@@ -2,6 +2,7 @@
 """Benchmark of the EGNN forward hot path (BASELINE.json metric: node-pairs/sec, dim=512 N=1024).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference|eager] [--dtype bf16|fp32]
+                    [--dump-outputs DIR]
 
 One "step" = one EGNN(dim=512) layer forward over one batch (B=4 graphs x N=1024 nodes, dense
 all-pairs = 4,194,304 node pairs) of synthetic N(0,1) inputs with the reference's default init
@@ -15,14 +16,18 @@ per step with CUDA events on the launch stream (L2 flushed between steps, flush 
 max over ranks.  `e2e` = the same through the public module API with pinned HOST tensors
 (H2D + D2H inside the timed region).  `roofline` describes the fused edge kernel, timed live by
 the library's own CUDA-event stage brackets (egnn_profile_*).  `cpu_baseline` = the UNMODIFIED
-reference's own torch forward (baseline/_ref, installed by baseline/install_ref.py) on the host cores,
+reference's own torch forward (oracle/_ref, installed by oracle/install_ref.py) on the host cores,
 one graph of the batch at a time (BASELINE.md section 3).  `gpu_eager_baseline` = the same unmodified
-reference in PyTorch eager on the same B200 (the ">= 10x" comparison of BASELINE.json's north_star).
+reference in PyTorch eager on the same GPU (the ">= 10x" comparison of BASELINE.json's north_star).
 `secondary` = the other four BASELINE configurations (c1, c3, c4 at 8 graphs per GPU, c5).
 
-`--impl reference` times the reference's own torch CPU forward (kind "reference"; if baseline/_ref is
+`--impl reference` times the reference's own torch CPU forward (kind "reference"; if oracle/_ref is
 absent, oracle/egnn_torch_port.py -- a torch restatement with the same ATen call sequence -- and kind
 "port"), all host threads, one graph of the same B=4 x N=1024 workload per step.
+
+`--dump-outputs DIR` writes what the timed path returned in its last timed step, `feats_out.npy` [B,N,dim] and
+`coors_out.npy` [B,N,3] (float32, 8 MB in all for c2), so that two builds can be compared output for output: the
+inputs and parameters depend only on the workload and the rank (fixed seeds).
 """
 from __future__ import annotations
 
@@ -60,14 +65,14 @@ def peaks():
         p = json.load(open(path))
         return dict(hbm_gbs=p["hbm_gbs"], bf16_tflops=p["bf16_tflops"], sm_max_mhz=p.get("sm_max_mhz", 1965.0),
                     source="measured (MEASURED_PEAKS.json)")
-    return dict(hbm_gbs=6650.0, bf16_tflops=1590.0, sm_max_mhz=1965.0, source="fallback (B200_PROFILING.md)")
+    return dict(hbm_gbs=3350.0, bf16_tflops=989.0, sm_max_mhz=1980.0, source="H100 SXM data sheet (dense bf16, 700 W)")
 
 
 # ----------------------------------------------------------------------------- clocks
 class ClockSampler:
     FIELDS = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
               "clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,"
-              "clocks_event_reasons.sw_power_cap")
+              "clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, index):
         self.rows, self.proc = [], None
@@ -92,18 +97,22 @@ class ClockSampler:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, pw, reasons = [], [], [], set()
+        sm, mx, pw, pl, reasons = [], [], [], [], set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
                 sm.append(float(r[0])); mx.append(float(r[1])); pw.append(float(r[2]))
             except Exception:
                 continue
+            try:
+                pl.append(float(r[7]))
+            except Exception:
+                pass
             for n, v in zip(names, r[3:7]):
                 if v.lower().startswith("active"):
                     reasons.add(n)
         return dict(sm_mhz=statistics.median(sm) if sm else None, sm_max_mhz=max(mx) if mx else None,
-                    power_w_max=max(pw) if pw else None, samples=len(sm), reasons=sorted(reasons))
+                    power_w_max=max(pw) if pw else None, power_limit_w=max(pl) if pl else None, samples=len(sm), reasons=sorted(reasons))
 
 
 # ----------------------------------------------------------------------------- workload
@@ -143,7 +152,7 @@ def equivariance_error(mod, feats, coors, dtype, device):
     """tests/test_equivariance.py:8-34 as a number: max|feats(Rx+t) - feats(x)|, max|coors(Rx+t) - (coors(x)R+t)|,
     reported absolute AND relative to the output magnitude (the c2 outputs are O(100): x_i + sum over 1024
     neighbours), plus the same figure for the unmodified reference in fp32 GPU-eager on the same inputs when
-    baseline/_ref is installed."""
+    oracle/_ref is installed."""
     g = torch.Generator().manual_seed(7)
     q, _ = torch.linalg.qr(torch.randn(3, 3, generator=g, dtype=torch.float64))
     t = torch.randn(1, 1, 3, generator=g, dtype=torch.float64)
@@ -175,10 +184,10 @@ def equivariance_error(mod, feats, coors, dtype, device):
     return out
 
 
-# ----------------------------------------------------------------------------- the reference (baseline/_ref)
+# ----------------------------------------------------------------------------- the reference (oracle/_ref)
 def load_reference():
-    """The UNMODIFIED reference package installed under baseline/_ref (baseline/install_ref.py), or None."""
-    ref_dir = os.path.join(REPO, "baseline", "_ref")
+    """The UNMODIFIED reference package installed under oracle/_ref (oracle/install_ref.py), or None."""
+    ref_dir = os.path.join(REPO, "oracle", "_ref")
     if not os.path.exists(os.path.join(ref_dir, "egnn_pytorch", "egnn_pytorch.py")):
         return None
     if ref_dir not in sys.path:
@@ -200,7 +209,7 @@ def bench_config(world, w, path=None):
 
 
 class CpuReference:
-    """The reference's own dense forward on the host cores: `EGNN(dim=512)` from baseline/_ref (kind 'reference'),
+    """The reference's own dense forward on the host cores: `EGNN(dim=512)` from oracle/_ref (kind 'reference'),
     else the torch restatement oracle/egnn_torch_port.py (kind 'port').  fp32, eval, no_grad, all host threads
     (BASELINE.md section 3); one graph of the B=4 batch per call -- B=4 at once needs > 62 GB of intermediates."""
 
@@ -245,7 +254,7 @@ class CpuReference:
         full = self.n == self.w["N"]
         what = "one full graph" if full else f"the first {self.n} of {self.w['N']} nodes of one graph (dense all-pairs on the sub-graph)"
         return (f"{calls} forward(s), each {what} of the B={self.w['B']} batch ({pairs} pairs, {secs:.1f} s); "
-                f"{'unmodified reference egnn_pytorch.EGNN (baseline/_ref)' if self.kind == 'reference' else 'torch restatement oracle/egnn_torch_port.py'}"
+                f"{'unmodified reference egnn_pytorch.EGNN (oracle/_ref)' if self.kind == 'reference' else 'torch restatement oracle/egnn_torch_port.py'}"
                 f", torch {torch.__version__} CPU fp32, torch.set_num_threads({self.threads})")
 
 
@@ -314,13 +323,16 @@ def time_ms(fn, iters, warm=3):
 
 
 def gpu_eager_baseline(name, dev, ours_ms):
-    """The unmodified reference in PyTorch eager on this GPU (bf16 and fp32), same workload, same B=4 batch at once."""
+    """The unmodified reference in PyTorch eager on this GPU (bf16 and fp32), same workload.  One step runs the B graphs
+    of the batch one after the other: the reference materialises [N,N,2E] intermediates per graph (c2 fp32: ~25 GB per
+    graph), and the whole batch at once does not fit in an 80 GB H100."""
     ref = load_reference()
     if ref is None:
-        return dict(unavailable="baseline/_ref not installed (python baseline/install_ref.py)")
+        return dict(unavailable="oracle/_ref not installed (python oracle/install_ref.py)")
     w = WORKLOADS[name]
     pairs = w["B"] * w["N"] * w["N"]
-    out = dict(kind="unmodified reference egnn_pytorch.EGNN (baseline/_ref), PyTorch eager, same GPU, inputs resident")
+    out = dict(kind="unmodified reference egnn_pytorch.EGNN (oracle/_ref), PyTorch eager, same GPU, inputs resident, "
+                    "one graph of the batch per call")
     for tag, dt, iters in (("bf16", torch.bfloat16, 5), ("fp32", torch.float32, 3)):
         try:
             torch.manual_seed(0)
@@ -329,7 +341,7 @@ def gpu_eager_baseline(name, dev, ours_ms):
             f = torch.randn(w["B"], w["N"], w["cfg"]["dim"], generator=g).to(dev, dt)
             x = torch.randn(w["B"], w["N"], w["C"], generator=g).to(dev, dt)
             torch.cuda.reset_peak_memory_stats(dev)
-            ms = time_ms(lambda: mod(f, x), iters, warm=2)
+            ms = time_ms(lambda: [mod(f[b:b + 1], x[b:b + 1]) for b in range(w["B"])], iters, warm=2)
             out[tag] = dict(ms_per_step=ms, pairs_per_s=pairs / ms * 1e3, peak_mem_gb=torch.cuda.max_memory_allocated(dev) / 2 ** 30,
                             speedup_of_this_repo=ms / ours_ms)
             del mod, f, x
@@ -415,7 +427,7 @@ def arm_ours(args):
     mod, feats, coors = build_workload(args.workload, dtype, dev, seed=rank)
     f_dev, x_dev = feats.to(dev, dtype), coors.to(dev)
     pairs_rank = w["B"] * w["N"] * w["N"]
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)        # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device=dev)        # > 50 MB L2
 
     def sync_all():
         torch.cuda.synchronize(dev)
@@ -439,10 +451,15 @@ def arm_ours(args):
     for a, b in evs:
         flush.zero_()                      # L2 flush between timed iterations (not timed)
         a.record()
-        mod(f_dev, x_dev)
+        last = mod(f_dev, x_dev)
         b.record()
     sync_all()
     clocks = sampler.stop() if sampler else None
+    if args.dump_outputs and rank == 0:
+        os.makedirs(args.dump_outputs, exist_ok=True)
+        for name, t in zip(("feats_out", "coors_out"), last):
+            np.save(os.path.join(args.dump_outputs, f"{name}.npy"), t.float().cpu().numpy())
+    del last
     ms_total = sum(a.elapsed_time(b) for a, b in evs)
     ms = (C.c_float * 4)(); spans = (C.c_int32 * 4)(); launches = C.c_int64()
     lib.egnn_profile_read(ms, spans, C.byref(launches), 1)
@@ -478,19 +495,15 @@ def arm_ours(args):
     pair_ms = ms[2] / max(1, spans[2])
     pair_s = pair_ms * 1e-3
     es = 2 if dtype == torch.bfloat16 else 4
-    sfu_peak = 148 * 16 * pk["sm_max_mhz"] * 1e6 / 1e9                 # G activations / s  (16 MUFU/clk/SM)
+    n_sm = torch.cuda.get_device_properties(dev).multi_processor_count
+    sfu_peak = n_sm * 16 * pk["sm_max_mhz"] * 1e6 / 1e9                # G activations / s  (16 MUFU/clk/SM)
     act_rate = pairs_rank * wp["act"] / pair_s / 1e9
-    traffic = None
-    tpath = os.path.join(REPO, "profiles", "traffic.json")
-    if os.path.exists(tpath):
-        traffic = json.load(open(tpath)).get(f"{args.workload}:{path}")
-    tensor_tf = pairs_rank * wp["tensor_flops"] / pair_s / 1e12 if path == "bf16-tcgen05" else 0.0
+    tensor_tf = pairs_rank * wp["tensor_flops"] / pair_s / 1e12 if path == "bf16-tc" else 0.0
     roofline = dict(
         bound="sfu", kernel="fused edge kernel (stage 2 of egnn_layer_forward)", path=path,
-        achieved=act_rate, peak=sfu_peak, unit="Gsilu/s", frac=act_rate / sfu_peak, traffic=traffic,
+        achieved=act_rate, peak=sfu_peak, unit="Gsilu/s", frac=act_rate / sfu_peak,
         note="split formulation: the binding unit is the MUFU/SFU pipe (SURVEY.md section 8(d)); "
-             f"peak = 148 SM x 16 MUFU/clk x {pk['sm_max_mhz']:.0f} MHz; the kernel's own instruction mix without any "
-             "synchronisation tops out at 15.0 of 16 /clk/SM (profiles/r02_pipe_bench.txt)",
+             f"peak = {n_sm} SM x 16 MUFU/clk x {pk['sm_max_mhz']:.0f} MHz",
         launch_ms=pair_ms, stage_ms_per_step={k: ms[i] / args.steps for i, k in
                                               enumerate(["select", "node_pre", "edge", "node_post"])},
         tensor=dict(achieved=tensor_tf, peak=pk["bf16_tflops"], unit="TFLOP/s", frac=tensor_tf / pk["bf16_tflops"],
@@ -503,8 +516,8 @@ def arm_ours(args):
     out = dict(
         metric="EGNN fwd node-pairs/sec (dim=512 N=1024)", value=value, unit="pairs/s", n_gpus=world,
         steps=args.steps, warmup=max(args.warmup, 3), ms_per_step=ms_per_step, higher_is_better=True, scaling="weak",
-        vs_baseline=None, dtype="bf16" if path == "bf16-tcgen05" else "f32", data="synthetic",
-        config=bench_config(world, w), kernel_path=path,
+        vs_baseline=None, dtype="bf16" if path == "bf16-tc" else "f32", data="synthetic",
+        config=bench_config(world, w), kernel_path=path, gpu=torch.cuda.get_device_name(dev),
         e2e=dict(value=e2e_value, unit="pairs/s", h2d_bytes_per_step=h2d, d2h_bytes_per_step=d2h,
                  ms_per_step=e2e_s / args.steps * 1e3),
         gpu_launches=int(launches.value), clocks=clocks, roofline=roofline)
@@ -559,7 +572,7 @@ def train_step_probe(workload, dev, pairs):
 
 
 def arm_reference(args):
-    """The reference's own torch forward on the host cores (baseline/_ref; torch restatement if absent), rank 0 only.
+    """The reference's own torch forward on the host cores (oracle/_ref; torch restatement if absent), rank 0 only.
     Each step = one graph of the B=4 x N=1024 batch (graphs cycle through the batch), sized down to a sub-graph only
     if the whole --steps/--warmup run would not end within a few minutes on this host."""
     world, rank = int(os.environ.get("WORLD_SIZE", "1")), int(os.environ.get("RANK", "0"))
@@ -602,7 +615,11 @@ def main():
     ap.add_argument("--dtype", default="bf16", choices=["bf16", "fp32"])
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--lean", action="store_true", help="metric, e2e and roofline only (profiling runs)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the outputs of the last timed step as DIR/<name>.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        ap.error("--dump-outputs writes the outputs of this library's timed path: use it with --impl ours")
     if args.impl == "cpu-sample":
         print(json.dumps(cpu_sample(args.workload)))
         return

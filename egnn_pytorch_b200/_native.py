@@ -2,7 +2,7 @@
 
 There is no CPU fallback: if the shared library is missing or does not export the expected
 symbols, importing the kernels fails loudly.  Build it with `python -m egnn_pytorch_b200.build`
-(or `__graft_entry__.build()`); it is compiled for sm_100a only.
+(or `__graft_entry__.build()`); it is compiled for sm_90a (H100) only.
 """
 from __future__ import annotations
 
@@ -154,7 +154,7 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise NativeLibraryError(
-            f"{LIB_PATH} not found: egnn_pytorch_b200 has no CPU fallback. Build the sm_100a library with "
+            f"{LIB_PATH} not found: egnn_pytorch_b200 has no CPU fallback. Build the sm_90a library with "
             f"`python -m egnn_pytorch_b200.build` (needs nvcc).")
     try:
         lib = C.CDLL(LIB_PATH)

@@ -1,4 +1,4 @@
-"""Build libegnn_b200.so in-tree with nvcc for sm_100a (cross-compiles without a GPU).
+"""Build libegnn_b200.so in-tree with nvcc for sm_90a (H100; cross-compiles without a GPU).
 
     python -m egnn_pytorch_b200.build [--force]
 """
@@ -16,7 +16,7 @@ LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libegnn_b200.so")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC",
 ]
 OBJ_DIR = os.path.join(HERE, "build")          # git-ignored; objects are rebuilt per source when stale
@@ -68,7 +68,7 @@ def build(force=False, verbose=False):
             sys.stderr.write(err)
     if failed:
         raise RuntimeError("nvcc failed building libegnn_b200.so")
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-shared", "-Xcompiler", "-fPIC", "-lcuda", "-o", LIB] + objs
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-shared", "-Xcompiler", "-fPIC", "-lcuda", "-o", LIB] + objs
     res = subprocess.run(cmd, capture_output=True, text=True)
     if res.returncode != 0:
         sys.stderr.write(res.stdout + res.stderr)

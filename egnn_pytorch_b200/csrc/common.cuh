@@ -1,4 +1,4 @@
-// Shared helpers for libegnn_b200 (sm_100a only).
+// Shared helpers for libegnn_b200 (sm_90a only).
 #pragma once
 
 #include <cuda_runtime.h>
@@ -6,6 +6,7 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <math.h>
+#include <mutex>
 
 #include "../../include/egnn_b200.h"
 
@@ -30,6 +31,21 @@ namespace egnn {
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline size_t round_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 __host__ __device__ inline int round_up_i(int a, int b) { return (a + b - 1) / b * b; }
+
+// Streaming-multiprocessor count of the current device (cached per device): grid sizes follow the GPU they run on.
+inline int sm_count(int* out) {
+  static std::mutex mu;
+  static int cached[64] = {0};
+  int dev = 0;
+  EGNN_CUDA_TRY(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  if (dev < 64 && cached[dev] > 0) { *out = cached[dev]; return EGNN_OK; }
+  int n = 0;
+  EGNN_CUDA_TRY(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
+  if (dev < 64) cached[dev] = n;
+  *out = n;
+  return EGNN_OK;
+}
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {
@@ -112,29 +128,14 @@ template <typename T> __device__ __forceinline__ T sq_acc(T a, T acc);
 template <> __device__ __forceinline__ float sq_acc<float>(float a, float acc) { return __fadd_rn(acc, __fmul_rn(a, a)); }
 template <> __device__ __forceinline__ double sq_acc<double>(double a, double acc) { return __dadd_rn(acc, __dmul_rn(a, a)); }
 
-// Two values that travel together through a contraction.  fp32: one 64-bit register pair and one packed FFMA2
-// (fma.rn.f32x2, the same IEEE fma per lane, so results are bit-identical to scalar code) per update -- the SIMT pair
-// kernels are issue-bound and most of their instructions are these contractions; fp64: two DFMAs.
-template <typename T> struct Pk2;
-template <> struct Pk2<float> {
-  unsigned long long v;
-  __device__ __forceinline__ static Pk2 make(float lo, float hi) {
-    Pk2 r;
-    asm("mov.b64 %0, {%1, %2};" : "=l"(r.v) : "f"(lo), "f"(hi));
-    return r;
-  }
-  __device__ __forceinline__ void fma(const Pk2& a, const Pk2& b) {       // this += a * b
-    asm("fma.rn.f32x2 %0, %1, %2, %0;" : "+l"(v) : "l"(a.v), "l"(b.v));
-  }
-  __device__ __forceinline__ float lo() const { float x, y; asm("mov.b64 {%0, %1}, %2;" : "=f"(x), "=f"(y) : "l"(v)); return x; }
-  __device__ __forceinline__ float hi() const { float x, y; asm("mov.b64 {%0, %1}, %2;" : "=f"(x), "=f"(y) : "l"(v)); return y; }
-};
-template <> struct Pk2<double> {
-  double x, y;
-  __device__ __forceinline__ static Pk2 make(double lo, double hi) { Pk2 r; r.x = lo; r.y = hi; return r; }
-  __device__ __forceinline__ void fma(const Pk2& a, const Pk2& b) { x = ::fma(a.x, b.x, x); y = ::fma(a.y, b.y, y); }
-  __device__ __forceinline__ double lo() const { return x; }
-  __device__ __forceinline__ double hi() const { return y; }
+// Two values that travel together through a contraction: two independent FMAs per update (Hopper has no packed
+// fp32 FMA, so fp32 and fp64 take the same form).
+template <typename T> struct Pk2 {
+  T x, y;
+  __device__ __forceinline__ static Pk2 make(T lo, T hi) { Pk2 r; r.x = lo; r.y = hi; return r; }
+  __device__ __forceinline__ void fma(const Pk2& a, const Pk2& b) { x = fma_t<T>(a.x, b.x, x); y = fma_t<T>(a.y, b.y, y); }
+  __device__ __forceinline__ T lo() const { return x; }
+  __device__ __forceinline__ T hi() const { return y; }
 };
 
 // 4 consecutive elements, 4-element aligned.

@@ -93,7 +93,9 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
       t.M = s.M; t.dim = s.dim; t.H = s.H; t.Hp = s.Hp; t.E = s.E;
       const size_t smem = tables_small_simt_smem<T>(s.dim, s.Hp);
       EGNN_TRY(ensure_dynamic_smem(tables_small_simt_kernel<T>, smem));
-      tables_small_simt_kernel<T><<<std::min(ceil_div(s.M, SN_WARPS), 4 * small_node_sms()), SN_WARPS * 32, smem, st>>>(t);
+      int sms = 0;
+      EGNN_TRY(sm_count(&sms));
+      tables_small_simt_kernel<T><<<std::min(ceil_div(s.M, SN_WARPS), 4 * sms), SN_WARPS * 32, smem, st>>>(t);
       EGNN_LAUNCH_CHECK();
       count_launch();
     } else {
@@ -157,7 +159,9 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
     n.do_norm = (d.flags & EGNN_FLAG_NORM_FEATS) ? 1 : 0;
     const size_t smem = node_small_simt_smem<T>(s.dim, s.m);
     EGNN_TRY(ensure_dynamic_smem(node_update_small_simt_kernel<T>, smem));
-    node_update_small_simt_kernel<T><<<std::min(ceil_div(Mr, SN_WARPS), 4 * small_node_sms()), SN_WARPS * 32, smem, st>>>(n);
+    int sms = 0;
+    EGNN_TRY(sm_count(&sms));
+    node_update_small_simt_kernel<T><<<std::min(ceil_div(Mr, SN_WARPS), 4 * sms), SN_WARPS * 32, smem, st>>>(n);
     EGNN_LAUNCH_CHECK();
     count_launch();
   } else if (uf) {
@@ -223,10 +227,12 @@ extern "C" int egnn_layer_pack_weights(const EgnnLayerDesc* desc, const EgnnLaye
   const Dims s = make_dims(*desc);
   if (desc->dtype == EGNN_DTYPE_BF16) return fast_pack_weights(*desc, *w, packed, packed_bytes, st);
   const SimtPackLayout L = simt_pack_layout(s);
+  int sms = 0;
+  EGNN_TRY(sm_count(&sms));
   if (desc->dtype == EGNN_DTYPE_F64)
-    simt_pack_kernel<double><<<148, 256, 0, st>>>(s, L, *w, desc->flags, static_cast<double*>(packed));
+    simt_pack_kernel<double><<<sms, 256, 0, st>>>(s, L, *w, desc->flags, static_cast<double*>(packed));
   else
-    simt_pack_kernel<float><<<148, 256, 0, st>>>(s, L, *w, desc->flags, static_cast<float*>(packed));
+    simt_pack_kernel<float><<<sms, 256, 0, st>>>(s, L, *w, desc->flags, static_cast<float*>(packed));
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
 }

@@ -44,7 +44,9 @@ static int launch_gemm_acc(const T* A, long ars, long aks, const T* B, long bks,
                            int Nc, int K, cudaStream_t st) {
   if (Mr <= 0 || Nc <= 0 || K <= 0) return EGNN_OK;
   const int tiles = ceil_div(Mr, 64) * ceil_div(Nc, 64);
-  int splits = std::max(1, std::min(ceil_div(296, tiles), ceil_div(K, 64)));
+  int sms = 0;
+  EGNN_TRY(sm_count(&sms));
+  int splits = std::max(1, std::min(ceil_div(2 * sms, tiles), ceil_div(K, 64)));     // about two CTAs per SM
   splits = std::min(splits, 65535);
   const int kper = round_up_i(ceil_div(K, splits), 16);
   splits = ceil_div(K, kper);
@@ -292,7 +294,9 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
   EGNN_TRY(launch_gemm_acc<T>(gP + s.Hp, 1, ldP, feats, dim, 1, gW1 + dim, s.E, s.H, dim, M, st));      // dW1_j = gB^T h
   EGNN_TRY(launch_colsum<T>(gP, ldP, M, s.H, static_cast<T*>(gr.w.edge_b1), st));                       // db1
 
-  unpack_grads_kernel<T><<<148, 256, 0, st>>>(s, L, d.flags, gpk, W1, static_cast<const T*>(w.label_emb), gr.w);
+  int sms = 0;
+  EGNN_TRY(sm_count(&sms));
+  unpack_grads_kernel<T><<<sms, 256, 0, st>>>(s, L, d.flags, gpk, W1, static_cast<const T*>(w.label_emb), gr.w);
   EGNN_LAUNCH_CHECK();
   (void)uc; (void)h1;
   return EGNN_OK;

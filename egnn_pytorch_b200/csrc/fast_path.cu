@@ -1,6 +1,6 @@
 // bf16 tensor-core path of the layer (EGNN_DTYPE_BF16): parameter packing, workspace layout and the
-// per-layer launch sequence   node tables (tcgen05 GEMM x2) -> fused edge kernel (tc_pair.cuh)
-//                             -> LayerNorm/concat -> node MLP (tcgen05 GEMM x2).
+// per-layer launch sequence   node tables (wgmma GEMM x2) -> fused edge kernel (tc_pair.cuh)
+//                             -> LayerNorm/concat -> node MLP (wgmma GEMM x2).
 // Option sets the tensor-core kernels do not cover return EGNN_ERR_UNSUPPORTED; the binding then runs
 // the fp32 SIMT kernels (never a CPU path).
 #include <stdlib.h>
@@ -133,7 +133,7 @@ __global__ void fast_pack_kernel(FastDims f, FastPack L, EgnnLayerWeights w, uin
     }
     wq[x] = 0.5f * v;
   }
-  // W2 [16][H] -> UMMA K-major core matrices: [slab = c/16][kc = (c%16)/8][nc = n/8][r = n%8][e = c%8]
+  // W2 [16][H] -> K-major core matrices: [slab = c/16][kc = (c%16)/8][nc = n/8][r = n%8][e = c%8]
   __nv_bfloat16* w2p = reinterpret_cast<__nv_bfloat16*>(out + L.w2p);
   for (size_t x = t0; x < (size_t)Hp * 16; x += stride) {
     const int e = (int)(x & 7), r = (int)((x >> 3) & 7), nc = (int)((x >> 6) & 1), kc = (int)((x >> 7) & 1);
@@ -240,24 +240,8 @@ int ensure_dyn_smem(K kernel, size_t bytes) {
   return EGNN_OK;
 }
 
-int sm_count(int* out) {
-  static std::mutex mu;
-  static int cached[64] = {0};
-  int dev = 0;
-  EGNN_CUDA_TRY(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lock(mu);
-  if (dev < 64 && cached[dev] > 0) { *out = cached[dev]; return EGNN_OK; }
-  int n = 0;
-  EGNN_CUDA_TRY(cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev));
-  if (dev < 64) cached[dev] = n;
-  *out = n;
-  return EGNN_OK;
-}
-
 // Optional start-up delay between the warpgroups of the persistent dense kernel (tc_pair.cuh), EGNN_B200_SKEW_NS.
-// Default 0: measured on B200 (profiles/r02_tc_pair_skew_sweep.txt) de-phasing the warpgroups' epilogues buys nothing --
-// the kernel is bound by per-warp latency (1/2/3/4 warps per sub-partition reach 0.28/0.47/0.58/0.67 of the MUFU
-// roofline), not by the pipe idling during the epilogues.
+// Default 0 (no de-phasing).
 uint32_t pair_skew_ns() {
   static const uint32_t v = [] {
     const char* e = getenv("EGNN_B200_SKEW_NS");
@@ -306,7 +290,9 @@ int fast_pack_weights(const EgnnLayerDesc& d, const EgnnLayerWeights& w, void* p
   const FastDims f = fast_dims(d);
   const FastPack L = fast_pack_layout(f);
   if (bytes < L.total) return EGNN_ERR_WORKSPACE;
-  fast_pack_kernel<<<296, 256, 0, st>>>(f, L, w, d.flags, static_cast<unsigned char*>(packed));
+  int sms = 0;
+  EGNN_TRY(sm_count(&sms));
+  fast_pack_kernel<<<2 * sms, 256, 0, st>>>(f, L, w, d.flags, static_cast<unsigned char*>(packed));
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
 }

@@ -1,4 +1,4 @@
-// bf16 tensor-core ("fast") path: tcgen05 / TMEM / TMA kernels for sm_100a (fast_path.cu).
+// bf16 tensor-core ("fast") path: wgmma / mma.sync / TMA kernels for sm_90a (fast_path.cu).
 #pragma once
 #include "common.cuh"
 

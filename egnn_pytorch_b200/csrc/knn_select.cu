@@ -257,7 +257,9 @@ static int launch_select(int B, int N, int C, int k, const void* coors, const ui
       attr_set[dev] = true;
     }
     // 16 rows per CTA halve the staging work per row; small problems keep 8 so that more SMs take part
-    const bool wide = (long)B * ceil_div(N, 16) >= 296;
+    int sms = 0;
+    EGNN_TRY(sm_count(&sms));
+    const bool wide = (long)B * ceil_div(N, 16) >= 2L * sms;
     dim3 grid(ceil_div(N, wide ? 16 : 8), B);
     const size_t smem = sel_smem_bytes<T>(C, wide ? 16 : 8);
     if (C == 3) {

@@ -80,7 +80,9 @@ static int launch_gemm(const T* A, int lda, const T* W, int ldw, const T* bias, 
   const size_t skinny_smem = (size_t)16 * ((K + V - 1) / V * V) * sizeof(T);
   if (Mr <= 16 && skinny_smem <= 96 * 1024) {
     // columns per warp: as many as still give about one CTA per SM (the kernel is bound by weight streaming)
-    const int cols = Nout >= 148 * SKINNY_WARPS * 4 ? 4 : (Nout >= 148 * SKINNY_WARPS * 2 ? 2 : 1);
+    int sms = 0;
+    EGNN_TRY(sm_count(&sms));
+    const int cols = Nout >= sms * SKINNY_WARPS * 4 ? 4 : (Nout >= sms * SKINNY_WARPS * 2 ? 2 : 1);
     const int grid = ceil_div(Nout, SKINNY_WARPS * cols);
     if (cols == 4) {
       EGNN_TRY(ensure_dynamic_smem(gemm_skinny_kernel<T, ACT, RES, 4>, skinny_smem));

@@ -149,7 +149,7 @@ gemm_nt_kernel(const T* __restrict__ A, int lda, const T* __restrict__ W, int ld
 // The latency-bound configs (BASELINE c1: 16 nodes, 12.7 MB of fp32 weights) are bound by how fast the WEIGHTS stream
 // from L2 / HBM: one CTA = 4 warps x COLS output columns, the <= 16 activation rows staged once in shared memory, every
 // lane pulls 16-byte pieces of its COLS weight rows (COLS independent 128-bit loads in flight per step) and keeps the
-// 16 x COLS partial sums in registers; COLS is picked by the launcher so that the grid fills the 148 SMs.
+// 16 x COLS partial sums in registers; COLS is picked by the launcher so that the grid fills the SMs of the device.
 constexpr int SKINNY_WARPS = 4;
 
 template <typename T> struct SkinnyVec;            // 16-byte vector of T
@@ -571,7 +571,7 @@ pair_kernel(const PairArgs<T> a) {
 // =====================================================================================
 // Dense all-pairs variant with register tiling over rows: a thread owns neighbour j and PP query rows, so every
 // W2 row fetched from shared memory feeds PP pairs (the thread-per-pair kernel above is bound by the 16
-// broadcast wavefronts per hidden channel that W2 costs; see profiles/).  One warp = PP rows x 32 neighbours,
+// broadcast wavefronts per hidden channel that W2 costs).  One warp = PP rows x 32 neighbours,
 // 4 warps per CTA; per-row sums are reduced with shuffles per j-tile and kept in shared memory.
 // =====================================================================================
 template <typename T>

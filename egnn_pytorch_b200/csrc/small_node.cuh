@@ -1,8 +1,8 @@
 // Per-node stages of the bf16 path for narrow layers (dim <= 64): one WARP per node, weights staged once per CTA in
 // shared memory (transposed, bf16), fp32 arithmetic.
 //
-// Why: with dim = 32 the per-node GEMMs of a layer are 9 k and 5 k FMAs per node -- the tcgen05 GEMM (TMEM allocation,
-// cp.async ring, 128-row tiles) spends 10-11 us of fixed latency on each of them, and the node update needs three
+// Why: with dim = 32 the per-node GEMMs of a layer are 9 k and 5 k FMAs per node -- the tile GEMM (cp.async ring,
+// 128-row tiles) spends microseconds of fixed latency on each of them, and the node update needs three
 // launches (LayerNorm+concat, Linear+SiLU, Linear+residual).  BASELINE configs 3 and 5 (EGNN_Network, dim 32) are made
 // of exactly these launches.  Here:
 //   tables_small_kernel      A' = 0.5 (h W1_i^T + b1) (fp32), B' = 0.5 h W1_j^T (bf16)            (egnn_pytorch.py:283-287,
@@ -23,15 +23,6 @@ constexpr int SN_DIM_MAX = 64;
 constexpr size_t SMALL_NODE_SMEM_MAX = 160 * 1024;   // staged weights beyond this: the GEMM path
 constexpr int SN_TABLES_M_MAX = 4096;                // the table kernel re-reads its weights per node (28 % FMA density): measured
                                                      // faster than the GEMMs at 1024 nodes (12 vs 20 us), slower at 8192 (35 vs 21 us)
-
-inline int small_node_sms() {
-  static int sms = 0;
-  if (!sms) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) sms = 148;
-  }
-  return sms;
-}
 
 struct TablesSmallArgs {
   const __nv_bfloat16* feats;      // [M][dim]

@@ -1,6 +1,5 @@
-// Thin inline-PTX layer over the Blackwell (sm_100a) primitives the tensor-core path uses:
-// mbarrier, tcgen05 (TMEM alloc / st / ld / mma / commit / fences), cp.async and TMA bulk copies,
-// and the UMMA shared-memory / instruction descriptors.  Single-CTA (cta_group::1) only.
+// Thin inline-PTX layer over the Hopper (sm_90a) primitives the tensor-core path uses: mbarrier, wgmma (shared-memory
+// descriptors, fence / commit / wait), warp-level mma.sync, cp.async and TMA bulk copies.
 #pragma once
 
 #include <cuda_runtime.h>
@@ -80,123 +79,66 @@ __device__ __forceinline__ void mbar_wait_a(uint32_t bar, uint32_t parity) {
 
 // ------------------------------------------------------------------ proxies / fences
 __device__ __forceinline__ void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// ------------------------------------------------------------------ TMEM allocation (one full warp calls these)
-template <int COLS>
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "n"(COLS) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int COLS>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(COLS) : "memory");
-}
-
-// ------------------------------------------------------------------ descriptors
-// Shared-memory matrix descriptor, K-major operand, no swizzle ("interleave") canonical layout:
-// 8x8 core matrices of 8 rows x 16 bytes stored contiguously (128 B); `lbo` = byte distance between
-// the two core matrices adjacent in K, `sbo` = byte distance between core matrices adjacent in M/N
-// (cute::UMMA::SmemDescriptor, CUTLASS 4.x mma_sm100_desc.hpp; version_ = 1 for Blackwell).
-__device__ __forceinline__ uint64_t smem_desc_kmajor_noswizzle(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;          // descriptor version (Blackwell)
-  return d;                        // base_offset 0, lbo_mode 0, layout_type 0 (SWIZZLE_NONE)
-}
-
-// K-major operand in the 128-byte-swizzle canonical layout: rows of 128 B (64 bf16), groups of 8 rows = 1024 B
-// (`sbo`), the 16-byte chunk index of a row XOR-ed with (row % 8).  Tile base 1024-byte aligned; a K=16 step
-// advances the start address by 32 B inside the swizzle atom.  (Measured on B200: the no-swizzle layout above is
-// read by the tensor core at ~16 B/clk, this one at full rate -- it matters for M=N=128 GEMM tiles, not for the
-// 512-byte W2 slabs of the fused edge kernels.)
-__device__ __forceinline__ uint64_t smem_desc_kmajor_sw128(uint32_t saddr) {
+// ------------------------------------------------------------------ wgmma (one warpgroup of 128 threads)
+// Shared-memory matrix descriptor of a K-major operand in the 128-byte-swizzle canonical layout: rows of 128 B
+// (64 bf16), groups of 8 rows = 1024 B (`sbo`), the 16-byte chunk index of a row XOR-ed with (row % 8).  Tile base
+// 1024-byte aligned; a K=16 step advances the start address by 32 B inside the swizzle atom.
+__device__ __forceinline__ uint64_t wgmma_desc_kmajor_sw128(uint32_t saddr) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)1 << 16;                      // LBO: unused for swizzled K-major
   d |= (uint64_t)(1024 >> 4) << 32;            // SBO: 8-row group stride
-  d |= (uint64_t)1 << 46;                      // descriptor version (Blackwell)
-  d |= (uint64_t)2 << 61;                      // layout_type = SWIZZLE_128B
+  d |= (uint64_t)1 << 62;                      // layout_type = SWIZZLE_128B
   return d;
 }
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
-// Instruction descriptor for kind::f16 with bf16 A/B, fp32 D, both operands K-major
-// (cute::UMMA::InstrDescriptor bit layout).
-__host__ __device__ constexpr uint32_t idesc_bf16_f32(int M, int N) {
-  return (1u << 4)                  // c_format  = F32
-         | (1u << 7)                // a_format  = BF16
-         | (1u << 10)               // b_format  = BF16
-         | (0u << 15) | (0u << 16)  // a_major, b_major = K
-         | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-
-// ------------------------------------------------------------------ MMA issue (one thread)
-// D[tmem] (+)= A[smem] * B[smem]
-__device__ __forceinline__ void mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
+// D (+)= A * B^T, M=64 N=128 K=16, bf16 operands (both K-major in shared memory), fp32 accumulators in registers.
+// Thread t of warp w of the warpgroup holds d[r] = D[16 w + t/4 + 8 ((r >> 1) & 1)][8 (r >> 2) + 2 (t % 4) + (r & 1)].
+__device__ __forceinline__ void wgmma_m64n128k16_ss(float (&d)[64], uint64_t a_desc, uint64_t b_desc, uint32_t accumulate) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem]
-__device__ __forceinline__ void mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}" ::"r"(d_tmem),
-      "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// Arrive on an mbarrier when all previously issued tcgen05.mma of this thread have completed
-// (implies tcgen05.fence::before_thread_sync).
-__device__ __forceinline__ void mma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mma_commit_a(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
-// ------------------------------------------------------------------ TMEM <-> registers (warp-wide, 32 lanes x 32 bit)
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t (&r)[32]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,"
-      "%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15]), "=r"(r[16]),
-        "=r"(r[17]), "=r"(r[18]), "=r"(r[19]), "=r"(r[20]), "=r"(r[21]), "=r"(r[22]), "=r"(r[23]), "=r"(r[24]),
-        "=r"(r[25]), "=r"(r[26]), "=r"(r[27]), "=r"(r[28]), "=r"(r[29]), "=r"(r[30]), "=r"(r[31])
-      : "r"(taddr)
-      : "memory");
-}
-// 16 lanes x 256 bit fragment store, 4 repeats along the columns (32 columns): thread t of the warp holds, for
-// every 8-column group n (regs 4n..4n+3), row t/4 (regs 4n, 4n+1) and row t/4 + 8 (regs 4n+2, 4n+3), columns
-// 2*(t%4) and 2*(t%4)+1 of the group -- the mma-accumulator-style layout.  The lane field of taddr selects the
-// 16-lane half (+0 / +16 inside the warp's quadrant).
-__device__ __forceinline__ void tmem_st_16x256b_x4(uint32_t taddr, const uint32_t (&r)[16]) {
-  asm volatile(
-      "tcgen05.st.sync.aligned.16x256b.x4.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};" ::"r"(taddr),
-      "r"(r[0]), "r"(r[1]), "r"(r[2]), "r"(r[3]), "r"(r[4]), "r"(r[5]), "r"(r[6]), "r"(r[7]), "r"(r[8]), "r"(r[9]),
-      "r"(r[10]), "r"(r[11]), "r"(r[12]), "r"(r[13]), "r"(r[14]), "r"(r[15])
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %66, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,"
+      "%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,"
+      "%62,%63}, %64, %65, p, 1, 1, 0, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]),
+        "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]),
+        "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]),
+        "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]),
+        "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]),
+        "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]),
+        "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "l"(a_desc), "l"(b_desc), "r"(accumulate)
       : "memory");
 }
 
-// one 8-column group (one K=16 slab of the A operand): 4 registers per thread, same fragment layout as above
-__device__ __forceinline__ void tmem_st_16x256b_x1(uint32_t taddr, uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3) {
-  asm volatile("tcgen05.st.sync.aligned.16x256b.x1.b32 [%0], {%1,%2,%3,%4};" ::"r"(taddr), "r"(r0), "r"(r1), "r"(r2), "r"(r3) : "memory");
+// ------------------------------------------------------------------ warp-level MMA (fused edge kernels)
+// D += A * B, M=16 N=8 K=16, bf16 operands and fp32 accumulators in registers (mma.sync fragment layouts: lane
+// (lr = l/4, lq = l%4) holds A rows lr / lr+8 and B / D column lr (B) or 2 lq, 2 lq + 1 (D)).
+__device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t b0, uint32_t b1) {
+  asm volatile(
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3])
+      : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
+}
+
+// One K=16 slab of the fused edge kernels' second GEMM (hidden [32 pairs x 16] . W2 slab^T [16 x 16]) for the 16 pair
+// rows of one half of a warp's 32.  The hidden fragment h[0..3] is what the producers pack: h[0] / h[1] = row lr,
+// channels 4 lq .. 4 lq + 3, h[2] / h[3] = the same for row lr + 8.  K is a reduction index, so the four channels of a
+// lane may stand at mma positions (2 lq, 2 lq + 1 | 2 lq + 8, 2 lq + 9) as long as the B fragment uses the same order:
+// then B of lane (lr, lq) for output column n = 8 nt + lr is channels 4 lq .. 4 lq + 3 of W2 row n -- one 8-byte load
+// from the core-matrix packing of W2 (slab s at byte 512 s: [kc = k/8][nc = n/8][n % 8][k % 8]).
+__device__ __forceinline__ void mma_w2_slab(float (&acc)[2][4], const uint32_t (&h)[4], const unsigned char* w2s, int slab, int lr, int lq) {
+#pragma unroll
+  for (int nt = 0; nt < 2; ++nt) {
+    const uint2 bw = *reinterpret_cast<const uint2*>(w2s + slab * 512 + (lq >> 1) * 256 + nt * 128 + lr * 16 + (lq & 1) * 8);
+    mma_16816(acc[nt], h[0], h[2], h[1], h[3], bw.x, bw.y);
+  }
 }
 
 // ------------------------------------------------------------------ copies into shared memory
@@ -219,17 +161,8 @@ __device__ __forceinline__ void tma_bulk_g2s(uint32_t saddr, const void* gptr, u
 template <int V> struct IntC { static constexpr int value = V; };     // compile-time int tag for generic lambdas
 
 // ------------------------------------------------------------------ scalar helpers
-// Packed fp32x2 FMA (Blackwell FFMA2): two independent a*b+c in one issue slot.
-__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) {
-  unsigned long long ra, rb, rc, rd;
-  asm("mov.b64 %0, {%1, %2};" : "=l"(ra) : "f"(a.x), "f"(a.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rb) : "f"(b.x), "f"(b.y));
-  asm("mov.b64 %0, {%1, %2};" : "=l"(rc) : "f"(c.x), "f"(c.y));
-  asm("fma.rn.f32x2 %0, %1, %2, %3;" : "=l"(rd) : "l"(ra), "l"(rb), "l"(rc));
-  float2 d;
-  asm("mov.b64 {%0, %1}, %2;" : "=f"(d.x), "=f"(d.y) : "l"(rd));
-  return d;
-}
+// a*b+c for two channels (two FFMAs; kept as one call so the producers read as channel pairs)
+__device__ __forceinline__ float2 ffma2(float2 a, float2 b, float2 c) { return make_float2(fmaf(a.x, b.x, c.x), fmaf(a.y, b.y, c.y)); }
 __device__ __forceinline__ float tanh_fast(float x) {
   float y;
   asm("tanh.approx.f32 %0, %1;" : "=f"(y) : "f"(x));
@@ -242,18 +175,9 @@ __device__ __forceinline__ uint32_t pack_bf16x2(float lo, float hi) {
   asm("cvt.rn.bf16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi), "f"(lo));
   return r;
 }
-// c + (low / high bf16 half of u), one mixed-precision FHADD.BF16 each: the packed operand is consumed
-// through the .H0/.H1 register selectors, so no unpack instruction (and no fp32 copy of B') is needed.
-__device__ __forceinline__ float add_bf16_lo(uint32_t u, float c) {
-  float y;
-  asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %1;\n\tadd.rn.f32.bf16 %0, lo, %2;\n\t}" : "=f"(y) : "r"(u), "f"(c));
-  return y;
-}
-__device__ __forceinline__ float add_bf16_hi(uint32_t u, float c) {
-  float y;
-  asm("{\n\t.reg .b16 lo, hi;\n\tmov.b32 {lo, hi}, %1;\n\tadd.rn.f32.bf16 %0, hi, %2;\n\t}" : "=f"(y) : "r"(u), "f"(c));
-  return y;
-}
+// c + (low / high bf16 half of u): a bf16 is the upper half of the fp32 with the same value
+__device__ __forceinline__ float add_bf16_lo(uint32_t u, float c) { return __uint_as_float(u << 16) + c; }
+__device__ __forceinline__ float add_bf16_hi(uint32_t u, float c) { return __uint_as_float(u & 0xFFFF0000u) + c; }
 
 }  // namespace tc
 }  // namespace egnn

@@ -1,12 +1,11 @@
-// tcgen05 GEMM for the per-node contractions of the layer (bf16 operands, fp32 accumulation in TMEM):
+// wgmma GEMM for the per-node contractions of the layer (bf16 operands, fp32 accumulation in registers):
 //     out[r, n] = act( scale * (sum_k A[r,k] W[n,k] + bias[n]) ) + R[r, n]
 // used for  A' = 0.5 (h W1_i^T + b1)  (fp32 out),  B' = 0.5 h W1_j^T  (bf16 out)   [split of egnn_pytorch.py:287]
 //           h1 = SiLU([LN(h) | m_i] Wn1^T + bn1),  h' = h1 Wn2^T + bn2 + h                   [egnn_pytorch.py:335-337]
 //
-// 128x128 output tile per CTA, BK = 64, a six-stage shared-memory ring filled with cp.async straight into the
-// UMMA swizzle-128B K-major layout (128-byte rows, 8-row groups), one elected thread issues
-// tcgen05.mma (M=128, N=128, K=16) x4 per stage, completion tracked with tcgen05.commit -> mbarrier,
-// epilogue reads the accumulator with tcgen05.ld (thread == row).
+// 128x128 output tile per CTA (one warpgroup), BK = 64, a three-stage shared-memory ring filled with cp.async straight
+// into the wgmma swizzle-128B K-major layout (128-byte rows, 8-row groups); per stage the warpgroup issues
+// wgmma (M=64, N=128, K=16) x 2 row halves x 4, accumulating in registers (2 x 64 fp32 per thread).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -47,22 +46,10 @@ __global__ void __launch_bounds__(128, 1) tc_gemm_kernel(const TcGemmPair gp) {
   g.M = second ? gp.p[1].M : gp.p[0].M; g.Nv = second ? gp.p[1].Nv : gp.p[0].Nv; g.Nout = second ? gp.p[1].Nout : gp.p[0].Nout;
   g.K = second ? gp.p[1].K : gp.p[0].K; g.scale = second ? gp.p[1].scale : gp.p[0].scale; g.act = second ? gp.p[1].act : gp.p[0].act;
   extern __shared__ __align__(1024) unsigned char smem_raw[];
-  __shared__ uint64_t full[GEMM_STAGES], mma_done[GEMM_STAGES];
-  __shared__ uint32_t tmem_base_s;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int m0 = blockIdx.y * GEMM_BM, n0 = ((int)blockIdx.x - (second ? gp.nt0 : 0)) * GEMM_BN;
   const uint32_t s_base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;       // swizzle-128B tiles need 1024-byte alignment
   unsigned char* smem = smem_raw + (s_base - tc::smem_u32(smem_raw));
-
-  if (tid == 0) {
-    for (int x = 0; x < GEMM_STAGES; ++x) { tc::mbar_init(&full[x], 128); tc::mbar_init(&mma_done[x], 1); }
-    tc::mbar_fence_init();
-  }
-  if (warp == 0) tc::tmem_alloc<128>(&tmem_base_s);
-  tc::tc_fence_before();
-  __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = tmem_base_s;
 
   const int nk = (g.K + GEMM_BK - 1) / GEMM_BK;
   // Copy mapping: 8 consecutive lanes fetch the 8 16-byte K-chunks of one row (one fully used 128-byte line per
@@ -87,62 +74,65 @@ __global__ void __launch_bounds__(128, 1) tc_gemm_kernel(const TcGemmPair gp) {
   };
 
   // Multi-stage ring.  Every thread copies its rows of stage kt+DIST, waits for its own copies of stage kt
-  // (cp.async.wait_group), makes them visible to the tensor core (fence.proxy.async) and arrives on full[kt];
-  // thread 0 then issues the stage's MMAs.  A slot is re-filled only after tcgen05.commit signalled mma_done.
-  constexpr uint32_t IDESC = tc::idesc_bf16_f32(128, 128);
+  // (cp.async.wait_group) and makes them visible to the tensor core (fence.proxy.async); after a barrier the
+  // warpgroup issues the stage's wgmma (rows 0..63 and 64..127 of the tile, K=16 x 4).  It then waits only for the
+  // PREVIOUS k-step's wgmma (wait_group 1) -- the last reader of slot (kt+DIST) % STAGES -- and, after a barrier that
+  // makes that true for every warp, refills the slot: the wgmma of stage kt keep running through the refill, the
+  // copy wait and the barrier of the next k-step.
+  float acc[2][64];
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int r = 0; r < 64; ++r) acc[h][r] = 0.f;
   for (int kt = 0; kt < GEMM_DIST; ++kt) {
     if (kt < nk) load_stage(kt);
     tc::cp_async_commit();
   }
   for (int kt = 0; kt < nk; ++kt) {
-    const int nxt = kt + GEMM_DIST;
-    if (nxt < nk) {
-      const int prev = nxt - GEMM_STAGES;            // iteration whose MMAs last read slot nxt % STAGES
-      if (prev >= 0) tc::mbar_wait(&mma_done[nxt % GEMM_STAGES], (prev / GEMM_STAGES) & 1);
-      load_stage(nxt);
-    }
-    tc::cp_async_commit();
-    tc::cp_async_wait<GEMM_DIST>();        // this thread's copies of stage kt have landed
+    tc::cp_async_wait<GEMM_DIST - 1>();    // this thread's copies of stage kt have landed
     tc::fence_proxy_async_smem();          // cp.async (generic proxy) -> tensor core (async proxy)
-    tc::mbar_arrive(&full[kt % GEMM_STAGES]);
-    if (tid == 0) {
-      tc::mbar_wait(&full[kt % GEMM_STAGES], (kt / GEMM_STAGES) & 1);
-      tc::tc_fence_after();
-      const uint32_t sA = s_base + (kt % GEMM_STAGES) * 2 * GEMM_TILE_BYTES, sW = sA + GEMM_TILE_BYTES;
+    __syncthreads();
+    const uint32_t sA = s_base + (kt % GEMM_STAGES) * 2 * GEMM_TILE_BYTES, sW = sA + GEMM_TILE_BYTES;
+    tc::wgmma_fence();
 #pragma unroll
-      for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
-        const uint64_t da = tc::smem_desc_kmajor_sw128(sA + kk * 32);   // K=16 step = 32 B inside the swizzle atom
-        const uint64_t dw = tc::smem_desc_kmajor_sw128(sW + kk * 32);
-        tc::mma_ss(tmem, da, dw, IDESC, (kt > 0 || kk > 0) ? 1u : 0u);
-      }
-      tc::mma_commit(&mma_done[kt % GEMM_STAGES]);
+    for (int kk = 0; kk < GEMM_BK / 16; ++kk) {
+      const uint64_t dw = tc::wgmma_desc_kmajor_sw128(sW + kk * 32);   // K=16 step = 32 B inside the swizzle atom
+#pragma unroll
+      for (int h = 0; h < 2; ++h)                                      // rows 64 h .. 64 h + 63: 8 row groups of 1024 B
+        tc::wgmma_m64n128k16_ss(acc[h], tc::wgmma_desc_kmajor_sw128(sA + h * 8192 + kk * 32), dw, 1u);
     }
+    tc::wgmma_commit();
+    tc::wgmma_wait<1>();                   // the wgmma of k-step kt-1 are done (this warp) ...
+    __syncthreads();                       // ... and every warp's: slot (kt+DIST) % STAGES is free
+    const int nxt = kt + GEMM_DIST;
+    if (nxt < nk) load_stage(nxt);
+    tc::cp_async_commit();
   }
-  // the last commit covers every MMA issued before it
-  tc::mbar_wait(&mma_done[(nk - 1) % GEMM_STAGES], ((nk - 1) / GEMM_STAGES) & 1);
-  tc::tc_fence_after();
+  tc::wgmma_wait<0>();
+  __syncthreads();                         // every warp's wgmma are done: the ring is free for the epilogue
 
-  // Epilogue.  tcgen05.ld hands every thread one ROW of the accumulator; storing rows from lanes would touch 32
-  // different lines per instruction, so each warp transposes its 32x32 block through shared memory (the pipeline
-  // buffers are free now) and writes with lane = column: 128-byte (fp32) / 64-byte (bf16) contiguous stores,
-  // bias and residual loaded once per column / coalesced.
-  float* stg = reinterpret_cast<float*>(smem) + warp * (32 * 33);
-  const uint32_t trow = tmem + ((uint32_t)(warp * 32) << 16);
+  // Epilogue.  The accumulator fragments are spread over the warpgroup (see wgmma_m64n128k16_ss); they go through
+  // shared memory (the pipeline buffers are free now) so that each warp then writes its 32 rows with lane = column:
+  // 128-byte (fp32) / 64-byte (bf16) contiguous stores, bias and residual loaded once per column / coalesced.
+  constexpr int LDS = GEMM_BN + 4;
+  float* stg = reinterpret_cast<float*>(smem);                    // [128][LDS]
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int r = 0; r < 64; r += 2) {
+      const int row = 64 * h + 16 * warp + (lane >> 2) + 8 * ((r >> 1) & 1), col = 8 * (r >> 2) + 2 * (lane & 3);
+      *reinterpret_cast<float2*>(stg + row * LDS + col) = make_float2(acc[h][r], acc[h][r + 1]);
+    }
+  __syncthreads();
 #pragma unroll 1
   for (int cb = 0; cb < GEMM_BN / 32; ++cb) {
     const int col0 = n0 + cb * 32;
     if (col0 >= g.Nout) break;
-    uint32_t r[32];
-    tc::tmem_ld32(trow + cb * 32, r);
-    tc::tmem_wait_ld();
-#pragma unroll
-    for (int q = 0; q < 32; ++q) stg[lane * 33 + q] = __uint_as_float(r[q]);
-    __syncwarp();
     const int col = col0 + lane;
     const bool cin = col < g.Nout, cv = col < g.Nv;
     const float bcol = (cv && g.bias) ? g.bias[col] : 0.f;
     // residual rows: all 32 loads are issued before the first one is consumed (one dependent global load per row
-    // made the residual GEMM latency-bound: 63 us for 8.6 GFLOP, 62 % of its stall samples on that load)
+    // makes the residual GEMM latency-bound)
     __nv_bfloat16 rres[32];
     if (g.R) {
 #pragma unroll
@@ -157,7 +147,7 @@ __global__ void __launch_bounds__(128, 1) tc_gemm_kernel(const TcGemmPair gp) {
       if (row >= g.M) break;
       float x = 0.f;
       if (cv) {
-        x = (stg[rr * 33 + lane] + bcol) * g.scale;
+        x = (stg[(warp * 32 + rr) * LDS + cb * 32 + lane] + bcol) * g.scale;
         if (g.act == 1) x = __fdividef(x, 1.0f + __expf(-x));
         if (g.R) x += __bfloat162float(rres[rr]);
       }
@@ -166,11 +156,7 @@ __global__ void __launch_bounds__(128, 1) tc_gemm_kernel(const TcGemmPair gp) {
         else static_cast<__nv_bfloat16*>(g.out)[(size_t)row * g.ldo + col] = __float2bfloat16(x);
       }
     }
-    __syncwarp();
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<128>(tmem);
 }
 
 }  // namespace egnn

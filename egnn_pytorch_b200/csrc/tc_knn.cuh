@@ -5,11 +5,11 @@
 // mask incl. valid_radius (:292-300), coors MLP / clamp / CoorsNorm (:302-315), pooling (:319-333).  The
 // neighbour lists come from egnn_knn_select (knn_select.cu).
 //
-// Same machinery as tc_pair.cuh (hidden values produced in fp32 registers, stored as the bf16 A operand into
-// TMEM with tcgen05.st.16x256b, tcgen05.mma M=128 N=16 K=16 against the W2 slab in shared memory, accumulators
-// in TMEM, issue duty rotating over the warps of a warpgroup and deferred by half a round).  What differs:
-//   * one WARP owns one query row i and its 32 neighbour slots (slot >= k is padding), so a warpgroup's 128
-//     MMA rows are 4 query rows x 32 slots and the reduction over j is a single warp shuffle tree;
+// Same machinery as tc_pair.cuh (hidden values produced in fp32 registers and packed to bf16 directly in the
+// mma.sync A-fragment layout, m16n8k16 MMAs against the W2 slab in shared memory, accumulators in registers).
+// What differs:
+//   * one WARP owns one query row i and its 32 neighbour slots (slot >= k is padding), so the reduction over j is a
+//     single warp shuffle tree;
 //   * the B' row of every pair is gathered from L2 (8-byte pieces, contiguous across the 4 lanes that share a
 //     pair) and used once: each 64-channel round re-fills its B' registers for the next chunk right after use;
 //   * up to 4 continuous edge channels per pair are folded in on the CUDA cores (We from shared memory);
@@ -28,8 +28,7 @@ namespace egnn {
 
 constexpr int TK_ROWS = 16;        // query rows per CTA (one per warp): 16, or 8 when two CTAs then fit on an SM
 constexpr int TK_KC = 64;
-constexpr int TK_SLOTS = 3;
-constexpr int TK_WGCOLS = 128;     // 16 accumulator + 3 x 32 operand columns (+16 spare)
+constexpr int TK_ACC_LD = 18;      // floats per slot row of the per-warp accumulator transpose tile
 constexpr int TK_QE = 4;           // edge channels folded per pair (edge_dim <= 4, zero padded)
 
 constexpr int TK_LEAN = 0, TK_EDGES = 1, TK_GEN = 2;
@@ -65,21 +64,21 @@ inline size_t tc_knn_smem_bytes(int Hp, int mode, int Q = 1, int rows = TK_ROWS)
   n += (size_t)tc_knn_wq_rows(mode, Q) * Hp * 4;   // wd | We | generic Wq
   n += (size_t)TP_EPI_FLOATS * 4;             // epilogue constants
   n += mode == TK_GEN ? (size_t)rows * Q * 32 * 4 : 0;   // per-warp scalar tile [Q][32 slots]
-  n += 64 + 32 * 8;                           // tmem pointer, mbarriers
+  n += (size_t)rows * 32 * TK_ACC_LD * 4;     // per-warp accumulator transpose tile [32 slots][TK_ACC_LD]
+  n += 64 + 8;                                // mbarrier
   return n + 128;
 }
 
-// Rows per CTA: a CTA runs its prologue (TMEM allocation, staging W2 / A' / channel weights, the dependent gathers of
+// Rows per CTA: a CTA runs its prologue (staging W2 / A' / channel weights, the dependent gathers of
 // neighbour indices, coordinates and edge channels), 17-odd chunks and the coors-MLP epilogue back to back, so with one
 // CTA per SM the MUFU pipe idles through every prologue and epilogue (c4: 52 us per CTA for 19 us of MUFU work).  With
-// ROWS = 8 (256 threads, 256 TMEM columns, half the A' rows) two CTAs are resident and cover each other's phases; the
+// ROWS = 8 (256 threads, half the A' rows) two CTAs are resident and cover each other's phases; the
 // host takes ROWS = 8 whenever two CTAs fit in shared memory (rows_per_cta below).
 inline int tc_knn_rows_per_cta(int Hp, int mode, int Q) { return 2 * (tc_knn_smem_bytes(Hp, mode, Q, 8) + 1024) <= 227 * 1024 ? 8 : 16; }
 
 template <int MODE, int ROWS>
 __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(const TcKnnArgs a) {
   constexpr int TK_THREADS = ROWS * 32;
-  constexpr int TK_TMEM = ROWS / 4 * TK_WGCOLS;                               // 512 | 256 columns
   constexpr bool EDGES = MODE == TK_EDGES, GEN = MODE == TK_GEN;
   constexpr int NX = GEN ? TP_CMAX : 3;                                       // coordinate registers
   constexpr int PW = GEN ? 16 + TP_CMAX + 1 : 20;                             // reduced record: 16 m | coords | count
@@ -92,12 +91,8 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
   float* wes = wds + Hp;                                                      // [QE][Hp] (EDGES only)
   float* epi = wds + (size_t)(GEN ? Q : EDGES ? 1 + TK_QE : 1) * Hp;
   float* stile = epi + TP_EPI_FLOATS;                                         // [16 warps][Q][32] (GEN only)
-  uint32_t* misc = reinterpret_cast<uint32_t*>(stile + (GEN ? ROWS * Q * 32 : 0));   // [0] tmem pointer
-  uint64_t* bars = reinterpret_cast<uint64_t*>(misc + 16);
-  uint64_t* full = bars;                      // [4][SLOTS]
-  uint64_t* empty = bars + 4 * TK_SLOTS;      // [4][SLOTS]
-  uint64_t* accdone = empty + 4 * TK_SLOTS;   // [4]
-  uint64_t* ldbar = accdone + 4;
+  float* accs = stile + (GEN ? ROWS * Q * 32 : 0);                            // [16 warps][32][TK_ACC_LD]
+  uint64_t* ldbar = reinterpret_cast<uint64_t*>(accs + ROWS * 32 * TK_ACC_LD);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.y, i0 = a.row0 + blockIdx.x * ROWS;
@@ -107,18 +102,12 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
   const bool upd_feats = a.flags & EGNN_FLAG_UPDATE_FEATS, upd_coors = a.flags & EGNN_FLAG_UPDATE_COORS;
 
   if (tid == 0) {
-    for (int x = 0; x < 4 * TK_SLOTS; ++x) { tc::mbar_init(&full[x], 128); tc::mbar_init(&empty[x], 1); }
-    for (int x = 0; x < 4; ++x) tc::mbar_init(&accdone[x], 1);
     tc::mbar_init(ldbar, 1);
     tc::mbar_fence_init();
   }
-  if (warp == 0) tc::tmem_alloc<TK_TMEM>(&misc[0]);
   for (int x = tid; x < TP_EPI_FLOATS; x += TK_THREADS) epi[x] = a.epi[x];
   for (int x = tid + rows_valid * Hp; x < ROWS * Hp; x += TK_THREADS) As[x] = 0.f;
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = misc[0];
 
   if (tid == 0) {
     const uint32_t w2_bytes = (uint32_t)Hp * 32, as_bytes = (uint32_t)rows_valid * Hp * 4;
@@ -134,11 +123,7 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
     if (EDGES) bulk(tc::smem_u32(wes), reinterpret_cast<const unsigned char*>(a.weh), we_bytes);
   }
 
-  const int g = warp >> 2, wq = warp & 3;
   const int lr = lane >> 2, lq = lane & 3;
-  const uint32_t tm_wg = tmem + g * TK_WGCOLS + ((uint32_t)(wq * 32) << 16);
-  constexpr uint32_t IDESC = tc::idesc_bf16_f32(128, 16);
-  const uint32_t w2a = tc::smem_u32(w2s);
 
   // ---- this warp's query row
   const bool iv = warp < rows_valid;
@@ -216,49 +201,27 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
       for (int sl = 0; sl < 4; ++sl) Bc[rho][sl] = sl < nsl0 ? __ldg(Bp[rho] + sl * 4) : make_uint2(0u, 0u);
   }
 
-  int pend_c = -1;
-  auto issue_pending = [&]() {
-    if (pend_c < 0) return;
-    const int pc = pend_c;
-    pend_c = -1;
-    if ((pc & 3) != wq) return;                       // rotating duty
-    const uint32_t pslot = (uint32_t)pc % TK_SLOTS;
-    tc::mbar_wait(&full[g * TK_SLOTS + pslot], ((uint32_t)pc / TK_SLOTS) & 1);
-    tc::tc_fence_after();
-    if (lane == 0) {
-      const uint32_t tm_g = tmem + g * TK_WGCOLS;
-      const int nk = pc + 1 == nchunks ? nsl_last : 4;
+  float acc[2][2][4];                                  // m_pre of slots [16 half, +16) x channels [8 nt, +8): mma.sync D fragments
 #pragma unroll
-      for (int kk = 0; kk < TK_KC / 16; ++kk) {
-        if (kk < nk) {
-          const uint64_t bd = tc::smem_desc_kmajor_noswizzle(w2a + (uint32_t)(pc * 4 + kk) * 512, 256u, 128u);
-          tc::mma_ts(tm_g, tm_g + 16 + pslot * 32 + kk * 8, bd, IDESC, (pc > 0 || kk > 0) ? 1u : 0u);
-        }
-      }
-      tc::mma_commit(&empty[g * TK_SLOTS + pslot]);
-      if (pc + 1 == nchunks) tc::mma_commit(&accdone[g]);
-    }
-    __syncwarp();
-  };
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+      for (int e = 0; e < 4; ++e) acc[h][nt][e] = 0.f;
 
   const float* Arow = As + (size_t)warp * Hp + lq * 4;
   // chunks with all 4 K slabs run with NSLC = 4 (the slab tests fold at compile time); only the last chunk of a hidden
   // width that is not a multiple of 64 takes the predicated instantiation (NSLC = 0)
   auto chunk = [&](const int c, auto nslc) {
     constexpr int NSLC = decltype(nslc)::value;
-    const uint32_t slot = (uint32_t)c % TK_SLOTS;
-    const uint32_t ta = tm_wg + 16 + slot * 32;
     const bool more = NSLC != 0 && c + 1 < nchunks;
     const int nsl = NSLC ? NSLC : nsl_last, nsl_next = c + 2 == nchunks ? nsl_last : 4;
     // Slab-major: the broadcast operands of a slab (A', w_d, edge-channel weights; 16 bytes per lane each, and every
     // LDS.128 costs four L1 wavefronts whatever the overlap between lanes) are fetched ONCE and used for all four slots of
     // the thread -- the kernel is bound by L1 wavefronts (ncu: 85 % of peak, 70 % of them these loads), not by the MUFU
-    // pipe.  The slot is therefore waited for at the top and every (half, slab) fragment goes to TMEM as soon as it is packed.
-    tc::mbar_wait(&empty[g * TK_SLOTS + slot], (((uint32_t)c / TK_SLOTS) & 1) ^ 1);
-    tc::tc_fence_after();
+    // pipe.  Every (half, slab) fragment is multiplied as soon as it is packed.
 #pragma unroll
     for (int sl = 0; sl < 4; ++sl) {
-      if (sl == 2) issue_pending();                         // chunk c-1's MMAs, if this warp has the duty (before the skip below)
       if (NSLC == 0 && sl >= nsl) continue;                 // tail chunk: slabs beyond H are neither computed nor multiplied
       const float4 av = *reinterpret_cast<const float4*>(Arow + c * TK_KC + sl * 16);
       float4 wv = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -292,7 +255,7 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
           const int rho = half * 2 + r2;
           const uint2 bb = Bc[rho][sl];
           const float d = dr[rho];
-          // packed FFMA2 (two channels per instruction) for w_d d + A', the edge channels and y + y tanh y
+          // channel pairs (tc::ffma2: two FFMAs) for w_d d + A', the edge channels and y + y tanh y
           float2 z01, z23;
           if (GEN) {
             z01 = make_float2(zg[GEN ? rho : 0][0], zg[GEN ? rho : 0][1]); z23 = make_float2(zg[GEN ? rho : 0][2], zg[GEN ? rho : 0][3]);
@@ -317,14 +280,10 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
           h4[r2 * 2 + 1] = tc::pack_bf16x2(h23.x, h23.y);
           if (more && sl < nsl_next) Bc[rho][sl] = __ldg(Bp[rho] + (c + 1) * 16 + sl * 4);
         }
-        // 16x256b fragment of slab sl: registers {0,1} -> slot lr (+16), {2,3} -> slot lr + 8 (+24)
-        tc::tmem_st_16x256b_x1(ta + ((uint32_t)(half * 16) << 16) + sl * 8, h4[0], h4[1], h4[2], h4[3]);
+        // A fragment of slab sl: registers {0,1} -> slot lr (+16), {2,3} -> slot lr + 8 (+24)
+        tc::mma_w2_slab(acc[half], h4, w2s, c * 4 + sl, lr, lq);
       }
     }
-    tc::tmem_wait_st();
-    tc::tc_fence_before();
-    tc::mbar_arrive(&full[g * TK_SLOTS + slot]);
-    pend_c = c;
   };
   {
     const int nfull = nsl_last == 4 ? nchunks : nchunks - 1;
@@ -332,20 +291,25 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
     for (int c = 0; c < nfull; ++c) chunk(c, tc::IntC<4>{});
     if (nfull < nchunks) chunk(nchunks - 1, tc::IntC<0>{});
   }
-  issue_pending();
 
   // ---- epilogue (pair mapping): one warp = one query row, shuffle tree over its 32 slots
-  tc::mbar_wait(&accdone[g], 0);
-  tc::tc_fence_after();
   {
     const float* W3 = epi; const float* b3 = epi + 1024; const float* w4 = b3 + 64;
     const float* b2 = w4 + 64; const float* gw = b2 + 16; const float* sc = gw + 16;
-    uint32_t r[16];
-    tc::tmem_ld16(tm_wg, r);
-    tc::tmem_wait_ld();
+    // accumulator fragments -> one slot row per lane, through this warp's transpose tile
+    float* myacc = accs + (size_t)warp * 32 * TK_ACC_LD;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+      for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+        for (int r2 = 0; r2 < 2; ++r2)
+          *reinterpret_cast<float2*>(myacc + (16 * h + 8 * r2 + lr) * TK_ACC_LD + 8 * nt + 2 * lq) =
+              make_float2(acc[h][nt][2 * r2], acc[h][nt][2 * r2 + 1]);
+    __syncwarp();
     float m[16];
 #pragma unroll
-    for (int o = 0; o < 16; ++o) m[o] = tc::silu_half_arg(0.5f * (__uint_as_float(r[o]) + b2[o]));
+    for (int o = 0; o < 16; ++o) m[o] = tc::silu_half_arg(0.5f * (myacc[lane * TK_ACC_LD + o] + b2[o]));
     if (a.flags & EGNN_FLAG_SOFT_EDGES) {
       float z = sc[0];
 #pragma unroll
@@ -402,9 +366,6 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
       }
     }
   }
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<TK_TMEM>(tmem);
 }
 
 }  // namespace egnn

@@ -1,4 +1,4 @@
-// The fused edge step on 5th-gen tensor cores (dense all-pairs, bf16 operands, fp32 accumulation).
+// The fused edge step on the tensor cores (dense all-pairs, bf16 operands, fp32 accumulation).
 //
 // Reference semantics: egnn_pytorch.py:232-233 (x_i - x_j, squared distance), :270-285 (fourier features, edge
 // input [h_i | h_j | d | e_ij]), :287 (edge MLP), :289-290 (gate), :292-333 (masks, coors MLP, clamp, both sums
@@ -10,34 +10,27 @@
 // handles any coordinate dimension C <= 8.
 //
 // PERSISTENT kernel: one CTA per SM walks "row groups" (TI = 4 query rows i of one graph) with a static stride.
-// W2 (UMMA core-matrix order) and Wq are staged ONCE per CTA with TMA bulk copies; the A' rows of row group
-// it+2 are prefetched into a two-deep ring while it / it+1 are being computed.  The 4 compute warpgroups
-// (128 threads each, 4 warps per SM sub-partition, 128 registers) are independent pipelines: warpgroup g owns
-// the j-tiles [512*jb + 128*g, +128) of every row group, has its own TMEM columns, mbarriers and pair-scalar
-// tile, and never waits for another warpgroup.  (An optional start-up skew, skew_ns, can de-phase the warpgroups so
-// that their MUFU-idle epilogues fall into different time windows; measured on B200 it buys nothing -- the kernel is
-// bound by per-warp dependency latency: with 1 / 2 / 3 / 4 warps per SM sub-partition it reaches 0.28 / 0.47 / 0.58 /
-// 0.67 of the MUFU roofline, i.e. every warp is stalled ~72 % of the time independently of the others -- so it is
-// off by default; profiles/r02_tc_pair_skew_sweep.txt.)
+// W2 (core-matrix order) and Wq are staged ONCE per CTA with TMA bulk copies; the A' rows of row group it+2 are
+// prefetched into a two-deep ring while it / it+1 are being computed.  The 2 compute warpgroups (128 threads each,
+// 2 warps per SM sub-partition, up to 255 registers) are independent pipelines: warpgroup g owns the j-tiles
+// [256*jb + 128*g, +128) of every row group, has its own pair-scalar tile, and never waits for the other warpgroup.
+// (An optional start-up skew, skew_ns, can de-phase the warpgroups so that their MUFU-idle epilogues fall into
+// different time windows; off by default.)
 //   * For each hidden chunk of 64 channels and each row i a warp produces the 64 bf16 hidden values of its 32
-//     pairs in registers (fp32 math, one MUFU.TANH per value) and stores them with tcgen05.st into a TMEM slot
-//     laid out as the MMA A operand (lane = pair, 32 columns = 64 bf16): the O(N^2 H) hidden tensor only ever
-//     exists 8 KB at a time, in TMEM.  H is padded to 16 (one K step), not 64: the last chunk runs 1..4 slabs.
-//   * The MMAs are issued by the compute warps themselves (a 17th warp would cut the register budget from
-//     128 to 96): after storing round n, warp n%4 of the warpgroup waits for the other three to arrive on
-//     the slot's `full` mbarrier and one lane issues tcgen05.mma.kind::f16 (M=128 pairs, N=16, K=16) per slab
-//     with A from TMEM and B = the W2 slab from shared memory, accumulating m_pre[i] (128 x 16 fp32) in
-//     TMEM across all chunks; tcgen05.commit releases the slot through its `empty` mbarrier.  The issue is
-//     deferred by half a round so the issuer never waits for its siblings.
-//   * After the last chunk each thread reads its own pair's 16 accumulators back (tcgen05.ld), applies
-//     SiLU / gate / coors MLP / mask / clamp in fp32 and the warp reduces over j with shuffles into per-warp
-//     partial sums in shared memory.  The LAST warpgroup to finish a row group (shared-memory counter) adds the
-//     16 partials in a fixed order (deterministic), writes m_i and x_i' once per row, and issues the TMA
-//     prefetch of row group it+2 into the ring slot that just became free.
+//     pairs in registers (fp32 math, one MUFU.TANH per value), packed directly in the mma.sync A-fragment layout,
+//     and multiplies each 16-channel slab with the W2 slab in shared memory right away (mma.sync m16n8k16, fp32
+//     accumulators in registers): the O(N^2 H) hidden tensor never leaves the registers.  H is padded to 16 (one
+//     K step), not 64: the last chunk runs 1..4 slabs.  The accumulators of the TI rows (m_pre[i], 32 pairs x 16
+//     per warp) stay in registers across all chunks -- 64 per thread, which is why a warpgroup has 255 registers.
+//   * After the last chunk the accumulators go through a per-warp shared-memory tile to the thread that owns the
+//     pair, which applies SiLU / gate / coors MLP / mask / clamp in fp32; the warp reduces over j with shuffles
+//     into per-warp partial sums in shared memory.  The LAST warpgroup to finish a row group (shared-memory
+//     counter) adds the partials in a fixed order (deterministic), writes m_i and x_i' once per row, and issues the
+//     TMA prefetch of row group it+2 into the ring slot that just became free.
 //
 // Thread <-> data mappings inside a compute warp:
-//   "pair" mapping     (geometry, epilogue, tcgen05.ld 32x32b): lane l owns pair row 32*wq + l of the tile;
-//   "fragment" mapping (hidden production, tcgen05.st 16x256b): lane (lr = l/4, lq = l%4) owns rows
+//   "pair" mapping     (geometry, epilogue): lane l owns pair row 32*wq + l of the tile;
+//   "fragment" mapping (hidden production, mma.sync A / D fragments): lane (lr = l/4, lq = l%4) owns rows
 //     lr + 8*rho (rho = 0..3) of the warp's 32-row quadrant and, in every 16-channel K-slab, channels
 //     4*lq .. 4*lq+3.  Lanes sharing lq read the same A'/Wq words (4 distinct addresses per warp instead
 //     of a 32-way broadcast, which cost one shared-memory wavefront per 4 bytes in the first version).
@@ -54,17 +47,15 @@ namespace egnn {
 #endif
 constexpr int TP_EPI_UNROLL = EPI_UNROLL;
 constexpr int TP_TI = 4;          // query rows per row group
-constexpr int TP_KC = 64;         // hidden channels per chunk (= 32 TMEM columns, 4 MMAs)
-constexpr int TP_SLOTS = 2;       // A-operand slots per warpgroup
-constexpr int TP_WG = 4;          // compute warpgroups
+constexpr int TP_KC = 64;         // hidden channels per chunk (4 K slabs)
+constexpr int TP_WG = 2;          // compute warpgroups
 constexpr int TP_CWARPS = TP_WG * 4;
-constexpr int TP_THREADS = TP_WG * 128;      // 16 warps = 4 per SM sub-partition, 128 registers each
+constexpr int TP_THREADS = TP_WG * 128;      // 8 warps = 2 per SM sub-partition, up to 255 registers each
 constexpr int TP_JB = TP_WG * 128;    // neighbours per block
-constexpr int TP_WGCOLS = 128;        // TMEM columns per warpgroup: TI*16 accumulators + SLOTS*32 operand
+constexpr int TP_ACC_LD = 18;         // floats per pair row of the per-warp accumulator transpose tile
 constexpr int TP_EPI_FLOATS = 64 * 16 + 64 + 64 + 16 + 16 + 4;   // W3 | b3 | w4 | b2 | gate_w | gate_b, b4, scale, 0
 constexpr int TP_QMAX = 12;           // per-pair scalar channels of the generic instantiation
 constexpr int TP_CMAX = 8;            // coordinate dimensions of the generic instantiation
-static_assert(TP_TI * 16 + TP_SLOTS * 32 == TP_WGCOLS && TP_WG * TP_WGCOLS == 512, "TMEM budget");
 
 struct TcPairArgs {
   int B, N, Hp, ldn;               // Hp: H rounded up to 16; ldn: row stride of node_in (bf16 elements)
@@ -105,11 +96,12 @@ inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
   n += (size_t)2 * TP_TI * Hp * 4;                          // A' rows, two-deep ring
   n += (size_t)TP_EPI_FLOATS * 4;                           // epilogue constants
   n += (size_t)2 * TP_CWARPS * TP_TI * TpCfg<GEN>::PW * 8;  // per-warp partial sums (fp64), per ring slot
-  n += (size_t)2 * TP_TI * TpCfg<GEN>::XC * 4 + 2 * TP_TI * 4 + 64;   // x_i, mask_i per ring slot; counters, tmem pointer
+  n += (size_t)TP_CWARPS * 32 * TP_ACC_LD * 4;               // per-warp accumulator transpose tile
+  n += (size_t)2 * TP_TI * TpCfg<GEN>::XC * 4 + 2 * TP_TI * 4 + 64;   // x_i, mask_i per ring slot; counters, flags
   n += (size_t)(GEN ? 0 : 1) * TP_TI * TP_JB * 4;           // lean: d_ij of the current tiles
   (void)Q;
   if (GEN) n += tc_pair_gen_scalar_bytes(Qf, Q - Qf);
-  n += 40 * 8;                                              // mbarriers
+  n += 8 * 8;                                               // mbarriers
   return n + 256;
 }
 
@@ -117,7 +109,7 @@ inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
 __device__ __forceinline__ void tp_wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }
 
 // End of a work item, run by the LAST warpgroup of the CTA to finish it (kept out of line: its registers must not add to the
-// pressure of the round loop).  jsplit == 1: add the 16 warps' partial sums and write m_i / x_i'.  jsplit > 1: publish this
+// pressure of the round loop).  jsplit == 1: add the warps' partial sums and write m_i / x_i'.  jsplit > 1: publish this
 // item's sums; the last of the row group's items (device-scope counter) adds the parts in order and writes the outputs.
 struct TpFinishArgs {               // the fields of TcPairArgs the finish needs, passed BY VALUE (a reference to the kernel
   int jsplit, N, C, ldn, has_mask;  // parameter block would force a local-memory copy of all of it)
@@ -199,18 +191,16 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
   // Sums ACROSS tiles are kept in fp64: the per-tile sums are fp32 (fixed shuffle tree), and adding a few hundred
   // fp32 numbers in fp64 is exact, so the result does not depend on how the tiles were dealt to warps, work items or
   // ranks (row-sharded == single GPU, bit for bit, whatever jsplit is).
-  double* part = reinterpret_cast<double*>(epi + TP_EPI_FLOATS);              // [2][16 warps][TI][PW]
+  double* part = reinterpret_cast<double*>(epi + TP_EPI_FLOATS);              // [2][CWARPS][TI][PW]
   float* xis = reinterpret_cast<float*>(part + 2 * TP_CWARPS * TP_TI * PW);   // [2][TI][XC]
   uint32_t* mki = reinterpret_cast<uint32_t*>(xis + 2 * TP_TI * XC);          // [2][TI]
-  uint32_t* misc = mki + 2 * TP_TI;                                           // [0..1] done counters, [2] tmem ptr, [4..7] last flags
+  uint32_t* misc = mki + 2 * TP_TI;                                           // [0..1] done counters, [4..] last flags
   const int Qf = GEN ? 1 + 2 * a.F : 1, Qh = Q - Qf;
   float* ssm = reinterpret_cast<float*>(misc + 16);                           // [WG][Qf][TI][128] fp32
   __nv_bfloat16* ssh = reinterpret_cast<__nv_bfloat16*>(ssm + (size_t)Qf * TP_TI * TP_JB);   // [WG][Qh][TI][128] bf16
-  uint64_t* bars = reinterpret_cast<uint64_t*>(ssh + (size_t)Qh * TP_TI * TP_JB);
-  uint64_t* full = bars;                          // [WG][SLOTS]
-  uint64_t* empty = bars + TP_WG * TP_SLOTS;      // [WG][SLOTS]
-  uint64_t* accdone = empty + TP_WG * TP_SLOTS;   // [WG]
-  uint64_t* ldbar = accdone + TP_WG;              // W2 / Wq staging
+  float* accs = reinterpret_cast<float*>(ssh + (size_t)Qh * TP_TI * TP_JB);    // [CWARPS][32][TP_ACC_LD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(accs + TP_CWARPS * 32 * TP_ACC_LD);
+  uint64_t* ldbar = bars;                         // W2 / Wq staging
   uint64_t* rowfull = ldbar + 1;                  // [2] A' ring
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -260,21 +250,15 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
 
   // ---------------- setup
   if (tid == 0) {
-    for (int x = 0; x < TP_WG * TP_SLOTS; ++x) { tc::mbar_init(&full[x], 128); tc::mbar_init(&empty[x], 1); }
-    for (int x = 0; x < TP_WG; ++x) tc::mbar_init(&accdone[x], 1);
     tc::mbar_init(ldbar, 1);
     tc::mbar_init(&rowfull[0], 1); tc::mbar_init(&rowfull[1], 1);
     tc::mbar_fence_init();
   }
-  if (warp == 0) tc::tmem_alloc<512>(&misc[2]);
   for (int x = tid; x < TP_EPI_FLOATS; x += TP_THREADS) epi[x] = a.epi[x];
   for (int x = tid; x < 2 * TP_TI * Hp; x += TP_THREADS) As[x] = 0.f;      // rows beyond a graph's end stay finite
   if (tid < 2) misc[tid] = 0;
   tc::fence_proxy_async_smem();                    // the zero fill above precedes TMA writes to the same buffers
-  tc::tc_fence_before();
   __syncthreads();
-  tc::tc_fence_after();
-  const uint32_t tmem = misc[2];
 
   if (tid == 0) {
     // TMA bulk staging, once per CTA: W2 slabs and the per-pair scalar columns
@@ -296,13 +280,9 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
     // =========================================================== compute warpgroups (independent pipelines)
     const int g = warp >> 2, wq = warp & 3, t128 = tid & 127;
     const int lr = lane >> 2, lq = lane & 3;
-    const uint32_t tm_wg = tmem + g * TP_WGCOLS + ((uint32_t)(wq * 32) << 16);    // this warp's lane quadrant
     float* swg = ssm + (size_t)g * Qf * TP_TI * 128;  // pair scalars of this warpgroup's tile: swg[(q*TI + i)*128 + pair]
     __nv_bfloat16* shg = ssh + (size_t)g * Qh * TP_TI * 128;
-    constexpr uint32_t IDESC = tc::idesc_bf16_f32(128, 16);
-    const uint32_t w2a = tc::smem_u32(w2s);           // W2 slab s at +512*s: K-adjacent core matrices 256 B apart, N-adjacent 128 B
-    const uint32_t full_a = tc::smem_u32(&full[g * TP_SLOTS]), empty_a = tc::smem_u32(&empty[g * TP_SLOTS]);   // + 8 * slot
-    const uint32_t accdone_a = tc::smem_u32(&accdone[g]);
+    float* myacc = accs + (size_t)warp * 32 * TP_ACC_LD;
     if (a.skew_ns && g > 0) {                         // de-phase the warpgroups (see the header)
       uint64_t t0, t1;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
@@ -314,8 +294,6 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
     const int active_wgs = min(TP_WG, (N + 127) / 128);
     const bool wg_active = g < active_wgs;
     if (wg_active) tc::mbar_wait(ldbar, 0);
-    uint32_t n = 0;                                   // rounds this warpgroup has produced
-    uint32_t tl = 0;                                  // tiles this warpgroup has finished (accdone phase)
     int it = 0;
     for (int item = blockIdx.x; wg_active && item < n_items; item += gridDim.x, ++it) {
       const int buf = it & 1;
@@ -379,54 +357,31 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
             for (int sl = 0; sl < 4; ++sl) Bc[rho][sl] = sl < nsl0 ? __ldg(Bp_(rho) + sl * 4) : make_uint2(0u, 0u);
         }
 
-        int pend_c = 0, pend_i = 0;
-        uint32_t pend_n = 0;
-        bool pend_valid = false;
-        auto issue_pending = [&]() {
-          if (!pend_valid) return;
-          pend_valid = false;
-          if ((pend_n & 3u) != (uint32_t)wq) return;      // rotating duty: warp (round % 4) of the warpgroup issues
-          const uint32_t pslot = pend_n & (TP_SLOTS - 1);
-          tc::mbar_wait_a(full_a + 8 * pslot, (pend_n / TP_SLOTS) & 1);
-          tc::tc_fence_after();
-          if (lane == 0) {
-            const uint32_t tm_g = tmem + g * TP_WGCOLS;
-            const int nk = pend_c + 1 == nchunks ? nsl_last : 4;
+        float acc[TP_TI][2][2][4];                      // m_pre[i] of rows [16 half, +16) x channels [8 nt, +8) (D fragments)
 #pragma unroll
-            for (int kk = 0; kk < TP_KC / 16; ++kk) {
-              if (kk < nk) {
-                const uint64_t bd = tc::smem_desc_kmajor_noswizzle(w2a + (uint32_t)(pend_c * 4 + kk) * 512, 256u, 128u);
-                tc::mma_ts(tm_g + pend_i * 16, tm_g + TP_TI * 16 + pslot * 32 + kk * 8, bd, IDESC, (pend_c > 0 || kk > 0) ? 1u : 0u);
-              }
-            }
-            tc::mma_commit_a(empty_a + 8 * pslot);
-            if (pend_c + 1 == nchunks && pend_i + 1 == TP_TI) tc::mma_commit_a(accdone_a);
-          }
-          __syncwarp();
-        };
+        for (int i = 0; i < TP_TI; ++i)
+#pragma unroll
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+              for (int e = 0; e < 4; ++e) acc[i][h][nt][e] = 0.f;
         // A chunk with all 4 K slabs runs with NSLC = 4 (every slab test folds at compile time); only the last chunk
         // of a hidden width that is not a multiple of 64 takes the predicated instantiation (NSLC = 0).
         auto chunk = [&](const int c, auto nslc) {
           constexpr int NSLC = decltype(nslc)::value;
           const int nsl = NSLC ? NSLC : nsl_last;                   // valid slabs of this chunk
           const int nsl_next = c + 2 == nchunks ? nsl_last : 4;     // ... and of the next one (prefetch)
-          // Register budget (same-box A/B, tools/ab_variants.sh; every step keeps 128 registers but leaves the compiler more
-          // of them for values in flight between MUFU issue and use): w_d and A' are read from shared memory at the point of
-          // use instead of being held for the chunk / round (-1.1 %, -0.6 %); one B' base pointer + stride (-0.4 %); the
-          // second half of a round stores every slab to TMEM as soon as it is packed (-0.5 %).  Tried and rejected: d_ij read
-          // at use (+1.0 %), slot wait at the top of the round with per-slab stores in both halves (+0.4 %), MMA issue one
-          // slab into the round instead of half a round (+3.1 %).
+          // Register budget: w_d and A' are read from shared memory at the point of use instead of being held for the chunk
+          // / round; one B' base pointer + stride; every slab is multiplied as soon as it is packed.
           // One round = the 64 hidden channels of chunk c for row i and this warp's 32 pairs.  In the last round
           // of a chunk (`reload`), every B' register is re-filled for chunk c+1 right after its last use, so the
           // L2 latency is covered by the rest of that round without a second register buffer.
-          // MMA issue is deferred by half a round: the MMAs of round n-1 are issued (by warp (n-1)%4 of the
-          // warpgroup) in the middle of round n, when the other three warps have long arrived, and the slot of
-          // round n is only waited for right before its first tcgen05.st.
-          auto round = [&](const int i, auto reload_tag) {
+          // The row index is a compile-time constant (IntC) so that acc[i] stays in registers.
+          auto round = [&](auto i_tag, auto reload_tag) {
+            constexpr int i = decltype(i_tag)::value;
             constexpr bool reload = decltype(reload_tag)::value != 0;
-            const uint32_t slot = n & (TP_SLOTS - 1);
             const float* Ai = Ab + (size_t)i * Hp + c * TP_KC + lq * 4;
-            const uint32_t ta = tm_wg + TP_TI * 16 + slot * 32;
             float dr[4];
             if (!GEN) {
 #pragma unroll
@@ -474,10 +429,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
               uint32_t hp[16];
 #pragma unroll
               for (int sl = 0; sl < 4; ++sl) {
-                if (NSLC == 0 && sl >= nsl) {              // tail chunk: slabs beyond H are not computed (no MUFU work) ...
-                  hp[sl * 4 + 0] = hp[sl * 4 + 1] = hp[sl * 4 + 2] = hp[sl * 4 + 3] = 0u;     // ... and never multiplied
-                  continue;
-                }
+                if (NSLC == 0 && sl >= nsl) continue;      // tail chunk: slabs beyond H are neither computed nor multiplied
 #pragma unroll
                 for (int r2 = 0; r2 < 2; ++r2) {
                   const int rho = half * 2 + r2;
@@ -497,37 +449,23 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
                   const float2 y23 = make_float2(tc::add_bf16_lo(bb.y, z23.x), tc::add_bf16_hi(bb.y, z23.y));
                   const float2 h01 = tc::ffma2(y01, make_float2(tc::tanh_fast(y01.x), tc::tanh_fast(y01.y)), y01);  // y + y tanh y
                   const float2 h23 = tc::ffma2(y23, make_float2(tc::tanh_fast(y23.x), tc::tanh_fast(y23.y)), y23);
-                  // 16x256b fragment: regs {0,1} of a slab -> row lr (+16), regs {2,3} -> row lr+8 (+24); even k low
+                  // A fragment: regs {0,1} of a slab -> row lr (+16), regs {2,3} -> row lr+8 (+24); even k low
                   hp[sl * 4 + r2 * 2 + 0] = tc::pack_bf16x2(h01.x, h01.y);
                   hp[sl * 4 + r2 * 2 + 1] = tc::pack_bf16x2(h23.x, h23.y);
                   if (reload && sl < nsl_next) Bc[rho][sl] = __ldg(Bp_(rho) + (c + 1) * 16 + sl * 4);
                 }
-                // second half: the slot is already ours (waited for in the first half) -- store every slab as soon as
-                // it is packed, so that its four staging registers are free for the next slab's values
-                if (half == 1) tc::tmem_st_16x256b_x1(ta + ((uint32_t)16 << 16) + sl * 8, hp[sl * 4], hp[sl * 4 + 1], hp[sl * 4 + 2], hp[sl * 4 + 3]);
+                const uint32_t h4[4] = {hp[sl * 4], hp[sl * 4 + 1], hp[sl * 4 + 2], hp[sl * 4 + 3]};
+                tc::mma_w2_slab(acc[i][half], h4, w2s, c * 4 + sl, lr, lq);
               }
-              if (half == 0) {
-                issue_pending();                          // round n-1's MMAs, if this warp has the duty
-                tc::mbar_wait_a(empty_a + 8 * slot, ((n / TP_SLOTS) & 1) ^ 1);
-                tc::tc_fence_after();
-              }
-              if (half == 0) tc::tmem_st_16x256b_x4(ta, hp);
             }
-            tc::tmem_wait_st();
-            tc::tc_fence_before();
-            tc::mbar_arrive_a(full_a + 8 * slot);
-            pend_c = c; pend_i = i; pend_n = n; pend_valid = true;
-            ++n;
           };
-          if constexpr (NSLC != 0) {
-#pragma unroll 1
-            for (int i = 0; i < TP_TI - 1; ++i) round(i, tc::IntC<0>{});
-            if (c + 1 < nchunks) round(TP_TI - 1, tc::IntC<1>{});
-            else round(TP_TI - 1, tc::IntC<0>{});
-          } else {                                        // the tail chunk is always the last one: nothing to prefetch
-#pragma unroll 1
-            for (int i = 0; i < TP_TI; ++i) round(i, tc::IntC<0>{});
-          }
+          static_assert(TP_TI == 4, "the rounds of a chunk are spelled out below");
+          round(tc::IntC<0>{}, tc::IntC<0>{});
+          round(tc::IntC<1>{}, tc::IntC<0>{});
+          round(tc::IntC<2>{}, tc::IntC<0>{});
+          // the last round of a full chunk re-fills B' for the next chunk; the tail chunk is always the last one
+          if (NSLC != 0 && c + 1 < nchunks) round(tc::IntC<3>{}, tc::IntC<1>{});
+          else round(tc::IntC<3>{}, tc::IntC<0>{});
         };
         {
           const int nfull = nsl_last == 4 ? nchunks : nchunks - 1;
@@ -535,22 +473,25 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
           for (int c = 0; c < nfull; ++c) chunk(c, tc::IntC<4>{});
           if (nfull < nchunks) chunk(nchunks - 1, tc::IntC<0>{});
         }
-        issue_pending();                                  // last round of the tile: also signals accdone
 
         // ---- epilogue of this tile: accumulators back to the owning thread (pair mapping)
-        tc::mbar_wait_a(accdone_a, tl & 1);
-        ++tl;
-        tc::tc_fence_after();
         const float* W3 = epi; const float* b3 = epi + 1024; const float* w4 = b3 + 64;
         const float* b2 = w4 + 64; const float* gw = b2 + 16; const float* sc = gw + 16;   // sc: gate_b, b4, scale
         float m[TP_TI][16];                              // m_ij of this thread's pair for the TI rows
 #pragma unroll
         for (int i = 0; i < TP_TI; ++i) {
-          uint32_t r[16];
-          tc::tmem_ld16(tm_wg + i * 16, r);
-          tc::tmem_wait_ld();
 #pragma unroll
-          for (int o = 0; o < 16; ++o) m[i][o] = tc::silu_half_arg(0.5f * (__uint_as_float(r[o]) + b2[o]));    // :183
+          for (int h = 0; h < 2; ++h)
+#pragma unroll
+            for (int nt = 0; nt < 2; ++nt)
+#pragma unroll
+              for (int r2 = 0; r2 < 2; ++r2)
+                *reinterpret_cast<float2*>(myacc + (16 * h + 8 * r2 + lr) * TP_ACC_LD + 8 * nt + 2 * lq) =
+                    make_float2(acc[i][h][nt][2 * r2], acc[i][h][nt][2 * r2 + 1]);
+          __syncwarp();
+#pragma unroll
+          for (int o = 0; o < 16; ++o) m[i][o] = tc::silu_half_arg(0.5f * (myacc[lane * TP_ACC_LD + o] + b2[o]));    // :183
+          __syncwarp();
           if (a.flags & EGNN_FLAG_SOFT_EDGES) {                                                               // :289-290
             float z = sc[0];
 #pragma unroll
@@ -560,14 +501,12 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
             for (int o = 0; o < 16; ++o) m[i][o] *= gate;
           }
         }
-        tc::tc_fence_before();                            // the accumulators may be overwritten by the next tile's MMAs
         float wgt[TP_TI];
 #pragma unroll
         for (int i = 0; i < TP_TI; ++i) wgt[i] = 0.f;
         if (upd_coors) {                                                                                      // :302-315
           // hidden unit u outermost: one W3 row (4 x LDS.128) serves all TI rows of this pair; the four rows are four
-          // independent FMA chains (same-box A/B, tools/ab_variants.sh: packing them two by two as FFMA2 is 1.4 % SLOWER
-          // on the whole kernel -- it halves the chains in flight and FFMA2 has no higher FMA throughput)
+          // independent FMA chains
 #pragma unroll TP_EPI_UNROLL
           for (int u = 0; u < 64; ++u) {
             const float4* w3 = reinterpret_cast<const float4*>(W3 + u * 16);
@@ -638,10 +577,6 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
     }
   }
 
-  // ---------------- teardown
-  tc::tc_fence_before();
-  __syncthreads();
-  if (warp == 0) tc::tmem_dealloc<512>(tmem);
 }
 
 }  // namespace egnn

@@ -4,7 +4,7 @@
 state-dict keys of lucidrains/egnn-pytorch (reference egnn_pytorch/egnn_pytorch.py:148-341 and
 :343-454), so a reference `state_dict()` loads unchanged -- but `forward` does not execute any
 PyTorch arithmetic for the edge step: it packs a POD descriptor and calls the hand-written
-sm_100a kernels of libegnn_b200.so through the C ABI (include/egnn_b200.h) on the current CUDA
+sm_90a kernels of libegnn_b200.so through the C ABI (include/egnn_b200.h) on the current CUDA
 stream.  PyTorch is used for parameter storage, device memory and streams only.
 
 There is no CPU compute path.  CPU tensors (the reference's own tests pass CPU float64) are
@@ -13,7 +13,7 @@ staged to the current CUDA device and the results copied back -- a transport con
 Element type -> kernel family
     float64 parameters  -> fp64 SIMT kernels      (parity with the fp64 oracle to ~1e-12)
     float32 parameters  -> fp32 SIMT kernels      ("accurate": the stated-fp32-tolerance path)
-    bfloat16 parameters -> tcgen05 bf16 tensor-core kernels with fp32 accumulation ("fast");
+    bfloat16 parameters -> bf16 tensor-core kernels (wgmma / mma.sync) with fp32 accumulation ("fast");
                            option combinations the tensor-core kernels do not cover run on the
                            fp32 SIMT kernels instead (still on the GPU; see `last_path`).
 `precision='fast'` / `'accurate'` overrides the choice for fp32/bf16 parameters.
@@ -63,12 +63,12 @@ def _compute_device(t: torch.Tensor) -> torch.device:
     if t.is_cuda:
         return t.device
     if not torch.cuda.is_available():
-        raise RuntimeError("egnn_pytorch_b200 needs a CUDA device (B200, sm_100a); there is no CPU fallback")
+        raise RuntimeError("egnn_pytorch_b200 needs a CUDA device (H100, sm_90a); there is no CPU fallback")
     return torch.device("cuda", torch.cuda.current_device())
 
 
 _KERNEL_DTYPE = {torch.float32: nat.DTYPE_F32, torch.float64: nat.DTYPE_F64, torch.bfloat16: nat.DTYPE_BF16}
-_PATH_NAME = {torch.float64: "fp64-simt", torch.float32: "fp32-simt", torch.bfloat16: "bf16-tcgen05"}
+_PATH_NAME = {torch.float64: "fp64-simt", torch.float32: "fp32-simt", torch.bfloat16: "bf16-tc"}
 
 
 def _ptr(t):
@@ -207,7 +207,7 @@ class EGNN(nn.Module):
         self.dropout_p = dropout
         self.init_eps = init_eps
         self.precision = precision
-        self.last_path = None          # 'fp64-simt' | 'fp32-simt' | 'bf16-tcgen05' of the last call
+        self.last_path = None          # 'fp64-simt' | 'fp32-simt' | 'bf16-tc' of the last call
         self.cache_policy = "version"  # 'version' | 'always' -- see invalidate_cache()
         self._stage = {}
         self._tc_unsupported = set()

@@ -15,7 +15,7 @@ the plumbing.
 The compute callable is injected, so the partition/exchange logic is testable on CPU with gloo
 (tests/test_multi_rank_cpu.py drives it with the oracle); on the GPU box it is the CUDA module.
 
-On B200s the all-gather of the row-sharded graph is NOT a host-driven collective: `PeerComm` wraps the library's
+On H100s the all-gather of the row-sharded graph is NOT a host-driven collective: `PeerComm` wraps the library's
 peer-memory communicator (`egnn_comm_*`, csrc/peer_comm.cu) -- one kernel per rank pushes the rank's rows into every
 peer's buffer with P2P stores over NVLink and waits on device-side epoch flags, enqueued on the layer's own stream
 (`row_sharded_layer_peer`).  torch.distributed is only used once, to exchange the 64-byte IPC handles.

@@ -1,5 +1,5 @@
 /*
- * egnn_b200.h -- C ABI of libegnn_b200.so, the B200 (sm_100a) implementation of the
+ * egnn_b200.h -- C ABI of libegnn_b200.so, the H100 (sm_90a) implementation of the
  * E(n)-equivariant message-passing layer of lucidrains/egnn-pytorch.
  *
  * The reference has no FFI: its boundary is the Python nn.Module API
@@ -44,7 +44,7 @@ extern "C" {
 /* ---- element types of feats / edges / weights / outputs ---------------------------- */
 #define EGNN_DTYPE_F32   0   /* SIMT fp32 kernels ("accurate" path)                       */
 #define EGNN_DTYPE_F64   1   /* SIMT fp64 kernels (the reference's tests run in fp64)     */
-#define EGNN_DTYPE_BF16  2   /* tcgen05 bf16 tensor-core kernels, fp32 accumulation       */
+#define EGNN_DTYPE_BF16  2   /* bf16 tensor-core kernels (wgmma / mma.sync), fp32 accum.   */
 
 /* ---- flags (EgnnLayerDesc.flags) ---------------------------------------------------- */
 #define EGNN_FLAG_NORM_FEATS    (1u << 0)   /* node_norm = LayerNorm  (egnn_pytorch.py:191)   */
@@ -228,7 +228,7 @@ int egnn_adj_expand(int32_t B, int32_t N, int32_t num_degrees, const uint8_t* ad
 int egnn_embed_nodes(int32_t dtype, int32_t B, int32_t N, int32_t dim, int32_t num_tokens, const int64_t* tokens,
                      const void* token_emb, const void* pos_emb, void* out, void* stream);
 
-/* The tcgen05 GEMM the bf16 path uses for its per-node contractions, exposed for unit tests:
+/* The wgmma GEMM the bf16 path uses for its per-node contractions, exposed for unit tests:
  * out[M,N] = act(scale * (A[M,K] W[N,K]^T + bias[N])), A/W bf16 row-major, K and N multiples of 8,
  * act 0 = none / 1 = SiLU, out fp32 (out_f32 = 1) or bf16. */
 int egnn_gemm_bf16(int32_t M, int32_t N, int32_t K, const void* A, const void* W, const float* bias,

@@ -1,7 +1,7 @@
 """Torch-CPU restatement of the reference's dense `EGNN.forward` -- TEST / BENCH INFRASTRUCTURE, NOT PRODUCT.
 
 Used ONLY as the fallback of `bench.py --impl reference` / `cpu_baseline` when the unmodified reference is not
-installed under baseline/_ref (then `kind` = "port" instead of "reference").  It keeps the reference's formulation
+installed under oracle/_ref (then `kind` = "port" instead of "reference").  It keeps the reference's formulation
 and its ATen call sequence for the dense all-pairs branch (egnn_pytorch.py:224-341): broadcast both feature
 operands to [B,N,N,d], concatenate [h_i | h_j | d] (:282-285), `Linear(E,2E) -> SiLU -> Linear(2E,m) -> SiLU`
 over the concatenation (:287), coors MLP and both sums (:302-333), node MLP with residual (:335-337) -- so it

@@ -10,12 +10,12 @@ for p in (REPO, os.path.join(REPO, "tests")):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (H100, sm_90a); select with -m gpu")
 
 
 def pytest_collection_modifyitems(config, items):
     """GPU tests are skipped (not failed) when no device is present, so a bare `pytest tests/`
-    also works in the CPU container; the driver selects with -m gpu / -m 'not gpu'."""
+    also works on a machine without a GPU; select with -m gpu / -m 'not gpu'."""
     try:
         import torch
         has_gpu = torch.cuda.is_available()
@@ -23,7 +23,7 @@ def pytest_collection_modifyitems(config, items):
         has_gpu = False
     if has_gpu:
         return
-    skip = pytest.mark.skip(reason="no CUDA device in this container")
+    skip = pytest.mark.skip(reason="no CUDA device on this machine")
     for item in items:
         if "gpu" in item.keywords:
             item.add_marker(skip)

@@ -36,12 +36,12 @@ def test_c1_exact_fp32_and_bf16():
     util.assert_close(out[1], want[1], atol=2e-6, rtol=1e-5, what="c1 coors")
     modb = util.make_module(case, torch.bfloat16)
     outb = util.run_module(modb, case, torch.bfloat16)
-    assert modb.last_path == "bf16-tcgen05"
+    assert modb.last_path == "bf16-tc"
     assert rel_err(outb[0], torch.from_numpy(want[0])) < 2e-2
 
 
 # ------------------------------------------------------------------ c2: EGNN(dim=512) dense, B=4, N=1024
-@pytest.mark.parametrize("dtype,path,tol", [(torch.bfloat16, "bf16-tcgen05", 2e-2), (torch.float32, "fp32-simt", 1e-4)],
+@pytest.mark.parametrize("dtype,path,tol", [(torch.bfloat16, "bf16-tc", 2e-2), (torch.float32, "fp32-simt", 1e-4)],
                          ids=["bf16", "fp32"])
 def test_c2_full_size_row_block_vs_oracle_and_properties(dtype, path, tol):
     B, N, d = 4, 1024, 512
@@ -121,7 +121,7 @@ def test_c4_two_graphs_row_block_vs_oracle_and_equivariance():
 
 
 def test_c4_bf16_tensor_core_knn_full_size():
-    """c4 as BASELINE.json states it (bf16): the gathered tcgen05 kernel at N=4096, k=32, edge_dim=4."""
+    """c4 as BASELINE.json states it (bf16): the gathered tensor-core kernel at N=4096, k=32, edge_dim=4."""
     B, N = 2, 4096
     spec = dict(kind="layer", cfg=dict(dim=256, edge_dim=4, num_nearest_neighbors=32), B=B, N=N, seed=4)
     case = cases.build_case(spec)
@@ -135,7 +135,7 @@ def test_c4_bf16_tensor_core_knn_full_size():
     coors = torch.from_numpy(ins["coors"]).float().cuda()
     edges = util.to_torch(ins["edges"], torch.bfloat16, "cuda")
     f, x = mod(feats, coors, edges)
-    assert mod.last_path == "bf16-tcgen05"
+    assert mod.last_path == "bf16-tc"
     wf, wx = cases.O.egnn_layer_forward(case["params"], case["cfg"], ins["feats"][1:2], ins["coors"][1:2], edges=ins["edges"][1:2],
                                         rows=(2000, 2064))
     assert rel_err(f[1:2, 2000:2064], torch.from_numpy(wf)) < 2e-2

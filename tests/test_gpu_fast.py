@@ -1,4 +1,4 @@
-"""The bf16 tensor-core path (tcgen05 GEMMs + the fused edge kernel) against the fp64 oracle.
+"""The bf16 tensor-core path (wgmma GEMMs + the fused edge kernels) against the fp64 oracle.
 
 Inputs and parameters are rounded to bf16 first, so the comparison isolates the kernels' internal
 rounding (bf16 B' table, bf16 hidden operand, bf16 m_i / h1, tanh.approx) from input quantisation.
@@ -107,7 +107,7 @@ def run_fast(spec):
 def test_fast_path_matches_oracle(name):
     case, mod, out = run_fast(FAST_SPECS[name])
     layers = [l[1] for l in mod.layers] if hasattr(mod, "layers") else [mod]
-    assert all(l.last_path == "bf16-tcgen05" for l in layers)
+    assert all(l.last_path == "bf16-tc" for l in layers)
     assert out[0].dtype == torch.bfloat16
     want = cases.run_oracle(case)
     f_scale = max(1e-3, float(np.abs(want[0]).max()))
@@ -138,7 +138,7 @@ def test_fast_path_row_range_equals_full_forward(name):
     for (r0, r1) in [(0, n // 3), (n // 3, n - 5), (n - 5, n), (7, 8)]:
         with torch.no_grad():
             f, x = mod(t("feats"), t("coors"), t("edges"), mask=t("mask"), _rows=(r0, r1))
-        assert mod.last_path == "bf16-tcgen05"
+        assert mod.last_path == "bf16-tc"
         assert torch.equal(f[:, r0:r1], full[0][:, r0:r1]) and torch.equal(x[:, r0:r1], full[1][:, r0:r1])
         keep = torch.ones(n, dtype=torch.bool, device="cuda"); keep[r0:r1] = False
         assert torch.equal(f[:, keep], t("feats")[:, keep]) and torch.equal(x[:, keep].float(), t("coors")[:, keep].float())

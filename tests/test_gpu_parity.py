@@ -1,5 +1,5 @@
-"""Parity of the CUDA path (through the module API -> C ABI -> sm_100a kernels) against the
-oracle and the committed reference outputs.  Needs a B200: `pytest -m gpu`.
+"""Parity of the CUDA path (through the module API -> C ABI -> sm_90a kernels) against the
+oracle and the committed reference outputs.  Needs an H100: `pytest -m gpu`.
 
 Tolerances (stated per SURVEY.md section 8(c)):
   fp64 kernels : atol 1e-9,  rtol 1e-9   (same algebra, different summation order)

@@ -20,7 +20,7 @@ HEADER = os.path.join(REPO, "include", "egnn_b200.h")
 @pytest.fixture(scope="module")
 def nat():
     from egnn_pytorch_b200 import build, _native
-    build.build()                     # nvcc cross-compiles sm_100a without a GPU
+    build.build()                     # nvcc cross-compiles sm_90a without a GPU
     _native.load()
     return _native
 
@@ -40,10 +40,10 @@ def test_library_exports_every_declared_symbol(nat):
     assert set(names) == set(nat.SYMBOLS), set(names) ^ set(nat.SYMBOLS)
 
 
-def test_library_is_sm100a_and_has_no_other_arch(nat):
+def test_library_is_sm90a_and_has_no_other_arch(nat):
     out = subprocess.run(["cuobjdump", "-lelf", nat.LIB_PATH], capture_output=True, text=True).stdout
-    assert "sm_100a" in out
-    assert not re.search(r"sm_(?!100a)\d+", out), out
+    assert "sm_90a" in out
+    assert not re.search(r"sm_(?!90a)\d+", out), out
 
 
 def test_ctypes_structs_match_c_layout(nat, tmp_path):

@@ -1,6 +1,6 @@
-"""Latency / throughput of the five BASELINE.json configurations on one B200: this repo vs the unmodified
-reference in PyTorch eager on the same GPU (if baseline/_ref is installed).  Writes one JSON line per config.
-    python tools/bench_configs.py > gpurun_out/configs.jsonl
+"""Latency / throughput of the five BASELINE.json configurations on one GPU: this repo vs the unmodified
+reference in PyTorch eager on the same GPU (if oracle/_ref is installed).  Writes one JSON line per config.
+    python tools/bench_configs.py > configs.jsonl
 c4 is run with the 8 graphs one GPU holds when B=64 is sharded over 8 GPUs."""
 import json
 import os
@@ -14,7 +14,7 @@ REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path[:0] = [REPO, os.path.join(REPO, "tests")]
 from egnn_pytorch_b200 import EGNN, EGNN_Network  # noqa: E402
 
-ONLY = [t for t in os.environ.get("ONLY", "").split(",") if t]      # e.g. ONLY=c4 NOREF=1 for an ncu capture
+ONLY = [t for t in os.environ.get("ONLY", "").split(",") if t]      # e.g. ONLY=c4 NOREF=1 for a profiler capture
 DTYPES = [t for t in os.environ.get("DTYPES", "bf16,fp32").split(",") if t]
 
 
@@ -25,7 +25,7 @@ def want(tag):
 try:
     if os.environ.get("NOREF"):
         raise ImportError
-    sys.path.insert(0, os.path.join(REPO, "baseline", "_ref"))
+    sys.path.insert(0, os.path.join(REPO, "oracle", "_ref"))
     import egnn_pytorch as ref
 except Exception:  # pragma: no cover
     ref = None

@@ -2,7 +2,7 @@
 reported a 0.0 difference to the reference for fp32 rows: stale memory or real?)"""
 import sys, os, torch
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__))); sys.path[:0] = [REPO]
-sys.path.insert(0, os.path.join(REPO, "baseline", "_ref"))
+sys.path.insert(0, os.path.join(REPO, "oracle", "_ref"))
 import egnn_pytorch as ref
 import egnn_pytorch_b200 as ours_pkg
 from egnn_pytorch_b200 import GraphedForward

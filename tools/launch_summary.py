@@ -1,5 +1,5 @@
 """Aggregate an `ncu --metrics gpu__time_duration.sum --csv` launch list by kernel name.
-    python tools/launch_summary.py gpurun_out/launches.csv [divide_by]"""
+    python tools/launch_summary.py launches.csv [divide_by]"""
 import collections
 import csv
 import re

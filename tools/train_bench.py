@@ -2,7 +2,7 @@
 
     python tools/train_bench.py [--b 4] [--n 1024] [--dim 512] [--k 0] [--ref-b 1] [--iters 5] [--no-ref]
 
-Prints one JSON line per arm.  The reference arm imports the unmodified reference from baseline/_ref; its batch is
+Prints one JSON line per arm.  The reference arm imports the unmodified reference from oracle/_ref; its batch is
 `--ref-b` graphs (its autograd graph keeps ~35 GB per graph at dim=512, N=1024 in fp32) and its time is reported per
 graph so the two arms compare per unit of work.
 """
@@ -75,7 +75,7 @@ def main():
                           edges_per_s=round(pairs / ms * 1e3, 1))))
     if a.no_ref:
         return
-    sys.path.insert(0, os.path.join(REPO, "baseline", "_ref"))
+    sys.path.insert(0, os.path.join(REPO, "oracle", "_ref"))
     from egnn_pytorch import EGNN as RefEGNN
     ref = RefEGNN(**kw).to(dev)
     try:
