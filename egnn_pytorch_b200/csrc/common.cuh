@@ -6,7 +6,9 @@
 #include <stdint.h>
 #include <stddef.h>
 #include <math.h>
+#include <map>
 #include <mutex>
+#include <utility>
 
 #include "../../include/egnn_b200.h"
 
@@ -28,6 +30,29 @@ namespace egnn {
 // Launch check that does not synchronise: catches bad configurations at enqueue time.
 #define EGNN_LAUNCH_CHECK() EGNN_CUDA_TRY(cudaPeekAtLastError())
 
+// Opt `kernel` in to `bytes` of dynamic shared memory on the current device.  One process-wide table remembers what
+// each (device, kernel) was raised to, so the attribute is set once per new maximum, never lowered (one kernel is
+// launched from several translation units with different needs), and a launch that needs no more costs no API call
+// beyond cudaGetDevice.
+inline int ensure_dynamic_smem(const void* kernel, size_t bytes) {
+  if (bytes <= 48 * 1024) return EGNN_OK;
+  static std::mutex mu;
+  static std::map<std::pair<int, const void*>, size_t> raised;
+  int dev = 0;
+  EGNN_CUDA_TRY(cudaGetDevice(&dev));
+  std::lock_guard<std::mutex> lock(mu);
+  size_t& cur = raised[{dev, kernel}];
+  if (cur < bytes) {
+    EGNN_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
+    cur = bytes;
+  }
+  return EGNN_OK;
+}
+template <typename... A>
+inline int ensure_dynamic_smem(void (*kernel)(A...), size_t bytes) {
+  return ensure_dynamic_smem(reinterpret_cast<const void*>(kernel), bytes);
+}
+
 __host__ __device__ inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 __host__ __device__ inline size_t round_up(size_t a, size_t b) { return (a + b - 1) / b * b; }
 __host__ __device__ inline int round_up_i(int a, int b) { return (a + b - 1) / b * b; }
@@ -46,6 +71,10 @@ inline int sm_count(int* out) {
   *out = n;
   return EGNN_OK;
 }
+
+// Neighbour lists of a layer with k > 0 (egnn_pytorch.py:237-260), ranked into *nbr_idx / *nbr_ok (workspace arrays
+// of [B,N,k]); in edge-list mode (io.nbr_idx set) the pointers are redirected to the caller's lists and *nbr_ok to null.
+int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st);
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {
@@ -127,16 +156,6 @@ template <> __device__ __forceinline__ double fma_t<double>(double a, double b, 
 template <typename T> __device__ __forceinline__ T sq_acc(T a, T acc);
 template <> __device__ __forceinline__ float sq_acc<float>(float a, float acc) { return __fadd_rn(acc, __fmul_rn(a, a)); }
 template <> __device__ __forceinline__ double sq_acc<double>(double a, double acc) { return __dadd_rn(acc, __dmul_rn(a, a)); }
-
-// Two values that travel together through a contraction: two independent FMAs per update (Hopper has no packed
-// fp32 FMA, so fp32 and fp64 take the same form).
-template <typename T> struct Pk2 {
-  T x, y;
-  __device__ __forceinline__ static Pk2 make(T lo, T hi) { Pk2 r; r.x = lo; r.y = hi; return r; }
-  __device__ __forceinline__ void fma(const Pk2& a, const Pk2& b) { x = fma_t<T>(a.x, b.x, x); y = fma_t<T>(a.y, b.y, y); }
-  __device__ __forceinline__ T lo() const { return x; }
-  __device__ __forceinline__ T hi() const { return y; }
-};
 
 // 4 consecutive elements, 4-element aligned.
 template <typename T> struct Vec4;

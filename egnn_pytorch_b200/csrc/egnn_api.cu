@@ -10,47 +10,6 @@
 
 namespace egnn {
 
-int knn_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
-                        const uint8_t* adj, int adj_batched, double valid_radius, int32_t* out_idx,
-                        uint8_t* out_ok, cudaStream_t st);
-int adj_neighbors_dispatch(int B, int N, int k, const uint8_t* adj, int adj_batched, int32_t* out_idx, uint8_t* out_ok,
-                           cudaStream_t st);
-
-template <typename T, int MP, bool KNN>
-static int launch_pair(const PairArgs<T>& a, cudaStream_t st) {
-  const size_t smem = pair_smem_bytes<T>(a.s, a.L, KNN);
-  EGNN_TRY(ensure_dynamic_smem(pair_kernel<T, MP, KNN>, smem));
-  const int TI = PAIR_THREADS / a.TS;
-  dim3 grid(ceil_div(a.s.row1 - a.s.row0, TI), a.s.B);
-  pair_kernel<T, MP, KNN><<<grid, PAIR_THREADS, smem, st>>>(a);
-  EGNN_LAUNCH_CHECK();
-  count_launch();
-  return EGNN_OK;
-}
-
-template <typename T, int MP, int PP>
-static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
-  const size_t smem = pair_tiled_smem_bytes<T>(a.s, a.L, PP);
-  EGNN_TRY(ensure_dynamic_smem(pair_dense_tiled_kernel<T, MP, PP>, smem));
-  dim3 grid(ceil_div(a.s.row1 - a.s.row0, 4 * PP), a.s.B);
-  if (a.hsplit > 1) {
-    PairArgs<T> a1 = a, a2 = a;
-    a1.phase = 1; a2.phase = 2;
-    a1.pre2_out = nullptr;                            // partial sums; phase 2 holds the full ones
-    dim3 g1(grid.x, grid.y, a.hsplit);
-    pair_dense_tiled_kernel<T, MP, PP><<<g1, PAIR_THREADS, smem, st>>>(a1);
-    EGNN_LAUNCH_CHECK();
-    pair_dense_tiled_kernel<T, MP, PP><<<grid, PAIR_THREADS, smem, st>>>(a2);
-    EGNN_LAUNCH_CHECK();
-    count_launch(2);
-    return EGNN_OK;
-  }
-  pair_dense_tiled_kernel<T, MP, PP><<<grid, PAIR_THREADS, smem, st>>>(a);
-  EGNN_LAUNCH_CHECK();
-  count_launch();
-  return EGNN_OK;
-}
-
 template <typename T>
 static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed,
                         const EgnnLayerIO& io, void* ws, size_t ws_bytes, cudaStream_t st) {
@@ -71,19 +30,7 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
   const RowMap ident{s.N, s.N, 0};
 
   // 1. neighbour lists (egnn_pytorch.py:237-260)
-  if (s.k > 0 && io.nbr_idx) {                       // edge-list mode: the caller's lists, no ranking
-    nbr_idx = const_cast<int32_t*>(io.nbr_idx);
-    nbr_ok = nullptr;
-  } else if (s.k > 0) {
-    StageTimer tm(st, STAGE_SELECT);
-    count_launch();
-    const double vr = (d.flags & EGNN_FLAG_ONLY_SPARSE) ? 0.0 : d.valid_radius;     // :250
-    if ((d.flags & EGNN_FLAG_ONLY_SPARSE) && io.mask && io.adj)      // every slot top-k could add is masked out: row scan
-      EGNN_TRY(adj_neighbors_dispatch(s.B, s.N, s.k, io.adj, (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0, nbr_idx, nbr_ok, st));
-    else
-      EGNN_TRY(knn_select_dispatch(d.dtype, s.B, s.N, s.C, s.k, io.coors, io.mask, io.adj,
-                                   (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0, vr, nbr_idx, nbr_ok, st));
-  }
+  if (s.k > 0) EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st));
   // 2. per-node tables  A = h W1[:, :dim]^T + b1,  B = h W1[:, dim:2dim]^T   (split of :287's Linear-1)
   {
     StageTimer tm(st, STAGE_NODE_PRE);
@@ -106,7 +53,7 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
     }
   }
   // 3. fused edge step
-  PairArgs<T> a;
+  PairArgs<T> a{};
   a.s = s; a.L = L; a.flags = d.flags; a.has_mask = io.mask != nullptr;
   a.clamp = (T)d.clamp;
   a.P = P; a.ldP = 2 * s.Hp;
@@ -128,19 +75,11 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
       int TS = 1;
       while (TS < s.k && TS < 32) TS <<= 1;
       a.TS = TS;
-      if (L.MP == 16) EGNN_TRY((launch_pair<T, 16, true>(a, st)));
-      else EGNN_TRY((launch_pair<T, 32, true>(a, st)));
+      EGNN_TRY((L.MP == 16 ? launch_pair<T, 16>(a, st) : launch_pair<T, 32>(a, st)));
+      count_launch();
     } else {
-      a.TS = 32;
-      constexpr int PP = 2;                                // rows per thread of the register-tiled dense kernel
-      int rc;
-      if (L.MP == 16) rc = launch_pair_tiled<T, 16, PP>(a, st);
-      else rc = launch_pair_tiled<T, 32, sizeof(T) == 4 ? 2 : 1>(a, st);
-      if (rc == EGNN_ERR_UNSUPPORTED) {                   // shared memory budget: thread-per-pair kernel
-        if (L.MP == 16) rc = launch_pair<T, 16, false>(a, st);
-        else rc = launch_pair<T, 32, false>(a, st);
-      }
-      EGNN_TRY(rc);
+      EGNN_TRY((L.MP == 16 ? launch_pair_dense<T, 16>(a, st) : launch_pair_dense<T, 32>(a, st)));
+      count_launch(wl.hsplit > 1 ? 2 : 1);
     }
   }
   // 4. node update  h' = node_mlp([LN(h) | m_i]) + h   (egnn_pytorch.py:335-337)

@@ -22,7 +22,7 @@ inline BwdWs bwd_ws_layout(const Dims& s, const SimtPackLayout& L, size_t es, ui
   w.gP = take((size_t)s.M * 2 * s.Hp * es);
   w.gpk = take(L.total * es);
   w.rec = take((size_t)s.M * J * rec_layout(s, L.MP).R * es);
-  w.pre2 = take(s.k == 0 ? (size_t)s.M * s.N * L.MP * es : 0);
+  w.pre2 = take((size_t)s.M * J * L.MP * es);
   w.h1pre = take(uf ? (size_t)s.M * 2 * s.dim * es : 0);
   w.ga = take(uf ? (size_t)s.M * 2 * s.dim * es : 0);
   w.g_node_in = take(uf ? (size_t)s.M * (s.dim + s.m) * es : 0);
@@ -65,96 +65,53 @@ static int launch_colsum(const T* X, long ld, int rows, int cols, T* out, cudaSt
   return EGNN_OK;
 }
 
-template <typename K>
-static int opt_in_smem(K kernel, size_t smem) { return ensure_dynamic_smem(kernel, smem); }
-
-// Dense: W2 silu(pre1) for every pair with the register-tiled forward kernel (its split-H "phase 1" stores exactly
-// that); returns EGNN_ERR_UNSUPPORTED when its shared memory does not fit, and bwd1 then recomputes by itself.
-template <typename T, int MP, int PP>
-static int launch_tiled_recompute(const BwdArgs<T>& a, T* pre2, cudaStream_t st) {
+// W2 silu(pre1) of every pair into pre2 when the forward did not keep it, by the forward's own edge kernels (with
+// the forward's dropout masks): for dense graphs the register-tiled kernel's split-H phase 1 over one split, which
+// stores exactly that; for neighbour lists pair_kernel with no node or coordinate update.
+template <typename T, int MP>
+static int recompute_pre2(const BwdArgs<T>& a, T* pre2, cudaStream_t st) {
   PairArgs<T> f;
-  f.s = a.s; f.L = a.L; f.flags = a.flags; f.has_mask = a.has_mask; f.TS = 32; f.clamp = a.clamp;
+  f.s = a.s; f.L = a.L; f.flags = a.flags; f.has_mask = a.has_mask; f.TS = a.TS; f.clamp = a.clamp;
   f.P = a.P; f.ldP = a.ldP; f.coors = a.coors; f.edges = a.edges; f.labels = a.labels; f.mask = a.mask;
-  f.nbr_idx = nullptr; f.nbr_ok = nullptr; f.packed = a.packed;
+  f.nbr_idx = a.nbr_idx; f.nbr_ok = a.nbr_ok; f.packed = a.packed;
   f.m_out = nullptr; f.ld_m = 0; f.coors_out = nullptr;
-  f.hpart = pre2; f.hsplit = 1; f.phase = 1;
+  f.hpart = nullptr; f.hsplit = 1; f.phase = 0;
   f.pre2_out = nullptr;
-  f.drop = a.drop;                                    // the recompute must draw the forward's masks
-  const size_t smem = pair_tiled_smem_bytes<T>(a.s, a.L, PP);
-  EGNN_TRY(opt_in_smem(pair_dense_tiled_kernel<T, MP, PP>, smem));
-  dim3 grid(ceil_div(a.s.N, 4 * PP), a.s.B, 1);
-  pair_dense_tiled_kernel<T, MP, PP><<<grid, PAIR_THREADS, smem, st>>>(f);
-  EGNN_LAUNCH_CHECK();
-  return EGNN_OK;
+  f.drop = a.drop;
+  if (a.s.k > 0) {
+    f.flags &= ~(uint32_t)(EGNN_FLAG_UPDATE_FEATS | EGNN_FLAG_UPDATE_COORS);
+    f.pre2_out = pre2;
+    return launch_pair<T, MP>(f, st);
+  }
+  f.hpart = pre2; f.phase = 1;
+  return launch_pair_dense<T, MP>(f, st);
 }
 
 template <typename T, int MP, bool KNN>
-static int launch_pair_bwd(BwdArgs<T>& a, bool saved_pre2, cudaStream_t st) {
+static int launch_pair_bwd(const BwdArgs<T>& a, cudaStream_t st) {
   const Dims& s = a.s;
-  if constexpr (!KNN) {
-    if (!saved_pre2) {
-    T* pre2 = const_cast<T*>(a.pre2);
-    const int rc = launch_tiled_recompute<T, MP, (MP == 32 && sizeof(T) == 8) ? 1 : 2>(a, pre2, st);
-    if (rc == EGNN_ERR_UNSUPPORTED) a.pre2 = nullptr;
-    else EGNN_TRY(rc);
-    }
-  }
-  const size_t smem1 = bwd1_smem_bytes<T>(s, a.L, KNN, (a.flags & EGNN_FLAG_SOFT_EDGES) != 0);
-  EGNN_TRY(opt_in_smem(pair_bwd1_kernel<T, MP, KNN>, smem1));
-  const int TI = PAIR_THREADS / a.TS;
-  dim3 g1(ceil_div(s.N, TI), s.B);
-  pair_bwd1_kernel<T, MP, KNN><<<g1, PAIR_THREADS, smem1, st>>>(a);
-  EGNN_LAUNCH_CHECK();
+  const dim3 g1(ceil_div(s.N, PAIR_THREADS / a.TS), s.B);
+  EGNN_TRY(launch_simt(pair_bwd1_kernel<T, MP, KNN>, g1, PAIR_THREADS,
+                       bwd1_smem_bytes<T>(s, a.L, (a.flags & EGNN_FLAG_SOFT_EDGES) != 0), st, a));
+  // bwd2: distance channel only (QR = 1), up to 8 channels in registers (lists only, QR = 8) or any (QR = 0); the
+  // dropout masks in their own instantiations
+  const bool simple = s.Q == 1 && s.label_dim == 0, drop = a.drop.thr != 0;
+  void (*bwd2)(BwdArgs<T>);
+  size_t smem2;
+  dim3 g2;
   if constexpr (KNN) {
-    const size_t smem2 = bwd2_knn_smem_bytes<T>(s, a.rl.R);
-    dim3 g2(ceil_div(s.N, a.TI2), ceil_div(s.Hp, BW2_TH), s.B);
-    if (s.Q == 1 && s.label_dim == 0) {
-      if (a.drop.thr) {
-        EGNN_TRY(opt_in_smem(pair_bwd2_knn_kernel<T, MP, 1, true>, smem2));
-        pair_bwd2_knn_kernel<T, MP, 1, true><<<g2, BW2_TH, smem2, st>>>(a);
-      } else {
-        EGNN_TRY(opt_in_smem(pair_bwd2_knn_kernel<T, MP, 1, false>, smem2));
-        pair_bwd2_knn_kernel<T, MP, 1, false><<<g2, BW2_TH, smem2, st>>>(a);
-      }
-    } else if (s.Q <= 8) {
-      if (a.drop.thr) {
-        EGNN_TRY(opt_in_smem(pair_bwd2_knn_kernel<T, MP, 8, true>, smem2));
-        pair_bwd2_knn_kernel<T, MP, 8, true><<<g2, BW2_TH, smem2, st>>>(a);
-      } else {
-        EGNN_TRY(opt_in_smem(pair_bwd2_knn_kernel<T, MP, 8, false>, smem2));
-        pair_bwd2_knn_kernel<T, MP, 8, false><<<g2, BW2_TH, smem2, st>>>(a);
-      }
-    } else {
-      if (a.drop.thr) {
-        EGNN_TRY(opt_in_smem(pair_bwd2_knn_kernel<T, MP, 0, true>, smem2));
-        pair_bwd2_knn_kernel<T, MP, 0, true><<<g2, BW2_TH, smem2, st>>>(a);
-      } else {
-        EGNN_TRY(opt_in_smem(pair_bwd2_knn_kernel<T, MP, 0, false>, smem2));
-        pair_bwd2_knn_kernel<T, MP, 0, false><<<g2, BW2_TH, smem2, st>>>(a);
-      }
-    }
+    smem2 = bwd2_knn_smem_bytes<T>(s, a.rl.R);
+    g2 = dim3(ceil_div(s.N, a.TI2), ceil_div(s.Hp, BW2_TH), s.B);
+    if (simple) bwd2 = drop ? pair_bwd2_knn_kernel<T, MP, 1, true> : pair_bwd2_knn_kernel<T, MP, 1, false>;
+    else if (s.Q <= 8) bwd2 = drop ? pair_bwd2_knn_kernel<T, MP, 8, true> : pair_bwd2_knn_kernel<T, MP, 8, false>;
+    else bwd2 = drop ? pair_bwd2_knn_kernel<T, MP, 0, true> : pair_bwd2_knn_kernel<T, MP, 0, false>;
   } else {
-    const size_t smem2 = bwd2_dense_smem_bytes<T>(s, a.rl.R);
-    dim3 g2(ceil_div(s.N, BW2_ROWS), ceil_div(s.Hp, BW2_TH), s.B);
-    if (s.Q == 1 && s.label_dim == 0) {
-      if (a.drop.thr) {
-        EGNN_TRY(opt_in_smem(pair_bwd2_dense_kernel<T, MP, 1, true>, smem2));
-        pair_bwd2_dense_kernel<T, MP, 1, true><<<g2, BW2_TH, smem2, st>>>(a);
-      } else {
-        EGNN_TRY(opt_in_smem(pair_bwd2_dense_kernel<T, MP, 1, false>, smem2));
-        pair_bwd2_dense_kernel<T, MP, 1, false><<<g2, BW2_TH, smem2, st>>>(a);
-      }
-    } else {
-      if (a.drop.thr) {
-        EGNN_TRY(opt_in_smem(pair_bwd2_dense_kernel<T, MP, 0, true>, smem2));
-        pair_bwd2_dense_kernel<T, MP, 0, true><<<g2, BW2_TH, smem2, st>>>(a);
-      } else {
-        EGNN_TRY(opt_in_smem(pair_bwd2_dense_kernel<T, MP, 0, false>, smem2));
-        pair_bwd2_dense_kernel<T, MP, 0, false><<<g2, BW2_TH, smem2, st>>>(a);
-      }
-    }
+    smem2 = bwd2_dense_smem_bytes<T>(s, a.rl.R);
+    g2 = dim3(ceil_div(s.N, BW2_ROWS), ceil_div(s.Hp, BW2_TH), s.B);
+    if (simple) bwd2 = drop ? pair_bwd2_dense_kernel<T, MP, 1, true> : pair_bwd2_dense_kernel<T, MP, 1, false>;
+    else bwd2 = drop ? pair_bwd2_dense_kernel<T, MP, 0, true> : pair_bwd2_dense_kernel<T, MP, 0, false>;
   }
-  EGNN_LAUNCH_CHECK();
+  EGNN_TRY(launch_simt(bwd2, g2, BW2_TH, smem2, st, a));
   pair_bwd3_kernel<T, KNN><<<g1, PAIR_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
@@ -269,21 +226,20 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
   a.g_coors_out = static_cast<const T*>(gr.g_coors_out);
   a.drop = make_drop(d.dropout_p, d.dropout_seed);
   const bool saved = io.pre2_out != nullptr;                 // the forward kept W2 silu(pre1) per pair
-  a.pre2 = saved ? static_cast<const T*>(io.pre2_out)
-                 : (s.k == 0 ? reinterpret_cast<const T*>(base + bl.pre2) : nullptr);
+  T* pre2 = saved ? static_cast<T*>(io.pre2_out) : reinterpret_cast<T*>(base + bl.pre2);
+  a.pre2 = pre2;
   a.rec = rec; a.gpk = gpk; a.gP = gP; a.g_coors = g_coors;
   a.g_edges = (s.edge_dim > 0) ? static_cast<T*>(gr.g_edges) : nullptr;
   if (s.k > 0) {
     int TS = 1;
     while (TS < s.k && TS < 32) TS <<= 1;
     a.TS = TS; a.TI2 = 16;
-    if (L.MP == 16) EGNN_TRY((launch_pair_bwd<T, 16, true>(a, false, st)));
-    else EGNN_TRY((launch_pair_bwd<T, 32, true>(a, false, st)));
   } else {
     a.TS = 32; a.TI2 = 32;
-    if (L.MP == 16) EGNN_TRY((launch_pair_bwd<T, 16, false>(a, saved, st)));
-    else EGNN_TRY((launch_pair_bwd<T, 32, false>(a, saved, st)));
   }
+  if (!saved) EGNN_TRY((L.MP == 16 ? recompute_pre2<T, 16>(a, pre2, st) : recompute_pre2<T, 32>(a, pre2, st)));
+  if (s.k > 0) EGNN_TRY((L.MP == 16 ? launch_pair_bwd<T, 16, true>(a, st) : launch_pair_bwd<T, 32, true>(a, st)));
+  else EGNN_TRY((L.MP == 16 ? launch_pair_bwd<T, 16, false>(a, st) : launch_pair_bwd<T, 32, false>(a, st)));
 
   // ---- per-node tables reversed: A = h W1[:, :dim]^T + b1, B = h W1[:, dim:2dim]^T
   T* gW1 = static_cast<T*>(gr.w.edge_w1);

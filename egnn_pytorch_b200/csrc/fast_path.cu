@@ -4,7 +4,6 @@
 // Option sets the tensor-core kernels do not cover return EGNN_ERR_UNSUPPORTED; the binding then runs
 // the fp32 SIMT kernels (never a CPU path).
 #include <stdlib.h>
-#include <mutex>
 #include "fast_path.h"
 #include "profile.h"
 #include "tc_gemm.cuh"
@@ -13,12 +12,6 @@
 #include "small_node.cuh"
 
 namespace egnn {
-
-int knn_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
-                        const uint8_t* adj, int adj_batched, double valid_radius, int32_t* out_idx,
-                        uint8_t* out_ok, cudaStream_t st);
-int adj_neighbors_dispatch(int B, int N, int k, const uint8_t* adj, int adj_batched, int32_t* out_idx, uint8_t* out_ok,
-                           cudaStream_t st);
 
 namespace {
 
@@ -224,22 +217,6 @@ FastWs fast_ws_layout(const FastDims& f, uint32_t flags) {
   return w;
 }
 
-// cudaFuncSetAttribute(MaxDynamicSharedMemorySize) once per (kernel, device), under a mutex: the only mutable
-// state of this file, written once per device and never shrunk.  TAG distinguishes kernels of identical type.
-template <int TAG, typename K>
-int ensure_dyn_smem(K kernel, size_t bytes) {
-  static std::mutex mu;
-  static size_t set[64] = {0};
-  int dev = 0;
-  EGNN_CUDA_TRY(cudaGetDevice(&dev));
-  std::lock_guard<std::mutex> lock(mu);
-  if (dev >= 64 || set[dev] < bytes) {
-    EGNN_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes));
-    if (dev < 64) set[dev] = bytes;
-  }
-  return EGNN_OK;
-}
-
 // Optional start-up delay between the warpgroups of the persistent dense kernel (tc_pair.cuh), EGNN_B200_SKEW_NS.
 // Default 0 (no de-phasing).
 uint32_t pair_skew_ns() {
@@ -253,7 +230,7 @@ uint32_t pair_skew_ns() {
 // one launch for one (g2 == nullptr) or two problems over the same rows
 int launch_tc_gemm(const TcGemmArgs& g, cudaStream_t st, const TcGemmArgs* g2 = nullptr) {
   if (g.M <= 0) return EGNN_OK;
-  EGNN_TRY((ensure_dyn_smem<0>(tc_gemm_kernel, GEMM_SMEM_BYTES)));
+  EGNN_TRY((ensure_dynamic_smem(tc_gemm_kernel, GEMM_SMEM_BYTES)));
   TcGemmPair gp;
   gp.p[0] = g;
   gp.p[1] = g2 ? *g2 : g;
@@ -337,7 +314,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
       t.b1 = reinterpret_cast<const float*>(pk + L.b1); t.Atab = Atab; t.Btab = Btab;
       t.M = s.M; t.N = s.N; t.dim = s.dim; t.Hp = f.Hp; t.row0 = r0; t.row1 = r1;
       const size_t smem = tables_small_smem(s.dim, f.Hp);
-      EGNN_TRY((ensure_dyn_smem<6>(tables_small_kernel, smem)));
+      EGNN_TRY((ensure_dynamic_smem(tables_small_kernel, smem)));
       int sms = 0;
       EGNN_TRY(sm_count(&sms));
       tables_small_kernel<<<std::min(ceil_div(s.M, SN_WARPS), 4 * sms), SN_WARPS * 32, smem, st>>>(t);
@@ -406,11 +383,11 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
       if (items < 2 * sms) a.skew_ns = 0;                      // too few row groups per CTA for the de-phasing to pay
       if (pair_is_lean(f)) {
         const size_t smem = tc_pair_smem_bytes<false>(f.Hp, 1);
-        EGNN_TRY((ensure_dyn_smem<1>(tc_pair_kernel<false>, smem)));
+        EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<false>, smem)));
         tc_pair_kernel<false><<<grid, TP_THREADS, smem, st>>>(a);
       } else {
         const size_t smem = tc_pair_smem_bytes<true>(f.Hp, f.QT, 1 + 2 * f.s.F);
-        EGNN_TRY((ensure_dyn_smem<2>(tc_pair_kernel<true>, smem)));
+        EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<true>, smem)));
         tc_pair_kernel<true><<<grid, TP_THREADS, smem, st>>>(a);
       }
       EGNN_LAUNCH_CHECK();
@@ -419,19 +396,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
   } else {         // neighbour lists: distance + top-k select, then the gathered fused edge kernel
     int32_t* nbr_idx = reinterpret_cast<int32_t*>(base + wl.nbr_idx);
     uint8_t* nbr_ok = base + wl.nbr_ok;
-    if (io.nbr_idx) {                                  // edge-list mode: the caller's lists, no ranking
-      nbr_idx = const_cast<int32_t*>(io.nbr_idx);
-      nbr_ok = nullptr;
-    } else {
-      StageTimer tm(st, STAGE_SELECT);
-      const double vr = (d.flags & EGNN_FLAG_ONLY_SPARSE) ? 0.0 : d.valid_radius;
-      if ((d.flags & EGNN_FLAG_ONLY_SPARSE) && io.mask && io.adj)      // every slot top-k could add is masked out: row scan
-        EGNN_TRY(adj_neighbors_dispatch(s.B, s.N, s.k, io.adj, (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0, nbr_idx, nbr_ok, st));
-      else
-        EGNN_TRY(knn_select_dispatch(EGNN_DTYPE_F32, s.B, s.N, s.C, s.k, io.coors, io.mask, io.adj,
-                                     (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0, vr, nbr_idx, nbr_ok, st));
-      count_launch();
-    }
+    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st));
     StageTimer tm(st, STAGE_PAIR);
     TcKnnArgs a{};
     a.B = s.B; a.N = s.N; a.Hp = f.Hp; a.ldn = f.Kn; a.dim = s.dim; a.k = s.k; a.edge_dim = s.edge_dim;
@@ -456,17 +421,17 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     const size_t smem = tc_knn_smem_bytes(f.Hp, mode, f.QT, rows);
     dim3 grid(ceil_div(R, rows), s.B);
     if (R > 0) {
-#define EGNN_TC_KNN_LAUNCH(TAG, MODE_, ROWS_)                                                  \
-  do {                                                                                          \
-    EGNN_TRY((ensure_dyn_smem<TAG>(tc_knn_kernel<MODE_, ROWS_>, smem)));                        \
-    tc_knn_kernel<MODE_, ROWS_><<<grid, ROWS_ * 32, smem, st>>>(a);                             \
+#define EGNN_TC_KNN_LAUNCH(MODE_, ROWS_)                                                  \
+  do {                                                                              \
+    EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_>, smem)));             \
+    tc_knn_kernel<MODE_, ROWS_><<<grid, ROWS_ * 32, smem, st>>>(a);                 \
   } while (0)
       if (mode == TK_LEAN) {
-        if (rows == 8) EGNN_TC_KNN_LAUNCH(3, TK_LEAN, 8); else EGNN_TC_KNN_LAUNCH(13, TK_LEAN, 16);
+        if (rows == 8) EGNN_TC_KNN_LAUNCH(TK_LEAN, 8); else EGNN_TC_KNN_LAUNCH(TK_LEAN, 16);
       } else if (mode == TK_EDGES) {
-        if (rows == 8) EGNN_TC_KNN_LAUNCH(4, TK_EDGES, 8); else EGNN_TC_KNN_LAUNCH(14, TK_EDGES, 16);
+        if (rows == 8) EGNN_TC_KNN_LAUNCH(TK_EDGES, 8); else EGNN_TC_KNN_LAUNCH(TK_EDGES, 16);
       } else {
-        if (rows == 8) EGNN_TC_KNN_LAUNCH(5, TK_GEN, 8); else EGNN_TC_KNN_LAUNCH(15, TK_GEN, 16);
+        if (rows == 8) EGNN_TC_KNN_LAUNCH(TK_GEN, 8); else EGNN_TC_KNN_LAUNCH(TK_GEN, 16);
       }
 #undef EGNN_TC_KNN_LAUNCH
       EGNN_LAUNCH_CHECK();
@@ -484,7 +449,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
       n.lnb = reinterpret_cast<const float*>(pk + L.lnb); n.out = fout;
       n.B = s.B; n.N = s.N; n.dim = s.dim; n.Kn = f.Kn; n.m = s.m; n.row0 = r0; n.row1 = r1; n.do_norm = (d.flags & EGNN_FLAG_NORM_FEATS) ? 1 : 0;
       const size_t smem = node_small_smem(s.dim, f.Kn);
-      EGNN_TRY((ensure_dyn_smem<7>(node_update_small_kernel, smem)));
+      EGNN_TRY((ensure_dynamic_smem(node_update_small_kernel, smem)));
       int sms = 0;
       EGNN_TRY(sm_count(&sms));
       node_update_small_kernel<<<std::min(ceil_div(s.B * R, SN_WARPS), 4 * sms), SN_WARPS * 32, smem, st>>>(n);

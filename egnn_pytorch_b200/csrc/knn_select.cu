@@ -13,6 +13,7 @@
 // warp-bitonic sort + merge, so the O(N^2) ranking matrix is never written.
 // k  > 32: one block per row sorts all N (rank, j) pairs in shared memory (bitonic).
 #include "common.cuh"
+#include "profile.h"
 
 namespace egnn {
 
@@ -351,6 +352,23 @@ int adj_neighbors_dispatch(int B, int N, int k, const uint8_t* adj, int adj_batc
   adj_neighbors_kernel<<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(B, N, k, adj, adj_batched, out_idx, out_ok);
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
+}
+
+int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st) {
+  if (io.nbr_idx) {                                  // edge-list mode: the caller's lists, no ranking
+    *nbr_idx = const_cast<int32_t*>(io.nbr_idx);
+    *nbr_ok = nullptr;
+    return EGNN_OK;
+  }
+  StageTimer tm(st, STAGE_SELECT);
+  count_launch();
+  const int adj_batched = (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0;
+  if ((d.flags & EGNN_FLAG_ONLY_SPARSE) && io.mask && io.adj)      // every slot top-k could add is masked out: row scan
+    return adj_neighbors_dispatch(d.B, d.N, d.k, io.adj, adj_batched, *nbr_idx, *nbr_ok, st);
+  const double vr = (d.flags & EGNN_FLAG_ONLY_SPARSE) ? 0.0 : d.valid_radius;     // egnn_pytorch.py:250
+  // coordinates are fp64 for the fp64 layer and fp32 otherwise (bf16 layers included)
+  return knn_select_dispatch(d.dtype == EGNN_DTYPE_F64 ? EGNN_DTYPE_F64 : EGNN_DTYPE_F32, d.B, d.N, d.C, d.k, io.coors,
+                             io.mask, io.adj, adj_batched, vr, *nbr_idx, *nbr_ok, st);
 }
 
 }  // namespace egnn

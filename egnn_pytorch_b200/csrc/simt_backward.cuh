@@ -1,9 +1,11 @@
 // Backward of the EGNN layer (SIMT fp32 / fp64), SURVEY.md section 8(f) rank 1.
 //
 // The reference trains through autograd over the materialised [B,N,J,2E] tensors (egnn_pytorch.py:224-341).
-// Here the forward is RECOMPUTED per pair in the split form of simt_kernels.cuh and differentiated by hand:
+// Here the forward is differentiated by hand in the split form of simt_kernels.cuh.  W2 silu(pre1) per pair (pre2)
+// comes from the forward (EgnnLayerIO.pre2_out) or is recomputed before bwd1 by a forward kernel that stores it:
+// the register-tiled kernel for dense graphs, pair_kernel for neighbour lists.
 //
-//   bwd1  thread per (i, slot) pair: recompute m_ij, differentiate the pair epilogue (coordinate MLP, CoorsNorm,
+//   bwd1  thread per (i, slot) pair: from pre2, recompute m_ij, differentiate the pair epilogue (coordinate MLP, CoorsNorm,
 //         clamp, masks, gate, pooling) and leave per pair  g_pre2[m] = dL/d(W2 hid + b2), the scalar channels f_q,
 //         coef = w_ij * scale and the CoorsNorm part of dL/d(dist)  in a [pairs][R] record; the small parameter
 //         gradients (coors_mlp, edge_gate, b2, coors_norm.scale) are reduced per CTA.
@@ -58,9 +60,8 @@ struct BwdArgs {
   const T* packed;
   const T* g_node_in; int ld_g;   // [M][dim+m]; dL/dm_i = columns dim..dim+m  (null when !update_feats)
   const T* g_coors_out;           // [B,N,C]
-  const T* pre2;                  // optional: W2 silu(pre1) per pair, row-major [B,N,J][MP]: saved by the forward
-                                  // (EgnnLayerIO.pre2_out) or, dense only, recomputed by the register-tiled forward
-                                  // kernel; null = bwd1 recomputes it itself
+  const T* pre2;                  // W2 silu(pre1) per pair, row-major [B,N,J][MP]: saved by the forward
+                                  // (EgnnLayerIO.pre2_out) or recomputed into the backward workspace
   T* rec;                         // [pairs][R]
   T* gpk;                         // gradient accumulators in SimtPackLayout order (zeroed by the caller)
   T* gP;                          // [M][2*Hp]: dL/dA | dL/dB (zeroed by the caller)
@@ -99,13 +100,9 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // bwd1
 // =====================================================================================
 template <typename T>
-inline size_t bwd1_smem_bytes(const Dims& s, const SimtPackLayout& L, bool knn, bool soft) {
+inline size_t bwd1_smem_bytes(const Dims& s, const SimtPackLayout& L, bool soft) {
   const int U = 4 * s.m;
   size_t n = 0;
-  n += (size_t)PAIR_CH * L.MP;                 // W2s
-  n += (size_t)s.Q * PAIR_CH;                  // wqs
-  if (!knn) n += (size_t)PAIR_CH * 33;         // Bs
-  if (s.Q > 1) n += (size_t)s.Q * PAIR_THREADS;  // fs
   n += (size_t)U * L.MP + 2 * U + 2 * L.MP + 4;   // w3s, b3s, w4s, misc
   n += (size_t)(soft ? 3 : 2) * PAIR_THREADS * L.MP;   // mms, gp2s, aux
   n += PAIR_THREADS;                           // gw0s
@@ -127,18 +124,13 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
   const int i = row_valid ? i_raw : 0;
   const int J = KNN ? s.k : s.N;
   const int U = 4 * s.m, UP = U + 1;
-  const int qd = 2 * s.F;
   const bool upd_feats = a.flags & EGNN_FLAG_UPDATE_FEATS;
   const bool upd_coors = a.flags & EGNN_FLAG_UPDATE_COORS;
   const bool soft = a.flags & EGNN_FLAG_SOFT_EDGES;
   const bool normc = a.flags & EGNN_FLAG_NORM_COORS;
   const bool clampf = a.flags & EGNN_FLAG_CLAMP;
 
-  T* W2s = reinterpret_cast<T*>(smem_raw);                 // [CH][MP]
-  T* wqs = W2s + PAIR_CH * MP;                             // [Q][CH]
-  T* Bs = wqs + s.Q * PAIR_CH;                             // [CH][33]      (dense only)
-  T* fs = Bs + (KNN ? 0 : PAIR_CH * 33);                   // [Q][128]      (Q > 1 only)
-  T* w3s = fs + (s.Q > 1 ? s.Q * PAIR_THREADS : 0);        // [U][MP]
+  T* w3s = reinterpret_cast<T*>(smem_raw);                 // [U][MP]
   T* b3s = w3s + U * MP;                                   // [U]
   T* w4s = b3s + U;                                        // [U]
   T* misc = w4s + U;                                       // b2[MP] | gate_w[MP] | gate_b, b4, scale, 0
@@ -155,12 +147,11 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
     w4s[x] = upd_coors ? pk[a.L.w4 + x] : T(0);
   }
   for (int x = tid; x < 2 * MP + 4; x += PAIR_THREADS) misc[x] = pk[a.L.misc + x];
-  // (visibility: the __syncthreads at the top of the chunk loop)
+  // (visibility: the __syncthreads at the top of the pair loop)
 
   const size_t node_i = (size_t)b * s.N + i;
   const T* xi = a.coors + node_i * s.C;
   const bool mask_i = a.has_mask ? (a.mask[node_i] != 0) : true;
-  const T* Arow = a.P + node_i * a.ldP;
   T gxo[PAIR_CMAX];
 #pragma unroll
   for (int c = 0; c < PAIR_CMAX; ++c) gxo[c] = (c < s.C) ? a.g_coors_out[node_i * s.C + c] : T(0);
@@ -172,20 +163,8 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
       T cnt = T(0);
       for (int s0 = 0; s0 < J; s0 += TS) {
         const int sidx = s0 + sl;
-        bool pv = row_valid && sidx < J;
-        int j = 0;
-        bool ok = true;
-        if (KNN) {
-          if (pv) {
-            const size_t o = node_i * s.k + sidx;
-            j = a.nbr_idx[o];
-            ok = a.nbr_ok ? a.nbr_ok[o] != 0 : true;
-            if (j < 0) { j = 0; pv = false; }
-          }
-        } else {
-          j = pv ? sidx : 0;
-        }
-        if (pv && mask_i && a.mask[(size_t)b * s.N + j] != 0 && ok) cnt += T(1);
+        const PairSlot ps = pair_slot<KNN>(a.nbr_idx, a.nbr_ok, s.k, node_i, sidx, row_valid && sidx < J);
+        if (ps.valid && mask_i && a.mask[(size_t)b * s.N + ps.j] != 0 && ps.ok) cnt += T(1);
       }
       for (int off = TS >> 1; off > 0; off >>= 1) cnt += shfl_xor_t<T>(cnt, off);
       inv = cnt > T(0) ? T(1) / cnt : T(0);
@@ -209,153 +188,44 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
   for (int s0 = 0; s0 < J; s0 += TS) {
     const int sidx = s0 + sl;
     const bool pair_exists = row_valid && sidx < J;
-    bool pair_valid = pair_exists;
-    int j = 0;
-    bool ok = true;
-    if (KNN) {
-      if (pair_valid) {
-        const size_t o = node_i * s.k + sidx;
-        j = a.nbr_idx[o];
-        ok = a.nbr_ok ? a.nbr_ok[o] != 0 : true;
-        if (j < 0) { j = 0; pair_valid = false; }
-      }
-    } else {
-      j = pair_valid ? sidx : 0;
-    }
+    const PairSlot ps = pair_slot<KNN>(a.nbr_idx, a.nbr_ok, s.k, node_i, sidx, pair_exists);
+    const int j = ps.j;
+    const bool pair_valid = ps.valid;
+    const size_t pair = node_i * s.N + j;
     T rel[PAIR_CMAX];
-    T d = T(0);
-    {
-      const T* xj = a.coors + ((size_t)b * s.N + j) * s.C;
-#pragma unroll
-      for (int c = 0; c < PAIR_CMAX; ++c) {
-        rel[c] = T(0);
-        if (c < s.C) { rel[c] = xi[c] - xj[c]; d = sq_acc<T>(rel[c], d); }
-      }
+    const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
+    if (pair_exists) {
+      T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
+      for (int q = 0; q < s.Q; ++q) r[a.rl.f + q] = pair_channel<T>(s, a.edges, pair, q, d);
     }
-    if (s.Q > 1) {
-      for (int q = 0; q < s.Q; ++q) {
-        T f;
-        if (q < s.F) f = sin(d / T(1 << q));
-        else if (q < 2 * s.F) f = cos(d / T(1 << (q - s.F)));
-        else if (q == qd) f = d;
-        else f = a.edges[((node_i) * s.N + j) * s.edge_dim + (q - s.Qd)];
-        fs[q * PAIR_THREADS + tid] = f;
-      }
-    }
-    int lab = 0;
-    if (a.labels) lab = a.labels[node_i * s.N + j];
-    const T* Brow = a.P + ((size_t)b * s.N + j) * a.ldP + s.Hp;
-    const T* tabrow = pk + a.L.tab + (size_t)lab * s.Hp;
 
-    Pk2<T> accp[MP / 2];
+    // ---- W2 silu(pre1) of this pair, as the forward (or its recompute) left it (empty slots were never stored: they
+    // read as zeros).  An accumulator wider than 32 registers (fp64, m_dim > 16) is read again for the second SiLU
+    // rather than held through the coordinate branch, where it would spill.
+    constexpr bool REREAD = MP * sizeof(T) > 32 * 4;
+    const T* pre2_src = a.pre2 + (node_i * (size_t)J + sidx) * MP;
+    auto load_pre2 = [&](T (&v)[MP]) {
 #pragma unroll
-    for (int o = 0; o < MP / 2; ++o) accp[o] = Pk2<T>::make(T(0), T(0));
-
-    // ---- forward recompute of W2 silu(pre1) (identical to pair_kernel), unless the caller already did it
-    if (a.pre2) {
-      __syncthreads();                               // tiles of the previous iteration fully consumed
-      if (pair_valid) {                              // (empty slots were never stored: keep their zeros)
-        const T* src = a.pre2 + (node_i * (size_t)J + sidx) * MP;
+      for (int o = 0; o < MP; ++o) v[o] = T(0);
+      if (pair_valid) {
 #pragma unroll
         for (int o = 0; o < MP; o += 4) {
-          Vec4<T> v;
-          v.load_g(src + o);
-          accp[o / 2] = Pk2<T>::make(v.v[0], v.v[1]);
-          accp[o / 2 + 1] = Pk2<T>::make(v.v[2], v.v[3]);
+          Vec4<T> t;
+          t.load_g(pre2_src + o);
+#pragma unroll
+          for (int z = 0; z < 4; ++z) v[o + z] = t.v[z];
         }
       }
-    }
-    for (int c0 = 0; c0 < (a.pre2 ? 0 : s.Hp); c0 += PAIR_CH) {
-      const int cn = min(PAIR_CH, s.Hp - c0);
-      __syncthreads();
-      for (int x = tid; x < cn * MP; x += PAIR_THREADS) W2s[x] = pk[a.L.w2t + (size_t)c0 * MP + x];
-      for (int x = tid; x < s.Q * cn; x += PAIR_THREADS) {
-        int q = x / cn, cc = x % cn;
-        wqs[q * PAIR_CH + cc] = pk[a.L.wq + (size_t)q * s.Hp + c0 + cc];
-      }
-      if (!KNN) {
-        const int cc = tid % PAIR_CH, jj0 = tid / PAIR_CH;
-        for (int jj = jj0; jj < 32; jj += PAIR_THREADS / PAIR_CH) {
-          T v = T(0);
-          if (cc < cn && s0 + jj < s.N) v = a.P[((size_t)b * s.N + s0 + jj) * a.ldP + s.Hp + c0 + cc];
-          Bs[cc * 33 + jj] = v;
-        }
-      }
-      __syncthreads();
-      for (int cc = 0; cc < cn; cc += 4) {
-        Vec4<T> av, wd;
-        av.load_g(Arow + c0 + cc);
-        wd.load(wqs + qd * PAIR_CH + cc);
-        T pre[4];
-        if (KNN) {
-          Vec4<T> bv;
-          bv.load_g(Brow + c0 + cc);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] = av.v[u] + bv.v[u];
-        } else {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] = av.v[u] + Bs[(cc + u) * 33 + sl];
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) pre[u] = fma_t(wd.v[u], d, pre[u]);
-        if (s.Q > 1) {
-          for (int q = 0; q < s.Q; ++q) {
-            if (q == qd) continue;
-            const T f = fs[q * PAIR_THREADS + tid];
-            Vec4<T> wv;
-            wv.load(wqs + q * PAIR_CH + cc);
-#pragma unroll
-            for (int u = 0; u < 4; ++u) pre[u] = fma_t(wv.v[u], f, pre[u]);
-          }
-        }
-        if (a.labels) {
-          Vec4<T> tv;
-          tv.load_g(tabrow + c0 + cc);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] += tv.v[u];
-        }
-        if (a.drop.thr) {                                // edge_mlp Dropout, same mask as the forward
-          const unsigned long long pkey = (((unsigned long long)b * s.N + i) * s.N + j) * s.Hp + c0 + cc;
-#pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] *= (T)drop_mul(a.drop, 0u, pkey + u);
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) {
-          const T hv = silu_acc<T>(pre[u]);             // egnn_pytorch.py:181
-          const Pk2<T> hdn = Pk2<T>::make(hv, hv);
-          const T* w2 = W2s + (cc + u) * MP;
-#pragma unroll
-          for (int v4 = 0; v4 < MP; v4 += 4) {
-            Vec4<T> wv;
-            wv.load(w2 + v4);
-            accp[v4 / 2].fma(hdn, Pk2<T>::make(wv.v[0], wv.v[1]));
-            accp[v4 / 2 + 1].fma(hdn, Pk2<T>::make(wv.v[2], wv.v[3]));
-          }
-        }
-      }
-    }
+    };
     T acc[MP];
-#pragma unroll
-    for (int o = 0; o < MP; o += 2) { acc[o] = accp[o / 2].lo(); acc[o + 1] = accp[o / 2].hi(); }
+    __syncthreads();                                 // shared tiles of the previous iteration fully consumed
+    load_pre2(acc);
 
     // ---- pair epilogue, forward
     T mm[MP];
-#pragma unroll
-    for (int o = 0; o < MP; ++o) mm[o] = silu_acc<T>(acc[o] + misc[o]);      // s2
-    T gate = T(1);
-    if (soft) {
-      T z = misc[2 * MP + 0];
-#pragma unroll
-      for (int o = 0; o < MP; ++o) z = fma_t(misc[MP + o], mm[o], z);
-      gate = sigmoid_acc<T>(z);
-#pragma unroll
-      for (int o = 0; o < MP; ++o) mm[o] *= gate;
-    }
+    const T gate = pair_message<T, MP>(acc, misc, a.flags, mm);      // mm = s2 * gate
     bool pm = pair_valid;
-    if (a.has_mask) {
-      const bool mask_j = a.mask[(size_t)b * s.N + j] != 0;
-      pm = pm && mask_i && mask_j && (KNN ? ok : true);
-    }
+    if (a.has_mask) pm = pm && mask_i && a.mask[(size_t)b * s.N + j] != 0 && ps.ok;
 
     // ---- backward through the coordinate branch (egnn_pytorch.py:302-315 reversed)
     T gmm[MP];
@@ -375,7 +245,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
           for (int z = 0; z < 4; ++z) t = fma_t(wv.v[z], mm[o + z], t);
         }
         if (a.drop.thr) {                                // coors_mlp Dropout: a dropped unit is stored as NaN (silu(0) = 0
-          const T f = (T)drop_mul(a.drop, 1u, (((unsigned long long)b * s.N + i) * s.N + j) * U + u);   // adds nothing)
+          const T f = (T)drop_mul(a.drop, 1u, (unsigned long long)pair * U + u);   // adds nothing)
           t = f == T(0) ? T(NAN) : t * f;
         }
         tt[tid * UP + u] = t;
@@ -436,7 +306,8 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
     }
 #pragma unroll
     for (int o = 0; o < MP; ++o) mms[tid * MP + o] = mm[o];
-    // ---- gate and the second SiLU (egnn_pytorch.py:287-290 reversed); s2 and silu'(pre2) recomputed from acc
+    // ---- gate and the second SiLU (egnn_pytorch.py:287-290 reversed); s2 and silu'(pre2) recomputed from pre2
+    if (REREAD) load_pre2(acc);
     T gz = T(0);
     if (soft) {
       T ggt = T(0);
@@ -463,11 +334,6 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
       T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
 #pragma unroll
       for (int o = 0; o < MP; ++o) r[a.rl.gpre2 + o] = gmm[o];
-      if (s.Q > 1) {
-        for (int q = 0; q < s.Q; ++q) r[a.rl.f + q] = fs[q * PAIR_THREADS + tid];
-      } else {
-        r[a.rl.f] = d;
-      }
       r[a.rl.coef] = coef;
       r[a.rl.gdn] = gdn;
     }
@@ -587,11 +453,11 @@ pair_bwd2_knn_kernel(const BwdArgs<T> a) {
     tabs[l * BW2_TH + tid] = hv ? pk[a.L.tab + (size_t)l * s.Hp + hh] : T(0);
     gtabs[l * BW2_TH + tid] = T(0);
   }
-  Pk2<T> w2p[MP / 2], gW2p[MP / 2];
+  T w2r[MP], gW2[MP];
 #pragma unroll
-  for (int o = 0; o < MP; o += 2) {
-    w2p[o / 2] = Pk2<T>::make(hv ? pk[a.L.w2t + (size_t)hh * MP + o] : T(0), hv ? pk[a.L.w2t + (size_t)hh * MP + o + 1] : T(0));
-    gW2p[o / 2] = Pk2<T>::make(T(0), T(0));
+  for (int o = 0; o < MP; ++o) {
+    w2r[o] = hv ? pk[a.L.w2t + (size_t)hh * MP + o] : T(0);
+    gW2[o] = T(0);
   }
   const T wq0 = hv ? pk[a.L.wq + (size_t)(2 * s.F) * s.Hp + hh] : T(0);
   T gwq0 = T(0);
@@ -672,19 +538,18 @@ pair_bwd2_knn_kernel(const BwdArgs<T> a) {
         }
         const T sg = sigmoid_bw(pre);
         const T a1 = pre * sg;
-        Pk2<T> ga1p = Pk2<T>::make(T(0), T(0));
-        const Pk2<T> a1p = Pk2<T>::make(a1, a1);
+        T ga1e[2] = {T(0), T(0)};                       // even / odd channels, summed at the end
 #pragma unroll
         for (int o = 0; o < MP; o += 4) {
           Vec4<T> gv;
           gv.load(r + o);
-          const Pk2<T> g01 = Pk2<T>::make(gv.v[0], gv.v[1]), g23 = Pk2<T>::make(gv.v[2], gv.v[3]);
-          ga1p.fma(w2p[o / 2], g01);
-          ga1p.fma(w2p[o / 2 + 1], g23);
-          gW2p[o / 2].fma(a1p, g01);
-          gW2p[o / 2 + 1].fma(a1p, g23);
+#pragma unroll
+          for (int z = 0; z < 4; ++z) {
+            ga1e[z & 1] = fma_t(w2r[o + z], gv.v[z], ga1e[z & 1]);
+            gW2[o + z] = fma_t(a1, gv.v[z], gW2[o + z]);
+          }
         }
-        const T ga1 = ga1p.lo() + ga1p.hi();
+        const T ga1 = ga1e[0] + ga1e[1];
         gp = ga1 * dsilu_from<T>(pre, sg);
         if (DROP) gp *= fdrop;
         gA += gp;
@@ -737,10 +602,7 @@ pair_bwd2_knn_kernel(const BwdArgs<T> a) {
   if (hv) {
     if (cur_row >= 0) a.gP[((size_t)b * N + i0 + cur_row) * a.ldP + hh] = gA;
 #pragma unroll
-    for (int o = 0; o < MP; o += 2) {
-      atomic_add_t<T>(a.gpk + a.L.w2t + (size_t)hh * MP + o, gW2p[o / 2].lo());
-      atomic_add_t<T>(a.gpk + a.L.w2t + (size_t)hh * MP + o + 1, gW2p[o / 2].hi());
-    }
+    for (int o = 0; o < MP; ++o) atomic_add_t<T>(a.gpk + a.L.w2t + (size_t)hh * MP + o, gW2[o]);
     if (SIMPLE) {
       atomic_add_t<T>(a.gpk + a.L.wq + (size_t)(2 * s.F) * s.Hp + hh, gwq0);
     } else {
@@ -816,11 +678,11 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
   for (int x = tid; x < 2 * BW2_ROWS * R; x += BW2_TH) recs[x] = T(0);     // rows >= nrows stay zero
   if (tid < 2 * BW2_ROWS) labs[tid] = 0;
   T gA[BW2_ROWS];
-  Pk2<T> w2p[MP / 2], gW2p[MP / 2];
+  T w2r[MP], gW2[MP];
 #pragma unroll
-  for (int o = 0; o < MP; o += 2) {
-    w2p[o / 2] = Pk2<T>::make(hv ? pk[a.L.w2t + (size_t)hh * MP + o] : T(0), hv ? pk[a.L.w2t + (size_t)hh * MP + o + 1] : T(0));
-    gW2p[o / 2] = Pk2<T>::make(T(0), T(0));
+  for (int o = 0; o < MP; ++o) {
+    w2r[o] = hv ? pk[a.L.w2t + (size_t)hh * MP + o] : T(0);
+    gW2[o] = T(0);
   }
 #pragma unroll
   for (int p = 0; p < BW2_ROWS; ++p) gA[p] = T(0);
@@ -881,19 +743,18 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
       }
       const T sg = sigmoid_bw(pre);
       const T a1 = pre * sg;
-      Pk2<T> ga1p = Pk2<T>::make(T(0), T(0));
-      const Pk2<T> a1p = Pk2<T>::make(a1, a1);
+      T ga1e[2] = {T(0), T(0)};                       // even / odd channels, summed at the end
 #pragma unroll
       for (int o = 0; o < MP; o += 4) {
         Vec4<T> gv;
         gv.load(r + o);
-        const Pk2<T> g01 = Pk2<T>::make(gv.v[0], gv.v[1]), g23 = Pk2<T>::make(gv.v[2], gv.v[3]);
-        ga1p.fma(w2p[o / 2], g01);
-        ga1p.fma(w2p[o / 2 + 1], g23);
-        gW2p[o / 2].fma(a1p, g01);
-        gW2p[o / 2 + 1].fma(a1p, g23);
+#pragma unroll
+        for (int z = 0; z < 4; ++z) {
+          ga1e[z & 1] = fma_t(w2r[o + z], gv.v[z], ga1e[z & 1]);
+          gW2[o + z] = fma_t(a1, gv.v[z], gW2[o + z]);
+        }
       }
-      const T ga1 = ga1p.lo() + ga1p.hi();
+      const T ga1 = ga1e[0] + ga1e[1];
       T gp = ga1 * dsilu_from<T>(pre, sg);
       if (DROP) gp *= fdrop;
       gA[p] += gp;
@@ -949,10 +810,7 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
     for (int p = 0; p < BW2_ROWS; ++p)
       if (p < nrows) a.gP[((size_t)b * N + i0 + p) * a.ldP + hh] = gA[p];
 #pragma unroll
-    for (int o = 0; o < MP; o += 2) {
-      atomic_add_t<T>(a.gpk + a.L.w2t + (size_t)hh * MP + o, gW2p[o / 2].lo());
-      atomic_add_t<T>(a.gpk + a.L.w2t + (size_t)hh * MP + o + 1, gW2p[o / 2].hi());
-    }
+    for (int o = 0; o < MP; ++o) atomic_add_t<T>(a.gpk + a.L.w2t + (size_t)hh * MP + o, gW2[o]);
     if (SIMPLE) {
       atomic_add_t<T>(a.gpk + a.L.wq + (size_t)(2 * s.F) * s.Hp + hh, gwq0);
     } else {
@@ -994,18 +852,12 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
   }
   for (int s0 = 0; s0 < J; s0 += TS) {
     const int sidx = s0 + sl;
-    if (!(row_valid && sidx < J)) continue;
-    int j = KNN ? a.nbr_idx[node_i * s.k + sidx] : sidx;
-    if (j < 0) continue;
+    const PairSlot ps = pair_slot<KNN>(a.nbr_idx, nullptr, s.k, node_i, sidx, row_valid && sidx < J);
+    if (!ps.valid) continue;
+    const int j = ps.j;
     const T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
-    const T* xj = a.coors + ((size_t)b * s.N + j) * s.C;
     T rel[PAIR_CMAX];
-    T d = T(0);
-#pragma unroll
-    for (int c = 0; c < PAIR_CMAX; ++c) {
-      rel[c] = T(0);
-      if (c < s.C) { rel[c] = xi[c] - xj[c]; d = sq_acc<T>(rel[c], d); }
-    }
+    const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
     T gd = r[a.rl.gf + qd] + r[a.rl.gdn];
     for (int q = 0; q < s.F; ++q) {                        // fourier_encode_dist :34-41 reversed
       const T sc = T(1 << q);

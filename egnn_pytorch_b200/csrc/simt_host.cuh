@@ -60,17 +60,50 @@ static SimtWs simt_ws_layout(const Dims& s, size_t es, uint32_t flags) {
   return w;
 }
 
-// Opt a kernel in to `smem` bytes of dynamic shared memory.  The attribute is read back first and only ever raised:
-// the same kernel template is launched from several translation units, so no TU-local cache may lower it.
-template <typename K>
-static int ensure_dynamic_smem(K kernel, size_t smem) {
-  if (smem > 220 * 1024) return EGNN_ERR_UNSUPPORTED;
-  if (smem <= 48 * 1024) return EGNN_OK;
-  cudaFuncAttributes attr;
-  EGNN_CUDA_TRY(cudaFuncGetAttributes(&attr, kernel));
-  if ((size_t)attr.maxDynamicSharedSizeBytes < smem)
-    EGNN_CUDA_TRY(cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+// Shared memory budget of the SIMT kernels.  A configuration over it is unsupported; the dense edge step then falls
+// back from two rows per thread to one.
+constexpr size_t SIMT_SMEM_MAX = 220 * 1024;
+
+// Opt in, launch one SIMT kernel with `smem` bytes of dynamic shared memory, and check the enqueue.
+template <typename Arg>
+static int launch_simt(void (*kernel)(Arg), dim3 grid, int threads, size_t smem, cudaStream_t st, const Arg& arg) {
+  if (smem > SIMT_SMEM_MAX) return EGNN_ERR_UNSUPPORTED;
+  EGNN_TRY(ensure_dynamic_smem(kernel, smem));
+  kernel<<<grid, threads, smem, st>>>(arg);
+  EGNN_LAUNCH_CHECK();
   return EGNN_OK;
+}
+
+// The edge step over neighbour lists.
+template <typename T, int MP>
+static int launch_pair(const PairArgs<T>& a, cudaStream_t st) {
+  dim3 grid(ceil_div(a.s.row1 - a.s.row0, PAIR_THREADS / a.TS), a.s.B);
+  return launch_simt(pair_kernel<T, MP>, grid, PAIR_THREADS, pair_smem_bytes<T>(a.s, a.L), st, a);
+}
+
+// The dense edge step at PP rows per thread; a.hsplit > 1 runs it as two phases over a split hidden axis.
+template <typename T, int MP, int PP>
+static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
+  const size_t smem = pair_tiled_smem_bytes<T>(a.s, a.L, PP);
+  dim3 grid(ceil_div(a.s.row1 - a.s.row0, 4 * PP), a.s.B);
+  if (a.hsplit > 1) {
+    PairArgs<T> a1 = a, a2 = a;
+    a1.phase = 1; a2.phase = 2;
+    a1.pre2_out = nullptr;                            // partial sums; phase 2 holds the full ones
+    EGNN_TRY(launch_simt(pair_dense_tiled_kernel<T, MP, PP>, dim3(grid.x, grid.y, a.hsplit), PAIR_THREADS, smem, st, a1));
+    return launch_simt(pair_dense_tiled_kernel<T, MP, PP>, grid, PAIR_THREADS, smem, st, a2);
+  }
+  return launch_simt(pair_dense_tiled_kernel<T, MP, PP>, grid, PAIR_THREADS, smem, st, a);
+}
+
+// The dense edge step at two rows per thread where its shared memory fits, else at one (fp64 with m_dim > 16:
+// one always).
+template <typename T, int MP>
+static int launch_pair_dense(const PairArgs<T>& a, cudaStream_t st) {
+  constexpr int PP = (MP == 32 && sizeof(T) == 8) ? 1 : 2;
+  const int rc = launch_pair_tiled<T, MP, PP>(a, st);
+  if (PP == 1 || rc != EGNN_ERR_UNSUPPORTED) return rc;
+  return launch_pair_tiled<T, MP, 1>(a, st);
 }
 
 template <typename T, int ACT, bool RES>

@@ -272,8 +272,9 @@ __global__ void ln_concat_kernel(const T* __restrict__ h, const T* __restrict__ 
 }
 
 // =====================================================================================
-// The fused edge step (reference egnn_pytorch.py:232-233, 270-333): one thread per (i, slot)
-// pair, 128 threads per CTA arranged as TI row-groups x TS slots (TS lanes of one warp).
+// The fused edge step (reference egnn_pytorch.py:232-233, 270-333).  pair_kernel walks neighbour lists, one thread
+// per (i, slot) pair; pair_dense_tiled_kernel walks all pairs.  The per-pair steps both forward kernels and the
+// backward share are stated once below.
 // =====================================================================================
 constexpr int PAIR_THREADS = 128;
 constexpr int PAIR_CH = 64;     // hidden-axis chunk staged in shared memory
@@ -285,7 +286,7 @@ struct PairArgs {
   SimtPackLayout L;
   uint32_t flags;
   int has_mask;
-  int TS;                    // slots per row group: 32 (dense) or pow2 >= min(k,32)
+  int TS;                    // neighbour lists: slots per row group, pow2 >= min(k,32); unused by the dense kernel
   T clamp;
   const T* P; int ldP;       // [M][2*Hp]: A | B
   const T* coors;            // [B,N,C]
@@ -304,18 +305,108 @@ struct PairArgs {
   DropCfg drop;                         // training-mode dropout of edge_mlp / coors_mlp hidden pre-activations (thr 0 = off)
 };
 
+// Slot `sidx` of row node_i -> neighbour j.  Dense: j = sidx.  Lists: j and its ok flag from the list; a -1 entry
+// (an empty slot of a caller-supplied list) makes the pair invalid and reads node 0 in its place.
+struct PairSlot { int j; bool ok, valid; };
+template <bool KNN>
+__device__ __forceinline__ PairSlot pair_slot(const int32_t* nbr_idx, const uint8_t* nbr_ok, int k, size_t node_i,
+                                              int sidx, bool exists) {
+  PairSlot p{0, true, exists};
+  if (KNN) {
+    if (exists) {
+      const size_t o = node_i * k + sidx;
+      p.j = nbr_idx[o];
+      p.ok = nbr_ok ? nbr_ok[o] != 0 : true;
+      if (p.j < 0) { p.j = 0; p.valid = false; }
+    }
+  } else {
+    p.j = exists ? sidx : 0;
+  }
+  return p;
+}
+
+// rel = x_i - x_j (zero beyond C) and the squared distance d (egnn_pytorch.py:232-233)
 template <typename T>
-inline size_t pair_smem_bytes(const Dims& s, const SimtPackLayout& L, bool knn) {
+__device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&rel)[PAIR_CMAX]) {
+  T d = T(0);
+#pragma unroll
+  for (int c = 0; c < PAIR_CMAX; ++c) {
+    rel[c] = T(0);
+    if (c < C) { rel[c] = xi[c] - xj[c]; d = sq_acc<T>(rel[c], d); }
+  }
+  return d;
+}
+
+// Scalar channel q of pair `pair` = (b * N + i) * N + j: fourier_encode_dist (egnn_pytorch.py:34-41), the squared
+// distance, then the continuous edge features.
+template <typename T>
+__device__ __forceinline__ T pair_channel(const Dims& s, const T* edges, size_t pair, int q, T d) {
+  if (q < s.F) return sin(d / T(1 << q));
+  if (q < 2 * s.F) return cos(d / T(1 << (q - s.F)));
+  if (q == 2 * s.F) return d;
+  return edges[pair * s.edge_dim + (q - s.Qd)];
+}
+
+// m_ij = silu(W2 hid + b2) (pad lanes: silu(0) = 0), times the soft-edge gate (egnn_pytorch.py:287-290).
+// misc = b2[MP] | gate_w[MP] | gate_b, ...  Returns the gate (1 without soft edges).
+template <typename T, int MP>
+__device__ __forceinline__ T pair_message(const T (&acc)[MP], const T* misc, uint32_t flags, T (&mm)[MP]) {
+#pragma unroll
+  for (int o = 0; o < MP; ++o) mm[o] = silu_acc<T>(acc[o] + misc[o]);
+  T gate = T(1);
+  if (flags & EGNN_FLAG_SOFT_EDGES) {
+    T z = misc[2 * MP + 0];
+#pragma unroll
+    for (int o = 0; o < MP; ++o) z = fma_t(misc[MP + o], mm[o], z);
+    gate = sigmoid_acc<T>(z);
+#pragma unroll
+    for (int o = 0; o < MP; ++o) mm[o] *= gate;
+  }
+  return gate;
+}
+
+// Coordinate weight of a pair (egnn_pytorch.py:302-313): coors_mlp(m_ij) with its dropout (stream 1), zero unless
+// the pair mask pm holds, clamped, zero for padding pairs, then CoorsNorm's scale / max(|rel|, 1e-8) (:74-77).
+template <typename T, int MP>
+__device__ __forceinline__ T pair_coord_weight(const PairArgs<T>& a, const T (&mm)[MP], const T* w3s, const T* b3s,
+                                               const T* w4s, const T* misc, size_t pair, bool pm, bool pair_valid, T d) {
+  const int U = 4 * a.s.m;
+  T w = misc[2 * MP + 1];
+  for (int u = 0; u < U; ++u) {
+    T t = b3s[u];
+    const T* w3 = w3s + u * MP;
+#pragma unroll
+    for (int o = 0; o < MP; o += 4) {
+      Vec4<T> wv;
+      wv.load(w3 + o);
+#pragma unroll
+      for (int z = 0; z < 4; ++z) t = fma_t(wv.v[z], mm[o + z], t);
+    }
+    if (a.drop.thr) t *= (T)drop_mul(a.drop, 1u, (unsigned long long)pair * U + u);    // coors_mlp Dropout, :205
+    w = fma_t(w4s[u], silu_acc<T>(t), w);
+  }
+  if (!pm) w = T(0);                                   // :309 (and padding lanes of the tile)
+  if (a.flags & EGNN_FLAG_CLAMP) w = w < -a.clamp ? -a.clamp : (w > a.clamp ? a.clamp : w);   // :313
+  if (!pair_valid) w = T(0);
+  if (a.flags & EGNN_FLAG_NORM_COORS) {
+    const T nrm = sqrt(d);
+    w *= misc[2 * MP + 2] / (nrm > T(1e-8) ? nrm : T(1e-8));
+  }
+  return w;
+}
+
+template <typename T>
+inline size_t pair_smem_bytes(const Dims& s, const SimtPackLayout& L) {
   size_t n = 0;
   n += (size_t)PAIR_CH * L.MP;                 // W2s
   n += (size_t)s.Q * PAIR_CH;                  // wqs
-  if (!knn) n += (size_t)PAIR_CH * 33;         // Bs
   if (s.Q > 1) n += (size_t)s.Q * PAIR_THREADS;  // fs
   n += (size_t)4 * s.m * L.MP + 8 * s.m + 2 * L.MP + 4;   // w3s, b3s, w4s, misc
   return round_up(n * sizeof(T), 16) + 16;
 }
 
-template <typename T, int MP, bool KNN>
+// Neighbour lists: 128 threads per CTA arranged as TI row-groups x TS slots (TS lanes of one warp).
+template <typename T, int MP>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -327,7 +418,7 @@ pair_kernel(const PairArgs<T> a) {
   const int i_raw = s.row0 + blockIdx.x * TI + g;
   const bool row_valid = i_raw < s.row1;
   const int i = row_valid ? i_raw : s.row0;
-  const int J = KNN ? s.k : s.N;
+  const int J = s.k;
   const int U = 4 * s.m;
   const int qd = 2 * s.F;                      // index of the raw squared distance in the Q channels
   const bool upd_feats = a.flags & EGNN_FLAG_UPDATE_FEATS;
@@ -336,8 +427,7 @@ pair_kernel(const PairArgs<T> a) {
   // ---- shared memory carve-up
   T* W2s = reinterpret_cast<T*>(smem_raw);                 // [CH][MP]
   T* wqs = W2s + PAIR_CH * MP;                             // [Q][CH]
-  T* Bs = wqs + s.Q * PAIR_CH;                             // [CH][33]      (dense only)
-  T* fs = Bs + (KNN ? 0 : PAIR_CH * 33);                   // [Q][128]      (Q > 1 only)
+  T* fs = wqs + s.Q * PAIR_CH;                             // [Q][128]      (Q > 1 only)
   T* w3s = fs + (s.Q > 1 ? s.Q * PAIR_THREADS : 0);        // [U][MP]
   T* b3s = w3s + U * MP;                                   // [U]
   T* w4s = b3s + U;                                        // [U]
@@ -351,9 +441,10 @@ pair_kernel(const PairArgs<T> a) {
   for (int x = tid; x < 2 * MP + 4; x += PAIR_THREADS) misc[x] = pk[a.L.misc + x];
   // (visibility is guaranteed by the __syncthreads inside the chunk loop below)
 
-  const T* xi = a.coors + ((size_t)b * s.N + i) * s.C;
-  const bool mask_i = a.has_mask ? (a.mask[(size_t)b * s.N + i] != 0) : true;
-  const T* Arow = a.P + ((size_t)b * s.N + i) * a.ldP;
+  const size_t node_i = (size_t)b * s.N + i;
+  const T* xi = a.coors + node_i * s.C;
+  const bool mask_i = a.has_mask ? (a.mask[node_i] != 0) : true;
+  const T* Arow = a.P + node_i * a.ldP;
 
   T msum[MP];
   T csum[PAIR_CMAX];
@@ -365,49 +456,23 @@ pair_kernel(const PairArgs<T> a) {
 
   for (int s0 = 0; s0 < J; s0 += TS) {
     const int sidx = s0 + sl;
-    bool pair_valid = row_valid && sidx < J;
-    int j = 0;
-    bool ok = true;
-    if (KNN) {
-      if (pair_valid) {
-        size_t o = ((size_t)b * s.N + i) * s.k + sidx;
-        j = a.nbr_idx[o];
-        ok = a.nbr_ok ? a.nbr_ok[o] != 0 : true;
-        if (j < 0) { j = 0; pair_valid = false; }      // empty slot of a caller-supplied neighbour list
-      }
-    } else {
-      j = pair_valid ? sidx : 0;
-    }
-    // ---- geometry (egnn_pytorch.py:232-233)
+    const PairSlot ps = pair_slot<true>(a.nbr_idx, a.nbr_ok, s.k, node_i, sidx, row_valid && sidx < J);
+    const int j = ps.j;
+    const bool pair_valid = ps.valid;
+    const size_t pair = node_i * s.N + j;
     T rel[PAIR_CMAX];
-    T d = T(0);
-    {
-      const T* xj = a.coors + ((size_t)b * s.N + j) * s.C;
-#pragma unroll
-      for (int c = 0; c < PAIR_CMAX; ++c) {
-        rel[c] = T(0);
-        if (c < s.C) { rel[c] = xi[c] - xj[c]; d = sq_acc<T>(rel[c], d); }
-      }
-    }
+    const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
     // ---- per-pair scalar channels other than d go through shared memory
-    if (s.Q > 1) {
-      for (int q = 0; q < s.Q; ++q) {
-        T f;
-        if (q < s.F) f = sin(d / T(1 << q));                     // fourier_encode_dist :34-41
-        else if (q < 2 * s.F) f = cos(d / T(1 << (q - s.F)));
-        else if (q == qd) f = d;
-        else f = a.edges[(((size_t)b * s.N + i) * s.N + j) * s.edge_dim + (q - s.Qd)];
-        fs[q * PAIR_THREADS + tid] = f;
-      }
-    }
+    if (s.Q > 1)
+      for (int q = 0; q < s.Q; ++q) fs[q * PAIR_THREADS + tid] = pair_channel<T>(s, a.edges, pair, q, d);
     int lab = 0;
-    if (a.labels) lab = a.labels[((size_t)b * s.N + i) * s.N + j];
+    if (a.labels) lab = a.labels[pair];
     const T* Brow = a.P + ((size_t)b * s.N + j) * a.ldP + s.Hp;
     const T* tabrow = pk + a.L.tab + (size_t)lab * s.Hp;
 
-    Pk2<T> accp[MP / 2];
+    T acc[MP];
 #pragma unroll
-    for (int o = 0; o < MP / 2; ++o) accp[o] = Pk2<T>::make(T(0), T(0));
+    for (int o = 0; o < MP; ++o) acc[o] = T(0);
 
     for (int c0 = 0; c0 < s.Hp; c0 += PAIR_CH) {
       const int cn = min(PAIR_CH, s.Hp - c0);      // multiple of 8
@@ -417,33 +482,17 @@ pair_kernel(const PairArgs<T> a) {
         int q = x / cn, cc = x % cn;
         wqs[q * PAIR_CH + cc] = pk[a.L.wq + (size_t)q * s.Hp + c0 + cc];
       }
-      if (!KNN) {
-        // B tile, transposed: Bs[cc][jj] = B[s0 + jj][c0 + cc]
-        const int cc = tid % PAIR_CH, jj0 = tid / PAIR_CH;
-        for (int jj = jj0; jj < 32; jj += PAIR_THREADS / PAIR_CH) {
-          T v = T(0);
-          if (cc < cn && s0 + jj < s.N) v = a.P[((size_t)b * s.N + s0 + jj) * a.ldP + s.Hp + c0 + cc];
-          Bs[cc * 33 + jj] = v;
-        }
-      }
       __syncthreads();
 
       for (int cc = 0; cc < cn; cc += 4) {
-        Vec4<T> av, wd;
+        // pre-activation of hidden channels c0+cc .. +3: A_i + B_j + Wq f + label row, then edge_mlp Dropout
+        Vec4<T> av, bv, wd;
         av.load_g(Arow + c0 + cc);
+        bv.load_g(Brow + c0 + cc);
         wd.load(wqs + qd * PAIR_CH + cc);
         T pre[4];
-        if (KNN) {
-          Vec4<T> bv;
-          bv.load_g(Brow + c0 + cc);
 #pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] = av.v[u] + bv.v[u];
-        } else {
-#pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] = av.v[u] + Bs[(cc + u) * 33 + sl];
-        }
-#pragma unroll
-        for (int u = 0; u < 4; ++u) pre[u] = fma_t(wd.v[u], d, pre[u]);
+        for (int u = 0; u < 4; ++u) pre[u] = fma_t(wd.v[u], d, av.v[u] + bv.v[u]);
         if (s.Q > 1) {
           for (int q = 0; q < s.Q; ++q) {
             if (q == qd) continue;
@@ -460,76 +509,38 @@ pair_kernel(const PairArgs<T> a) {
 #pragma unroll
           for (int u = 0; u < 4; ++u) pre[u] += tv.v[u];
         }
-        if (a.drop.thr) {                                // edge_mlp Dropout, egnn_pytorch.py:180
-          const unsigned long long pkey = (((unsigned long long)b * s.N + i) * s.N + j) * s.Hp + c0 + cc;
+        if (a.drop.thr) {                                // egnn_pytorch.py:180
+          const unsigned long long pkey = (unsigned long long)pair * s.Hp + c0 + cc;
 #pragma unroll
           for (int u = 0; u < 4; ++u) pre[u] *= (T)drop_mul(a.drop, 0u, pkey + u);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const T hv = silu_acc<T>(pre[u]);             // egnn_pytorch.py:181
-          const Pk2<T> hdn = Pk2<T>::make(hv, hv);
           const T* w2 = W2s + (cc + u) * MP;
 #pragma unroll
           for (int v4 = 0; v4 < MP; v4 += 4) {
             Vec4<T> wv;
             wv.load(w2 + v4);
-            accp[v4 / 2].fma(hdn, Pk2<T>::make(wv.v[0], wv.v[1]));
-            accp[v4 / 2 + 1].fma(hdn, Pk2<T>::make(wv.v[2], wv.v[3]));
+#pragma unroll
+            for (int z = 0; z < 4; ++z) acc[v4 + z] = fma_t(hv, wv.v[z], acc[v4 + z]);
           }
         }
       }
     }
-    T acc[MP];
-#pragma unroll
-    for (int o = 0; o < MP; o += 2) { acc[o] = accp[o / 2].lo(); acc[o + 1] = accp[o / 2].hi(); }
 
-    if (a.pre2_out && pair_valid) {                  // kept for backward: [B,N,J][MP], J = N (dense) or k
-      T* dst = a.pre2_out + (KNN ? ((size_t)b * s.N + i) * s.k + sidx : ((size_t)b * s.N + i) * s.N + j) * MP;
+    if (a.pre2_out && pair_valid) {                  // kept for backward: [B,N,k][MP]
+      T* dst = a.pre2_out + (node_i * s.k + sidx) * MP;
 #pragma unroll
       for (int o = 0; o < MP; ++o) dst[o] = acc[o];
     }
     // ---- epilogue for this pair: m_ij, gate, coordinate weight, masks (egnn_pytorch.py:287-322)
     T mm[MP];
-#pragma unroll
-    for (int o = 0; o < MP; ++o) mm[o] = silu_acc<T>(acc[o] + misc[o]);     // pad lanes: silu(0) = 0
-    if (a.flags & EGNN_FLAG_SOFT_EDGES) {
-      T z = misc[2 * MP + 0];
-#pragma unroll
-      for (int o = 0; o < MP; ++o) z = fma_t(misc[MP + o], mm[o], z);
-      const T gate = sigmoid_acc<T>(z);
-#pragma unroll
-      for (int o = 0; o < MP; ++o) mm[o] *= gate;
-    }
+    pair_message<T, MP>(acc, misc, a.flags, mm);
     bool pm = pair_valid;
-    if (a.has_mask) {
-      const bool mask_j = a.mask[(size_t)b * s.N + j] != 0;
-      pm = pm && mask_i && mask_j && (KNN ? ok : true);
-    }
+    if (a.has_mask) pm = pm && mask_i && a.mask[(size_t)b * s.N + j] != 0 && ps.ok;
     if (upd_coors) {
-      T w = misc[2 * MP + 1];
-      for (int u = 0; u < U; ++u) {
-        T t = b3s[u];
-        const T* w3 = w3s + u * MP;
-#pragma unroll
-        for (int o = 0; o < MP; o += 4) {
-          Vec4<T> wv;
-          wv.load(w3 + o);
-#pragma unroll
-          for (int z = 0; z < 4; ++z) t = fma_t(wv.v[z], mm[o + z], t);
-        }
-        if (a.drop.thr) t *= (T)drop_mul(a.drop, 1u, (((unsigned long long)b * s.N + i) * s.N + j) * U + u);    // coors_mlp Dropout, :205
-        w = fma_t(w4s[u], silu_acc<T>(t), w);
-      }
-      if (!pm) w = T(0);                                   // :309 (and padding lanes of the tile)
-      if (a.flags & EGNN_FLAG_CLAMP) w = w < -a.clamp ? -a.clamp : (w > a.clamp ? a.clamp : w);   // :313
-      if (!pair_valid) w = T(0);
-      T scale = T(1);
-      if (a.flags & EGNN_FLAG_NORM_COORS) {                // CoorsNorm :74-77
-        const T nrm = sqrt(d);
-        scale = misc[2 * MP + 2] / (nrm > T(1e-8) ? nrm : T(1e-8));
-      }
-      w *= scale;
+      const T w = pair_coord_weight<T, MP>(a, mm, w3s, b3s, w4s, misc, pair, pm, pair_valid, d);
 #pragma unroll
       for (int c = 0; c < PAIR_CMAX; ++c) csum[c] = fma_t(w, rel[c], csum[c]);
     }
@@ -549,7 +560,6 @@ pair_kernel(const PairArgs<T> a) {
     cnt += shfl_xor_t<T>(cnt, off);
   }
   if (sl == 0 && row_valid) {
-    const size_t node = (size_t)b * s.N + i;
     if (upd_feats) {
       T inv = T(1);
       if (a.flags & EGNN_FLAG_POOL_MEAN) {
@@ -558,21 +568,22 @@ pair_kernel(const PairArgs<T> a) {
       }
 #pragma unroll
       for (int o = 0; o < MP; ++o)
-        if (o < s.m) a.m_out[node * a.ld_m + o] = msum[o] * inv;
+        if (o < s.m) a.m_out[node_i * a.ld_m + o] = msum[o] * inv;
     }
     if (upd_coors) {
 #pragma unroll
       for (int c = 0; c < PAIR_CMAX; ++c)
-        if (c < s.C) a.coors_out[node * s.C + c] = csum[c] + xi[c];   // :315
+        if (c < s.C) a.coors_out[node_i * s.C + c] = csum[c] + xi[c];   // :315
     }
   }
 }
 
 // =====================================================================================
 // Dense all-pairs variant with register tiling over rows: a thread owns neighbour j and PP query rows, so every
-// W2 row fetched from shared memory feeds PP pairs (the thread-per-pair kernel above is bound by the 16
-// broadcast wavefronts per hidden channel that W2 costs).  One warp = PP rows x 32 neighbours,
-// 4 warps per CTA; per-row sums are reduced with shuffles per j-tile and kept in shared memory.
+// W2 row fetched from shared memory feeds PP pairs (a thread-per-pair kernel is bound by the 16 broadcast
+// wavefronts per hidden channel that W2 costs).  One warp = PP rows x 32 neighbours, 4 warps per CTA; per-row sums
+// are reduced with shuffles per j-tile and kept in shared memory (PP > 1) or in registers (PP = 1, the variant for
+// configurations whose per-pair channels leave no shared memory to spare).
 // =====================================================================================
 template <typename T>
 inline size_t pair_tiled_smem_bytes(const Dims& s, const SimtPackLayout& L, int PP) {
@@ -582,7 +593,7 @@ inline size_t pair_tiled_smem_bytes(const Dims& s, const SimtPackLayout& L, int 
   n += (size_t)PAIR_CH * 33;                           // Bs
   if (s.Q > 1) n += (size_t)PP * s.Q * PAIR_THREADS;   // fs
   n += (size_t)4 * s.m * L.MP + 8 * s.m + 2 * L.MP + 4;   // w3s, b3s, w4s, misc
-  n += (size_t)4 * PP * (L.MP + PAIR_CMAX + 4);        // per-row running sums
+  if (PP > 1) n += (size_t)4 * PP * (L.MP + PAIR_CMAX + 4);   // per-row running sums
   return round_up(n * sizeof(T), 16) + 16;
 }
 
@@ -596,6 +607,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
   const int U = 4 * s.m;
   const int qd = 2 * s.F;
   constexpr int RS = MP + PAIR_CMAX + 4;          // row-sum record: m[MP] | csum[CMAX] | cnt | pad
+  constexpr int RN = MP + PAIR_CMAX + 1;          // used part of the record
   const bool upd_feats = a.flags & EGNN_FLAG_UPDATE_FEATS;
   const bool upd_coors = a.flags & EGNN_FLAG_UPDATE_COORS;
 
@@ -607,7 +619,8 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
   T* b3s = w3s + U * MP;
   T* w4s = b3s + U;
   T* misc = w4s + U;
-  T* rows = misc + 2 * MP + 4;                    // [4 warps][PP][RS]
+  T* rows = misc + 2 * MP + 4;                    // [4 warps][PP][RS]   (PP > 1)
+  T rlo = T(0), rhi = T(0);                       // PP = 1: lane l keeps elements l and l + 32 of its warp's record
 
   const T* pk = a.packed;
   if (upd_coors) {
@@ -615,7 +628,8 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
     for (int x = tid; x < U; x += PAIR_THREADS) { b3s[x] = pk[a.L.b3 + x]; w4s[x] = pk[a.L.w4 + x]; }
   }
   for (int x = tid; x < 2 * MP + 4; x += PAIR_THREADS) misc[x] = pk[a.L.misc + x];
-  for (int x = tid; x < 4 * PP * RS; x += PAIR_THREADS) rows[x] = T(0);
+  if (PP > 1)
+    for (int x = tid; x < 4 * PP * RS; x += PAIR_THREADS) rows[x] = T(0);
   __syncthreads();                                // constants visible (phase 2 never enters the chunk loop)
 
   int irow[PP];
@@ -634,41 +648,25 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
   for (int s0 = 0; s0 < s.N; s0 += 32) {
     const int jraw = s0 + lane;
     const bool jv = jraw < s.N;
-    const int j = jv ? jraw : 0;
-    T xj[PAIR_CMAX];
-    {
-      const T* xjp = a.coors + ((size_t)b * s.N + j) * s.C;
-#pragma unroll
-      for (int c = 0; c < PAIR_CMAX; ++c) xj[c] = c < s.C ? xjp[c] : T(0);
-    }
+    const int j = pair_slot<false>(nullptr, nullptr, 0, 0, jraw, jv).j;
+    const T* xj = a.coors + ((size_t)b * s.N + j) * s.C;     // re-read in the epilogue rather than held through the chunk loop
     T d[PP];
     int lab[PP];
 #pragma unroll
     for (int p = 0; p < PP; ++p) {
-      const T* xi = a.coors + ((size_t)b * s.N + irow[p]) * s.C;
-      T dd = T(0);
-#pragma unroll
-      for (int c = 0; c < PAIR_CMAX; ++c)
-        if (c < s.C) dd = sq_acc<T>(xi[c] - xj[c], dd);
-      d[p] = dd;
-      lab[p] = a.labels ? a.labels[((size_t)b * s.N + irow[p]) * s.N + j] : 0;
-      if (s.Q > 1) {
-        for (int q = 0; q < s.Q; ++q) {
-          T f;
-          if (q < s.F) f = sin(dd / T(1 << q));
-          else if (q < 2 * s.F) f = cos(dd / T(1 << (q - s.F)));
-          else if (q == qd) f = dd;
-          else f = a.edges[(((size_t)b * s.N + irow[p]) * s.N + j) * s.edge_dim + (q - s.Qd)];
-          fs[(p * s.Q + q) * PAIR_THREADS + tid] = f;
-        }
-      }
+      const size_t pair = ((size_t)b * s.N + irow[p]) * s.N + j;
+      T rel[PAIR_CMAX];
+      d[p] = pair_geometry<T>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel);
+      lab[p] = a.labels ? a.labels[pair] : 0;
+      if (s.Q > 1)
+        for (int q = 0; q < s.Q; ++q) fs[(p * s.Q + q) * PAIR_THREADS + tid] = pair_channel<T>(s, a.edges, pair, q, d[p]);
     }
 
-    Pk2<T> accp[PP][MP / 2];
+    T acc[PP][MP];
 #pragma unroll
     for (int p = 0; p < PP; ++p)
 #pragma unroll
-      for (int o = 0; o < MP / 2; ++o) accp[p][o] = Pk2<T>::make(T(0), T(0));
+      for (int o = 0; o < MP; ++o) acc[p][o] = T(0);
 
     int c_begin = 0, c_end = s.Hp;
     if (a.phase == 1) {
@@ -687,6 +685,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
         wqs[q * PAIR_CH + cc] = pk[a.L.wq + (size_t)q * s.Hp + c0 + cc];
       }
       {
+        // B tile, transposed: Bs[cc][jj] = B[s0 + jj][c0 + cc]
         const int cc = tid % PAIR_CH, jj0 = tid / PAIR_CH;
         for (int jj = jj0; jj < 32; jj += PAIR_THREADS / PAIR_CH) {
           T v = T(0);
@@ -740,31 +739,21 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
           const T* w2 = W2s + (cc + u) * MP;
-          Pk2<T> hdn[PP];
+          T hv[PP];
 #pragma unroll
-          for (int p = 0; p < PP; ++p) {
-            const T hv = silu_acc<T>(pre[p][u]);
-            hdn[p] = Pk2<T>::make(hv, hv);
-          }
+          for (int p = 0; p < PP; ++p) hv[p] = silu_acc<T>(pre[p][u]);
 #pragma unroll
           for (int v4 = 0; v4 < MP; v4 += 4) {
             Vec4<T> wv;
             wv.load(w2 + v4);
-            const Pk2<T> w01 = Pk2<T>::make(wv.v[0], wv.v[1]), w23 = Pk2<T>::make(wv.v[2], wv.v[3]);
 #pragma unroll
-            for (int p = 0; p < PP; ++p) {
-              accp[p][v4 / 2].fma(hdn[p], w01);
-              accp[p][v4 / 2 + 1].fma(hdn[p], w23);
-            }
+            for (int p = 0; p < PP; ++p)
+#pragma unroll
+              for (int z = 0; z < 4; ++z) acc[p][v4 + z] = fma_t(hv[p], wv.v[z], acc[p][v4 + z]);
           }
         }
       }
     }
-    T acc[PP][MP];
-#pragma unroll
-    for (int p = 0; p < PP; ++p)
-#pragma unroll
-      for (int o = 0; o < MP; o += 2) { acc[p][o] = accp[p][o / 2].lo(); acc[p][o + 1] = accp[p][o / 2].hi(); }
 
     if (a.phase != 0) {
       // split hidden axis: partial sums go through global memory, summed in split order (deterministic)
@@ -798,47 +787,20 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
 #pragma unroll
     for (int p = 0; p < PP; ++p) {
       T mm[MP];
-#pragma unroll
-      for (int o = 0; o < MP; ++o) mm[o] = silu_acc<T>(acc[p][o] + misc[o]);
-      if (a.flags & EGNN_FLAG_SOFT_EDGES) {
-        T z = misc[2 * MP + 0];
-#pragma unroll
-        for (int o = 0; o < MP; ++o) z = fma_t(misc[MP + o], mm[o], z);
-        const T gate = sigmoid_acc<T>(z);
-#pragma unroll
-        for (int o = 0; o < MP; ++o) mm[o] *= gate;
-      }
+      pair_message<T, MP>(acc[p], misc, a.flags, mm);
       const bool pair_valid = rvalid[p] && jv;
       const bool pm = pair_valid && (a.has_mask ? (mask_i[p] && mask_j) : true);
       T rec[RS];
 #pragma unroll
       for (int x = 0; x < RS; ++x) rec[x] = T(0);
       if (upd_coors) {
-        T w = misc[2 * MP + 1];
-        for (int u = 0; u < U; ++u) {
-          T t = b3s[u];
-          const T* w3 = w3s + u * MP;
-#pragma unroll
-          for (int o = 0; o < MP; o += 4) {
-            Vec4<T> wv;
-            wv.load(w3 + o);
-#pragma unroll
-            for (int z = 0; z < 4; ++z) t = fma_t(wv.v[z], mm[o + z], t);
-          }
-          if (a.drop.thr) t *= (T)drop_mul(a.drop, 1u, (((unsigned long long)b * s.N + irow[p]) * s.N + j) * U + u);   // :205
-          w = fma_t(w4s[u], silu_acc<T>(t), w);
-        }
-        if (!pm) w = T(0);
-        if (a.flags & EGNN_FLAG_CLAMP) w = w < -a.clamp ? -a.clamp : (w > a.clamp ? a.clamp : w);
-        if (!pair_valid) w = T(0);
-        if (a.flags & EGNN_FLAG_NORM_COORS) {
-          const T nrm = sqrt(d[p]);
-          w *= misc[2 * MP + 2] / (nrm > T(1e-8) ? nrm : T(1e-8));
-        }
-        const T* xi = a.coors + ((size_t)b * s.N + irow[p]) * s.C;
+        const size_t pair = ((size_t)b * s.N + irow[p]) * s.N + j;
+        const T w = pair_coord_weight<T, MP>(a, mm, w3s, b3s, w4s, misc, pair, pm, pair_valid, d[p]);
+        T rel[PAIR_CMAX];
+        pair_geometry<T>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel);
 #pragma unroll
         for (int c = 0; c < PAIR_CMAX; ++c)
-          if (c < s.C) rec[MP + c] = w * (xi[c] - xj[c]);
+          if (c < s.C) rec[MP + c] = w * rel[c];
       }
       if (upd_feats && pm) {
 #pragma unroll
@@ -848,14 +810,39 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
 #pragma unroll
       for (int off = 16; off > 0; off >>= 1)
 #pragma unroll
-        for (int x = 0; x < MP + PAIR_CMAX + 1; ++x) rec[x] += shfl_xor_t<T>(rec[x], off);
-      if (lane == 0) {
+        for (int x = 0; x < RN; ++x) rec[x] += shfl_xor_t<T>(rec[x], off);
+      if (PP == 1) {
 #pragma unroll
-        for (int x = 0; x < MP + PAIR_CMAX + 1; ++x) myrows[p * RS + x] += rec[x];
+        for (int x = 0; x < RN; ++x) {
+          if (x == lane) rlo += rec[x];
+          if (x == lane + 32) rhi += rec[x];
+        }
+      } else if (lane == 0) {
+#pragma unroll
+        for (int x = 0; x < RN; ++x) myrows[p * RS + x] += rec[x];
       }
     }
   }
 
+  if constexpr (PP == 1) {
+    const T cnt = shfl_idx_t<T>(MP + PAIR_CMAX < 32 ? rlo : rhi, (MP + PAIR_CMAX) % 32);
+    if (a.phase != 1 && rvalid[0]) {
+      const size_t node = (size_t)b * s.N + irow[0];
+      T inv = T(1);
+      if (a.flags & EGNN_FLAG_POOL_MEAN) {
+        if (a.has_mask) inv = cnt > T(0) ? T(1) / cnt : T(0);
+        else inv = T(1) / T(s.N);
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int e = lane + 32 * h;
+        const T v = h ? rhi : rlo;
+        if (upd_feats && e < s.m) a.m_out[node * a.ld_m + e] = v * inv;
+        if (upd_coors && e >= MP && e < MP + s.C) a.coors_out[node * s.C + e - MP] = v + a.coors[node * s.C + e - MP];
+      }
+    }
+    return;
+  }
   __syncwarp();
   if (a.phase != 1 && lane < PP && rvalid[0]) {
     // lane p writes row p (rvalid is monotone in p)

@@ -42,6 +42,19 @@ def test_cuda_matches_oracle_and_golden(name, dtype):
     assert layer.last_path == ("fp64-simt" if dtype == torch.float64 else "fp32-simt")
 
 
+def test_dense_fp64_with_many_pair_channels_matches_oracle():
+    """fourier_features=30 and edge_dim=16 give 77 per-pair scalar channels: the register-tiled dense kernel's shared
+    memory does not fit at two rows per thread in fp64, so the edge step runs at one row per thread."""
+    spec = dict(kind="layer", cfg=dict(dim=8, fourier_features=30, edge_dim=16), B=1, N=20, seed=41, init="xavier")
+    case = cases.build_case(spec)
+    mod = util.make_module(case, torch.float64)
+    out = util.run_module(mod, case, torch.float64)
+    want = cases.run_oracle(case)
+    util.assert_close(out[0], want[0], what="feats vs oracle", **TOL[torch.float64])
+    util.assert_close(out[1], want[1], what="coors vs oracle", **TOL[torch.float64])
+    assert mod.last_path == "fp64-simt"
+
+
 def test_cpu_tensors_are_staged_and_returned_on_cpu():
     """The reference's tests call the layer with CPU float64 tensors (tests/test_equivariance.py:28)."""
     case = cases.build_case(cases.SPECS["dense_edges"])
