@@ -31,10 +31,25 @@ inline BwdWs bwd_ws_layout(const Dims& s, const SimtPackLayout& L, size_t es, ui
   return w;
 }
 
+// Shared memory of bwd1 and bwd2, sized by the functions their launches use (launch_pair_bwd).
+template <typename T>
+inline bool backward_smem_fits(const Dims& s, uint32_t flags) {
+  const SimtPackLayout L = simt_pack_layout(s);
+  const int R = rec_layout(s, L.MP).R;
+  const size_t bwd1 = bwd1_smem_bytes<T>(s, L, (flags & EGNN_FLAG_SOFT_EDGES) != 0);
+  const size_t bwd2 = s.k > 0 ? bwd2_knn_smem_bytes<T>(s, R) : bwd2_dense_smem_bytes<T>(s, R);
+  return bwd1 <= SIMT_SMEM_MAX && bwd2 <= SIMT_SMEM_MAX;
+}
+
+// Everything the backward kernels cannot run.  The training forward calls this first (through
+// egnn_layer_backward_workspace_bytes), so such a configuration fails before the forward instead of in the backward.
 inline int backward_supported(const EgnnLayerDesc& d) {
   if (d.dtype != EGNN_DTYPE_F32 && d.dtype != EGNN_DTYPE_F64) return EGNN_ERR_UNSUPPORTED;
   if (!(d.row_begin == 0 && (d.row_end == 0 || d.row_end == d.N))) return EGNN_ERR_UNSUPPORTED;
   if (d.label_dim > 0 && d.num_labels > BW2_MAXLAB) return EGNN_ERR_UNSUPPORTED;
+  const Dims s = make_dims(d);
+  const bool fits = d.dtype == EGNN_DTYPE_F64 ? backward_smem_fits<double>(s, d.flags) : backward_smem_fits<float>(s, d.flags);
+  if (!fits) return EGNN_ERR_UNSUPPORTED;
   return EGNN_OK;
 }
 

@@ -320,16 +320,18 @@ def upstream_grads(case):
     return rs.standard_normal((B, N, d)), rs.standard_normal((B, N, C))
 
 
-def run_oracle_grad(case):
-    """-> dict(feats|None, coors, edges|None, params{key: grad}) from the numpy backward oracle."""
+def run_oracle_grad(case, neighbors=None):
+    """-> dict(feats|None, coors, edges|None, params{key: grad}) from the numpy backward oracle.  `neighbors` (layers
+    only): the edge-list form, [B,N,k] with -1 for empty slots."""
     from oracle import egnn_oracle_grad as G
     ins = case["inputs"]
     gf, gx = upstream_grads(case)
     if case["kind"] == "network":
+        assert neighbors is None
         return G.egnn_network_backward(case["params"], case["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
                                        ins.get("edges"), ins.get("mask"), gf, gx)
     return G.egnn_layer_backward(case["params"], case["cfg"], ins["feats"], ins["coors"], ins.get("edges"),
-                                 ins.get("mask"), ins.get("adj_mat"), gf, gx)
+                                 ins.get("mask"), ins.get("adj_mat"), gf, gx, neighbors=neighbors)
 
 
 def flatten_grads(r):

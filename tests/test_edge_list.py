@@ -4,7 +4,9 @@ structure of reference egnn_pytorch_geometric.py:182-267 in the dense layer's co
 
 CPU part: the edge-list oracle is pinned to the reference-pinned gather oracle on the lists the top-k would pick,
 and its gradient restatement to finite differences.  GPU part: random lists with empty (-1) slots, duplicate-free,
-in fp64 / fp32 / bf16 forward and fp64 backward."""
+in fp64 / fp32 / bf16 forward and fp64 / fp32 backward (with W2 silu(pre1) saved by the forward or recomputed)."""
+import functools
+
 import numpy as np
 import pytest
 import torch
@@ -23,6 +25,16 @@ EDGE_CASES = {
     "fourier_c5":   (dict(dim=12, fourier_features=2, norm_feats=True), 1, 16, 5, 5, True, "xavier"),
     "k33":          (dict(dim=8, edge_dim=2), 1, 48, 33, 3, False, "xavier"),
     "default_init": (dict(dim=32, edge_dim=4), 2, 40, 9, 3, True, "default"),
+    # tile boundaries of the neighbour-list kernels (test_gpu_tile_boundaries.py checks that they stay covered): the
+    # slot group TS of pair_kernel / bwd1 / bwd3 (next power of two >= k, at most 32) with one or two slot passes,
+    # the 32-slot steps and 16-row CTAs of bwd2 (N not a multiple of 16), and bwd2's per-pair channel instantiations
+    # QR = 1 (Q = 1), 8 (Q <= 8) and 0 (Q > 8)
+    "k3_q1":        (dict(dim=16, m_pool_method="mean"), 2, 37, 3, 3, True, "xavier"),
+    "k17_q5_c2":    (dict(dim=16, fourier_features=2, soft_edges=True), 2, 70, 17, 2, True, "xavier"),
+    "k32_q10":      (dict(dim=12, edge_dim=9, norm_coors=True), 1, 100, 32, 3, False, "xavier"),
+    "k48_c5_mean":  (dict(dim=8, edge_dim=2, m_pool_method="mean", coor_weights_clamp_value=1.0), 2, 70, 48, 5, True, "xavier"),
+    "k64_q1":       (dict(dim=8, m_pool_method="mean"), 1, 100, 64, 3, False, "xavier"),
+    "k33_mdim24":   (dict(dim=12, m_dim=24, edge_dim=1), 2, 37, 33, 3, True, "xavier"),   # fp64: 32-wide accumulators
 }
 
 
@@ -124,28 +136,34 @@ def test_edge_list_forward_bf16_matches_oracle(name):
     assert ferr < 1e-2 and cerr < 1e-2, (name, mod.last_path, ferr, cerr)
 
 
-@pytest.mark.gpu
-@pytest.mark.parametrize("name", ["plain", "edges_mask", "mean_mask", "mean_nomask", "fourier_c5"])
-def test_edge_list_backward_matches_grad_oracle(name):
+BACKWARD_CASES = ["plain", "edges_mask", "mean_mask", "mean_nomask", "fourier_c5", "k33", "k3_q1", "k17_q5_c2", "k32_q10",
+                  "k48_c5_mean", "k64_q1", "k33_mdim24"]
+
+
+@functools.lru_cache(maxsize=None)
+def _grad_case(name):
+    """(case, neighbour lists, flat oracle gradients) of an EDGE_CASES entry; the oracle runs once per case."""
     case, nb = build(name)
-    ins, cfg = case["inputs"], case["cfg"]
-    mod = util.make_module(case, torch.float64, device="cuda").requires_grad_(True)
-    t = lambda key: util.to_torch(ins.get(key), torch.float64, "cuda")
-    f, x = t("feats").requires_grad_(True), t("coors").requires_grad_(True)
-    e = t("edges")
-    if e is not None:
-        e.requires_grad_(True)
-    gf_np, gx_np = cases.upstream_grads(case)
-    gf, gx = torch.from_numpy(gf_np).cuda(), torch.from_numpy(gx_np).cuda()
-    with torch.enable_grad():
-        fo, xo = mod(f, x, e, mask=t("mask"), neighbors=torch.from_numpy(nb).cuda())
-        ((fo * gf).sum() + (xo * gx).sum()).backward()
-    want = G.egnn_layer_backward(case["params"], cfg, ins["feats"], ins["coors"], ins.get("edges"), ins.get("mask"), None,
-                                 gf_np, gx_np, neighbors=nb)
-    checks = [("feats", f.grad, want["feats"]), ("coors", x.grad, want["coors"])]
-    if e is not None:
-        checks.append(("edges", e.grad, want["edges"]))
-    checks += [(k, p.grad, want["params"][k]) for k, p in mod.named_parameters()]
-    for what, got, ref in checks:
-        scale = max(1.0, float(np.abs(ref).max()))
-        assert util.max_err(got, ref) / scale < 1e-8, (name, what, util.max_err(got, ref), scale)
+    return case, nb, cases.flatten_grads(cases.run_oracle_grad(case, neighbors=nb))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", BACKWARD_CASES)
+def test_edge_list_backward_matches_grad_oracle(name):
+    case, nb, want = _grad_case(name)
+    got = util.module_grads(case, torch.float64, neighbors=nb)
+    util.compare(got, want, 1e-8, f"{name} vs oracle")
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", BACKWARD_CASES)
+@pytest.mark.parametrize("dtype,mode", [(torch.float64, "recompute"), (torch.float32, "saved"), (torch.float32, "recompute")],
+                         ids=["fp64-recompute", "fp32-saved", "fp32-recompute"])
+def test_edge_list_backward_fp32_and_recompute_match_grad_oracle(name, dtype, mode, monkeypatch):
+    """The other three instantiations of the list backward: the fp32 kernels (bwd2's ex2.approx sigmoid among them),
+    and both types with W2 silu(pre1) recomputed by pair_kernel instead of saved by the forward."""
+    if mode == "recompute":
+        monkeypatch.setenv("EGNN_B200_SAVE_PAIR_MB", "0")
+    case, nb, want = _grad_case(name)
+    got = util.module_grads(case, dtype, neighbors=nb)
+    util.compare(got, want, 1e-8 if dtype == torch.float64 else util.grad_tol(case, dtype), f"{name} {mode} vs oracle")

@@ -19,7 +19,7 @@ import util
 pytestmark = pytest.mark.gpu
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 NAMES = list(cases.SPECS)
-TOL = {torch.float64: dict(atol=1e-9, rtol=1e-9), torch.float32: dict(atol=2e-5, rtol=1e-4)}
+TOL = util.TOL
 
 
 @pytest.mark.parametrize("dtype", [torch.float64, torch.float32], ids=["fp64", "fp32"])

@@ -87,6 +87,32 @@ def test_host_side_validation_without_gpu(nat):
     assert lib.egnn_adj_workspace_bytes(1, 8192, C.byref(nb)) == 0 and nb.value == 2 * 8192 * 256 * 4
 
 
+def test_backward_preflight_checks_the_shared_memory_of_the_backward_kernels(nat):
+    """egnn_layer_backward_workspace_bytes (which the training forward calls before it launches anything) sizes bwd1 and
+    bwd2 as their launches do and rejects what exceeds the 220 KB SIMT budget, dense and neighbour lists alike."""
+    lib = nat.load()
+    nb = C.c_size_t()
+    uf_uc = nat.FLAG_UPDATE_FEATS | nat.FLAG_UPDATE_COORS
+    base = dict(abi_version=nat.ABI_VERSION, B=2, N=40, C=3, dim=16, edge_dim=0, label_dim=0, num_labels=0, m_dim=16,
+                fourier=0, k=0, flags=uf_uc, valid_radius=1e30, clamp=0.0, row_begin=0, row_end=0, reserved=0)
+    soft = uf_uc | nat.FLAG_SOFT_EDGES
+    over_in_fp64 = [dict(m_dim=32),                                  # bwd1: 234,032 B
+                    dict(m_dim=24, flags=soft),                      # bwd1: 225,328 B
+                    dict(dim=8, fourier=30, edge_dim=16)]            # dense bwd2: 77 channels, about 311 KB
+    fits = [dict(m_dim=24), dict(m_dim=20, flags=soft), dict(m_dim=17), dict(label_dim=4, num_labels=16),
+            dict(dim=8, fourier=30, edge_dim=16, m_dim=32)]         # (the last in fp32 only: see below)
+    rc = lambda **kw: lib.egnn_layer_backward_workspace_bytes(C.byref(nat.LayerDesc(**dict(base, **kw))), C.byref(nb))
+    for k in (0, 20):
+        for cfg in over_in_fp64:
+            assert rc(dtype=nat.DTYPE_F64, k=k, **cfg) == -3, (cfg, k)
+            assert rc(dtype=nat.DTYPE_F32, k=k, **cfg) == 0, (cfg, k)
+        for cfg in fits[:-1]:
+            assert rc(dtype=nat.DTYPE_F64, k=k, **cfg) == 0, (cfg, k)
+        assert rc(dtype=nat.DTYPE_F32, k=k, **fits[-1]) == 0
+        for dt in (nat.DTYPE_F32, nat.DTYPE_F64):
+            assert rc(dtype=dt, k=k, label_dim=4, num_labels=17) == -3        # label rows of bwd2's shared table
+
+
 @pytest.mark.parametrize("name", ["dense_everything", "knn_edges_mask", "dense_no_feats", "dense_no_coors",
                                   "net_c5_xavier", "net_edge_tokens", "net_c3_small"])
 def test_reference_state_dict_loads_unchanged(name):

@@ -1,11 +1,17 @@
 """Helpers shared by the GPU parity tests, smoke() and bench.py: build the product modules from
-a tests/cases.py case and move numpy inputs to torch."""
+a tests/cases.py case, move numpy inputs to torch, and run / compare forward and backward."""
 from __future__ import annotations
 
 import numpy as np
 import torch
 
 import cases
+
+# Forward tolerances against the fp64 oracle (stated per SURVEY.md section 8(c)):
+#   fp64 kernels : atol 1e-9,  rtol 1e-9   (same algebra, different summation order)
+#   fp32 kernels : atol 2e-5,  rtol 1e-4   (the reference's own fp32-vs-fp64 deviation is <= 5e-6 at these sizes,
+#                  BASELINE.md section 2)
+TOL = {torch.float64: dict(atol=1e-9, rtol=1e-9), torch.float32: dict(atol=2e-5, rtol=1e-4)}
 
 
 def to_torch(x, dtype, device):
@@ -35,6 +41,55 @@ def run_module(mod, case, dtype, device="cuda", **kw):
     if case["kind"] == "network":
         return mod(t("feats"), t("coors"), adj_mat=t("adj_mat"), edges=t("edges"), mask=t("mask"), **kw)
     return mod(t("feats"), t("coors"), t("edges"), mask=t("mask"), adj_mat=t("adj_mat"), **kw)
+
+
+def module_grads(case, dtype, device="cuda", neighbors=None):
+    """Run forward + backward of the product module; -> flat {name: float64 numpy gradient}.  `neighbors` (numpy
+    [B,N,k], -1 = empty slot) runs a layer in edge-list mode."""
+    mod = make_module(case, dtype, device=device)
+    mod.requires_grad_(True)
+    ins = case["inputs"]
+    t = lambda name: to_torch(ins.get(name), dtype, device)
+    feats, coors, edges = t("feats"), t("coors"), t("edges")
+    leaves = {"coors": coors.requires_grad_(True)}
+    if feats.is_floating_point():
+        leaves["feats"] = feats.requires_grad_(True)
+    if edges is not None and edges.is_floating_point():
+        leaves["edges"] = edges.requires_grad_(True)
+    gf, gx = (torch.from_numpy(g).to(device=device, dtype=dtype) for g in cases.upstream_grads(case))
+    with torch.enable_grad():
+        if case["kind"] == "network":
+            fo, xo = mod(feats, coors, adj_mat=t("adj_mat"), edges=edges, mask=t("mask"))
+        elif neighbors is not None:
+            fo, xo = mod(feats, coors, edges, mask=t("mask"), neighbors=torch.from_numpy(neighbors).to(device))
+        else:
+            fo, xo = mod(feats, coors, edges, mask=t("mask"), adj_mat=t("adj_mat"))
+        assert fo.requires_grad and xo.requires_grad
+        ((fo * gf).sum() + (xo * gx).sum()).backward()
+    out = {f"in.{k}": v.grad.double().cpu().numpy() for k, v in leaves.items()}
+    for k, p in mod.named_parameters():
+        out[f"p.{k}"] = (torch.zeros_like(p) if p.grad is None else p.grad).double().cpu().numpy()
+    return out
+
+
+def compare(got, want, tol, what):
+    """Every gradient within `tol` of the reference, relative to max(1, its largest magnitude)."""
+    assert set(got) == set(want), (what, sorted(set(got) ^ set(want)))
+    bad = []
+    for k in sorted(want):
+        scale = max(1.0, float(np.abs(want[k]).max()))
+        err = float(np.abs(got[k] - want[k]).max()) / scale
+        if not np.isfinite(got[k]).all() or err > tol:
+            bad.append(f"{k}: rel err {err:.3e}")
+    assert not bad, f"{what}: " + "; ".join(bad)
+
+
+def grad_tol(case, dtype):
+    """Gradient tolerance of `compare` against the fp64 backward oracle."""
+    if dtype == torch.float64:
+        # CoorsNorm: the oracle (like the reference) carries ~1e-9 of cancellation noise from the 1/eps self pair
+        return 1e-7 if "norm_coors" in str(case["spec"]["cfg"]) else 1e-9
+    return 5e-4
 
 
 def max_err(a, b):
