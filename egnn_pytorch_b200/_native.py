@@ -9,7 +9,7 @@ from __future__ import annotations
 import ctypes as C
 import os
 
-ABI_VERSION = 3
+ABI_VERSION = 4
 
 DTYPE_F32, DTYPE_F64, DTYPE_BF16 = 0, 1, 2
 
@@ -22,6 +22,7 @@ FLAG_POOL_MEAN = 1 << 5
 FLAG_CLAMP = 1 << 6
 FLAG_ONLY_SPARSE = 1 << 7
 FLAG_ADJ_BATCHED = 1 << 8
+FLAG_EDGES_PER_SLOT = 1 << 9
 
 ERR_UNSUPPORTED = -3
 

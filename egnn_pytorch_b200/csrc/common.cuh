@@ -103,6 +103,15 @@ inline Dims make_dims(const EgnnLayerDesc& d) {
   return s;
 }
 
+// The edge-feature row of slot `slot` of row node_i = b*N + i, whose neighbour is j: [B,N,k,edge_dim] per slot under
+// EGNN_FLAG_EDGES_PER_SLOT, else [B,N,N,edge_dim] per pair.  Every reader and the per-slot gradient store use this one
+// rule.  A slot beyond k (a padding lane) reads slot 0, which always exists.
+template <typename E>
+__device__ __forceinline__ E* edge_row(E* edges, bool per_slot, size_t node_i, int slot, int j, int N, int k, int edge_dim) {
+  const size_t r = per_slot ? node_i * k + (slot < k ? slot : 0) : node_i * N + j;
+  return edges + r * edge_dim;
+}
+
 // ------------------------------------------------------------------ dropout (training mode, egnn_pytorch.py:176-208)
 // nn.Dropout(p) sits between Linear-1 and SiLU of edge_mlp / node_mlp / coors_mlp.  The masks are never stored: every
 // kernel (forward, recompute, backward) regenerates the keep/drop decision of an element from a counter hash of

@@ -211,7 +211,8 @@ extern "C" int egnn_layer_forward_host(const EgnnLayerDesc* desc, const EgnnLaye
   const size_t es = elem_size(desc->dtype);
   const size_t cs = desc->dtype == EGNN_DTYPE_F64 ? 8 : 4;
   const size_t nf = (size_t)s.M * s.dim * es, nc = (size_t)s.M * s.C * cs;
-  const size_t ne = hio->edges ? (size_t)s.M * s.N * s.edge_dim * es : 0;
+  const size_t erows = (desc->flags & EGNN_FLAG_EDGES_PER_SLOT) ? (size_t)s.k : (size_t)s.N;   // edge rows per node
+  const size_t ne = hio->edges ? (size_t)s.M * erows * s.edge_dim * es : 0;
   const size_t nl = hio->edge_labels ? (size_t)s.M * s.N : 0;
   const size_t nm = hio->mask ? (size_t)s.M : 0;
   const size_t na = hio->adj ? (size_t)((desc->flags & EGNN_FLAG_ADJ_BATCHED) ? s.B : 1) * s.N * s.N : 0;

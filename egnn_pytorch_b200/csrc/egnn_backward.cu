@@ -44,6 +44,7 @@ extern "C" int egnn_layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWei
   if (!io->feats || !io->coors) return EGNN_ERR_NULL;
   if (desc->edge_dim > 0 && !io->edges) return EGNN_ERR_NULL;
   if (desc->label_dim > 0 && !io->edge_labels) return EGNN_ERR_NULL;
+  if ((desc->flags & EGNN_FLAG_EDGES_PER_SLOT) && !io->nbr_idx) return EGNN_ERR_SHAPE;
   EGNN_TRY(check_grad_ptrs(*desc, grads));
   if (((uintptr_t)workspace | (uintptr_t)fwd_workspace) & 0xFF) return EGNN_ERR_ALIGN;
   cudaStream_t st = static_cast<cudaStream_t>(stream);

@@ -193,7 +193,10 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
   EGNN_TRY(zero(gr.w.coors_w2, (size_t)4 * m * es));
   EGNN_TRY(zero(gr.w.coors_b2, es));
   EGNN_TRY(zero(gr.w.label_emb, (size_t)s.num_labels * s.label_dim * es));
-  if (gr.g_edges && s.k > 0) EGNN_TRY(zero(gr.g_edges, (size_t)M * s.N * s.edge_dim * es));
+  // neighbour lists: bwd3 adds dL/d edges into [B,N,N,e] with atomics, or stores them per slot ([B,N,k,e]) -- empty slots
+  // are skipped, so they keep these zeros
+  const size_t edge_rows = (d.flags & EGNN_FLAG_EDGES_PER_SLOT) ? (size_t)s.k : (size_t)s.N;
+  if (gr.g_edges && s.k > 0) EGNN_TRY(zero(gr.g_edges, (size_t)M * edge_rows * s.edge_dim * es));
   // residual / identity paths: h' = ... + h (:337, :339), x' = x + ... (:315, :317)
   EGNN_CUDA_TRY(cudaMemcpyAsync(g_feats, go, (size_t)M * dim * es, cudaMemcpyDeviceToDevice, st));
   EGNN_CUDA_TRY(cudaMemcpyAsync(g_coors, gr.g_coors_out, (size_t)M * s.C * es, cudaMemcpyDeviceToDevice, st));

@@ -52,7 +52,7 @@ struct BwdArgs {
   T clamp;
   const T* P; int ldP;        // forward tables [M][2*Hp]: A | B
   const T* coors;
-  const T* edges;
+  const T* edges;                 // [B,N,N,edge_dim], [B,N,k,edge_dim] under EGNN_FLAG_EDGES_PER_SLOT, | null
   const uint8_t* labels;
   const uint8_t* mask;
   const int32_t* nbr_idx;
@@ -66,7 +66,7 @@ struct BwdArgs {
   T* gpk;                         // gradient accumulators in SimtPackLayout order (zeroed by the caller)
   T* gP;                          // [M][2*Hp]: dL/dA | dL/dB (zeroed by the caller)
   T* g_coors;                     // [B,N,C], pre-loaded with g_coors_out
-  T* g_edges;                     // [B,N,N,edge_dim] | null
+  T* g_edges;                     // [B,N,N,edge_dim], [B,N,k,edge_dim] under EGNN_FLAG_EDGES_PER_SLOT, | null
   DropCfg drop;                   // the forward's dropout configuration (masks are regenerated, never stored)
 };
 
@@ -196,7 +196,8 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
     const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
     if (pair_exists) {
       T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
-      for (int q = 0; q < s.Q; ++q) r[a.rl.f + q] = pair_channel<T>(s, a.edges, pair, q, d);
+      const T* erow = edge_row(a.edges, KNN && (a.flags & EGNN_FLAG_EDGES_PER_SLOT), node_i, sidx, j, s.N, s.k, s.edge_dim);
+      for (int q = 0; q < s.Q; ++q) r[a.rl.f + q] = pair_channel<T>(s, erow, q, d);
     }
 
     // ---- W2 silu(pre1) of this pair, as the forward (or its recompute) left it (empty slots were never stored: they
@@ -850,6 +851,7 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
     gxo[c] = (c < s.C) ? a.g_coors_out[node_i * s.C + c] : T(0);
     gxi[c] = T(0);
   }
+  const bool per_slot = KNN && (a.flags & EGNN_FLAG_EDGES_PER_SLOT);
   for (int s0 = 0; s0 < J; s0 += TS) {
     const int sidx = s0 + sl;
     const PairSlot ps = pair_slot<KNN>(a.nbr_idx, nullptr, s.k, node_i, sidx, row_valid && sidx < J);
@@ -863,10 +865,10 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
       const T sc = T(1 << q);
       gd += (r[a.rl.gf + q] * cos(d / sc) - r[a.rl.gf + s.F + q] * sin(d / sc)) / sc;
     }
-    if (a.g_edges) {
-      T* ge = a.g_edges + (node_i * s.N + j) * s.edge_dim;
+    if (a.g_edges) {      // per-slot edges: this thread alone owns the slot, so a plain store, no atomic
+      T* ge = edge_row(a.g_edges, per_slot, node_i, sidx, j, s.N, s.k, s.edge_dim);
       for (int e = 0; e < s.edge_dim; ++e) {
-        if (KNN) atomic_add_t<T>(ge + e, r[a.rl.gf + s.Qd + e]);
+        if (KNN && !per_slot) atomic_add_t<T>(ge + e, r[a.rl.gf + s.Qd + e]);
         else ge[e] = r[a.rl.gf + s.Qd + e];
       }
     }

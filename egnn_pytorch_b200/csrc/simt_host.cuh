@@ -28,6 +28,8 @@ static int validate_desc(const EgnnLayerDesc* d) {
   if (!(d->dropout_p >= 0.0 && d->dropout_p < 1.0)) return EGNN_ERR_SHAPE;
   if (d->dropout_p > 0.0 && d->dtype == EGNN_DTYPE_BF16) return EGNN_ERR_UNSUPPORTED;     // training runs the fp32 / fp64 kernels
   if (d->row_begin < 0 || d->row_end < 0 || d->row_end > d->N || d->row_begin > d->row_end) return EGNN_ERR_SHAPE;
+  // per-slot edges follow the slots of caller-supplied lists; the library's own top-k has no order they could follow
+  if ((d->flags & EGNN_FLAG_EDGES_PER_SLOT) && (d->k == 0 || d->edge_dim == 0)) return EGNN_ERR_SHAPE;
   return EGNN_OK;
 }
 
@@ -150,6 +152,7 @@ static int check_ptrs(const EgnnLayerDesc& d, const EgnnLayerWeights* w, const E
     if (!io->feats || !io->coors || !io->feats_out || !io->coors_out) return EGNN_ERR_NULL;
     if (d.edge_dim > 0 && !io->edges) return EGNN_ERR_NULL;
     if (d.label_dim > 0 && !io->edge_labels) return EGNN_ERR_NULL;
+    if ((d.flags & EGNN_FLAG_EDGES_PER_SLOT) && !io->nbr_idx) return EGNN_ERR_SHAPE;
     const uintptr_t all = (uintptr_t)io->feats | (uintptr_t)io->feats_out | (uintptr_t)io->edges;
     if (all & 0xF) return EGNN_ERR_ALIGN;
   }

@@ -290,7 +290,7 @@ struct PairArgs {
   T clamp;
   const T* P; int ldP;       // [M][2*Hp]: A | B
   const T* coors;            // [B,N,C]
-  const T* edges;            // [B,N,N,edge_dim] | null
+  const T* edges;            // [B,N,N,edge_dim], [B,N,k,edge_dim] under EGNN_FLAG_EDGES_PER_SLOT, | null
   const uint8_t* labels;     // [B,N,N] | null
   const uint8_t* mask;       // [B,N] | null
   const int32_t* nbr_idx;    // [B,N,k] (KNN)
@@ -337,14 +337,14 @@ __device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&
   return d;
 }
 
-// Scalar channel q of pair `pair` = (b * N + i) * N + j: fourier_encode_dist (egnn_pytorch.py:34-41), the squared
-// distance, then the continuous edge features.
+// Scalar channel q of a pair: fourier_encode_dist (egnn_pytorch.py:34-41), the squared distance, then the continuous
+// edge features from the pair's edge row `erow` (edge_row).
 template <typename T>
-__device__ __forceinline__ T pair_channel(const Dims& s, const T* edges, size_t pair, int q, T d) {
+__device__ __forceinline__ T pair_channel(const Dims& s, const T* erow, int q, T d) {
   if (q < s.F) return sin(d / T(1 << q));
   if (q < 2 * s.F) return cos(d / T(1 << (q - s.F)));
   if (q == 2 * s.F) return d;
-  return edges[pair * s.edge_dim + (q - s.Qd)];
+  return erow[q - s.Qd];
 }
 
 // m_ij = silu(W2 hid + b2) (pad lanes: silu(0) = 0), times the soft-edge gate (egnn_pytorch.py:287-290).
@@ -463,8 +463,10 @@ pair_kernel(const PairArgs<T> a) {
     T rel[PAIR_CMAX];
     const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
     // ---- per-pair scalar channels other than d go through shared memory
-    if (s.Q > 1)
-      for (int q = 0; q < s.Q; ++q) fs[q * PAIR_THREADS + tid] = pair_channel<T>(s, a.edges, pair, q, d);
+    if (s.Q > 1) {
+      const T* erow = edge_row(a.edges, a.flags & EGNN_FLAG_EDGES_PER_SLOT, node_i, sidx, j, s.N, s.k, s.edge_dim);
+      for (int q = 0; q < s.Q; ++q) fs[q * PAIR_THREADS + tid] = pair_channel<T>(s, erow, q, d);
+    }
     int lab = 0;
     if (a.labels) lab = a.labels[pair];
     const T* Brow = a.P + ((size_t)b * s.N + j) * a.ldP + s.Hp;
@@ -659,7 +661,8 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
       d[p] = pair_geometry<T>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel);
       lab[p] = a.labels ? a.labels[pair] : 0;
       if (s.Q > 1)
-        for (int q = 0; q < s.Q; ++q) fs[(p * s.Q + q) * PAIR_THREADS + tid] = pair_channel<T>(s, a.edges, pair, q, d[p]);
+        for (int q = 0; q < s.Q; ++q)
+          fs[(p * s.Q + q) * PAIR_THREADS + tid] = pair_channel<T>(s, a.edges + pair * s.edge_dim, q, d[p]);
     }
 
     T acc[PP][MP];

@@ -46,7 +46,7 @@ struct TcKnnArgs {
   const __nv_bfloat16* w2p;        // W2 in core-matrix order
   const float* epi;
   const float* coors;              // [B][N][3]
-  const __nv_bfloat16* edges;      // [B][N][N][edge_dim] | null
+  const __nv_bfloat16* edges;      // [B][N][N][edge_dim], [B][N][k][edge_dim] under EGNN_FLAG_EDGES_PER_SLOT, | null
   const uint8_t* mask;             // [B][N] | null
   const int32_t* nbr_idx;          // [B][N][k]
   const uint8_t* nbr_ok;           // [B][N][k]
@@ -162,7 +162,8 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
     }
     q += 2 * a.F;
     const size_t pij = ((size_t)b * N + i) * N + j;
-    for (int e = 0; e < a.edge_dim; ++e) myS[(q + e) * 32 + lane] = __bfloat162float(a.edges[pij * a.edge_dim + e]);
+    const __nv_bfloat16* erow = edge_row(a.edges, a.flags & EGNN_FLAG_EDGES_PER_SLOT, nodei, lane, j, N, K, a.edge_dim);
+    for (int e = 0; e < a.edge_dim; ++e) myS[(q + e) * 32 + lane] = __bfloat162float(erow[e]);
     q += a.edge_dim;
     if (a.num_labels > 0) {
       const int lab = a.labels[pij];
@@ -180,8 +181,8 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
     dr[rho] = __shfl_sync(0xffffffffu, dmine, lr + 8 * rho);
 #pragma unroll
     for (int q = 0; q < TK_QE; ++q) ef[rho][q] = 0.f;
-    if (EDGES) {
-      const __nv_bfloat16* ep = a.edges + (((size_t)b * N + i) * N + jf[rho]) * a.edge_dim;
+    if (EDGES) {      // per-slot edges: the warp's 32 slots are one contiguous run of 32 * edge_dim values
+      const __nv_bfloat16* ep = edge_row(a.edges, a.flags & EGNN_FLAG_EDGES_PER_SLOT, nodei, lr + 8 * rho, jf[rho], N, K, a.edge_dim);
 #pragma unroll
       for (int q = 0; q < TK_QE; ++q) if (q < a.edge_dim) ef[rho][q] = __bfloat162float(ep[q]);
     }

@@ -284,25 +284,49 @@ class EGNN(nn.Module):
         return torch.float32
 
     # -------------------------------------------------------------- forward
-    def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, _edge_labels=None,
-                _label_emb=None, _k_hint=None, _rows=None):
+    def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, neighbor_edges=None,
+                _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
         """Reference signature `forward(feats, coors, edges=None, mask=None, adj_mat=None)` (egnn_pytorch.py:224).
 
         `neighbors` (additive, keyword-only): int tensor [B, N, k] of neighbour indices, -1 = empty slot.  When
         given, the layer runs on exactly these edges and the O(N^2) distance / top-k pass is skipped -- the
-        edge-list mode of SURVEY.md section 8(f) (`edge_index_to_neighbors` converts a PyG-style edge_index)."""
+        edge-list mode of SURVEY.md section 8(f) (`edge_index_to_neighbors` converts a PyG-style edge_index).
+
+        `neighbor_edges` (additive, keyword-only, needs `neighbors`, replaces `edges`): float tensor
+        [B, N, k, edge_dim] of edge features per neighbour slot -- slot s of node i holds the features of the edge
+        neighbors[b, i, s] -> i -- so a sparse graph needs no [B, N, N, edge_dim] tensor.  Its gradient has the same
+        shape (0 in empty slots)."""
+        if neighbor_edges is not None:
+            edges = self._check_neighbor_edges(feats, edges, neighbors, neighbor_edges, _label_emb)
         if torch.is_grad_enabled():             # (the parameter scan is skipped entirely under torch.no_grad())
             fields = self._state_fields()
             if (feats.requires_grad or coors.requires_grad or (edges is not None and edges.requires_grad) or
                     (_label_emb is not None and _label_emb.requires_grad) or any(p.requires_grad for _, _, _, p in fields)):
                 return self._forward_train(fields, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb,
-                                           _k_hint, _rows)
+                                           _k_hint, _rows, neighbor_edges is not None)
             with torch.no_grad():
                 return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint,
-                                          _rows)
-        return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows)
+                                          _rows, slot_edges=neighbor_edges is not None)
+        return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
+                                  slot_edges=neighbor_edges is not None)
 
-    def _forward_train(self, fields, feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows):
+    def _check_neighbor_edges(self, feats, edges, neighbors, neighbor_edges, label_emb):
+        """Misuse of `neighbor_edges` raises here, before anything is staged or launched; -> the tensor to run with."""
+        if neighbors is None:
+            raise ValueError("neighbor_edges needs neighbors=: its slots follow the caller's neighbour lists")
+        if edges is not None:
+            raise ValueError("pass edge features either as edges [B, N, N, edge_dim] or as neighbor_edges "
+                             "[B, N, k, edge_dim], not both")
+        edge_dim = self.edge_dim - (0 if label_emb is None else label_emb.shape[1])
+        b, n = feats.shape[:2]
+        want = (b, n, neighbors.shape[-1], edge_dim)
+        if edge_dim == 0 or tuple(neighbor_edges.shape) != want or not neighbor_edges.is_floating_point():
+            raise ValueError(f"neighbor_edges must be a float tensor of shape (B, N, k, edge_dim) = {want} for this layer "
+                             f"(edge_dim > 0), got {neighbor_edges.dtype} {tuple(neighbor_edges.shape)}")
+        return neighbor_edges
+
+    def _forward_train(self, fields, feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
+                       slot_edges=False):
         if rows is not None:
             raise NotImplementedError("a row range (_rows) cannot be differentiated: call it under torch.no_grad() for "
                                       "inference, or shard the batch (parallel.batch_sharded_call) for training")
@@ -310,12 +334,13 @@ class EGNN(nn.Module):
 
         def run():
             return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, None,
-                                      train=True, param_fields=[f for _, _, f, _ in fields])
+                                      train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges)
 
         return _EGNNLayerFunction.apply(run, feats, coors, edges, label_emb, *params)
 
     def _forward_impl(self, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
-                      train=False, param_fields=None):
+                      train=False, param_fields=None, slot_edges=False):
+        """`slot_edges`: `edges` holds features per neighbour slot, [B, N, k, edge_dim] (forward's `neighbor_edges`)."""
         lib = nat.load()
         dev = _compute_device(feats)
         b, n, d = feats.shape
@@ -336,6 +361,8 @@ class EGNN(nn.Module):
         adj_u8 = None
         k = 0
         flags = self._flags()
+        if slot_edges:
+            flags |= nat.FLAG_EDGES_PER_SLOT
         nbr = None
         if neighbors is not None:
             assert neighbors.dim() == 3 and neighbors.shape[:2] == (b, n), "neighbors must be [B, N, k]"
@@ -482,10 +509,15 @@ class EGNN(nn.Module):
         return outs + (saved,)
 
 
-def edge_index_to_neighbors(edge_index, num_nodes, k=None):
+def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
     """PyG-style `edge_index` [2, E] (messages flow source j = edge_index[0] -> target i = edge_index[1], one graph)
     -> padded neighbour lists [1, N, k] for `EGNN.forward(..., neighbors=...)`; -1 marks empty slots.  Glue code:
-    a stable sort by target node, nothing on the hot path."""
+    a stable sort by target node, nothing on the hot path.
+
+    With `edge_attr` [E, e] (PyG's per-edge features) it returns `(neighbors, neighbor_edges)`: neighbor_edges
+    [1, N, k, e] holds each edge's features in that edge's slot (same order, same truncation at k, zeros in empty
+    slots), for `EGNN.forward(..., neighbors=, neighbor_edges=)`.  It is built by indexing, so gradients flow back
+    to edge_attr."""
     src, dst = edge_index[0].long(), edge_index[1].long()
     order = torch.argsort(dst, stable=True)
     src, dst = src[order], dst[order]
@@ -496,7 +528,13 @@ def edge_index_to_neighbors(edge_index, num_nodes, k=None):
     out = torch.full((num_nodes, kmax), -1, dtype=torch.int32, device=src.device)
     keep = slot < kmax
     out[dst[keep], slot[keep]] = src[keep].to(torch.int32)
-    return out.unsqueeze(0)
+    if edge_attr is None:
+        return out.unsqueeze(0)
+    assert edge_attr.dim() == 2 and edge_attr.shape[0] == src.numel(), "edge_attr must be [E, edge_dim]"
+    keep_idx = order[keep]
+    slot_attr = edge_attr.new_zeros((num_nodes, kmax, edge_attr.shape[1])).index_put(
+        (dst[keep], slot[keep]), edge_attr[keep_idx])
+    return out.unsqueeze(0), slot_attr.unsqueeze(0)
 
 
 # ----------------------------------------------------------------------------- global attention

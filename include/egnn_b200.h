@@ -28,8 +28,9 @@
 extern "C" {
 #endif
 
-#define EGNN_ABI_VERSION 3   /* 2: EgnnLayerIO grew nbr_idx + pre2_out; backward entry points added
-                                3: peer-memory all-gather communicator (egnn_comm_*), egnn_global_attn_* */
+#define EGNN_ABI_VERSION 4   /* 2: EgnnLayerIO grew nbr_idx + pre2_out; backward entry points added
+                                3: peer-memory all-gather communicator (egnn_comm_*), egnn_global_attn_*
+                                4: EGNN_FLAG_EDGES_PER_SLOT (io.edges / g_edges per neighbour slot) */
 
 /* ---- error codes ------------------------------------------------------------------- */
 #define EGNN_OK                 0
@@ -57,6 +58,10 @@ extern "C" {
 #define EGNN_FLAG_ONLY_SPARSE   (1u << 7)   /* only_sparse_neighbors: valid_radius := 0 (:250);
                                                the caller passes k = max adjacency row sum   */
 #define EGNN_FLAG_ADJ_BATCHED   (1u << 8)   /* io.adj is [B,N,N] instead of [N,N] (:245)      */
+#define EGNN_FLAG_EDGES_PER_SLOT (1u << 9)  /* io.edges / grads.g_edges are [B,N,k,edge_dim], aligned with the caller's
+                                               io.nbr_idx: slot s of row i holds edge nbr_idx[b,i,s] -> i.  Needs
+                                               k > 0 and edge_dim > 0 (else EGNN_ERR_SHAPE) and io.nbr_idx != NULL
+                                               (EGNN_ERR_SHAPE from egnn_layer_forward / egnn_layer_backward) */
 
 /*
  * Static description of one layer call.  E = 2*dim + 2*fourier + 1 + edge_dim + label_dim
@@ -121,7 +126,8 @@ typedef struct EgnnLayerWeights {
 typedef struct EgnnLayerIO {
   const void*    feats;      /* [B, N, dim]                                               */
   const void*    coors;      /* [B, N, C]                                                 */
-  const void*    edges;      /* [B, N, N, edge_dim] or NULL when edge_dim == 0            */
+  const void*    edges;      /* [B, N, N, edge_dim], or [B, N, k, edge_dim] per neighbour slot under
+                                EGNN_FLAG_EDGES_PER_SLOT; NULL when edge_dim == 0                */
   const uint8_t* edge_labels;/* [B, N, N] label index per pair, or NULL when label_dim == 0 */
   const uint8_t* mask;       /* [B, N] 0/1, or NULL (= the reference's mask=None)         */
   const uint8_t* adj;        /* [N, N] or [B, N, N] 0/1 (EGNN_FLAG_ADJ_BATCHED), or NULL;
@@ -186,7 +192,9 @@ typedef struct EgnnLayerGrads {
   const void* g_coors_out;   /* [B, N, C]    dL/d coors_out (input)                         */
   void*       g_feats;       /* [B, N, dim]  dL/d feats                                     */
   void*       g_coors;       /* [B, N, C]    dL/d coors                                     */
-  void*       g_edges;       /* [B, N, N, edge_dim] dL/d edges, or NULL (not wanted / edge_dim == 0) */
+  void*       g_edges;       /* [B, N, N, edge_dim] dL/d edges, or NULL (not wanted / edge_dim == 0).
+                                Under EGNN_FLAG_EDGES_PER_SLOT [B, N, k, edge_dim]: one plain store per slot, no
+                                atomics across slots; empty (-1) slots get 0                     */
   EgnnLayerWeightGrads w;
 } EgnnLayerGrads;
 
