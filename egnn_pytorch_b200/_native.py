@@ -23,6 +23,7 @@ FLAG_CLAMP = 1 << 6
 FLAG_ONLY_SPARSE = 1 << 7
 FLAG_ADJ_BATCHED = 1 << 8
 FLAG_EDGES_PER_SLOT = 1 << 9
+FLAG_ROW_PARTIAL_GRADS = 1 << 10
 
 ERR_UNSUPPORTED = -3
 

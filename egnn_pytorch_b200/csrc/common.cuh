@@ -103,6 +103,20 @@ inline Dims make_dims(const EgnnLayerDesc& d) {
   return s;
 }
 
+// Row blocks (EGNN_FLAG_ROW_PARTIAL_GRADS with a range other than all rows): the per-pair buffers (pre2, the backward
+// record) hold the block's rows only, B x (row1 - row0), row i at i - row0.  The pair kernels take this as a template
+// parameter BLK, so the instantiations without a row block keep the plain node-order arithmetic and their arguments.
+inline bool row_block(const Dims& s, uint32_t flags) {
+  return (flags & EGNN_FLAG_ROW_PARTIAL_GRADS) && (s.row0 != 0 || s.row1 != s.N);
+}
+// Rows per graph of the per-pair buffers.
+inline int pair_rows(const Dims& s, uint32_t flags) { return row_block(s, flags) ? s.row1 - s.row0 : s.N; }
+// Row of node (b, i) in the per-pair buffers.
+template <bool BLK>
+__host__ __device__ __forceinline__ size_t pair_row(const Dims& s, int b, int i) {
+  return BLK ? (size_t)b * (s.row1 - s.row0) + (i - s.row0) : (size_t)b * s.N + i;
+}
+
 // The edge-feature row of slot `slot` of row node_i = b*N + i, whose neighbour is j: [B,N,k,edge_dim] per slot under
 // EGNN_FLAG_EDGES_PER_SLOT, else [B,N,N,edge_dim] per pair.  Every reader and the per-slot gradient store use this one
 // rule.  A slot beyond k (a padding lane) reads slot 0, which always exists.

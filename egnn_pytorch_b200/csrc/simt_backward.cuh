@@ -60,7 +60,7 @@ struct BwdArgs {
   const T* packed;
   const T* g_node_in; int ld_g;   // [M][dim+m]; dL/dm_i = columns dim..dim+m  (null when !update_feats)
   const T* g_coors_out;           // [B,N,C]
-  const T* pre2;                  // W2 silu(pre1) per pair, row-major [B,N,J][MP]: saved by the forward
+  const T* pre2;                  // W2 silu(pre1) per pair, row-major [B,N,J][MP] (rows by pair_row): saved by the forward
                                   // (EgnnLayerIO.pre2_out) or recomputed into the backward workspace
   T* rec;                         // [pairs][R]
   T* gpk;                         // gradient accumulators in SimtPackLayout order (zeroed by the caller)
@@ -81,11 +81,18 @@ __device__ __forceinline__ float sigmoid_bw(float x) {
 __device__ __forceinline__ double sigmoid_bw(double x) { return 1.0 / (1.0 + exp(-x)); }
 
 // Record index of pair (b, i, slot).  kNN: row-major (b, i, slot).  Dense: (b, j, i) -- "column-major" -- so that the
-// records of 32 consecutive rows i for one neighbour j are contiguous, which is what a bwd2 CTA streams.
-template <bool KNN>
-__device__ __forceinline__ size_t rec_index(int b, int N, int J, int i, int slot) {
-  return KNN ? ((size_t)b * N + i) * J + slot : ((size_t)b * N + slot) * N + i;
+// records of 32 consecutive rows i for one neighbour j are contiguous, which is what a bwd2 CTA streams.  Rows count
+// from row0 over row1 - row0 per graph for a row block (BLK, pair_row), so its record is sized by the block.
+template <bool KNN, bool BLK>
+__device__ __forceinline__ size_t rec_index(const Dims& s, int b, int N, int J, int i, int slot) {
+  if (!BLK) return KNN ? ((size_t)b * N + i) * J + slot : ((size_t)b * N + slot) * N + i;
+  const int R = s.row1 - s.row0, r = i - s.row0;
+  return KNN ? ((size_t)b * R + r) * J + slot : ((size_t)b * N + slot) * R + r;
 }
+
+// The i-rows a backward pair kernel covers: the row block (BLK), else all N rows.
+template <bool BLK> __device__ __forceinline__ int rows_begin(const Dims& s) { return BLK ? s.row0 : 0; }
+template <bool BLK> __device__ __forceinline__ int rows_end(const Dims& s) { return BLK ? s.row1 : s.N; }
 
 __device__ __forceinline__ void cp_async_elem(void* smem_dst, const float* g) {
   asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"((uint32_t)__cvta_generic_to_shared(smem_dst)), "l"(g) : "memory");
@@ -110,7 +117,7 @@ inline size_t bwd1_smem_bytes(const Dims& s, const SimtPackLayout& L, bool soft)
   return round_up(n * sizeof(T), 16) + 16;
 }
 
-template <typename T, int MP, bool KNN>
+template <typename T, int MP, bool KNN, bool BLK>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd1_kernel(const BwdArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -119,9 +126,9 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
   const int TS = a.TS, TI = PAIR_THREADS / TS;
   const int g = tid / TS, sl = tid % TS;
   const int b = blockIdx.y;
-  const int i_raw = blockIdx.x * TI + g;
-  const bool row_valid = i_raw < s.N;
-  const int i = row_valid ? i_raw : 0;
+  const int i_raw = rows_begin<BLK>(s) + blockIdx.x * TI + g;
+  const bool row_valid = i_raw < rows_end<BLK>(s);
+  const int i = row_valid ? i_raw : rows_begin<BLK>(s);
   const int J = KNN ? s.k : s.N;
   const int U = 4 * s.m, UP = U + 1;
   const bool upd_feats = a.flags & EGNN_FLAG_UPDATE_FEATS;
@@ -195,7 +202,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
     T rel[PAIR_CMAX];
     const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
     if (pair_exists) {
-      T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
+      T* r = a.rec + rec_index<KNN, BLK>(s, b, s.N, J, i, sidx) * a.rl.R;
       const T* erow = edge_row(a.edges, KNN && (a.flags & EGNN_FLAG_EDGES_PER_SLOT), node_i, sidx, j, s.N, s.k, s.edge_dim);
       for (int q = 0; q < s.Q; ++q) r[a.rl.f + q] = pair_channel<T>(s, erow, q, d);
     }
@@ -204,7 +211,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
     // read as zeros).  An accumulator wider than 32 registers (fp64, m_dim > 16) is read again for the second SiLU
     // rather than held through the coordinate branch, where it would spill.
     constexpr bool REREAD = MP * sizeof(T) > 32 * 4;
-    const T* pre2_src = a.pre2 + (node_i * (size_t)J + sidx) * MP;
+    const T* pre2_src = a.pre2 + ((BLK ? pair_row<true>(s, b, i) : node_i) * (size_t)J + sidx) * MP;
     auto load_pre2 = [&](T (&v)[MP]) {
 #pragma unroll
       for (int o = 0; o < MP; ++o) v[o] = T(0);
@@ -332,7 +339,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
       gmm[o] = gp2;                                   // reuse as the value written to the record
     }
     if (pair_exists) {
-      T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
+      T* r = a.rec + rec_index<KNN, BLK>(s, b, s.N, J, i, sidx) * a.rl.R;
 #pragma unroll
       for (int o = 0; o < MP; ++o) r[a.rl.gpre2 + o] = gmm[o];
       r[a.rl.coef] = coef;
@@ -418,20 +425,20 @@ inline size_t bwd2_knn_smem_bytes(const Dims& s, int R) {
   return round_up(n * sizeof(T), 16) + 4 * BW2_PB * sizeof(int) + 16;
 }
 
-template <typename T, int MP, int QR, bool DROP>
+template <typename T, int MP, int QR, bool DROP, bool BLK>
 __global__ void __launch_bounds__(BW2_TH)
 pair_bwd2_knn_kernel(const BwdArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const Dims& s = a.s;
   const int tid = threadIdx.x, lane = tid & 31;
   const int b = blockIdx.z;
-  const int i0 = blockIdx.x * a.TI2;
+  const int i0 = rows_begin<BLK>(s) + blockIdx.x * a.TI2;
   const int h0 = blockIdx.y * BW2_TH;
   const int hh = h0 + tid;
   const bool hv = hh < s.Hp;
   const int N = s.N, R = a.rl.R, Q = s.Q, k = s.k;
   const int NL = s.label_dim > 0 ? s.num_labels : 0;
-  const int nrows = min(a.TI2, N - i0);
+  const int nrows = min(a.TI2, (BLK ? s.row1 : N) - i0);
   const int nch = ceil_div(k, BW2_PB);
   const int nsteps = nrows * nch;
 
@@ -475,7 +482,7 @@ pair_bwd2_knn_kernel(const BwdArgs<T> a) {
   auto prefetch = [&](int t, int buf) {
     const int row = t / nch, c0 = (t % nch) * BW2_PB, kc = min(BW2_PB, k - c0);
     const size_t node = (size_t)b * N + i0 + row;
-    const T* src = a.rec + rec_index<true>(b, N, k, i0 + row, c0) * R;
+    const T* src = a.rec + rec_index<true, BLK>(s, b, N, k, i0 + row, c0) * R;
     T* dst = recs + buf * BW2_PB * R;
     for (int x = tid; x < kc * R; x += BW2_TH) cp_async_elem(dst + x, src + x);
     if (tid < BW2_PB) {
@@ -594,7 +601,7 @@ pair_bwd2_knn_kernel(const BwdArgs<T> a) {
         }
         v += shfl_xor_t<T>(v, 1);
         v += shfl_xor_t<T>(v, 2);
-        if (qt == 0 && live) atomic_add_t<T>(a.rec + rec_index<true>(b, N, k, i0 + row, c0 + p) * R + a.rl.gf + q, v);
+        if (qt == 0 && live) atomic_add_t<T>(a.rec + rec_index<true, BLK>(s, b, N, k, i0 + row, c0 + p) * R + a.rl.gf + q, v);
       }
     }
     cp_async_wait_all();
@@ -640,20 +647,20 @@ inline size_t bwd2_dense_smem_bytes(const Dims& s, int R) {
   return round_up(n * sizeof(T), 16) + 2 * BW2_ROWS * sizeof(int) + 16;
 }
 
-template <typename T, int MP, int QR, bool DROP>
+template <typename T, int MP, int QR, bool DROP, bool BLK>
 __global__ void __launch_bounds__(BW2_TH)
 pair_bwd2_dense_kernel(const BwdArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const Dims& s = a.s;
   const int tid = threadIdx.x, lane = tid & 31;
   const int b = blockIdx.z;
-  const int i0 = blockIdx.x * BW2_ROWS;
+  const int i0 = rows_begin<BLK>(s) + blockIdx.x * BW2_ROWS;
   const int h0 = blockIdx.y * BW2_TH;
   const int hh = h0 + tid;
   const bool hv = hh < s.Hp;
   const int N = s.N, R = a.rl.R, Q = s.Q;
   const int NL = s.label_dim > 0 ? s.num_labels : 0;
-  const int nrows = min(BW2_ROWS, N - i0);
+  const int nrows = min(BW2_ROWS, (BLK ? s.row1 : N) - i0);
 
   T* As = reinterpret_cast<T*>(smem_raw);        // [32][128]
   T* wqs = As + BW2_ROWS * BW2_TH;               // [Q][128]
@@ -701,7 +708,7 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
   __syncthreads();
 
   auto prefetch = [&](int j, int buf) {
-    const T* src = a.rec + rec_index<false>(b, N, N, i0, j) * R;
+    const T* src = a.rec + rec_index<false, BLK>(s, b, N, N, i0, j) * R;
     T* dst = recs + buf * BW2_ROWS * R;
     for (int x = tid; x < nrows * R; x += BW2_TH) cp_async_elem(dst + x, src + x);
     if (!SIMPLE && NL && tid < nrows) labs[buf * BW2_ROWS + tid] = a.labels[((size_t)b * N + i0 + tid) * N + j];
@@ -800,7 +807,7 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
         }
         v += shfl_xor_t<T>(v, 1);
         v += shfl_xor_t<T>(v, 2);
-        if (qt == 0 && p < nrows) atomic_add_t<T>(a.rec + rec_index<false>(b, N, N, i0 + p, j) * R + a.rl.gf + q, v);
+        if (qt == 0 && p < nrows) atomic_add_t<T>(a.rec + rec_index<false, BLK>(s, b, N, N, i0 + p, j) * R + a.rl.gf + q, v);
       }
     }
     cp_async_wait_all();
@@ -830,7 +837,7 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
 // =====================================================================================
 // bwd3: dL/d(dist) -> coordinates and edges.  Same thread <-> pair mapping as bwd1.
 // =====================================================================================
-template <typename T, bool KNN>
+template <typename T, bool KNN, bool BLK>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd3_kernel(const BwdArgs<T> a) {
   const Dims& s = a.s;
@@ -838,9 +845,9 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
   const int TS = a.TS, TI = PAIR_THREADS / TS;
   const int g = tid / TS, sl = tid % TS;
   const int b = blockIdx.y;
-  const int i_raw = blockIdx.x * TI + g;
-  const bool row_valid = i_raw < s.N;
-  const int i = row_valid ? i_raw : 0;
+  const int i_raw = rows_begin<BLK>(s) + blockIdx.x * TI + g;
+  const bool row_valid = i_raw < rows_end<BLK>(s);
+  const int i = row_valid ? i_raw : rows_begin<BLK>(s);
   const int J = KNN ? s.k : s.N;
   const int qd = 2 * s.F;
   const size_t node_i = (size_t)b * s.N + i;
@@ -857,7 +864,7 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
     const PairSlot ps = pair_slot<KNN>(a.nbr_idx, nullptr, s.k, node_i, sidx, row_valid && sidx < J);
     if (!ps.valid) continue;
     const int j = ps.j;
-    const T* r = a.rec + rec_index<KNN>(b, s.N, J, i, sidx) * a.rl.R;
+    const T* r = a.rec + rec_index<KNN, BLK>(s, b, s.N, J, i, sidx) * a.rl.R;
     T rel[PAIR_CMAX];
     const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
     T gd = r[a.rl.gf + qd] + r[a.rl.gdn];
@@ -898,12 +905,17 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
 // =====================================================================================
 // Per-node pieces
 // =====================================================================================
+// Node rows of a row block (EGNN_FLAG_ROW_PARTIAL_GRADS) are addressed through a RowMap by the per-node backward
+// kernels; ACC_PLAIN keeps the plain row index (every row, in order).  For gemm_acc_kernel the map applies to the output
+// rows r of A and C (ACC_ROWS) or to the reduction index k of A and B (ACC_K).
+constexpr int ACC_PLAIN = 0, ACC_ROWS = 1, ACC_K = 2;
+
 // C[r, c] += sum_k A(r, k) B(k, c),  A(r,k) = A[r*ars + k*aks],  B(k,c) = B[k*bks + c*bcs]; K split over gridDim.z.
 // Always accumulates with atomics: the caller zero-fills C or wants the sum.
-template <typename T>
+template <typename T, int MAP>
 __global__ void __launch_bounds__(256)
 gemm_acc_kernel(const T* __restrict__ A, long ars, long aks, const T* __restrict__ Bm, long bks, long bcs,
-                T* __restrict__ Cm, long ldc, int Mr, int Nc, int K, int kper) {
+                T* __restrict__ Cm, long ldc, int Mr, int Nc, int K, int kper, RowMap map) {
   __shared__ T As[16][64 + 4];
   __shared__ T Bs[16][64 + 4];
   const int tid = threadIdx.x, tx = tid % 16, ty = tid / 16;
@@ -922,13 +934,20 @@ gemm_acc_kernel(const T* __restrict__ A, long ars, long aks, const T* __restrict
       {
         const int row = a_rows_fast ? idx % 64 : idx / 16, kk = a_rows_fast ? idx / 64 : idx % 16;
         T v = T(0);
-        if (m0 + row < Mr && k0 + kk < kend) v = A[(long)(m0 + row) * ars + (long)(k0 + kk) * aks];
+        if (m0 + row < Mr && k0 + kk < kend) {
+          const long ar = MAP == ACC_ROWS ? (long)map(m0 + row) : (long)(m0 + row);
+          const long ak = MAP == ACC_K ? (long)map(k0 + kk) : (long)(k0 + kk);
+          v = A[ar * ars + ak * aks];
+        }
         As[kk][row] = v;
       }
       {
         const int col = b_cols_fast ? idx % 64 : idx / 16, kk = b_cols_fast ? idx / 64 : idx % 16;
         T v = T(0);
-        if (n0 + col < Nc && k0 + kk < kend) v = Bm[(long)(k0 + kk) * bks + (long)(n0 + col) * bcs];
+        if (n0 + col < Nc && k0 + kk < kend) {
+          const long bk = MAP == ACC_K ? (long)map(k0 + kk) : (long)(k0 + kk);
+          v = Bm[bk * bks + (long)(n0 + col) * bcs];
+        }
         Bs[kk][col] = v;
       }
     }
@@ -949,22 +968,23 @@ gemm_acc_kernel(const T* __restrict__ A, long ars, long aks, const T* __restrict
   for (int i = 0; i < 4; ++i) {
     const int r = m0 + ty * 4 + i;
     if (r >= Mr) continue;
+    const long rr = MAP == ACC_ROWS ? (long)map(r) : (long)r;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
       const int c = n0 + tx * 4 + j;
-      if (c < Nc) atomic_add_t<T>(Cm + (long)r * ldc + c, acc[i][j]);
+      if (c < Nc) atomic_add_t<T>(Cm + rr * ldc + c, acc[i][j]);
     }
   }
 }
 
-// out[c] += sum_r X[r*ld + c]
-template <typename T>
-__global__ void colsum_acc_kernel(const T* __restrict__ X, long ld, int rows, int cols, T* __restrict__ out) {
+// out[c] += sum_r X[row(r)*ld + c], row(r) = map(r) when MAP, else r
+template <typename T, bool MAP>
+__global__ void colsum_acc_kernel(const T* __restrict__ X, long ld, int rows, int cols, T* __restrict__ out, RowMap map) {
   __shared__ T part[8][33];
   const int c = blockIdx.x * 32 + threadIdx.x;
   T s = T(0);
   if (c < cols)
-    for (int r = blockIdx.y * 8 + threadIdx.y; r < rows; r += gridDim.y * 8) s += X[(long)r * ld + c];
+    for (int r = blockIdx.y * 8 + threadIdx.y; r < rows; r += gridDim.y * 8) s += X[(MAP ? (long)map(r) : (long)r) * ld + c];
   part[threadIdx.y][threadIdx.x] = s;
   __syncthreads();
   if (threadIdx.y == 0 && c < cols) {
@@ -975,24 +995,27 @@ __global__ void colsum_acc_kernel(const T* __restrict__ X, long ld, int rows, in
   }
 }
 
-// g[x] = g[x] * silu'(drop(pre[x])) * drop'   (node_mlp: Linear -> Dropout -> SiLU, egnn_pytorch.py:197-199; x = row * cols + col
-// is the element index the forward GEMM epilogue hashed)
-template <typename T>
-__global__ void dsilu_mul_kernel(T* __restrict__ g, const T* __restrict__ pre, size_t n, DropCfg drop) {
+// g[e] = g[e] * silu'(drop(pre[e])) * drop'   (node_mlp: Linear -> Dropout -> SiLU, egnn_pytorch.py:197-199; e = row * cols + col
+// is the element index the forward GEMM epilogue hashed).  Element x of the n = rows * cols walked is e = x, or with MAP
+// the element of row map(x / cols).
+template <typename T, bool MAP>
+__global__ void dsilu_mul_kernel(T* __restrict__ g, const T* __restrict__ pre, size_t n, int cols, RowMap map, DropCfg drop) {
   for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < n; x += (size_t)gridDim.x * blockDim.x) {
-    T p = pre[x], f = T(1);
-    if (drop.thr) { f = (T)drop_mul(drop, 2u, (unsigned long long)x); p *= f; }
-    g[x] *= dsilu_from<T>(p, sigmoid_acc<T>(p)) * f;
+    const size_t e = MAP ? map((int)(x / cols)) * cols + x % cols : x;
+    T p = pre[e], f = T(1);
+    if (drop.thr) { f = (T)drop_mul(drop, 2u, (unsigned long long)e); p *= f; }
+    g[e] *= dsilu_from<T>(p, sigmoid_acc<T>(p)) * f;
   }
 }
 
-// LayerNorm backward (or identity) of the first `dim` columns of g_node_in, one warp per row:
+// LayerNorm backward (or identity) of the first `dim` columns of g_node_in, one warp per row (row map(r) with MAP):
 //   g_feats[row] += d(node_norm)/dh . g_normed;  gyx[row] = g_normed * xhat  (for dL/dgamma by column sum)
-template <typename T>
+template <typename T, bool MAP>
 __global__ void ln_bwd_kernel(const T* __restrict__ h, const T* __restrict__ gamma, const T* __restrict__ g_node_in,
-                              int ld_g, T* __restrict__ g_feats, T* __restrict__ gyx, int dim, int M, int do_norm) {
-  const int row = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
-  if (row >= M) return;
+                              int ld_g, T* __restrict__ g_feats, T* __restrict__ gyx, int dim, int M, int do_norm, RowMap map) {
+  const int r = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x % 32;
+  if (r >= M) return;
+  const size_t row = MAP ? map(r) : (size_t)r;
   const T* x = h + (size_t)row * dim;
   const T* gy = g_node_in + (size_t)row * ld_g;
   T* go = g_feats + (size_t)row * dim;

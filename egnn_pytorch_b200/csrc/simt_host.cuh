@@ -80,7 +80,8 @@ static int launch_simt(void (*kernel)(Arg), dim3 grid, int threads, size_t smem,
 template <typename T, int MP>
 static int launch_pair(const PairArgs<T>& a, cudaStream_t st) {
   dim3 grid(ceil_div(a.s.row1 - a.s.row0, PAIR_THREADS / a.TS), a.s.B);
-  return launch_simt(pair_kernel<T, MP>, grid, PAIR_THREADS, pair_smem_bytes<T>(a.s, a.L), st, a);
+  void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_kernel<T, MP, true> : pair_kernel<T, MP, false>;
+  return launch_simt(kernel, grid, PAIR_THREADS, pair_smem_bytes<T>(a.s, a.L), st, a);
 }
 
 // The dense edge step at PP rows per thread; a.hsplit > 1 runs it as two phases over a split hidden axis.
@@ -88,14 +89,15 @@ template <typename T, int MP, int PP>
 static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
   const size_t smem = pair_tiled_smem_bytes<T>(a.s, a.L, PP);
   dim3 grid(ceil_div(a.s.row1 - a.s.row0, 4 * PP), a.s.B);
-  if (a.hsplit > 1) {
+  if (a.hsplit > 1) {                                 // (all rows only: simt_hsplit)
     PairArgs<T> a1 = a, a2 = a;
     a1.phase = 1; a2.phase = 2;
     a1.pre2_out = nullptr;                            // partial sums; phase 2 holds the full ones
-    EGNN_TRY(launch_simt(pair_dense_tiled_kernel<T, MP, PP>, dim3(grid.x, grid.y, a.hsplit), PAIR_THREADS, smem, st, a1));
-    return launch_simt(pair_dense_tiled_kernel<T, MP, PP>, grid, PAIR_THREADS, smem, st, a2);
+    EGNN_TRY(launch_simt(pair_dense_tiled_kernel<T, MP, PP, false>, dim3(grid.x, grid.y, a.hsplit), PAIR_THREADS, smem, st, a1));
+    return launch_simt(pair_dense_tiled_kernel<T, MP, PP, false>, grid, PAIR_THREADS, smem, st, a2);
   }
-  return launch_simt(pair_dense_tiled_kernel<T, MP, PP>, grid, PAIR_THREADS, smem, st, a);
+  void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_dense_tiled_kernel<T, MP, PP, true> : pair_dense_tiled_kernel<T, MP, PP, false>;
+  return launch_simt(kernel, grid, PAIR_THREADS, smem, st, a);
 }
 
 // The dense edge step at two rows per thread where its shared memory fits, else at one (fp64 with m_dim > 16:

@@ -301,7 +301,8 @@ struct PairArgs {
   // tiny graphs only (pair_dense_tiled_kernel): the hidden axis is split over gridDim.z CTAs in phase 1, which
   // store partial m_pre sums to hpart [hsplit][B][N][N][MP]; phase 2 adds them up in a fixed order and finishes.
   T* hpart; int hsplit; int phase;      // phase 0 = single pass
-  T* pre2_out;                          // optional: [B,N,J][MP] W2 silu(pre1) per pair (J = N dense, k lists), kept for backward
+  T* pre2_out;                          // optional: [B,N,J][MP] W2 silu(pre1) per pair (J = N dense, k lists), kept for backward;
+                                        // rows by pair_row ([B,R,J][MP] for a row block under EGNN_FLAG_ROW_PARTIAL_GRADS)
   DropCfg drop;                         // training-mode dropout of edge_mlp / coors_mlp hidden pre-activations (thr 0 = off)
 };
 
@@ -406,7 +407,8 @@ inline size_t pair_smem_bytes(const Dims& s, const SimtPackLayout& L) {
 }
 
 // Neighbour lists: 128 threads per CTA arranged as TI row-groups x TS slots (TS lanes of one warp).
-template <typename T, int MP>
+// BLK: pre2_out is block-relative (pair_row).
+template <typename T, int MP, bool BLK>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -531,8 +533,8 @@ pair_kernel(const PairArgs<T> a) {
       }
     }
 
-    if (a.pre2_out && pair_valid) {                  // kept for backward: [B,N,k][MP]
-      T* dst = a.pre2_out + (node_i * s.k + sidx) * MP;
+    if (a.pre2_out && pair_valid) {                  // kept for backward: [B,N,k][MP] (rows of pair_row)
+      T* dst = a.pre2_out + ((BLK ? pair_row<true>(s, b, i) : node_i) * s.k + sidx) * MP;
 #pragma unroll
       for (int o = 0; o < MP; ++o) dst[o] = acc[o];
     }
@@ -599,7 +601,7 @@ inline size_t pair_tiled_smem_bytes(const Dims& s, const SimtPackLayout& L, int 
   return round_up(n * sizeof(T), 16) + 16;
 }
 
-template <typename T, int MP, int PP>
+template <typename T, int MP, int PP, bool BLK>     // BLK: pre2_out / hpart are block-relative (pair_row)
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_dense_tiled_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -763,8 +765,8 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
 #pragma unroll
       for (int p = 0; p < PP; ++p) {
         if (!(rvalid[p] && jv)) continue;
-        const size_t pair = ((size_t)b * s.N + irow[p]) * s.N + j;
-        const size_t stride = (size_t)s.B * s.N * s.N * MP;
+        const size_t pair = pair_row<BLK>(s, b, irow[p]) * s.N + j;    // (the backward's recompute of pre2 lands here)
+        const size_t stride = (size_t)s.B * (BLK ? s.row1 - s.row0 : s.N) * s.N * MP;
         if (a.phase == 1) {
 #pragma unroll
           for (int o = 0; o < MP; ++o) a.hpart[blockIdx.z * stride + pair * MP + o] = acc[p][o];
@@ -780,7 +782,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
 #pragma unroll
       for (int p = 0; p < PP; ++p) {
         if (!(rvalid[p] && jv)) continue;
-        T* dst = a.pre2_out + (((size_t)b * s.N + irow[p]) * s.N + j) * MP;
+        T* dst = a.pre2_out + (pair_row<BLK>(s, b, irow[p]) * s.N + j) * MP;
 #pragma unroll
         for (int o = 0; o < MP; ++o) dst[o] = acc[p][o];
       }

@@ -167,6 +167,13 @@ class _EGNNLayerFunction(torch.autograd.Function):
             nat.check("egnn_layer_backward",
                       lib.egnn_layer_backward(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]), C.byref(sv["io"]),
                                               _ptr(sv["ws"]), C.byref(grads), _ptr(ws), ws.numel(), stream))
+            if sv["rows"] is not None:
+                # a row block returns its inputs unchanged outside [r0, r1): the identity's gradient for those rows (the
+                # library's partial gradients cover the block's own outputs only)
+                r0, r1 = sv["rows"]
+                for g_in, g_out in ((g_feats, g_f), (g_coors, g_x)):
+                    g_in[:, :r0] += g_out[:, :r0]
+                    g_in[:, r1:] += g_out[:, r1:]
         ctx.saved = None
         back = lambda g, m: None if (g is None or m is None) else g.to(device=m[1], dtype=m[0])
         out = [None, back(g_feats, ctx.meta[0]), back(g_coors, ctx.meta[1]), back(g_edges, ctx.meta[2]),
@@ -327,13 +334,13 @@ class EGNN(nn.Module):
 
     def _forward_train(self, fields, feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
                        slot_edges=False):
-        if rows is not None:
-            raise NotImplementedError("a row range (_rows) cannot be differentiated: call it under torch.no_grad() for "
-                                      "inference, or shard the batch (parallel.batch_sharded_call) for training")
+        """With a row range (`_rows=(r0, r1)`) the layer is differentiated as the function it returns: rows r0:r1 are the
+        layer's output, every other row is its input unchanged.  The library's backward then yields this block's share
+        of every gradient (EGNN_FLAG_ROW_PARTIAL_GRADS): the blocks of a partition of the rows sum to the full gradient."""
         params = [p for _, _, _, p in fields]
 
         def run():
-            return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, None,
+            return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
                                       train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges)
 
         return _EGNNLayerFunction.apply(run, feats, coors, edges, label_emb, *params)
@@ -363,6 +370,8 @@ class EGNN(nn.Module):
         flags = self._flags()
         if slot_edges:
             flags |= nat.FLAG_EDGES_PER_SLOT
+        if train and _rows is not None:
+            flags |= nat.FLAG_ROW_PARTIAL_GRADS          # backward of the row block only; per-pair buffers sized by it
         nbr = None
         if neighbors is not None:
             assert neighbors.dim() == 3 and neighbors.shape[:2] == (b, n), "neighbors must be [B, N, k]"
@@ -420,12 +429,15 @@ class EGNN(nn.Module):
                 float(self.valid_radius), float(self.coor_weights_clamp_value or 0.0))
         cc = self._call_cache.get(ckey)
         if cc is None:
+            r_lo, r_hi = (0, 0) if rows is None else rows
+            if rows is not None and r_lo == r_hi:
+                r_lo = r_hi = n                          # an empty block (the descriptor's 0, 0 means all rows)
             desc = nat.LayerDesc(
                 abi_version=nat.ABI_VERSION, dtype=_KERNEL_DTYPE[kdt], B=b, N=n, C=c, dim=self.dim,
                 edge_dim=cont_edge_dim, label_dim=label_dim, num_labels=0 if label_emb is None else label_emb.shape[0],
                 m_dim=self.m_dim, fourier=self.fourier_features, k=k, flags=flags,
                 valid_radius=float(self.valid_radius), clamp=float(self.coor_weights_clamp_value or 0.0),
-                row_begin=0 if rows is None else rows[0], row_end=0 if rows is None else rows[1], reserved=0,
+                row_begin=r_lo, row_end=r_hi, reserved=0,
                 dropout_p=0.0, dropout_seed=0)
             nb = C.c_size_t()
             nat.check("egnn_layer_workspace_bytes", lib.egnn_layer_workspace_bytes(C.byref(desc), C.byref(nb)))
@@ -470,11 +482,13 @@ class EGNN(nn.Module):
                 f_out.copy_(f_in)
                 x_out.copy_(x_in)
             # training: keep the per-pair pre-activations of edge_mlp's second SiLU (64 B per pair in fp32) so
-            # that backward need not recompute them, unless that exceeds EGNN_B200_SAVE_PAIR_MB (default 1024)
+            # that backward need not recompute them, unless that exceeds EGNN_B200_SAVE_PAIR_MB (default 1024).  A row
+            # block keeps the pairs of its own rows only: [B, r1 - r0, J, MP]
             pre2 = None
             if train:
                 mp = 16 if self.m_dim <= 16 else 32
-                nbytes = b * n * (k if k > 0 else n) * mp * f_in.element_size()
+                n_rows = n if rows is None else rows[1] - rows[0]
+                nbytes = b * n_rows * (k if k > 0 else n) * mp * f_in.element_size()
                 if nbytes <= float(os.environ.get("EGNN_B200_SAVE_PAIR_MB", "1024")) * 2 ** 20:
                     pre2 = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             # the library reads EgnnLayerIO during the call only: inference re-fills one struct per layer, training
@@ -495,16 +509,17 @@ class EGNN(nn.Module):
                 nat.check("egnn_layer_backward_workspace_bytes", lib.egnn_layer_backward_workspace_bytes(C.byref(desc), C.byref(nbb)))
             # training keeps the workspace (per-node tables, pooled messages, neighbour lists) for backward
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if train else _workspace(dev, ws_bytes, stream_handle)
-            nat.check("egnn_layer_forward",
-                      lib.egnn_layer_forward(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io), _ptr(ws),
-                                             ws.numel(), stream))
+            if train or rows is None or rows[0] != rows[1]:      # an empty row block computes nothing in inference
+                nat.check("egnn_layer_forward",
+                          lib.egnn_layer_forward(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io), _ptr(ws),
+                                                 ws.numel(), stream))
         object.__setattr__(self, "last_path", _PATH_NAME[kdt])
         outs = (f_out if (f_out.dtype == feats.dtype and f_out.device == feats.device) else f_out.to(device=feats.device, dtype=feats.dtype),
                 x_out if (x_out.dtype == coors.dtype and x_out.device == coors.device) else x_out.to(device=coors.device, dtype=coors.dtype))
         if not train:
             return outs
         saved = dict(dev=dev, kdt=kdt, cdt=cdt, desc=desc, w=w, packed=packed, io=io, ws=ws, tensors=T,
-                     f_in=f_in, x_in=x_in, e_in=e_in, param_fields=param_fields,
+                     f_in=f_in, x_in=x_in, e_in=e_in, param_fields=param_fields, rows=rows,
                      keep=(m_in, l_in, adj_u8, nbr, lab_w, pre2))      # everything io points at stays alive
         return outs + (saved,)
 

@@ -11,6 +11,10 @@ the plumbing.
 * Training on batch shards: every rank differentiates the loss of its own graphs; the parameter gradients are
   the only thing exchanged -- `allreduce_gradients` sums them in a few flat buckets (one collective per
   bucket: the whole EGNN(512) layer is 12.8 MB in fp32, i.e. one launch-latency-bound all-reduce over NVLink).
+* Training on row shards of one graph: the gather is differentiable.  Its backward all-reduces (sums) the
+  full-size gradient of [coors | feats] and keeps this rank's rows; each rank's layer backward covers its own
+  row block only (EGNN_FLAG_ROW_PARTIAL_GRADS, per-pair memory ~ rows / world), so the parameter gradients are
+  partial sums that the same `allreduce_gradients` completes.
 
 The compute callable is injected, so the partition/exchange logic is testable on CPU with gloo
 (tests/test_multi_rank_cpu.py drives it with the oracle); on the GPU box it is the CUDA module.
@@ -74,19 +78,45 @@ def batch_sharded_call(fn, tensors: dict, batch: int, gather: bool = True, group
     return tuple(_all_gather_var(o, sizes, group) for o in outs)
 
 
+class _GatherRows(torch.autograd.Function):
+    """All-gather of the per-rank row blocks along dim 0.  Every rank's rows feed every rank's layer (as neighbours j),
+    so the gradient of a rank's block is the SUM over ranks of the gradient of the gathered array, taken at the block's
+    rows: one all-reduce of the full-size gradient, then a slice (gloo has no reduce-scatter; the payload is only
+    N x (C + dim)).  Every rank must run its backward: the all-reduce is a collective."""
+
+    @staticmethod
+    def forward(ctx, local, sizes, rank, group):
+        ctx.sizes, ctx.rank, ctx.group = sizes, rank, group
+        return _all_gather_var(local, sizes, group)
+
+    @staticmethod
+    def backward(ctx, g):
+        g = g.clone(memory_format=torch.contiguous_format)
+        dist.all_reduce(g, op=dist.ReduceOp.SUM, group=ctx.group)
+        r0 = sum(ctx.sizes[:ctx.rank])
+        return g[r0:r0 + ctx.sizes[ctx.rank]], None, None, None
+
+
 def row_sharded_layer_call(layer_fn, feats_local, coors_local, n_total: int, group=None, **kw):
     """One layer of a row-sharded single graph.
 
     feats_local [B, R_rank, dim], coors_local [B, R_rank, C] hold this rank's node block.  The single
     exchange step all-gathers both along the node axis; `layer_fn(feats_all, coors_all, rows=(r0, r1), **kw)`
-    must return full-size outputs of which only rows r0:r1 are meaningful.  Returns the local blocks."""
+    must return full-size outputs of which only rows r0:r1 are meaningful.  Returns the local blocks.
+
+    Training: the call is differentiable.  `layer_fn` must differentiate as the function it returns (an `EGNN` called
+    with `_rows=` does), and the gather's backward sums the gradient of the gathered array over the ranks and hands each
+    rank its own rows, so gradients reach `feats_local` / `coors_local` and layers chain.  After `loss.backward()` every
+    rank holds its block's PARTIAL sum of each parameter gradient: `allreduce_gradients(params)` (sum, not average)
+    completes them.  With dropout, every rank must draw the same per-call seed (e.g. the same `torch.manual_seed` on
+    every rank): the masks are keyed on global pair indices, so the sharded step then equals the single-GPU step."""
     rank, world = dist.get_rank(group), dist.get_world_size(group)
     sizes = [shard_range(n_total, r, world)[1] - shard_range(n_total, r, world)[0] for r in range(world)]
     r0, r1 = shard_range(n_total, rank, world)
     # one payload: [coors | feats] along the channel axis, node axis first for the gather
     wide = torch.promote_types(coors_local.dtype, feats_local.dtype)      # bf16 feats ride in fp32: exact
     payload = torch.cat([coors_local.to(wide), feats_local.to(wide)], dim=-1).transpose(0, 1).contiguous()
-    full = _all_gather_var(payload, sizes, group).transpose(0, 1)
+    full = _GatherRows.apply(payload, sizes, rank, group).transpose(0, 1)
     c = coors_local.shape[-1]
     coors_all = full[..., :c].to(coors_local.dtype).contiguous()
     feats_all = full[..., c:].to(feats_local.dtype).contiguous()
@@ -190,19 +220,15 @@ def row_payload_layout(n_total: int, c: int, dim: int, feat_bytes: int, batch: i
     return feats_off, feats_off + batch * n_total * dim * feat_bytes
 
 
-def row_sharded_layer_peer(comm: PeerComm, layer, feats_local, coors_local, n_total: int, **kw):
-    """One layer of a row-sharded single graph with the peer-memory all-gather.
-
-    feats_local [B, R_rank, dim] (module dtype), coors_local [B, R_rank, C] float32: this rank's node block (rows
-    `shard_range(n_total, rank, world)`).  Pushes both into every rank's gather buffer (one kernel, NVLink), then runs
-    `layer(feats_all, coors_all, _rows=(r0, r1), **kw)` on the gathered arrays.  Returns the local output blocks."""
+def _peer_gather(comm: PeerComm, feats_local, coors_local, n_total: int):
+    """-> (feats_all, coors_all): views of the communicator's gather buffer, valid until the call after next."""
     dev = feats_local.device
     b, _, dim = feats_local.shape
     c = coors_local.shape[-1]
-    r0, r1 = shard_range(n_total, comm.rank, comm.world)
+    r0, _ = shard_range(n_total, comm.rank, comm.world)
     feats_off, total = row_payload_layout(n_total, c, dim, feats_local.element_size(), b)
     assert total <= comm.payload_bytes, "PeerComm payload too small for this graph"
-    coors_local = coors_local.float().contiguous()
+    coors_local = coors_local.contiguous()
     feats_local = feats_local.contiguous()
     segs = []
     for g in range(b):            # rows of one graph are contiguous in both the local block and the gathered array
@@ -211,6 +237,49 @@ def row_sharded_layer_peer(comm: PeerComm, layer, feats_local, coors_local, n_to
     buf = comm.allgather(segs, dev)
     coors_all = buf[:b * n_total * c * 4].view(torch.float32).view(b, n_total, c)
     feats_all = buf[feats_off:total].view(feats_local.dtype).view(b, n_total, dim)
+    return feats_all, coors_all
+
+
+class _PeerGatherRows(torch.autograd.Function):
+    """The peer-memory all-gather under autograd.  The gathered arrays are copied out of the communicator's buffer into
+    tensors torch owns: the layer saves its inputs for backward, and the buffer is rewritten by the call after next --
+    raw memory whose reuse the saved-tensor version check cannot see.  Backward as `_GatherRows`: one all-reduce (sum) of
+    the full-size gradients over `comm.group`, then this rank's rows."""
+
+    @staticmethod
+    def forward(ctx, feats_local, coors_local, comm, n_total):
+        ctx.group, ctx.rows = comm.group, shard_range(n_total, comm.rank, comm.world)
+        feats_all, coors_all = _peer_gather(comm, feats_local, coors_local, n_total)
+        return feats_all.clone(), coors_all.clone()
+
+    @staticmethod
+    def backward(ctx, g_f, g_x):
+        wide = torch.promote_types(g_x.dtype, g_f.dtype)
+        flat = torch.cat([g_x.to(wide).reshape(-1), g_f.to(wide).reshape(-1)])
+        dist.all_reduce(flat, op=dist.ReduceOp.SUM, group=ctx.group)
+        g_x_all = flat[:g_x.numel()].view(g_x.shape)
+        g_f_all = flat[g_x.numel():].view(g_f.shape)
+        r0, r1 = ctx.rows
+        return g_f_all[:, r0:r1].to(g_f.dtype), g_x_all[:, r0:r1].to(g_x.dtype), None, None
+
+
+def row_sharded_layer_peer(comm: PeerComm, layer, feats_local, coors_local, n_total: int, **kw):
+    """One layer of a row-sharded single graph with the peer-memory all-gather.
+
+    feats_local [B, R_rank, dim] (module dtype), coors_local [B, R_rank, C] float32: this rank's node block (rows
+    `shard_range(n_total, rank, world)`).  Pushes both into every rank's gather buffer (one kernel, NVLink), then runs
+    `layer(feats_all, coors_all, _rows=(r0, r1), **kw)` on the gathered arrays.  Returns the local output blocks.
+
+    Under `torch.no_grad()` the layer reads the gathered arrays in place.  With grad mode on they are copied into tensors
+    torch owns (the layer may save them for backward), and the call differentiates like `row_sharded_layer_call`: gradients
+    reach `feats_local` / `coors_local`, and `allreduce_gradients` (sum) completes the parameter gradients."""
+    r0, r1 = shard_range(n_total, comm.rank, comm.world)
+    coors_local = coors_local.float()
+    # under grad the layer may save its inputs whatever `layer` is (a module, a lambda around one, ...): always copy
+    if torch.is_grad_enabled():
+        feats_all, coors_all = _PeerGatherRows.apply(feats_local, coors_local, comm, n_total)
+    else:
+        feats_all, coors_all = _peer_gather(comm, feats_local, coors_local, n_total)
     f_out, x_out = layer(feats_all, coors_all, _rows=(r0, r1), **kw)
     return f_out[:, r0:r1], x_out[:, r0:r1]
 

@@ -30,7 +30,12 @@ extern "C" {
 
 #define EGNN_ABI_VERSION 4   /* 2: EgnnLayerIO grew nbr_idx + pre2_out; backward entry points added
                                 3: peer-memory all-gather communicator (egnn_comm_*), egnn_global_attn_*
-                                4: EGNN_FLAG_EDGES_PER_SLOT (io.edges / g_edges per neighbour slot) */
+                                4: EGNN_FLAG_EDGES_PER_SLOT (io.edges / g_edges per neighbour slot);
+                                   EGNN_FLAG_ROW_PARTIAL_GRADS (backward of a row block) added later as one more flag bit,
+                                   the descriptor unchanged.  A version-4 library that predates it ignores the bit, and its
+                                   backward preflight (egnn_layer_backward_workspace_bytes, which a training caller runs
+                                   before the forward) still rejects the row range with EGNN_ERR_UNSUPPORTED: a mismatch
+                                   fails loudly before anything is written into block-sized buffers */
 
 /* ---- error codes ------------------------------------------------------------------- */
 #define EGNN_OK                 0
@@ -62,6 +67,11 @@ extern "C" {
                                                io.nbr_idx: slot s of row i holds edge nbr_idx[b,i,s] -> i.  Needs
                                                k > 0 and edge_dim > 0 (else EGNN_ERR_SHAPE) and io.nbr_idx != NULL
                                                (EGNN_ERR_SHAPE from egnn_layer_forward / egnn_layer_backward) */
+#define EGNN_FLAG_ROW_PARTIAL_GRADS (1u << 10) /* training of a row block [row_begin, row_end) (row-sharded graphs): pass the
+                                               same desc to egnn_layer_forward and egnn_layer_backward.  io.pre2_out and the
+                                               backward's per-pair buffers are sized by the block, [B, R, J, *] with
+                                               R = row_end - row_begin; egnn_layer_backward returns the gradient of
+                                               sum_{b, i in block} <g_out[b,i], out[b,i]>.  See EgnnLayerGrads */
 
 /*
  * Static description of one layer call.  E = 2*dim + 2*fourier + 1 + edge_dim + label_dim
@@ -141,7 +151,8 @@ typedef struct EgnnLayerIO {
                                 and MP = 16 when m_dim <= 16, else 32.  egnn_layer_forward stores the per-pair
                                 pre-activation of edge_mlp's second SiLU there; egnn_layer_backward, given the same
                                 pointer, skips recomputing it -- a speed / memory trade (64 B per pair in fp32).
-                                NULL = nothing stored, backward recomputes. */
+                                NULL = nothing stored, backward recomputes.  Under EGNN_FLAG_ROW_PARTIAL_GRADS
+                                [B, R, J, MP]: the pairs of rows [row_begin, row_end) only, row i at i - row_begin. */
 } EgnnLayerIO;
 
 int         egnn_abi_version(void);
@@ -175,9 +186,17 @@ int egnn_layer_forward_host(const EgnnLayerDesc* desc, const EgnnLayerWeights* w
 /*
  * Backward of one layer (SURVEY.md section 8(f) rank 1): what autograd computes through the reference's
  * EGNN.forward (egnn_pytorch.py:224-341).  fp32 / fp64 kernels only (EGNN_ERR_UNSUPPORTED for bf16 and for a row
- * range).  The edge step is recomputed pair by pair, so the only saved state is the forward WORKSPACE:
- * `fwd_workspace` must be the buffer egnn_layer_forward ran on with the same desc / io, unmodified since.
- * Gradient buffers are OVERWRITTEN (not accumulated into).  Neighbour selection contributes no gradient.
+ * range without EGNN_FLAG_ROW_PARTIAL_GRADS).  The edge step is recomputed pair by pair, so the only saved state is
+ * the forward WORKSPACE: `fwd_workspace` must be the buffer egnn_layer_forward ran on with the same desc / io,
+ * unmodified since.  Gradient buffers are OVERWRITTEN (not accumulated into).  Neighbour selection contributes no
+ * gradient.
+ *
+ * Row blocks (EGNN_FLAG_ROW_PARTIAL_GRADS with a row range): the gradient of sum_{b, i in [row_begin, row_end)}
+ * <g_out[b,i], out[b,i]>.  Only the block's rows of g_feats_out / g_coors_out are read.  g_feats, g_coors, g_edges and
+ * every weight gradient keep their full shapes and hold this block's contribution: the block's own rows (residual,
+ * node update, dL/dA_i), the neighbour-side terms of every row j (dL/dB_j, dL/dx_j, edges), 0 where there are none.
+ * Summed over the blocks of a partition of the rows they give the gradient of the whole layer.  Dropout masks are keyed
+ * on global indices, so the blocks see the masks of the whole-graph call with the same seed.
  */
 typedef struct EgnnLayerWeightGrads {   /* one buffer per EgnnLayerWeights field, same shape and dtype; NULL for
                                            modules the flags disable */
