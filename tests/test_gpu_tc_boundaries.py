@@ -1,0 +1,531 @@
+"""Tile and schedule boundaries of the bf16 tensor-core layer, against a rounding-matched reference.
+
+The fp64 oracle gate of test_gpu_fast.py (1e-2 of the output scale) has to allow for every bf16 rounding of the
+kernels, so it cannot see errors of that size in the edge kernels.  tests/tc_reference.py rounds where the kernels
+round; what is left between it and a correct kernel is tanh.approx, fp32 arithmetic and bf16 rounding-boundary flips,
+so the gates below can be two orders of magnitude tighter on the coordinate output.
+
+The case table crosses the boundaries of the launch code (fast_path.cu, tc_pair.cuh, tc_knn.cuh, small_node.cuh),
+mirrored in `geometry` and held there by test_table_covers_every_boundary:
+  tc_pair   j-split 1 / 2 / 4 / 8 (full graphs and row ranges); one active warpgroup (N <= 128); partial and empty
+            warpgroup tiles (N = 127 / 128 / 129 / 255 / 256 / 257); 1..3 valid rows in the last row group, at graph
+            ends and at row-range ends; ring reuse (more than 2 items per CTA, odd laps); last hidden chunk of 1..4 K
+            slabs; batches (the last graph reads B' into the table's pad rows); the generic instantiation at its
+            limits (Q = 12 per-pair channels, C = 8) with fourier features, edges and degree labels through EGNN_Network;
+            padded, random and fully masked graphs; mean pooling, clamp, soft edges, CoorsNorm
+  tc_knn    k = 1 / 8 / 31 / 32; the lean, edges and generic instantiations at 8 and 16 rows per CTA, each with a
+            partial last CTA; caller lists with -1 slots (mean without a mask too); per-slot edges; row ranges
+  node path small-node kernels (dim <= 64, B*N <= 4096), tc_gemm tables at dim <= 64 with B*N > 4096, dim > 64
+Every case uses xavier weights, so that the coordinate update is O(1) and the messages move the features
+(test_every_case_sees_the_edge_kernel checks that on the reference).
+
+Gates against the rounding-matched reference, per case (measured: the worst value over the table on an H100 80GB HBM3;
+each tolerance is about 4x that, `TOL`):
+  feats   max and mean |error| in bf16 ulps of the reference value (ulps below 1 % of the tensor's scale are
+          counted at that floor)
+  coors   per row: max |error| over the row / that row's update; over all rows: RMS error / RMS update
+plus the gate of test_gpu_fast.py against the fp64 oracle.  Large cases compare row windows (`check`) that include
+the first and last rows of every graph and of the range."""
+import functools
+
+import numpy as np
+import pytest
+import torch
+
+import cases
+import tc_reference as T
+import util
+from oracle import egnn_oracle as O
+
+L, NW = "layer", "network"
+
+# Worst value over the table, measured on an H100 80GB HBM3 (700 W power limit), and the tolerance: 4x that.
+#   f_ulp_max   33      (k8_edges8_slot: values near the 1 % floor)      -> 132
+#   f_ulp_mean  0.0645  (k32_lean16)                                      -> 0.26
+#   c_row       2.0e-3  (p_n256)                                          -> 8e-3
+#   c_rms       9.1e-5  (k8_gemm_tables)                                  -> 3.6e-4
+# For scale: packing the hidden values with round-toward-zero instead of round-to-nearest gives f_ulp_mean 0.1 - 1.6,
+# c_row 1e-3 - 0.28 and c_rms 3e-4 - 7e-3 over the same table.
+TOL = dict(f_ulp_max=132.0, f_ulp_mean=0.26, c_row=8e-3, c_rms=3.6e-4)
+
+CASES = {
+    # ---------------- dense all-pairs (tc_pair_kernel)
+    # j-split 1, 7 items on the first CTAs (ring slots reused, odd laps), padded graphs
+    "p_js1_ring":      dict(kind=L, cfg=dict(dim=16), B=5, N=700, seed=401, mask="padded",
+                            check=[(0, 8), (344, 352), (690, 700)]),
+    # j-split 2, 1 valid row in the last row group, 3-slab tail chunk, random mask
+    "p_js2_n701":      dict(kind=L, cfg=dict(dim=24, soft_edges=True), B=2, N=701, seed=402, mask="random",
+                            check=[(0, 8), (400, 404), (693, 701)]),
+    # j-split 4 over a whole graph; generic instantiation (fourier + edges, Q = 9), 2-slab tail chunk
+    "p_js4_full":      dict(kind=L, cfg=dict(dim=16, fourier_features=2, edge_dim=4), B=1, N=1100, seed=403,
+                            check=[(0, 8), (548, 556), (1092, 1100)]),
+    # j-split 4 on a row range ending with 3 valid rows; 4-slab last chunk (Hp = 128); two graphs
+    "p_js4_range":     dict(kind=L, cfg=dict(dim=24, fourier_features=2, edge_dim=4, norm_coors=True), B=2, N=1024,
+                            seed=404, rows=(0, 63), mask="padded"),
+    # j-split 8 on a row range ending with 1 valid row
+    "p_js8_range":     dict(kind=L, cfg=dict(dim=16, coor_weights_clamp_value=2.0), B=1, N=2048, seed=405, rows=(5, 34)),
+    # one active warpgroup; mean over a mask with one fully masked graph
+    "p_n100_empty":    dict(kind=L, cfg=dict(dim=64, m_pool_method="mean"), B=3, N=100, seed=406, mask="one_empty"),
+    # warpgroup tiles: partial (127, 255), exactly full (128, 256), one pair in the second tile (129) / the next block (257)
+    "p_n127_clamp":    dict(kind=L, cfg=dict(dim=32, coor_weights_clamp_value=0.3), B=2, N=127, seed=407),
+    "p_n128_soft":     dict(kind=L, cfg=dict(dim=32, soft_edges=True), B=2, N=128, seed=408, mask="random"),
+    "p_n129_norm":     dict(kind=L, cfg=dict(dim=32, norm_coors=True), B=2, N=129, seed=409),
+    "p_n255_mean":     dict(kind=L, cfg=dict(dim=40, m_pool_method="mean"), B=2, N=255, seed=410),
+    "p_n256":          dict(kind=L, cfg=dict(dim=48), B=2, N=256, seed=411, mask="padded"),
+    "p_n257_rows":     dict(kind=L, cfg=dict(dim=32, edge_dim=2), B=3, N=257, seed=412, rows=(97, 257)),
+    # GEMM node path and GEMM tables (dim > 64), 2 valid rows in the last row group
+    "p_d72_n258":      dict(kind=L, cfg=dict(dim=72, norm_feats=True, m_pool_method="mean"), B=2, N=258, seed=413,
+                            mask="padded"),
+    # GEMM tables at dim <= 64 (B*N > 4096) with the small node kernels
+    "p_gemm_tables":   dict(kind=L, cfg=dict(dim=32), B=3, N=1400, seed=414, check=[(0, 4), (700, 704), (1396, 1400)]),
+    # generic instantiation at its limits: C = 8, and Q = 12 (d, 2 x 2 fourier, 3 edges, 4 degree labels)
+    "p_c8_mean_clamp": dict(kind=L, cfg=dict(dim=32, fourier_features=3, m_pool_method="mean",
+                                             coor_weights_clamp_value=1.0), B=2, N=90, C=8, seed=415, mask="random"),
+    "p_net_q12_c8":    dict(kind=NW, cfg=dict(depth=1, dim=16, fourier_features=2, edge_dim=3, num_adj_degrees=3,
+                                              adj_dim=2, soft_edges=True), B=2, N=150, C=8, seed=416, adj="chain",
+                            edges=True, mask="padded"),
+    # ---------------- neighbour lists (tc_knn_kernel), caller-supplied lists
+    "k1_lean8":        dict(kind=L, cfg=dict(dim=32), B=2, N=203, k=1, seed=420),
+    "k8_edges8_slot":  dict(kind=L, cfg=dict(dim=64, edge_dim=4), B=2, N=150, k=8, seed=421, holes=True,
+                            slot_edges=True, mask="padded"),
+    "k31_gen8_mean":   dict(kind=L, cfg=dict(dim=32, fourier_features=2, m_pool_method="mean"), B=2, N=100, k=31,
+                            seed=422, holes=True),
+    "k8_gen8_c5":      dict(kind=L, cfg=dict(dim=32, edge_dim=2, soft_edges=True, norm_coors=True), B=2, N=77, C=5,
+                            k=8, seed=423, mask="random"),
+    "k32_lean16":      dict(kind=L, cfg=dict(dim=344, coor_weights_clamp_value=3.0), B=1, N=150, k=32, seed=424,
+                            holes=True),
+    "k32_edges16":     dict(kind=L, cfg=dict(dim=280, edge_dim=4), B=1, N=100, k=32, seed=425, holes=True,
+                            mask="random"),
+    "k31_gen16_rows":  dict(kind=L, cfg=dict(dim=264, fourier_features=2, edge_dim=1, m_pool_method="mean"), B=2, N=150,
+                            k=31, seed=426, holes=True, slot_edges=True, mask="padded", rows=(19, 140)),
+    "k32_d128_rows":   dict(kind=L, cfg=dict(dim=128, soft_edges=True), B=2, N=120, k=32, seed=427, rows=(3, 117)),
+    "k8_gemm_tables":  dict(kind=L, cfg=dict(dim=32, m_pool_method="mean"), B=1, N=5000, k=8, seed=428, holes=True,
+                            check=[(0, 16), (2500, 2516), (4990, 5000)]),
+}
+
+# ------------------------------------------------------------------ launch geometry (mirrors the launch code)
+
+H100_SMS = 132
+TP_TI, TP_JB, TP_KC, TP_JSPLIT_MAX, TP_QMAX, TP_CMAX = 4, 256, 64, 8, 12, 8
+TP_EPI_FLOATS = 64 * 16 + 64 + 64 + 16 + 16 + 4
+TK_QE, TK_LEAN, TK_EDGES, TK_GEN = 4, 0, 1, 2
+SN_DIM_MAX, SN_TABLES_M_MAX = 64, 4096
+SMEM_MAX = 227 * 1024
+
+
+def _ceil(a, b):
+    return -(-a // b)
+
+
+def _knn_smem(Hp, mode, Q, rows):
+    """tc_knn_smem_bytes (tc_knn.cuh)."""
+    wq_rows = 1 if mode == TK_LEAN else (1 + TK_QE if mode == TK_EDGES else Q)
+    n = Hp * 32 + rows * Hp * 4 + wq_rows * Hp * 4 + TP_EPI_FLOATS * 4
+    n += rows * Q * 32 * 4 if mode == TK_GEN else 0
+    return n + rows * 32 * 18 * 4 + 64 + 8 + 128
+
+
+def _pair_smem(Hp, Q, Qf, gen):
+    """tc_pair_smem_bytes (tc_pair.cuh)."""
+    PW, XC = (28, 8) if gen else (20, 4)
+    n = Hp * 32 + Q * Hp * 4 + 2 * TP_TI * Hp * 4 + TP_EPI_FLOATS * 4 + 2 * 8 * TP_TI * PW * 8 + 8 * 32 * 18 * 4
+    n += 2 * TP_TI * XC * 4 + 2 * TP_TI * 4 + 64 + (0 if gen else TP_TI * TP_JB * 4)
+    n += TP_TI * TP_JB * (Qf * 4 + (Q - Qf) * 2) if gen else 0
+    return n + 64 + 256
+
+
+def layer_shape(spec):
+    """(layer cfg, continuous edge channels, degree labels) of a case."""
+    if spec["kind"] == NW:
+        ncfg = O.network_cfg(**spec["cfg"])
+        cfg = ncfg["layer"]
+        nlab = ncfg["num_adj_degrees"] + 1 if ncfg["num_adj_degrees"] is not None and ncfg["adj_dim"] > 0 else 0
+        return cfg, cfg["edge_dim"] - (ncfg["adj_dim"] if nlab else 0), nlab, (ncfg["adj_dim"] if nlab else 0)
+    cfg = O.layer_cfg(**spec["cfg"])
+    return cfg, cfg["edge_dim"], 0, 0
+
+
+def geometry(spec, sms=H100_SMS):
+    """What the launch code (fast_path.cu) runs a case with."""
+    cfg, ed, nlab, label_dim = layer_shape(spec)
+    dim, F = cfg["dim"], cfg["fourier_features"]
+    B, N, C, k = spec["B"], spec["N"], spec.get("C", 3), spec.get("k", 0)
+    r0, r1 = spec.get("rows") or (0, N)
+    R = r1 - r0
+    E = 2 * dim + 1 + 2 * F + ed + label_dim
+    Hp = _ceil(2 * E, 16) * 16
+    QT = 1 + 2 * F + ed + nlab
+    nchunks = _ceil(Hp, TP_KC)
+    M = B * N
+    g = dict(dim=dim, B=B, N=N, C=C, k=k, R=R, Hp=Hp, Q=QT, F=F, edge_dim=ed, labels=nlab,
+             nsl_last=(Hp - (nchunks - 1) * TP_KC) // 16, rows_range=spec.get("rows") is not None,
+             tables="small" if dim <= SN_DIM_MAX and M <= SN_TABLES_M_MAX else "tc_gemm",
+             node="small" if dim <= SN_DIM_MAX else "tc_gemm")
+    if k == 0:
+        gen = not (C == 3 and QT == 1)
+        items = B * _ceil(R, TP_TI)
+        njb = _ceil(N, TP_JB)
+        js = 1
+        while js < TP_JSPLIT_MAX and items * js < 6 * sms and js * 2 <= njb:
+            js *= 2
+        n_items = items * js
+        grid = min(n_items, sms)
+        g.update(kernel="tc_pair<generic>" if gen else "tc_pair<lean>", jsplit=js, items=n_items, grid=grid,
+                 laps=_ceil(n_items, grid), active_wgs=min(2, _ceil(N, 128)),
+                 last_rows_valid=R - TP_TI * (_ceil(R, TP_TI) - 1),
+                 supported=QT <= TP_QMAX and C <= TP_CMAX and _pair_smem(Hp, QT, 1 + 2 * F, gen) <= SMEM_MAX)
+    else:
+        mode = TK_LEAN if ed == 0 else (TK_EDGES if ed <= TK_QE else TK_GEN)
+        if not (C == 3 and F == 0 and nlab == 0):
+            mode = TK_GEN
+        rows = 8 if 2 * (_knn_smem(Hp, mode, QT, 8) + 1024) <= SMEM_MAX else 16
+        g.update(kernel=f"tc_knn<{['LEAN', 'EDGES', 'GEN'][mode]},{rows}>", mode=mode, ROWS=rows,
+                 last_rows_valid=R - rows * (_ceil(R, rows) - 1),
+                 supported=k <= 32 and (mode != TK_GEN or QT <= TP_QMAX) and _knn_smem(Hp, mode, QT, 16) <= SMEM_MAX)
+    return g
+
+
+def test_table_covers_every_boundary():
+    """Each boundary the table is meant to reach, recomputed from the specs: an edit to a shape that drops one fails
+    here.  The SM count is the H100's 132, or the device's when one is present."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else H100_SMS
+    geo = {n: geometry(s, sms) for n, s in CASES.items()}
+    assert all(g["supported"] for g in geo.values()), [n for n, g in geo.items() if not g["supported"]]
+    pair = {n: g for n, g in geo.items() if g["k"] == 0}
+    knn = {n: g for n, g in geo.items() if g["k"] > 0}
+    want = {
+        "jsplit 1 / 2 / 4 / 8": {g["jsplit"] for g in pair.values()} >= {1, 2, 4, 8},
+        "jsplit 4 on a full graph": any(g["jsplit"] == 4 and not g["rows_range"] for g in pair.values()),
+        "jsplit 4 and 8 on row ranges": {g["jsplit"] for g in pair.values() if g["rows_range"]} >= {4, 8},
+        "one active warpgroup": any(g["active_wgs"] == 1 for g in pair.values()),
+        "N 127 / 128 / 129 / 255 / 256 / 257": {g["N"] for g in pair.values()} >= {127, 128, 129, 255, 256, 257},
+        "last row group 1 / 2 / 3 rows at a graph end": {g["last_rows_valid"] for g in pair.values()
+                                                         if not g["rows_range"]} >= {1, 2, 3},
+        "last row group 1 / 3 rows at a range end": {g["last_rows_valid"] for g in pair.values()
+                                                     if g["rows_range"]} >= {1, 3},
+        "ring reuse, odd laps": any(g["items"] > 2 * g["grid"] and g["laps"] % 2 == 1 for g in pair.values()),
+        "dense last chunk 1 / 2 / 3 / 4 slabs": {g["nsl_last"] for g in pair.values()} >= {1, 2, 3, 4},
+        "dense batches": any(g["B"] >= 2 and g["N"] % 128 != 0 for g in pair.values()),
+        "dense lean and generic": {g["kernel"] for g in pair.values()} == {"tc_pair<lean>", "tc_pair<generic>"},
+        "dense Q 12, C 8, labels": any(g["Q"] == TP_QMAX and g["C"] == TP_CMAX and g["labels"] > 0
+                                       for g in pair.values()),
+        "dense fourier and edges": any(g["F"] > 0 and g["edge_dim"] > 0 for g in pair.values()),
+        "knn k 1 / 8 / 31 / 32": {g["k"] for g in knn.values()} >= {1, 8, 31, 32},
+        "knn every instantiation at 8 and 16 rows": {g["kernel"] for g in knn.values()} >= {
+            f"tc_knn<{m},{r}>" for m in ("LEAN", "EDGES", "GEN") for r in (8, 16)},
+        "knn partial last CTA at 8 and 16 rows": {g["ROWS"] for g in knn.values() if g["last_rows_valid"] < g["ROWS"]}
+        == {8, 16},
+        "knn 16 rows with more than 8 valid rows": any(g["ROWS"] == 16 and g["R"] > 8 for g in knn.values()),
+        "knn row ranges": any(g["rows_range"] for g in knn.values()),
+        "small tables + small node": any(g["tables"] == "small" and g["node"] == "small" for g in geo.values()),
+        "tc_gemm tables at dim <= 64": any(g["tables"] == "tc_gemm" and g["dim"] <= 64 for g in geo.values())
+        and any(g["tables"] == "tc_gemm" and g["dim"] <= 64 for g in pair.values()),
+        "GEMM node path (dim > 64)": any(g["node"] == "tc_gemm" for g in pair.values())
+        and any(g["node"] == "tc_gemm" for g in knn.values()),
+    }
+    missing = [k for k, v in want.items() if not v]
+    assert not missing, missing
+    opts = [(s.get("mask"), s["cfg"]) for s in CASES.values()]
+    assert {m for m, _ in opts} >= {"padded", "random", "one_empty", None}
+    for key in ("soft_edges", "norm_coors", "coor_weights_clamp_value", "norm_feats"):
+        assert any(key in c for _, c in opts), key
+    assert any(c.get("m_pool_method") == "mean" and s.get("k") and not s.get("mask") for s in CASES.values()
+               for c in [s["cfg"]]), "mean over lists without a mask"
+    assert any(s.get("holes") for s in CASES.values()) and any(s.get("slot_edges") for s in CASES.values())
+
+
+# ------------------------------------------------------------------ inputs and the reference
+
+
+def _bf16(a):
+    return torch.from_numpy(np.asarray(a, np.float64)).float().bfloat16().double().numpy()
+
+
+@functools.lru_cache(maxsize=None)
+def build(name):
+    """The case with bf16 parameters / features / edges and fp32 coordinates, plus its neighbour lists."""
+    spec = CASES[name]
+    case = cases.build_case(dict({k: v for k, v in spec.items() if k not in ("check", "rows")}, init="xavier"))
+    ins = case["inputs"]
+    case["params"] = {k: _bf16(v) for k, v in case["params"].items()}
+    if np.issubdtype(np.asarray(ins["feats"]).dtype, np.floating):
+        ins["feats"] = _bf16(ins["feats"])
+    ins["coors"] = np.asarray(ins["coors"], np.float32).astype(np.float64)
+    if ins.get("edges") is not None and np.issubdtype(np.asarray(ins["edges"]).dtype, np.floating):
+        ins["edges"] = _bf16(ins["edges"])
+    k = spec.get("k", 0)
+    if k:
+        B, N = spec["B"], spec["N"]
+        rs = np.random.RandomState(spec["seed"] + 7)
+        if spec.get("slot_edges"):      # distinct neighbours per row: the oracle takes per-slot edges as [B, N, N, e]
+            nbr = rs.uniform(size=(B, N, N)).argsort(-1)[..., :k]
+        else:
+            nbr = rs.randint(0, N, (B, N, k))
+        if spec.get("holes"):
+            holes = rs.uniform(size=nbr.shape) < 0.2
+            holes[:, ::2, -1] = False                                   # the last slot stays in use on half the rows
+            nbr[holes] = -1
+        ins["neighbors"] = nbr
+        if spec.get("slot_edges"):
+            ins["edges"] = _bf16(rs.standard_normal((B, N, k, case["cfg"]["edge_dim"])))
+    return case
+
+
+def windows(name):
+    spec = CASES[name]
+    return spec.get("check") or [spec.get("rows") or (0, spec["N"])]
+
+
+def reference(name, rounding=True, messages=True):
+    """[(window, feats, coors)] of the reference over the case's check windows."""
+    case = build(name)
+    ins = case["inputs"]
+    if case["kind"] == NW:
+        assert messages
+        f, x = T.tc_network_forward(case["params"], case["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
+                                    ins.get("edges"), ins.get("mask"), rounding=rounding)
+        return [((0, CASES[name]["N"]), f, x)]
+    spec = CASES[name]
+    out = []
+    for w in windows(name):
+        f, x = T.tc_layer_forward(case["params"], case["cfg"], ins["feats"], ins["coors"], edges=ins.get("edges"),
+                                  mask=ins.get("mask"), neighbors=ins.get("neighbors"),
+                                  slot_edges=bool(spec.get("slot_edges")), rows=w, rounding=rounding,
+                                  messages=messages)
+        out.append((w, f, x))
+    return out
+
+
+@functools.lru_cache(maxsize=None)
+def reference_cached(name):
+    return reference(name)
+
+
+def oracle(name):
+    """[(window, feats, coors)] of the fp64 oracle over the same windows."""
+    case = build(name)
+    ins = case["inputs"]
+    if case["kind"] == NW:
+        f, x = cases.run_oracle(case)
+        return [((0, CASES[name]["N"]), f, x)]
+    if "neighbors" in ins:
+        e = ins.get("edges")
+        if CASES[name].get("slot_edges"):          # per-slot edges -> the dense [B, N, N, e] tensor the oracle takes
+            B, N, k = ins["neighbors"].shape
+            dense = np.zeros((B, N, N, e.shape[-1]))
+            b_, i_, s_ = np.nonzero(ins["neighbors"] >= 0)
+            dense[b_, i_, ins["neighbors"][b_, i_, s_]] = e[b_, i_, s_]      # (`build` draws these lists without repeats)
+            e = dense
+        f, x = O.egnn_layer_forward_edge_list(case["params"], case["cfg"], ins["feats"], ins["coors"], ins["neighbors"],
+                                              edges=e, mask=ins.get("mask"))
+        return [(w, f[:, w[0]:w[1]], x[:, w[0]:w[1]]) for w in windows(name)]
+    return [(w,) + tuple(O.egnn_layer_forward(case["params"], case["cfg"], ins["feats"], ins["coors"],
+                                              edges=ins.get("edges"), mask=ins.get("mask"), rows=w))
+            for w in windows(name)]
+
+
+def test_every_case_sees_the_edge_kernel():
+    """On the reference: the coordinate update of every case is O(0.1 - 1) per row or larger, and the messages move
+    the features by more than 2 % of their scale (several bf16 ulps), so an error in the edge kernel shows in both outputs."""
+    for name in CASES:
+        case = build(name)
+        x_in = case["inputs"]["coors"]
+        ref = reference_cached(name)
+        upd = np.concatenate([np.abs(x - x_in[:, w[0]:w[1]]).max(-1).ravel() for w, _, x in ref])
+        live = upd[upd > 0]
+        assert live.size > 0.5 * upd.size and np.median(live) > 0.1, (name, np.median(live) if live.size else 0)
+        if case["kind"] == NW:
+            continue
+        nomsg = reference(name, messages=False)
+        share = max(float(np.abs(f - f0).max() / np.abs(f).max()) for (_, f, _), (_, f0, _) in zip(ref, nomsg))
+        assert share > 0.02, (name, share)
+
+
+@pytest.mark.parametrize("name", ["p_js2_n701", "p_js4_range", "p_c8_mean_clamp", "k8_edges8_slot", "k31_gen16_rows"])
+def test_reference_rounding_stays_within_the_oracle_gate(name):
+    """The rounded reference is within the bf16 gate of test_gpu_fast.py of the fp64 oracle (it models the kernels'
+    rounding, not a different function)."""
+    for (w, f, x), (_, fo, xo) in zip(reference_cached(name), oracle(name)):
+        x_in = build(name)["inputs"]["coors"][:, w[0]:w[1]]
+        assert np.abs(f - fo).max() <= 1e-2 * np.abs(fo).max(), name
+        assert np.abs(x - xo).max() <= 1e-2 * max(np.abs(xo - x_in).max(), 1.0), name
+
+
+# ------------------------------------------------------------------ the reference pinned to the oracles (CPU)
+
+PIN_LAYER = ["dense_everything", "dense_c5", "dense_mean", "dense_clamp", "dense_soft_edges", "dense_norm_coors",
+             "dense_mask_random", "dense_no_feats", "dense_no_coors", "knn_edges_mask", "knn_radius_mask",
+             "knn_radius_nomask", "knn_mean_fourier", "knn_norm_coors", "knn_k32_c5", "adj_sparse_random"]
+PIN_NETWORK = ["net_adj_dense", "net_adj_degrees", "net_c5_xavier", "net_edge_tokens", "net_c3_xavier"]
+
+
+@pytest.mark.parametrize("name", PIN_LAYER + PIN_NETWORK)
+def test_unrounded_reference_equals_the_oracle(name):
+    c = cases.build_case(cases.SPECS[name])
+    ins = c["inputs"]
+    want = cases.run_oracle(c)
+    if c["kind"] == NW:
+        got = T.tc_network_forward(c["params"], c["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
+                                   ins.get("edges"), ins.get("mask"), rounding=False)
+    else:
+        cfg, nbr, ok = c["cfg"], None, None
+        if cfg["num_nearest_neighbors"] > 0 or cfg["only_sparse_neighbors"]:
+            nbr, ok, _ = O.neighbour_selection(cfg, ins["coors"], ins.get("mask"), ins.get("adj_mat"))
+        got = T.tc_layer_forward(c["params"], cfg, ins["feats"], ins["coors"], edges=ins.get("edges"),
+                                 mask=ins.get("mask"), neighbors=nbr, nbr_ok=ok, rounding=False)
+    for g, w in zip(got, want):
+        assert np.abs(g - w).max() <= 1e-12 * max(1.0, np.abs(w).max()), name
+
+
+@pytest.mark.parametrize("mean", [False, True])
+@pytest.mark.parametrize("masked", [False, True])
+def test_unrounded_reference_equals_the_edge_list_oracle(masked, mean):
+    """Caller lists with -1 slots and per-slot edges (edge-list mode) against oracle.egnn_layer_forward_edge_list."""
+    spec = dict(kind=L, cfg=dict(dim=16, edge_dim=2, fourier_features=1, soft_edges=True, norm_coors=True,
+                                 coor_weights_clamp_value=0.8, m_pool_method="mean" if mean else "sum"),
+                B=2, N=23, seed=430, init="xavier", mask="random" if masked else "none")
+    c = cases.build_case(spec)
+    ins = c["inputs"]
+    rs = np.random.RandomState(5)
+    k = 6
+    nbr = np.stack([np.stack([rs.permutation(23)[:k] for _ in range(23)]) for _ in range(2)])
+    nbr[rs.uniform(size=nbr.shape) < 0.25] = -1
+    slot = rs.standard_normal((2, 23, k, 2))
+    dense = np.zeros((2, 23, 23, 2))
+    b_, i_, s_ = np.nonzero(nbr >= 0)
+    dense[b_, i_, nbr[b_, i_, s_]] = slot[b_, i_, s_]
+    want = O.egnn_layer_forward_edge_list(c["params"], c["cfg"], ins["feats"], ins["coors"], nbr, edges=dense,
+                                          mask=ins.get("mask"))
+    for edges, per_slot in ((dense, False), (slot, True)):
+        got = T.tc_layer_forward(c["params"], c["cfg"], ins["feats"], ins["coors"], edges=edges, mask=ins.get("mask"),
+                                 neighbors=nbr, slot_edges=per_slot, rounding=False)
+        for g, w in zip(got, want):
+            assert np.abs(g - w).max() <= 1e-12 * max(1.0, np.abs(w).max())
+
+
+def test_rounded_reference_stays_within_the_oracle_gate_on_pinned_cases():
+    for name in ["dense_everything", "knn_edges_mask", "net_adj_dense"]:
+        c = cases.build_case(cases.SPECS[name])
+        c["params"] = {k: _bf16(v) for k, v in c["params"].items()}
+        ins = c["inputs"]
+        for key in ("feats", "coors", "edges"):
+            if ins.get(key) is not None and np.issubdtype(np.asarray(ins[key]).dtype, np.floating):
+                ins[key] = _bf16(ins[key])
+        want = cases.run_oracle(c)
+        if c["kind"] == NW:
+            got = T.tc_network_forward(c["params"], c["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
+                                       ins.get("edges"), ins.get("mask"))
+        else:
+            nbr, ok = None, None
+            if c["cfg"]["num_nearest_neighbors"] > 0:
+                nbr, ok, _ = O.neighbour_selection(c["cfg"], ins["coors"], ins.get("mask"), None)
+            got = T.tc_layer_forward(c["params"], c["cfg"], ins["feats"], ins["coors"], edges=ins.get("edges"),
+                                     mask=ins.get("mask"), neighbors=nbr, nbr_ok=ok)
+        assert np.abs(got[0] - want[0]).max() <= 1e-2 * np.abs(want[0]).max(), name
+        assert np.abs(got[1] - want[1]).max() <= 1e-2 * max(np.abs(want[1] - ins["coors"]).max(), 1.0), name
+
+
+# ------------------------------------------------------------------ the GPU runs
+
+
+def run_gpu(name, rows="spec"):
+    """Forward of the case on the bf16 path; -> (feats [B,N,dim] float64, coors [B,N,C] float64) as numpy."""
+    case = build(name)
+    spec = CASES[name]
+    ins = case["inputs"]
+    rows = spec.get("rows") if rows == "spec" else rows
+    mod = util.make_module(case, torch.bfloat16)
+    dev = "cuda"
+    coors = torch.from_numpy(ins["coors"]).float().to(dev)
+    mask = None if ins.get("mask") is None else torch.from_numpy(ins["mask"]).to(dev)
+    tb = lambda a: None if a is None else torch.from_numpy(np.asarray(a, np.float64)).to(dev, torch.bfloat16)
+    with torch.no_grad():
+        if case["kind"] == NW:
+            f, x = mod(torch.from_numpy(ins["feats"]).to(dev) if not np.issubdtype(ins["feats"].dtype, np.floating)
+                       else tb(ins["feats"]), coors, adj_mat=torch.from_numpy(ins["adj_mat"]).to(dev),
+                       edges=tb(ins.get("edges")), mask=mask)
+            layers = [l[1] for l in mod.layers]
+        else:
+            kw = dict(mask=mask, _rows=rows)
+            edges = tb(ins.get("edges"))
+            if "neighbors" in ins:
+                kw["neighbors"] = torch.from_numpy(ins["neighbors"]).to(dev)
+                if spec.get("slot_edges"):
+                    kw["neighbor_edges"], edges = edges, None
+            f, x = mod(tb(ins["feats"]), coors, edges, **kw)
+            layers = [mod]
+    assert all(l.last_path == "bf16-tc" for l in layers), name
+    assert f.dtype == torch.bfloat16 and x.dtype == torch.float32
+    return f, x
+
+
+def metrics(name, f, x):
+    """The four gate values of one GPU output against the rounding-matched reference."""
+    x_in = build(name)["inputs"]["coors"]
+    fu, fe, cr, ce, cu = [], [], [], [], []
+    for w, rf, rx in reference_cached(name):
+        gf = f[:, w[0]:w[1]].double().cpu().numpy()
+        gx = x[:, w[0]:w[1]].double().cpu().numpy()
+        floor = 1e-2 * np.abs(rf).max()
+        ulp = 2.0 ** (np.floor(np.log2(np.maximum(np.abs(rf), floor))) - 7)
+        fu.append((np.abs(gf - rf) / ulp).ravel())
+        upd = rx - x_in[:, w[0]:w[1]]
+        err = np.abs(gx - rx).max(-1)
+        row_upd = np.abs(upd).max(-1)
+        cr.append((err / np.maximum(row_upd, 1e-3 * np.abs(upd).max() + 1e-30)).ravel())
+        ce.append((gx - rx).ravel())
+        cu.append(upd.ravel())
+    fu, cr, ce, cu = (np.concatenate(a) for a in (fu, cr, ce, cu))
+    return dict(f_ulp_max=float(fu.max()), f_ulp_mean=float(fu.mean()), c_row=float(cr.max()),
+                c_rms=float(np.sqrt((ce ** 2).mean() / max((cu ** 2).mean(), 1e-300))))
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", list(CASES))
+def test_matches_rounding_matched_reference(name):
+    f, x = run_gpu(name)
+    assert np.isfinite(f.float().cpu().numpy()).all() and np.isfinite(x.cpu().numpy()).all()
+    m = metrics(name, f, x)
+    g = geometry(CASES[name], torch.cuda.get_device_properties(0).multi_processor_count)
+    sched = f"jsplit={g['jsplit']}" if g["k"] == 0 else f"ROWS={g['ROWS']}"
+    print(f"TCB {name} {g['kernel']} {sched} Hp={g['Hp']} nsl_last={g['nsl_last']} "
+          + " ".join(f"{k}={v:.3e}" for k, v in m.items()))
+    bad = {k: v for k, v in m.items() if not v <= TOL[k]}
+    assert not bad, (name, bad)
+    # ... and the gate of test_gpu_fast.py against the fp64 oracle
+    x_in = build(name)["inputs"]["coors"]
+    for w, of, ox in oracle(name):
+        gf = f[:, w[0]:w[1]].double().cpu().numpy()
+        gx = x[:, w[0]:w[1]].double().cpu().numpy()
+        assert np.abs(gf - of).max() <= 1e-2 * max(1e-3, np.abs(of).max()), name
+        assert np.abs(gx - ox).max() <= 1e-2 * max(np.abs(ox - x_in[:, w[0]:w[1]]).max(), 1.0), name
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,full_js", [("p_js8_range", 2), ("p_js4_range", 2)])
+def test_jsplit_row_range_is_bit_identical_to_the_full_forward(name, full_js):
+    """DESIGN's claim for the row-sharded dense kernel: the fp64 sums across tiles make the rows independent of how
+    the j-blocks were dealt, so a row range run at j-split 4 / 8 equals the full forward (j-split 1 / 2) bit for bit.
+    Two calls in a row are identical too: the j-split arrival counters are left at zero."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    spec = CASES[name]
+    r0, r1 = spec["rows"]
+    assert geometry(dict(spec, rows=None), sms)["jsplit"] == full_js and geometry(spec, sms)["jsplit"] > full_js
+    f_full, x_full = run_gpu(name, rows=None)
+    f1, x1 = run_gpu(name)
+    f2, x2 = run_gpu(name)
+    assert torch.equal(f1, f2) and torch.equal(x1, x2)
+    assert torch.equal(f1[:, r0:r1], f_full[:, r0:r1]) and torch.equal(x1[:, r0:r1], x_full[:, r0:r1])
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name", ["k32_lean16", "k31_gen16_rows"])
+def test_knn_16_rows_row_range_is_bit_identical(name):
+    """The 16-row neighbour-list kernel on a row range that starts off the CTA grid equals its full forward."""
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    assert geometry(CASES[name], sms)["ROWS"] == 16
+    n = CASES[name]["N"]
+    f_full, x_full = run_gpu(name, rows=None)
+    for r0, r1 in [(5, n - 3), (37, 38)]:
+        f, x = run_gpu(name, rows=(r0, r1))
+        assert torch.equal(f[:, r0:r1], f_full[:, r0:r1]) and torch.equal(x[:, r0:r1], x_full[:, r0:r1])
