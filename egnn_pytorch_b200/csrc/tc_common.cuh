@@ -133,12 +133,20 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a
 // lane may stand at mma positions (2 lq, 2 lq + 1 | 2 lq + 8, 2 lq + 9) as long as the B fragment uses the same order:
 // then B of lane (lr, lq) for output column n = 8 nt + lr is channels 4 lq .. 4 lq + 3 of W2 row n -- one 8-byte load
 // from the core-matrix packing of W2 (slab s at byte 512 s: [kc = k/8][nc = n/8][n % 8][k % 8]).
-__device__ __forceinline__ void mma_w2_slab(float (&acc)[2][4], const uint32_t (&h)[4], const unsigned char* w2s, int slab, int lr, int lq) {
+__device__ __forceinline__ void w2_slab_frag(uint2 (&bw)[2], const unsigned char* w2s, int slab, int lr, int lq) {
 #pragma unroll
-  for (int nt = 0; nt < 2; ++nt) {
-    const uint2 bw = *reinterpret_cast<const uint2*>(w2s + slab * 512 + (lq >> 1) * 256 + nt * 128 + lr * 16 + (lq & 1) * 8);
-    mma_16816(acc[nt], h[0], h[2], h[1], h[3], bw.x, bw.y);
-  }
+  for (int nt = 0; nt < 2; ++nt)
+    bw[nt] = *reinterpret_cast<const uint2*>(w2s + slab * 512 + (lq >> 1) * 256 + nt * 128 + lr * 16 + (lq & 1) * 8);
+}
+// ... the multiply with fragments loaded by w2_slab_frag (one load serves several hidden fragments)
+__device__ __forceinline__ void mma_w2_frag(float (&acc)[2][4], const uint32_t (&h)[4], const uint2 (&bw)[2]) {
+#pragma unroll
+  for (int nt = 0; nt < 2; ++nt) mma_16816(acc[nt], h[0], h[2], h[1], h[3], bw[nt].x, bw[nt].y);
+}
+__device__ __forceinline__ void mma_w2_slab(float (&acc)[2][4], const uint32_t (&h)[4], const unsigned char* w2s, int slab, int lr, int lq) {
+  uint2 bw[2];
+  w2_slab_frag(bw, w2s, slab, lr, lq);
+  mma_w2_frag(acc, h, bw);
 }
 
 // ------------------------------------------------------------------ copies into shared memory

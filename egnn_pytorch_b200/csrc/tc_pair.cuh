@@ -11,29 +11,35 @@
 //
 // PERSISTENT kernel: one CTA per SM walks "row groups" (TI = 4 query rows i of one graph) with a static stride.
 // W2 (core-matrix order) and Wq are staged ONCE per CTA with TMA bulk copies; the A' rows of row group it+2 are
-// prefetched into a two-deep ring while it / it+1 are being computed.  The 2 compute warpgroups (128 threads each,
-// 2 warps per SM sub-partition, up to 255 registers) are independent pipelines: warpgroup g owns the j-tiles
-// [256*jb + 128*g, +128) of every row group, has its own pair-scalar tile, and never waits for the other warpgroup.
+// prefetched into a two-deep ring while it / it+1 are being computed.  The WG compute warpgroups (128 threads each)
+// are independent pipelines: warpgroup g owns the j-tile [256*jb + TW*g, +TW) of every j-block (TW = 256 / WG pairs),
+// has its own pair-scalar tile, and never waits for another warpgroup.  Two layouts (template parameters WG, PPW):
+//   WG = 2, PPW = 32 pairs per warp: 256 threads, 2 warps per SM sub-partition, up to 255 registers (the default);
+//   WG = 4, PPW = 16 pairs per warp: 512 threads, 4 warps per SM sub-partition, at most 128 registers (lean
+//     instantiation only, on request, EGNN_B200_TC_PAIR_WG=4, where its shared memory fits; measured no faster on
+//     the H100, DESIGN.md section 6).
 // (An optional start-up skew, skew_ns, can de-phase the warpgroups so that their MUFU-idle epilogues fall into
 // different time windows; off by default.)
-//   * For each hidden chunk of 64 channels and each row i a warp produces the 64 bf16 hidden values of its 32
+//   * For each hidden chunk of 64 channels and each row i a warp produces the 64 bf16 hidden values of its PPW
 //     pairs in registers (fp32 math, one MUFU.TANH per value), packed directly in the mma.sync A-fragment layout,
 //     and multiplies each 16-channel slab with the W2 slab in shared memory right away (mma.sync m16n8k16, fp32
 //     accumulators in registers): the O(N^2 H) hidden tensor never leaves the registers.  H is padded to 16 (one
-//     K step), not 64: the last chunk runs 1..4 slabs.  The accumulators of the TI rows (m_pre[i], 32 pairs x 16
-//     per warp) stay in registers across all chunks -- 64 per thread, which is why a warpgroup has 255 registers.
-//   * After the last chunk the accumulators go through a per-warp shared-memory tile to the thread that owns the
-//     pair, which applies SiLU / gate / coors MLP / mask / clamp in fp32; the warp reduces over j with shuffles
-//     into per-warp partial sums in shared memory.  The LAST warpgroup to finish a row group (shared-memory
-//     counter) adds the partials in a fixed order (deterministic), writes m_i and x_i' once per row, and issues the
-//     TMA prefetch of row group it+2 into the ring slot that just became free.
+//     K step), not 64: the last chunk runs 1..4 slabs.  The accumulators of the TI rows (m_pre[i], PPW pairs x 16
+//     per warp) stay in registers across all chunks: 2 * PPW per thread (32 at PPW = 16, 64 at PPW = 32).
+//   * After the last chunk each lane applies the message SiLU to its accumulators in the fragment mapping, and the
+//     messages go through a per-warp shared-memory tile (one row at a time) to the lane that owns the pair, which
+//     applies gate / coors MLP / mask / clamp in fp32; the warp reduces over j with shuffles into per-warp partial
+//     sums in shared memory.  The LAST warpgroup to finish a row group (shared-memory counter) adds the partials in
+//     a fixed order (deterministic), writes m_i and x_i' once per row, and issues the TMA prefetch of row group it+2
+//     into the ring slot that just became free.
 //
-// Thread <-> data mappings inside a compute warp:
-//   "pair" mapping     (geometry, epilogue): lane l owns pair row 32*wq + l of the tile;
-//   "fragment" mapping (hidden production, mma.sync A / D fragments): lane (lr = l/4, lq = l%4) owns rows
-//     lr + 8*rho (rho = 0..3) of the warp's 32-row quadrant and, in every 16-channel K-slab, channels
-//     4*lq .. 4*lq+3.  Lanes sharing lq read the same A'/Wq words (4 distinct addresses per warp instead
-//     of a 32-way broadcast, which cost one shared-memory wavefront per 4 bytes in the first version).
+// Thread <-> data mappings inside a compute warp (its pairs are PPW*wq .. PPW*wq + PPW-1 of the warpgroup tile):
+//   "pair" mapping     (geometry, epilogue): lane l owns pair l % PPW of the warp and the RPL = TI*PPW/32 rows
+//     RPL*(l / PPW) .. +RPL-1 (PPW = 32: all 4 rows; PPW = 16: rows 2*(l/16), 2*(l/16)+1);
+//   "fragment" mapping (hidden production, mma.sync A / D fragments): lane (lr = l/4, lq = l%4) owns pairs
+//     lr + 8*rho (rho < PPW/8) of the warp and, in every 16-channel K-slab, channels 4*lq .. 4*lq+3.  Lanes sharing
+//     lq read the same A'/Wq words (4 distinct addresses per warp instead of a 32-way broadcast, which cost one
+//     shared-memory wavefront per 4 bytes in the first version).
 #pragma once
 
 #include <cuda_bf16.h>
@@ -48,11 +54,8 @@ namespace egnn {
 constexpr int TP_EPI_UNROLL = EPI_UNROLL;
 constexpr int TP_TI = 4;          // query rows per row group
 constexpr int TP_KC = 64;         // hidden channels per chunk (4 K slabs)
-constexpr int TP_WG = 2;          // compute warpgroups
-constexpr int TP_CWARPS = TP_WG * 4;
-constexpr int TP_THREADS = TP_WG * 128;      // 8 warps = 2 per SM sub-partition, up to 255 registers each
-constexpr int TP_JB = TP_WG * 128;    // neighbours per block
-constexpr int TP_ACC_LD = 18;         // floats per pair row of the per-warp accumulator transpose tile
+constexpr int TP_JB = 256;            // neighbours per block: WG warpgroups x 4 warps x PPW pairs in both layouts
+constexpr int TP_ACC_LD = 18;         // floats per pair row of the per-warp message transpose tile
 constexpr int TP_EPI_FLOATS = 64 * 16 + 64 + 64 + 16 + 16 + 4;   // W3 | b3 | w4 | b2 | gate_w | gate_b, b4, scale, 0
 constexpr int TP_QMAX = 12;           // per-pair scalar channels of the generic instantiation
 constexpr int TP_CMAX = 8;            // coordinate dimensions of the generic instantiation
@@ -88,15 +91,17 @@ template <bool GEN> struct TpCfg {
 // continuous edge channels / one-hot labels in bf16 (Qh planes; both are exactly representable: edges arrive as bf16).
 inline size_t tc_pair_gen_scalar_bytes(int Qf, int Qh) { return (size_t)TP_TI * TP_JB * (Qf * 4 + Qh * 2); }
 
-template <bool GEN>
+// shared memory of the kernel with WG compute warpgroups (the 2-warpgroup layout needs the least)
+template <bool GEN, int WG>
 inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
+  constexpr int CWARPS = WG * 4, PPW = TP_JB / CWARPS;
   size_t n = 0;
   n += (size_t)Hp * 32;                                     // W2 slabs
   n += (size_t)Q * Hp * 4;                                  // Wq
   n += (size_t)2 * TP_TI * Hp * 4;                          // A' rows, two-deep ring
   n += (size_t)TP_EPI_FLOATS * 4;                           // epilogue constants
-  n += (size_t)2 * TP_CWARPS * TP_TI * TpCfg<GEN>::PW * 8;  // per-warp partial sums (fp64), per ring slot
-  n += (size_t)TP_CWARPS * 32 * TP_ACC_LD * 4;               // per-warp accumulator transpose tile
+  n += (size_t)2 * CWARPS * TP_TI * TpCfg<GEN>::PW * 8;     // per-warp partial sums (fp64), per ring slot
+  n += (size_t)CWARPS * PPW * TP_ACC_LD * 4;                // per-warp message transpose tile (one row)
   n += (size_t)2 * TP_TI * TpCfg<GEN>::XC * 4 + 2 * TP_TI * 4 + 64;   // x_i, mask_i per ring slot; counters, flags
   n += (size_t)(GEN ? 0 : 1) * TP_TI * TP_JB * 4;           // lean: d_ij of the current tiles
   (void)Q;
@@ -105,7 +110,7 @@ inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
   return n + 256;
 }
 
-// named barrier over one warpgroup (ids 1..4; id 0 is __syncthreads)
+// named barrier over one warpgroup (ids 1..WG; id 0 is __syncthreads)
 __device__ __forceinline__ void tp_wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }
 
 // End of a work item, run by the LAST warpgroup of the CTA to finish it (kept out of line: its registers must not add to the
@@ -116,7 +121,7 @@ struct TpFinishArgs {               // the fields of TcPairArgs the finish needs
   uint32_t flags;
   double* gpart; unsigned int* gcount; __nv_bfloat16* m_out; float* coors_out;
 };
-template <bool GEN>
+template <bool GEN, int CWARPS>
 __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* partb, uint32_t* misc, const float* xi, int item, int b,
                                             int i0, int rows_valid, int active_wgs, int g, int t128) {
   constexpr int PW = TpCfg<GEN>::PW, XC = TpCfg<GEN>::XC;
@@ -158,7 +163,7 @@ __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* 
               }
             } else {
 #pragma unroll
-              for (int wv = 0; wv < TP_CWARPS; ++wv)
+              for (int wv = 0; wv < CWARPS; ++wv)
                 if (wv < active_wgs * 4) s += pb[(size_t)wv * TP_TI * PW + o];      // idle warpgroups never wrote theirs
               for (int wv = 0; wv < active_wgs * 4; ++wv) cnt += pb[(size_t)wv * TP_TI * PW + PW - 1];
             }
@@ -176,9 +181,15 @@ __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* 
         }
 }
 
-template <bool GEN>
-__global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs a) {
+template <bool GEN, int WG, int PPW>
+__global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a) {
+  static_assert(WG * 4 * PPW == TP_JB && (PPW == 16 || PPW == 32), "a j-block is WG warpgroups x 4 warps x PPW pairs");
+  static_assert(!GEN || WG == 2, "the generic chunk loop needs more than the 128 registers of 4 warpgroups");
   constexpr int PW = TpCfg<GEN>::PW, XC = TpCfg<GEN>::XC;
+  constexpr int CWARPS = WG * 4, THREADS = WG * 128;
+  constexpr int TW = 4 * PPW;              // pairs of a warpgroup's j-tile
+  constexpr int NH = PPW / 16;             // m16 halves of a warp's pairs (fragment mapping)
+  constexpr int RPL = TP_TI * PPW / 32;    // rows of a lane's pair (pair mapping)
   // carve the dynamic shared memory directly (no integer round trip) so every access stays in the
   // shared state space (LDS/STS, not generic LD/ST); nothing here needs more than 128-byte alignment
   extern __shared__ __align__(128) unsigned char sm[];
@@ -192,14 +203,14 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
   // fp32 numbers in fp64 is exact, so the result does not depend on how the tiles were dealt to warps, work items or
   // ranks (row-sharded == single GPU, bit for bit, whatever jsplit is).
   double* part = reinterpret_cast<double*>(epi + TP_EPI_FLOATS);              // [2][CWARPS][TI][PW]
-  float* xis = reinterpret_cast<float*>(part + 2 * TP_CWARPS * TP_TI * PW);   // [2][TI][XC]
+  float* xis = reinterpret_cast<float*>(part + 2 * CWARPS * TP_TI * PW);      // [2][TI][XC]
   uint32_t* mki = reinterpret_cast<uint32_t*>(xis + 2 * TP_TI * XC);          // [2][TI]
-  uint32_t* misc = mki + 2 * TP_TI;                                           // [0..1] done counters, [4..] last flags
+  uint32_t* misc = mki + 2 * TP_TI;        // [0..1] done counters, [4 + g] / [8 + g] last-warpgroup / last-item flags
   const int Qf = GEN ? 1 + 2 * a.F : 1, Qh = Q - Qf;
-  float* ssm = reinterpret_cast<float*>(misc + 16);                           // [WG][Qf][TI][128] fp32
-  __nv_bfloat16* ssh = reinterpret_cast<__nv_bfloat16*>(ssm + (size_t)Qf * TP_TI * TP_JB);   // [WG][Qh][TI][128] bf16
-  float* accs = reinterpret_cast<float*>(ssh + (size_t)Qh * TP_TI * TP_JB);    // [CWARPS][32][TP_ACC_LD]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(accs + TP_CWARPS * 32 * TP_ACC_LD);
+  float* ssm = reinterpret_cast<float*>(misc + 16);                           // [WG][Qf][TI][TW] fp32
+  __nv_bfloat16* ssh = reinterpret_cast<__nv_bfloat16*>(ssm + (size_t)Qf * TP_TI * TP_JB);   // [WG][Qh][TI][TW] bf16
+  float* accs = reinterpret_cast<float*>(ssh + (size_t)Qh * TP_TI * TP_JB);    // [CWARPS][PPW][TP_ACC_LD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(accs + CWARPS * PPW * TP_ACC_LD);
   uint64_t* ldbar = bars;                         // W2 / Wq staging
   uint64_t* rowfull = ldbar + 1;                  // [2] A' ring
 
@@ -254,8 +265,8 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
     tc::mbar_init(&rowfull[0], 1); tc::mbar_init(&rowfull[1], 1);
     tc::mbar_fence_init();
   }
-  for (int x = tid; x < TP_EPI_FLOATS; x += TP_THREADS) epi[x] = a.epi[x];
-  for (int x = tid; x < 2 * TP_TI * Hp; x += TP_THREADS) As[x] = 0.f;      // rows beyond a graph's end stay finite
+  for (int x = tid; x < TP_EPI_FLOATS; x += THREADS) epi[x] = a.epi[x];
+  for (int x = tid; x < 2 * TP_TI * Hp; x += THREADS) As[x] = 0.f;         // rows beyond a graph's end stay finite
   if (tid < 2) misc[tid] = 0;
   tc::fence_proxy_async_smem();                    // the zero fill above precedes TMA writes to the same buffers
   __syncthreads();
@@ -280,18 +291,20 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
     // =========================================================== compute warpgroups (independent pipelines)
     const int g = warp >> 2, wq = warp & 3, t128 = tid & 127;
     const int lr = lane >> 2, lq = lane & 3;
-    float* swg = ssm + (size_t)g * Qf * TP_TI * 128;  // pair scalars of this warpgroup's tile: swg[(q*TI + i)*128 + pair]
-    __nv_bfloat16* shg = ssh + (size_t)g * Qh * TP_TI * 128;
-    float* myacc = accs + (size_t)warp * 32 * TP_ACC_LD;
+    const int pp = wq * PPW + lane % PPW;            // pair mapping: this lane's pair in the warpgroup tile ...
+    const int rb = lane / PPW * RPL;                 // ... and its first row
+    float* swg = ssm + (size_t)g * Qf * TP_TI * TW;  // pair scalars of this warpgroup's tile: swg[(q*TI + i)*TW + pair]
+    __nv_bfloat16* shg = ssh + (size_t)g * Qh * TP_TI * TW;
+    float* myacc = accs + (size_t)warp * PPW * TP_ACC_LD;
     if (a.skew_ns && g > 0) {                         // de-phase the warpgroups (see the header)
       uint64_t t0, t1;
       asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
       const uint64_t until = t0 + (uint64_t)a.skew_ns * g;
       do { __nanosleep(1000); asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); } while (t1 < until);
     }
-    // warpgroups whose j-tiles all lie beyond the graph (N <= 128 g) have nothing to do in ANY row group: they leave
+    // warpgroups whose j-tiles all lie beyond the graph (N <= TW g) have nothing to do in ANY row group: they leave
     // now instead of spinning on the ring barriers next to the working warps of their SM sub-partitions
-    const int active_wgs = min(TP_WG, (N + 127) / 128);
+    const int active_wgs = min(WG, (N + TW - 1) / TW);
     const bool wg_active = g < active_wgs;
     if (wg_active) tc::mbar_wait(ldbar, 0);
     int it = 0;
@@ -303,158 +316,199 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
       const float* Ab = As + (size_t)buf * TP_TI * Hp;
       const float* xi = xis + buf * TP_TI * XC;
       const uint32_t* mk = mki + buf * TP_TI;
-      double* mypart = part + ((size_t)buf * TP_CWARPS + warp) * TP_TI * PW;
+      double* mypart = part + ((size_t)buf * CWARPS + warp) * TP_TI * PW;
       for (int x = lane; x < TP_TI * PW; x += 32) mypart[x] = 0.0;
       __syncwarp();
 
       for (int jb = item % a.jsplit; jb < njb; jb += a.jsplit) {
-        if (jb * TP_JB + g * 128 >= N) break;           // this warpgroup's tile lies beyond the graph
-        // ---- pair mapping: geometry (and the other per-pair scalar channels) of (i, j) for the rows i
-        const int j = jb * TP_JB + g * 128 + t128;
+        if (jb * TP_JB + g * TW >= N) break;            // this warpgroup's tile lies beyond the graph
+        // ---- pair mapping: geometry (and the other per-pair scalar channels) of (i, j) for this lane's rows i
+        // (lean: x_j and mask_j are read here and again in the epilogue rather than held across the chunk loop, which
+        //  the 128 registers of the 4-warpgroup layout need; the generic instantiation holds them)
+        const int j = jb * TP_JB + g * TW + pp;
         const bool jv = j < N;
-        const size_t nodej = (size_t)b * N + (jv ? j : N - 1);
-        float xj[GEN ? TP_CMAX : 3];
+        auto load_xj = [&](float (&xj)[GEN ? TP_CMAX : 3]) {
+          const size_t nodej = (size_t)b * N + (jv ? j : N - 1);
 #pragma unroll
-        for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) xj[c] = (!GEN || c < C) ? a.coors[nodej * C + c] : 0.f;
-        const bool mask_j = jv && (a.has_mask ? a.mask[nodej] != 0 : true);
+          for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) xj[c] = (!GEN || c < C) ? a.coors[nodej * C + c] : 0.f;
+          return jv && (a.has_mask ? a.mask[nodej] != 0 : true);                                           // mask_j
+        };
         __syncwarp();                                   // previous tile's readers of swg are done
+        float xj[GEN ? TP_CMAX : 3];
+        const bool mask_j0 = load_xj(xj);
 #pragma unroll
-        for (int i = 0; i < TP_TI; ++i) {
+        for (int r = 0; r < RPL; ++r) {
+          const int i = rb + r;
           float d = 0.f;
 #pragma unroll
-          for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float r = xi[i * XC + c] - xj[c]; d = fmaf(r, r, d); }
-          swg[i * 128 + t128] = d;
+          for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float rc = xi[i * XC + c] - xj[c]; d = fmaf(rc, rc, d); }
+          swg[i * TW + pp] = d;
           if (GEN) {
             int q = 1;
             for (int f = 0; f < a.F; ++f) {                                                       // :34-41
               const float sc = d * exp2f(-(float)f);
-              swg[((q + f) * TP_TI + i) * 128 + t128] = sinf(sc);
-              swg[((q + a.F + f) * TP_TI + i) * 128 + t128] = cosf(sc);
+              swg[((q + f) * TP_TI + i) * TW + pp] = sinf(sc);
+              swg[((q + a.F + f) * TP_TI + i) * TW + pp] = cosf(sc);
             }
             const size_t pij = ((size_t)b * N + min(i0 + i, N - 1)) * N + (jv ? j : N - 1);
-            for (int e = 0; e < a.edge_dim; ++e) shg[(e * TP_TI + i) * 128 + t128] = a.edges[pij * a.edge_dim + e];
+            for (int e = 0; e < a.edge_dim; ++e) shg[(e * TP_TI + i) * TW + pp] = a.edges[pij * a.edge_dim + e];
             if (a.num_labels > 0) {
               const int lab = a.labels[pij];
               for (int l = 0; l < a.num_labels; ++l)
-                shg[((a.edge_dim + l) * TP_TI + i) * 128 + t128] = __float2bfloat16((l == lab) ? 1.f : 0.f);
+                shg[((a.edge_dim + l) * TP_TI + i) * TW + pp] = __float2bfloat16((l == lab) ? 1.f : 0.f);
             }
           }
         }
         __syncwarp();
-        // ---- fragment mapping: B' rows of this lane's 4 pairs
+        // ---- fragment mapping: B' rows of this lane's 2 * NH pairs
         // (rows lr + 8 rho of the tile are 8 table rows apart: one base pointer + a stride instead of four pointers.  Rows
         //  beyond the graph are NOT clamped: they read the next graph's rows or the 128 padding rows of the table, and
         //  their pairs are discarded by `jv` -- NaN-safe, every use is a select)
-        const uint2* Bp0 = reinterpret_cast<const uint2*>(a.Btab + ((size_t)b * N + jb * TP_JB + g * 128 + wq * 32 + lr) * Hp + 4 * lq);
+        const uint2* Bp0 = reinterpret_cast<const uint2*>(a.Btab + ((size_t)b * N + jb * TP_JB + g * TW + wq * PPW + lr) * Hp + 4 * lq);
         const int Bstride = 8 * Hp / 4;                 // uint2 units between rows lr + 8 rho and lr + 8 (rho + 1)
 #define Bp_(rho) (Bp0 + (rho) * Bstride)
-        uint2 Bc[4][4];                                 // [rho][slab] B' of the current chunk (bf16 x4 each)
+        // lean: a two-slab ring of B' (see the lean chunk below); generic: B' of the whole chunk
+        constexpr int BCS = GEN ? 4 : 2;
+        uint2 Bc[2 * NH][BCS];                          // [rho][slab % BCS] B' (bf16 x4 each)
         {
           const int nsl0 = nchunks == 1 ? nsl_last : 4;
 #pragma unroll
-          for (int rho = 0; rho < 4; ++rho)
+          for (int rho = 0; rho < 2 * NH; ++rho)
 #pragma unroll
-            for (int sl = 0; sl < 4; ++sl) Bc[rho][sl] = sl < nsl0 ? __ldg(Bp_(rho) + sl * 4) : make_uint2(0u, 0u);
+            for (int sl = 0; sl < BCS; ++sl) Bc[rho][sl] = sl < nsl0 ? __ldg(Bp_(rho) + sl * 4) : make_uint2(0u, 0u);
         }
 
-        float acc[TP_TI][2][2][4];                      // m_pre[i] of rows [16 half, +16) x channels [8 nt, +8) (D fragments)
+        float acc[TP_TI][NH][2][4];                     // m_pre[i] of pairs [16 half, +16) x channels [8 nt, +8) (D fragments)
 #pragma unroll
         for (int i = 0; i < TP_TI; ++i)
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+          for (int h = 0; h < NH; ++h)
 #pragma unroll
             for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
               for (int e = 0; e < 4; ++e) acc[i][h][nt][e] = 0.f;
+        float dr[GEN ? 1 : TP_TI][2 * NH];              // lean: d_ij of this lane's fragment pairs, for the whole tile
+        if (!GEN) {
+#pragma unroll
+          for (int i = 0; i < TP_TI; ++i)
+#pragma unroll
+            for (int rho = 0; rho < 2 * NH; ++rho) dr[GEN ? 0 : i][rho] = swg[i * TW + wq * PPW + lr + 8 * rho];
+        }
+        // 8 hidden values (2 pairs x 4 channels of one K slab) from their pre-activation / 2 without B' (z), + B', SiLU,
+        // packed as the mma.sync A fragment: regs {0,1} -> pair lr (+16), regs {2,3} -> pair lr+8 (+24); even k low
+        auto hidden = [&](uint32_t (&h4)[4], const float2 (&z)[2][2], const uint2 (&bb)[2]) {
+#pragma unroll
+          for (int r2 = 0; r2 < 2; ++r2) {
+            const float2 y01 = make_float2(tc::add_bf16_lo(bb[r2].x, z[r2][0].x), tc::add_bf16_hi(bb[r2].x, z[r2][0].y));
+            const float2 y23 = make_float2(tc::add_bf16_lo(bb[r2].y, z[r2][1].x), tc::add_bf16_hi(bb[r2].y, z[r2][1].y));
+            const float2 h01 = tc::ffma2(y01, make_float2(tc::tanh_fast(y01.x), tc::tanh_fast(y01.y)), y01);  // y + y tanh y
+            const float2 h23 = tc::ffma2(y23, make_float2(tc::tanh_fast(y23.x), tc::tanh_fast(y23.y)), y23);
+            h4[r2 * 2 + 0] = tc::pack_bf16x2(h01.x, h01.y);
+            h4[r2 * 2 + 1] = tc::pack_bf16x2(h23.x, h23.y);
+          }
+        };
         // A chunk with all 4 K slabs runs with NSLC = 4 (every slab test folds at compile time); only the last chunk
-        // of a hidden width that is not a multiple of 64 takes the predicated instantiation (NSLC = 0).
-        auto chunk = [&](const int c, auto nslc) {
+        // of a hidden width that is not a multiple of 64 takes the predicated instantiation (NSLC = 0).  The loops are
+        // fully unrolled (or the row is a compile-time tag), so that acc[i] and B' stay in registers.
+        //
+        // Lean: slab outermost, then the TI rows.  The W2 fragments and the distance column of W1 of a slab are loaded
+        // once and serve all rows, and are dead after it -- no per-chunk register copy of them.  B' is a two-slab
+        // ring: right after the last row of a slab has used its B' registers they are re-filled with the slab two
+        // ahead (in this chunk or the next), so the L2 latency is covered by a whole slab of work.
+        auto chunk_lean = [&](const int c, auto nslc) {
           constexpr int NSLC = decltype(nslc)::value;
           const int nsl = NSLC ? NSLC : nsl_last;                   // valid slabs of this chunk
           const int nsl_next = c + 2 == nchunks ? nsl_last : 4;     // ... and of the next one (prefetch)
-          // Register budget: w_d and A' are read from shared memory at the point of use instead of being held for the chunk
-          // / round; one B' base pointer + stride; every slab is multiplied as soon as it is packed.
-          // One round = the 64 hidden channels of chunk c for row i and this warp's 32 pairs.  In the last round
-          // of a chunk (`reload`), every B' register is re-filled for chunk c+1 right after its last use, so the
-          // L2 latency is covered by the rest of that round without a second register buffer.
-          // The row index is a compile-time constant (IntC) so that acc[i] stays in registers.
+          const bool more = NSLC != 0 && c + 1 < nchunks;           // a next chunk follows (the tail chunk is the last)
+#pragma unroll
+          for (int sl = 0; sl < 4; ++sl) {
+            if (NSLC == 0 && sl >= nsl) continue;        // tail chunk: slabs beyond H are neither computed nor multiplied
+            const int s = c * 4 + sl;                    // K slab (16 hidden channels)
+            uint2 bw[2];
+            tc::w2_slab_frag(bw, w2s, s, lr, lq);
+            const float4 wv = *reinterpret_cast<const float4*>(wqs + s * 16 + lq * 4);
+#pragma unroll
+            for (int i = 0; i < TP_TI; ++i) {
+              const float4 av = *reinterpret_cast<const float4*>(Ab + (size_t)i * Hp + s * 16 + lq * 4);
+#pragma unroll
+              for (int half = 0; half < NH; ++half) {    // pairs (lr, lr+8), then (lr+16, lr+24)
+                float2 z[2][2];                          // [r2][channel pair]: wd*d + A'
+#pragma unroll
+                for (int r2 = 0; r2 < 2; ++r2) {
+                  const float d = dr[GEN ? 0 : i][half * 2 + r2];
+                  const float2 dd = make_float2(d, d);
+                  z[r2][0] = tc::ffma2(make_float2(wv.x, wv.y), dd, make_float2(av.x, av.y));
+                  z[r2][1] = tc::ffma2(make_float2(wv.z, wv.w), dd, make_float2(av.z, av.w));
+                }
+                const uint2 bb[2] = {Bc[half * 2][sl % BCS], Bc[half * 2 + 1][sl % BCS]};
+                uint32_t h4[4];
+                hidden(h4, z, bb);
+                tc::mma_w2_frag(acc[i][half], h4, bw);
+              }
+            }
+            // B' of slab sl + 2 into the ring slot slab sl just freed
+            if (sl + 2 < 4 ? sl + 2 < nsl : more && sl - 2 < nsl_next) {
+#pragma unroll
+              for (int rho = 0; rho < 2 * NH; ++rho) Bc[rho][sl % BCS] = __ldg(Bp_(rho) + (s + 2) * 4);
+            }
+          }
+        };
+        // Generic: row outermost.  One round = the 64 hidden channels of chunk c for row i and this warp's pairs; the
+        // per-pair scalar channels go in q outermost (a runtime loop over Q), each s_q read once for all 4 slabs.  In
+        // the last round of a chunk (`reload`) every B' register is re-filled for chunk c+1 right after its last use.
+        auto chunk_gen = [&](const int c, auto nslc) {
+          constexpr int NSLC = decltype(nslc)::value;
+          const int nsl = NSLC ? NSLC : nsl_last;
+          const int nsl_next = c + 2 == nchunks ? nsl_last : 4;
           auto round = [&](auto i_tag, auto reload_tag) {
             constexpr int i = decltype(i_tag)::value;
             constexpr bool reload = decltype(reload_tag)::value != 0;
             const float* Ai = Ab + (size_t)i * Hp + c * TP_KC + lq * 4;
-            float dr[4];
-            if (!GEN) {
 #pragma unroll
-              for (int rho = 0; rho < 4; ++rho) dr[rho] = swg[i * 128 + wq * 32 + lr + 8 * rho];
-            }
+            for (int half = 0; half < NH; ++half) {
+              float2 z[4][2][2];                         // [slab][r2][channel pair]: A' + sum_q Wq s_q
 #pragma unroll
-            for (int half = 0; half < 2; ++half) {       // rows (lr, lr+8), then (lr+16, lr+24)
-              // GEN: z = A' + sum_q Wq s_q (pre-activation / 2 without B') for 2 pairs x 16 channels, q outermost
-              float2 z[GEN ? 4 : 1][2][2];               // [slab][r2][channel pair]
-              if (GEN) {
+              for (int sl = 0; sl < 4; ++sl) {
+                const float4 av = sl < nsl ? *reinterpret_cast<const float4*>(Ai + sl * 16) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+                for (int r2 = 0; r2 < 2; ++r2) {
+                  z[sl][r2][0] = make_float2(av.x, av.y);
+                  z[sl][r2][1] = make_float2(av.z, av.w);
+                }
+              }
+#pragma unroll 1
+              for (int q = 0; q < Q; ++q) {
+                float s0, s1;
+                if (q < Qf) {
+                  const float* sq = swg + (q * TP_TI + i) * TW + wq * PPW + lr + 16 * half;
+                  s0 = sq[0]; s1 = sq[8];
+                } else {
+                  const __nv_bfloat16* sq = shg + ((q - Qf) * TP_TI + i) * TW + wq * PPW + lr + 16 * half;
+                  s0 = __bfloat162float(sq[0]); s1 = __bfloat162float(sq[8]);
+                }
+                const float2 ss0 = make_float2(s0, s0), ss1 = make_float2(s1, s1);
+                const float* wrow = wqs + (size_t)q * Hp + c * TP_KC + lq * 4;
 #pragma unroll
                 for (int sl = 0; sl < 4; ++sl) {
-                  const float4 av = sl < nsl ? *reinterpret_cast<const float4*>(Ai + sl * 16) : make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll
-                  for (int r2 = 0; r2 < 2; ++r2) {
-                    z[GEN ? sl : 0][r2][0] = make_float2(av.x, av.y);
-                    z[GEN ? sl : 0][r2][1] = make_float2(av.z, av.w);
-                  }
-                }
-#pragma unroll 1
-                for (int q = 0; q < Q; ++q) {
-                  float s0, s1;
-                  if (q < Qf) {
-                    const float* sq = swg + (q * TP_TI + i) * 128 + wq * 32 + lr + 16 * half;
-                    s0 = sq[0]; s1 = sq[8];
-                  } else {
-                    const __nv_bfloat16* sq = shg + ((q - Qf) * TP_TI + i) * 128 + wq * 32 + lr + 16 * half;
-                    s0 = __bfloat162float(sq[0]); s1 = __bfloat162float(sq[8]);
-                  }
-                  const float2 ss0 = make_float2(s0, s0), ss1 = make_float2(s1, s1);
-                  const float* wrow = wqs + (size_t)q * Hp + c * TP_KC + lq * 4;
-#pragma unroll
-                  for (int sl = 0; sl < 4; ++sl) {
-                    if (sl < nsl) {
-                      const float4 wv = *reinterpret_cast<const float4*>(wrow + sl * 16);
-                      float2 (&zz)[2][2] = z[GEN ? sl : 0];
-                      zz[0][0] = tc::ffma2(make_float2(wv.x, wv.y), ss0, zz[0][0]);
-                      zz[0][1] = tc::ffma2(make_float2(wv.z, wv.w), ss0, zz[0][1]);
-                      zz[1][0] = tc::ffma2(make_float2(wv.x, wv.y), ss1, zz[1][0]);
-                      zz[1][1] = tc::ffma2(make_float2(wv.z, wv.w), ss1, zz[1][1]);
-                    }
+                  if (sl < nsl) {
+                    const float4 wv = *reinterpret_cast<const float4*>(wrow + sl * 16);
+                    z[sl][0][0] = tc::ffma2(make_float2(wv.x, wv.y), ss0, z[sl][0][0]);
+                    z[sl][0][1] = tc::ffma2(make_float2(wv.z, wv.w), ss0, z[sl][0][1]);
+                    z[sl][1][0] = tc::ffma2(make_float2(wv.x, wv.y), ss1, z[sl][1][0]);
+                    z[sl][1][1] = tc::ffma2(make_float2(wv.z, wv.w), ss1, z[sl][1][1]);
                   }
                 }
               }
-              uint32_t hp[16];
 #pragma unroll
               for (int sl = 0; sl < 4; ++sl) {
-                if (NSLC == 0 && sl >= nsl) continue;      // tail chunk: slabs beyond H are neither computed nor multiplied
+                if (NSLC == 0 && sl >= nsl) continue;
+                const uint2 bb[2] = {Bc[half * 2][sl % BCS], Bc[half * 2 + 1][sl % BCS]};
+                uint32_t h4[4];
+                hidden(h4, z[sl], bb);
+                if (reload && sl < nsl_next) {
 #pragma unroll
-                for (int r2 = 0; r2 < 2; ++r2) {
-                  const int rho = half * 2 + r2;
-                  const uint2 bb = Bc[rho][sl];
-                  float2 z01, z23;
-                  if (GEN) {
-                    z01 = z[GEN ? sl : 0][r2][0]; z23 = z[GEN ? sl : 0][r2][1];
-                  } else {
-                    const float4 av = *reinterpret_cast<const float4*>(Ai + sl * 16);
-                    const float d = dr[rho];
-                    const float2 dd = make_float2(d, d);
-                    const float4 wv = *reinterpret_cast<const float4*>(wqs + c * TP_KC + sl * 16 + lq * 4);
-                    z01 = tc::ffma2(make_float2(wv.x, wv.y), dd, make_float2(av.x, av.y));   // wd*d + A'
-                    z23 = tc::ffma2(make_float2(wv.z, wv.w), dd, make_float2(av.z, av.w));
-                  }
-                  const float2 y01 = make_float2(tc::add_bf16_lo(bb.x, z01.x), tc::add_bf16_hi(bb.x, z01.y));  // + B'
-                  const float2 y23 = make_float2(tc::add_bf16_lo(bb.y, z23.x), tc::add_bf16_hi(bb.y, z23.y));
-                  const float2 h01 = tc::ffma2(y01, make_float2(tc::tanh_fast(y01.x), tc::tanh_fast(y01.y)), y01);  // y + y tanh y
-                  const float2 h23 = tc::ffma2(y23, make_float2(tc::tanh_fast(y23.x), tc::tanh_fast(y23.y)), y23);
-                  // A fragment: regs {0,1} of a slab -> row lr (+16), regs {2,3} -> row lr+8 (+24); even k low
-                  hp[sl * 4 + r2 * 2 + 0] = tc::pack_bf16x2(h01.x, h01.y);
-                  hp[sl * 4 + r2 * 2 + 1] = tc::pack_bf16x2(h23.x, h23.y);
-                  if (reload && sl < nsl_next) Bc[rho][sl] = __ldg(Bp_(rho) + (c + 1) * 16 + sl * 4);
+                  for (int r2 = 0; r2 < 2; ++r2) Bc[half * 2 + r2][sl % BCS] = __ldg(Bp_(half * 2 + r2) + (c + 1) * 16 + sl * 4);
                 }
-                const uint32_t h4[4] = {hp[sl * 4], hp[sl * 4 + 1], hp[sl * 4 + 2], hp[sl * 4 + 3]};
                 tc::mma_w2_slab(acc[i][half], h4, w2s, c * 4 + sl, lr, lq);
               }
             }
@@ -467,6 +521,10 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
           if (NSLC != 0 && c + 1 < nchunks) round(tc::IntC<3>{}, tc::IntC<1>{});
           else round(tc::IntC<3>{}, tc::IntC<0>{});
         };
+        auto chunk = [&](const int c, auto nslc) {
+          if constexpr (GEN) chunk_gen(c, nslc);
+          else chunk_lean(c, nslc);
+        };
         {
           const int nfull = nsl_last == 4 ? nchunks : nchunks - 1;
 #pragma unroll 1
@@ -474,38 +532,51 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
           if (nfull < nchunks) chunk(nchunks - 1, tc::IntC<0>{});
         }
 
-        // ---- epilogue of this tile: accumulators back to the owning thread (pair mapping)
+        // ---- epilogue of this tile: the message SiLU in the fragment mapping (elementwise: every lane busy), then the
+        //      messages through the per-warp tile, one row at a time, to the lanes that own the pair (pair mapping)
         const float* W3 = epi; const float* b3 = epi + 1024; const float* w4 = b3 + 64;
         const float* b2 = w4 + 64; const float* gw = b2 + 16; const float* sc = gw + 16;   // sc: gate_b, b4, scale
-        float m[TP_TI][16];                              // m_ij of this thread's pair for the TI rows
+        float m[RPL][16];                                // m_ij of this lane's pair for its RPL rows
+        {
+          float b2f[2][2];                               // b2 of this lane's D-fragment channels 8 nt + 2 lq + e
 #pragma unroll
-        for (int i = 0; i < TP_TI; ++i) {
+          for (int nt = 0; nt < 2; ++nt) { b2f[nt][0] = b2[8 * nt + 2 * lq]; b2f[nt][1] = b2[8 * nt + 2 * lq + 1]; }
 #pragma unroll
-          for (int h = 0; h < 2; ++h)
+          for (int i = 0; i < TP_TI; ++i) {
 #pragma unroll
-            for (int nt = 0; nt < 2; ++nt)
+            for (int h = 0; h < NH; ++h)
 #pragma unroll
-              for (int r2 = 0; r2 < 2; ++r2)
-                *reinterpret_cast<float2*>(myacc + (16 * h + 8 * r2 + lr) * TP_ACC_LD + 8 * nt + 2 * lq) =
-                    make_float2(acc[i][h][nt][2 * r2], acc[i][h][nt][2 * r2 + 1]);
-          __syncwarp();
+              for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
-          for (int o = 0; o < 16; ++o) m[i][o] = tc::silu_half_arg(0.5f * (myacc[lane * TP_ACC_LD + o] + b2[o]));    // :183
-          __syncwarp();
-          if (a.flags & EGNN_FLAG_SOFT_EDGES) {                                                               // :289-290
-            float z = sc[0];
+                for (int r2 = 0; r2 < 2; ++r2)                                                                // :183
+                  *reinterpret_cast<float2*>(myacc + (16 * h + 8 * r2 + lr) * TP_ACC_LD + 8 * nt + 2 * lq) =
+                      make_float2(tc::silu_half_arg(0.5f * (acc[i][h][nt][2 * r2] + b2f[nt][0])),
+                                  tc::silu_half_arg(0.5f * (acc[i][h][nt][2 * r2 + 1] + b2f[nt][1])));
+            __syncwarp();
+            if (i / RPL == lane / PPW) {                 // (always, at PPW = 32)
 #pragma unroll
-            for (int o = 0; o < 16; ++o) z = fmaf(gw[o], m[i][o], z);
-            const float gate = 0.5f + 0.5f * tc::tanh_fast(0.5f * z);
-#pragma unroll
-            for (int o = 0; o < 16; ++o) m[i][o] *= gate;
+              for (int o = 0; o < 16; ++o) m[i % RPL][o] = myacc[(lane % PPW) * TP_ACC_LD + o];
+            }
+            __syncwarp();
           }
         }
-        float wgt[TP_TI];
+        const bool mask_j = GEN ? mask_j0 : load_xj(xj);
+        if (a.flags & EGNN_FLAG_SOFT_EDGES) {                                                                 // :289-290
 #pragma unroll
-        for (int i = 0; i < TP_TI; ++i) wgt[i] = 0.f;
+          for (int r = 0; r < RPL; ++r) {
+            float z = sc[0];
+#pragma unroll
+            for (int o = 0; o < 16; ++o) z = fmaf(gw[o], m[r][o], z);
+            const float gate = 0.5f + 0.5f * tc::tanh_fast(0.5f * z);
+#pragma unroll
+            for (int o = 0; o < 16; ++o) m[r][o] *= gate;
+          }
+        }
+        float wgt[RPL];
+#pragma unroll
+        for (int r = 0; r < RPL; ++r) wgt[r] = 0.f;
         if (upd_coors) {                                                                                      // :302-315
-          // hidden unit u outermost: one W3 row (4 x LDS.128) serves all TI rows of this pair; the four rows are four
+          // hidden unit u outermost: one W3 row (4 x LDS.128) serves all RPL rows of this pair; the rows are
           // independent FMA chains
 #pragma unroll TP_EPI_UNROLL
           for (int u = 0; u < 64; ++u) {
@@ -513,48 +584,50 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
             const float4 wa = w3[0], wb = w3[1], wc = w3[2], wd4 = w3[3];
             const float bu = b3[u], w4u = w4[u];
 #pragma unroll
-            for (int i = 0; i < TP_TI; ++i) {
+            for (int r = 0; r < RPL; ++r) {
               float tt = bu;
-              tt = fmaf(wa.x, m[i][0], tt); tt = fmaf(wa.y, m[i][1], tt); tt = fmaf(wa.z, m[i][2], tt); tt = fmaf(wa.w, m[i][3], tt);
-              tt = fmaf(wb.x, m[i][4], tt); tt = fmaf(wb.y, m[i][5], tt); tt = fmaf(wb.z, m[i][6], tt); tt = fmaf(wb.w, m[i][7], tt);
-              tt = fmaf(wc.x, m[i][8], tt); tt = fmaf(wc.y, m[i][9], tt); tt = fmaf(wc.z, m[i][10], tt); tt = fmaf(wc.w, m[i][11], tt);
-              tt = fmaf(wd4.x, m[i][12], tt); tt = fmaf(wd4.y, m[i][13], tt); tt = fmaf(wd4.z, m[i][14], tt); tt = fmaf(wd4.w, m[i][15], tt);
-              wgt[i] = fmaf(w4u, tc::silu_half_arg(0.5f * tt), wgt[i]);
+              tt = fmaf(wa.x, m[r][0], tt); tt = fmaf(wa.y, m[r][1], tt); tt = fmaf(wa.z, m[r][2], tt); tt = fmaf(wa.w, m[r][3], tt);
+              tt = fmaf(wb.x, m[r][4], tt); tt = fmaf(wb.y, m[r][5], tt); tt = fmaf(wb.z, m[r][6], tt); tt = fmaf(wb.w, m[r][7], tt);
+              tt = fmaf(wc.x, m[r][8], tt); tt = fmaf(wc.y, m[r][9], tt); tt = fmaf(wc.z, m[r][10], tt); tt = fmaf(wc.w, m[r][11], tt);
+              tt = fmaf(wd4.x, m[r][12], tt); tt = fmaf(wd4.y, m[r][13], tt); tt = fmaf(wd4.z, m[r][14], tt); tt = fmaf(wd4.w, m[r][15], tt);
+              wgt[r] = fmaf(w4u, tc::silu_half_arg(0.5f * tt), wgt[r]);
             }
           }
         }
 #pragma unroll
-        for (int i = 0; i < TP_TI; ++i) {
+        for (int r = 0; r < RPL; ++r) {
+          const int i = rb + r;
           const bool pm = jv && (mk[i] != 0) && (a.has_mask ? mask_j : true);
-          float w = wgt[i] + sc[1];
+          float w = wgt[r] + sc[1];
           if (upd_coors) {
             if (!pm) w = 0.f;                                                                                 // :309
             if (a.flags & EGNN_FLAG_CLAMP) w = fminf(fmaxf(w, -a.clamp), a.clamp);                            // :313
-            if (a.flags & EGNN_FLAG_NORM_COORS) w *= sc[2] / fmaxf(sqrtf(swg[i * 128 + t128]), 1e-8f);        // :74-77
+            if (a.flags & EGNN_FLAG_NORM_COORS) w *= sc[2] / fmaxf(sqrtf(swg[i * TW + pp]), 1e-8f);           // :74-77
           } else {
             w = 0.f;
           }
           float v[PW];
 #pragma unroll
-          for (int o = 0; o < 16; ++o) v[o] = pm ? m[i][o] : 0.f;                                             // :322
+          for (int o = 0; o < 16; ++o) v[o] = pm ? m[r][o] : 0.f;                                             // :322
 #pragma unroll
           for (int c = 0; c < PW - 17; ++c) {
             constexpr int NX = GEN ? TP_CMAX : 3;
             v[16 + c] = (c < NX && (!GEN || c < C)) ? w * (xi[i * XC + (c < NX ? c : 0)] - xj[c < NX ? c : 0]) : 0.f;
           }
           v[PW - 1] = pm ? 1.f : 0.f;
+          // sum over the warp's pairs: the PPW lanes that hold row i (the whole warp, or one half of it)
 #pragma unroll
-          for (int off = 16; off > 0; off >>= 1)
+          for (int off = PPW / 2; off > 0; off >>= 1)
 #pragma unroll
             for (int o = 0; o < PW; ++o) v[o] += __shfl_xor_sync(0xffffffffu, v[o], off);
-          if (lane == 0) {
+          if (lane % PPW == 0) {
 #pragma unroll
             for (int o = 0; o < PW; ++o) mypart[i * PW + o] += (double)v[o];
           }
         }
       }
 
-      // ---- this warpgroup is done with the row group: the last of the four finishes it
+      // ---- this warpgroup is done with the row group: the last of the WG finishes it
       __syncwarp();
       tp_wg_sync(g);                                       // all partial sums of this warpgroup are in shared memory
       if (t128 == 0) {
@@ -569,7 +642,7 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
         TpFinishArgs fa;
         fa.jsplit = a.jsplit; fa.N = N; fa.C = C; fa.ldn = a.ldn; fa.has_mask = a.has_mask; fa.flags = a.flags;
         fa.gpart = a.gpart; fa.gcount = a.gcount; fa.m_out = a.m_out; fa.coors_out = a.coors_out;
-        tp_finish_item<GEN>(fa, part + (size_t)buf * TP_CWARPS * TP_TI * PW, misc, xi, item, b, i0, rows_valid, active_wgs, g, t128);
+        tp_finish_item<GEN, CWARPS>(fa, part + (size_t)buf * CWARPS * TP_TI * PW, misc, xi, item, b, i0, rows_valid, active_wgs, g, t128);
         tp_wg_sync(g);                                     // every reader of ring slot `buf` is done
         const int nxt = item + 2 * gridDim.x;
         if (nxt < n_items) stage_item(nxt, buf, t128, [&]() { tp_wg_sync(g); });
