@@ -74,7 +74,9 @@ inline int sm_count(int* out) {
 
 // Neighbour lists of a layer with k > 0 (egnn_pytorch.py:237-260), ranked into *nbr_idx / *nbr_ok (workspace arrays
 // of [B,N,k]); in edge-list mode (io.nbr_idx set) the pointers are redirected to the caller's lists and *nbr_ok to null.
-int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st);
+// box: [B,C] periodic box lengths in the coordinates' type (distances are minimum-image distances), or null.
+int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
+                     const void* box = nullptr);
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {
@@ -179,6 +181,21 @@ template <> __device__ __forceinline__ double fma_t<double>(double a, double b, 
 template <typename T> __device__ __forceinline__ T sq_acc(T a, T acc);
 template <> __device__ __forceinline__ float sq_acc<float>(float a, float acc) { return __fadd_rn(acc, __fmul_rn(a, a)); }
 template <> __device__ __forceinline__ double sq_acc<double>(double a, double acc) { return __dadd_rn(acc, __dmul_rn(a, a)); }
+
+// ------------------------------------------------------------------ periodic boundaries (minimum image)
+// Axis c of graph b's box as the kernels use it: the length L and 1/L, both 0 on an axis that is not periodic (L = 0
+// or +inf) and beyond C, so that min_image leaves such an axis unchanged.  Read once per row or CTA, never per pair.
+template <typename T>
+__device__ __forceinline__ void box_axis(const T* box, int b, int C, int c, T& L, T& inv) {
+  const T l = c < C ? box[(size_t)b * C + c] : T(0);
+  const bool periodic = l > T(0) && l < T(INFINITY);
+  L = periodic ? l : T(0);
+  inv = periodic ? T(1) / l : T(0);
+}
+// rel - L rint(rel / L): the minimum-image difference (rounding half to even, as rintf / rint / np.rint)
+template <typename T> __device__ __forceinline__ T min_image(T r, T L, T inv);
+template <> __device__ __forceinline__ float min_image<float>(float r, float L, float inv) { return fmaf(-L, rintf(r * inv), r); }
+template <> __device__ __forceinline__ double min_image<double>(double r, double L, double inv) { return fma(-L, rint(r * inv), r); }
 
 // 4 consecutive elements, 4-element aligned.
 template <typename T> struct Vec4;

@@ -94,7 +94,7 @@ static int launch_colsum(const T* X, long ld, int rows, int cols, T* out, cudaSt
 // W2 silu(pre1) of every pair into pre2 when the forward did not keep it, by the forward's own edge kernels (with
 // the forward's dropout masks): for dense graphs the register-tiled kernel's split-H phase 1 over one split, which
 // stores exactly that; for neighbour lists pair_kernel with no node or coordinate update.
-template <typename T, int MP>
+template <typename T, int MP, bool PBC>
 static int recompute_pre2(const BwdArgs<T>& a, T* pre2, cudaStream_t st) {
   PairArgs<T> f;
   f.s = a.s; f.L = a.L; f.flags = a.flags; f.has_mask = a.has_mask; f.TS = a.TS; f.clamp = a.clamp;
@@ -104,23 +104,25 @@ static int recompute_pre2(const BwdArgs<T>& a, T* pre2, cudaStream_t st) {
   f.hpart = nullptr; f.hsplit = 1; f.phase = 0;
   f.pre2_out = nullptr;
   f.drop = a.drop;
+  f.box = a.box;
   if (a.s.k > 0) {
     f.flags &= ~(uint32_t)(EGNN_FLAG_UPDATE_FEATS | EGNN_FLAG_UPDATE_COORS);
     f.pre2_out = pre2;
-    return launch_pair<T, MP>(f, st);
+    return launch_pair<T, MP, PBC>(f, st);
   }
   f.hpart = pre2; f.phase = 1;
-  return launch_pair_dense<T, MP>(f, st);
+  return launch_pair_dense<T, MP, PBC>(f, st);
 }
 
-// BLK: a row block (its own instantiations, so that the whole-graph kernels keep their plain row arithmetic)
-template <typename T, int MP, bool KNN, bool BLK>
+// BLK: a row block (its own instantiations, so that the whole-graph kernels keep their plain row arithmetic).
+// PBC: periodic geometry in bwd1 / bwd3 (bwd2 reads the pair records only).
+template <typename T, int MP, bool KNN, bool BLK, bool PBC>
 static int launch_pair_bwd(const BwdArgs<T>& a, cudaStream_t st) {
   const Dims& s = a.s;
   const int rows = s.row1 - s.row0;                 // the i-rows of the call (all N unless a row block); the last CTA
                                                     // of each grid masks the rows past row1
   const dim3 g1(ceil_div(rows, PAIR_THREADS / a.TS), s.B);
-  EGNN_TRY(launch_simt(pair_bwd1_kernel<T, MP, KNN, BLK>, g1, PAIR_THREADS,
+  EGNN_TRY(launch_simt(pair_bwd1_kernel<T, MP, KNN, BLK, PBC>, g1, PAIR_THREADS,
                        bwd1_smem_bytes<T>(s, a.L, (a.flags & EGNN_FLAG_SOFT_EDGES) != 0), st, a));
   // bwd2: distance channel only (QR = 1), up to 8 channels in registers (lists only, QR = 8) or any (QR = 0); the
   // dropout masks in their own instantiations
@@ -141,14 +143,27 @@ static int launch_pair_bwd(const BwdArgs<T>& a, cudaStream_t st) {
     else bwd2 = drop ? pair_bwd2_dense_kernel<T, MP, 0, true, BLK> : pair_bwd2_dense_kernel<T, MP, 0, false, BLK>;
   }
   EGNN_TRY(launch_simt(bwd2, g2, BW2_TH, smem2, st, a));
-  pair_bwd3_kernel<T, KNN, BLK><<<g1, PAIR_THREADS, 0, st>>>(a);
+  pair_bwd3_kernel<T, KNN, BLK, PBC><<<g1, PAIR_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
 }
 
+// The edge step reversed for one choice of (row block, neighbour lists, periodic box).
+template <typename T, bool PBC>
+static int launch_edge_bwd(const BwdArgs<T>& a, T* pre2, bool saved, bool part, cudaStream_t st) {
+  const int MP = a.L.MP;
+  if (!saved) EGNN_TRY((MP == 16 ? recompute_pre2<T, 16, PBC>(a, pre2, st) : recompute_pre2<T, 32, PBC>(a, pre2, st)));
+  if (part) {
+    if (a.s.k > 0) return MP == 16 ? launch_pair_bwd<T, 16, true, true, PBC>(a, st) : launch_pair_bwd<T, 32, true, true, PBC>(a, st);
+    return MP == 16 ? launch_pair_bwd<T, 16, false, true, PBC>(a, st) : launch_pair_bwd<T, 32, false, true, PBC>(a, st);
+  }
+  if (a.s.k > 0) return MP == 16 ? launch_pair_bwd<T, 16, true, false, PBC>(a, st) : launch_pair_bwd<T, 32, true, false, PBC>(a, st);
+  return MP == 16 ? launch_pair_bwd<T, 16, false, false, PBC>(a, st) : launch_pair_bwd<T, 32, false, false, PBC>(a, st);
+}
+
 template <typename T>
 int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed, const EgnnLayerIO& io,
-                         const void* fwd_ws, const EgnnLayerGrads& gr, void* ws, size_t ws_bytes, cudaStream_t st) {
+                  const void* box, const void* fwd_ws, const EgnnLayerGrads& gr, void* ws, size_t ws_bytes, cudaStream_t st) {
   const Dims s = make_dims(d);
   const SimtPackLayout L = simt_pack_layout(s);
   const SimtWs fl = simt_ws_layout(s, sizeof(T), d.flags);
@@ -302,14 +317,9 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
   } else {
     a.TS = 32; a.TI2 = 32;
   }
-  if (!saved) EGNN_TRY((L.MP == 16 ? recompute_pre2<T, 16>(a, pre2, st) : recompute_pre2<T, 32>(a, pre2, st)));
-  if (part) {
-    if (s.k > 0) EGNN_TRY((L.MP == 16 ? launch_pair_bwd<T, 16, true, true>(a, st) : launch_pair_bwd<T, 32, true, true>(a, st)));
-    else EGNN_TRY((L.MP == 16 ? launch_pair_bwd<T, 16, false, true>(a, st) : launch_pair_bwd<T, 32, false, true>(a, st)));
-  } else {
-    if (s.k > 0) EGNN_TRY((L.MP == 16 ? launch_pair_bwd<T, 16, true, false>(a, st) : launch_pair_bwd<T, 32, true, false>(a, st)));
-    else EGNN_TRY((L.MP == 16 ? launch_pair_bwd<T, 16, false, false>(a, st) : launch_pair_bwd<T, 32, false, false>(a, st)));
-  }
+  a.box = static_cast<const T*>(box);
+  if (box) EGNN_TRY((launch_edge_bwd<T, true>(a, pre2, saved, part, st)));
+  else EGNN_TRY((launch_edge_bwd<T, false>(a, pre2, saved, part, st)));
 
   // ---- per-node tables reversed: A = h W1[:, :dim]^T + b1, B = h W1[:, dim:2dim]^T.  dL/dA is 0 outside the row block,
   // so its terms run over the block's rows; dL/dB (every j) over all rows

@@ -237,11 +237,11 @@ int pair_wg() {
   return e && strtol(e, nullptr, 10) == 4 ? 4 : 2;
 }
 
-template <bool GEN, int WG>
+template <bool GEN, int WG, bool PBC = false>
 int launch_tc_pair(const TcPairArgs& a, int grid, size_t smem, cudaStream_t st) {
   constexpr int PPW = TP_JB / (4 * WG);
-  EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<GEN, WG, PPW>, smem)));
-  tc_pair_kernel<GEN, WG, PPW><<<grid, WG * 128, smem, st>>>(a);
+  EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<GEN, WG, PPW, PBC>, smem)));
+  tc_pair_kernel<GEN, WG, PPW, PBC><<<grid, WG * 128, smem, st>>>(a);
   count_pair_layout(WG);
   return EGNN_OK;
 }
@@ -300,7 +300,7 @@ int fast_workspace_bytes(const EgnnLayerDesc& d, size_t* out) {
 }
 
 int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed, const EgnnLayerIO& io,
-                 void* ws, size_t ws_bytes, cudaStream_t st) {
+                 const void* box, void* ws, size_t ws_bytes, cudaStream_t st) {
   (void)w;
   EGNN_TRY(fast_supported(d));
   const FastDims f = fast_dims(d);
@@ -379,6 +379,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     a.mask = io.mask;
     a.m_out = uf ? node_in + s.dim : nullptr;
     a.coors_out = uc ? static_cast<float*>(io.coors_out) : nullptr;
+    a.box = static_cast<const float*>(box);
     if (f.L > 0 && !io.edge_labels) return EGNN_ERR_NULL;
     if (s.edge_dim > 0 && !io.edges) return EGNN_ERR_NULL;
     int sms = 0;
@@ -402,8 +403,11 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
       if (items < 2 * sms) a.skew_ns = 0;                      // too few row groups per CTA for the de-phasing to pay
       // 2 warpgroups (2 warps per SM sub-partition); the lean instantiation runs 4 when asked for and the shared memory
       // allows.  The generic one always runs 2: its row-outermost chunk loop holds the pre-activations of a whole chunk
-      // and does not fit 128 registers.
-      if (pair_is_lean(f)) {
+      // and does not fit 128 registers.  A periodic layer runs the 2-warpgroup periodic instantiations (DESIGN section 5).
+      if (box) {
+        if (pair_is_lean(f)) EGNN_TRY((launch_tc_pair<false, 2, true>(a, grid, tc_pair_smem_bytes<false, 2>(f.Hp, 1), st)));
+        else EGNN_TRY((launch_tc_pair<true, 2, true>(a, grid, tc_pair_smem_bytes<true, 2>(f.Hp, f.QT, 1 + 2 * f.s.F), st)));
+      } else if (pair_is_lean(f)) {
         const size_t smem4 = tc_pair_smem_bytes<false, 4>(f.Hp, 1);
         if (pair_wg() == 4 && smem4 <= 227 * 1024) EGNN_TRY((launch_tc_pair<false, 4>(a, grid, smem4, st)));
         else EGNN_TRY((launch_tc_pair<false, 2>(a, grid, tc_pair_smem_bytes<false, 2>(f.Hp, 1), st)));
@@ -416,7 +420,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
   } else {         // neighbour lists: distance + top-k select, then the gathered fused edge kernel
     int32_t* nbr_idx = reinterpret_cast<int32_t*>(base + wl.nbr_idx);
     uint8_t* nbr_ok = base + wl.nbr_ok;
-    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st));
+    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box));
     StageTimer tm(st, STAGE_PAIR);
     TcKnnArgs a{};
     a.B = s.B; a.N = s.N; a.Hp = f.Hp; a.ldn = f.Kn; a.dim = s.dim; a.k = s.k; a.edge_dim = s.edge_dim;
@@ -436,6 +440,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     a.nbr_idx = nbr_idx; a.nbr_ok = nbr_ok;
     a.m_out = uf ? node_in + s.dim : nullptr;
     a.coors_out = uc ? static_cast<float*>(io.coors_out) : nullptr;
+    a.box = static_cast<const float*>(box);
     const int mode = knn_mode(f);
     const int rows = tc_knn_rows_per_cta(f.Hp, mode, f.QT);         // 8 (two CTAs per SM) when shared memory allows
     const size_t smem = tc_knn_smem_bytes(f.Hp, mode, f.QT, rows);
@@ -443,8 +448,13 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     if (R > 0) {
 #define EGNN_TC_KNN_LAUNCH(MODE_, ROWS_)                                                  \
   do {                                                                              \
-    EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_>, smem)));             \
-    tc_knn_kernel<MODE_, ROWS_><<<grid, ROWS_ * 32, smem, st>>>(a);                 \
+    if (box) {                                                                      \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, true>, smem)));     \
+      tc_knn_kernel<MODE_, ROWS_, true><<<grid, ROWS_ * 32, smem, st>>>(a);         \
+    } else {                                                                        \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_>, smem)));           \
+      tc_knn_kernel<MODE_, ROWS_><<<grid, ROWS_ * 32, smem, st>>>(a);               \
+    }                                                                               \
   } while (0)
       if (mode == TK_LEAN) {
         if (rows == 8) EGNN_TC_KNN_LAUNCH(TK_LEAN, 8); else EGNN_TC_KNN_LAUNCH(TK_LEAN, 16);

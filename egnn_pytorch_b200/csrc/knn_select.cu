@@ -27,13 +27,19 @@ struct SelArgs {
   T valid_radius;
   int32_t* out_idx;
   uint8_t* out_ok;
+  const T* box;              // [B,C] periodic box lengths (PBC instantiations only)
 };
 
-template <typename T>
-__device__ __forceinline__ T rank_of(const SelArgs<T>& a, int b, int i, int j, const T* xi, bool mask_i) {
+// pb (PBC only): the box of graph b as L[8] | 1/L[8] (box_axis)
+template <typename T, bool PBC>
+__device__ __forceinline__ T rank_of(const SelArgs<T>& a, int b, int i, int j, const T* xi, bool mask_i, const T* pb) {
   const T* xj = a.coors + ((size_t)b * a.N + j) * a.C;
   T d = T(0);
-  for (int c = 0; c < a.C; ++c) d = sq_acc<T>(xi[c] - xj[c], d);
+  for (int c = 0; c < a.C; ++c) {
+    T r = xi[c] - xj[c];
+    if constexpr (PBC) r = min_image<T>(r, pb[c], pb[8 + c]);
+    d = sq_acc<T>(r, d);
+  }
   if (a.mask && !(mask_i && a.mask[(size_t)b * a.N + j])) d = T(1e5);
   if (a.adj) {
     if (i == j) d = T(-1);
@@ -92,7 +98,8 @@ inline size_t sel_smem_bytes(int C, int warps = SEL_WARPS_MAX) {
 
 // CDIM = 3: the coordinate loops are exactly three steps (the generic instantiation, CDIM = 0, issues all eight predicated
 // steps per candidate -- 125 instead of ~55 instructions per trip of the scan, which is 63 % of the kernel; ncu source page)
-template <typename T, int SEL_WARPS, int CDIM>
+// PBC: ranks by the minimum-image distance under a.box.
+template <typename T, int SEL_WARPS, int CDIM, bool PBC = false>
 __global__ void __launch_bounds__(SEL_WARPS * 32)
 knn_warp_select_kernel(const SelArgs<T> a) {
   constexpr int NC = CDIM ? CDIM : 8;
@@ -111,6 +118,11 @@ knn_warp_select_kernel(const SelArgs<T> a) {
 #pragma unroll
   for (int c = 0; c < NC; ++c) xi[c] = (CDIM || c < a.C) ? a.coors[row * a.C + c] : T(0);
   const bool mask_i = a.mask ? a.mask[row] != 0 : true;
+  T bl[PBC ? NC : 1], binv[PBC ? NC : 1];          // the box of graph b, once per row (box_axis)
+  if constexpr (PBC) {
+#pragma unroll
+    for (int c = 0; c < NC; ++c) box_axis<T>(a.box, b, a.C, c, bl[c], binv[c]);
+  }
   const uint8_t* adjrow = a.adj ? a.adj + ((size_t)(a.adj_batched ? b : 0) * a.N + i) * a.N : nullptr;
   const T INF = T(INFINITY);
   const int IMAX = 0x7fffffff;
@@ -147,7 +159,11 @@ knn_warp_select_kernel(const SelArgs<T> a) {
           T d = T(0);
 #pragma unroll
           for (int c = 0; c < NC; ++c)
-            if (CDIM || c < a.C) d = sq_acc<T>(xi[c] - xs[c * SEL_JC + jj], d);
+            if (CDIM || c < a.C) {
+              T r = xi[c] - xs[c * SEL_JC + jj];
+              if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
+              d = sq_acc<T>(r, d);
+            }
           if (a.mask && !(mask_i && ms[jj])) d = T(1e5);
           if (adjrow) {
             if (i == j) d = T(-1);
@@ -199,7 +215,7 @@ knn_warp_select_kernel(const SelArgs<T> a) {
 }
 
 // k > 32: block-wide bitonic sort of all N candidates in shared memory.
-template <typename T>
+template <typename T, bool PBC = false>
 __global__ void __launch_bounds__(256)
 knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   extern __shared__ __align__(16) unsigned char sel_smem[];
@@ -209,8 +225,15 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   const int b = row / a.N, i = row % a.N;
   const T* xi = a.coors + (size_t)row * a.C;
   const bool mask_i = a.mask ? a.mask[row] != 0 : true;
+  T* pb = nullptr;
+  if constexpr (PBC) {
+    __shared__ T box_s[16];
+    pb = box_s;
+    if (threadIdx.x < 8) box_axis<T>(a.box, b, a.C, threadIdx.x, pb[threadIdx.x], pb[8 + threadIdx.x]);
+    __syncthreads();
+  }
   for (int j = threadIdx.x; j < Npad; j += blockDim.x) {
-    keys[j] = j < a.N ? rank_of<T>(a, b, i, j, xi, mask_i) : T(INFINITY);
+    keys[j] = j < a.N ? rank_of<T, PBC>(a, b, i, j, xi, mask_i, pb) : T(INFINITY);
     idxs[j] = j < a.N ? j : 0x7fffffff;
   }
   __syncthreads();
@@ -236,10 +259,12 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   }
 }
 
-template <typename T>
+template <typename T, bool PBC>
 static int launch_select(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const uint8_t* adj,
-                         int adj_batched, double valid_radius, int32_t* out_idx, uint8_t* out_ok, cudaStream_t st) {
+                         int adj_batched, double valid_radius, int32_t* out_idx, uint8_t* out_ok, const void* box,
+                         cudaStream_t st) {
   SelArgs<T> a;
+  a.box = static_cast<const T*>(box);
   a.B = B; a.N = N; a.C = C; a.k = k;
   a.coors = static_cast<const T*>(coors);
   a.mask = mask; a.adj = adj; a.adj_batched = adj_batched;
@@ -251,9 +276,9 @@ static int launch_select(int B, int N, int C, int k, const void* coors, const ui
     int dev = 0;
     EGNN_CUDA_TRY(cudaGetDevice(&dev));
     if (dev < 64 && !attr_set[dev]) {
-      EGNN_CUDA_TRY(cudaFuncSetAttribute(knn_warp_select_kernel<T, 16, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      EGNN_CUDA_TRY(cudaFuncSetAttribute(knn_warp_select_kernel<T, 16, 0, PBC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)sel_smem_bytes<T>(8, 16)));
-      EGNN_CUDA_TRY(cudaFuncSetAttribute(knn_warp_select_kernel<T, 8, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      EGNN_CUDA_TRY(cudaFuncSetAttribute(knn_warp_select_kernel<T, 8, 0, PBC>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)sel_smem_bytes<T>(8, 8)));
       attr_set[dev] = true;
     }
@@ -264,32 +289,35 @@ static int launch_select(int B, int N, int C, int k, const void* coors, const ui
     dim3 grid(ceil_div(N, wide ? 16 : 8), B);
     const size_t smem = sel_smem_bytes<T>(C, wide ? 16 : 8);
     if (C == 3) {
-      if (wide) knn_warp_select_kernel<T, 16, 3><<<grid, 16 * 32, smem, st>>>(a);
-      else knn_warp_select_kernel<T, 8, 3><<<grid, 8 * 32, smem, st>>>(a);
+      if (wide) knn_warp_select_kernel<T, 16, 3, PBC><<<grid, 16 * 32, smem, st>>>(a);
+      else knn_warp_select_kernel<T, 8, 3, PBC><<<grid, 8 * 32, smem, st>>>(a);
     } else {
-      if (wide) knn_warp_select_kernel<T, 16, 0><<<grid, 16 * 32, smem, st>>>(a);
-      else knn_warp_select_kernel<T, 8, 0><<<grid, 8 * 32, smem, st>>>(a);
+      if (wide) knn_warp_select_kernel<T, 16, 0, PBC><<<grid, 16 * 32, smem, st>>>(a);
+      else knn_warp_select_kernel<T, 8, 0, PBC><<<grid, 8 * 32, smem, st>>>(a);
     }
   } else {
     int Npad = 1;
     while (Npad < N) Npad <<= 1;
     const size_t smem = (size_t)Npad * (sizeof(T) + sizeof(int));
     if (smem > 200 * 1024) return EGNN_ERR_UNSUPPORTED;     // N too large for the k>32 path
-    EGNN_CUDA_TRY(cudaFuncSetAttribute(knn_block_sort_kernel<T>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    knn_block_sort_kernel<T><<<rows, 256, smem, st>>>(a, Npad);
+    EGNN_CUDA_TRY(cudaFuncSetAttribute(knn_block_sort_kernel<T, PBC>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    knn_block_sort_kernel<T, PBC><<<rows, 256, smem, st>>>(a, Npad);
   }
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
 }
 
+// box: [B,C] periodic box lengths in the coordinates' type, or null (the layer's select only: egnn_knn_select has none)
 int knn_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
                         const uint8_t* adj, int adj_batched, double valid_radius, int32_t* out_idx,
-                        uint8_t* out_ok, cudaStream_t st) {
+                        uint8_t* out_ok, cudaStream_t st, const void* box = nullptr) {
   if (!coors || !out_idx) return EGNN_ERR_NULL;
   if (B <= 0 || B > 65535 || N <= 0 || C <= 0 || C > 8 || k <= 0 || k > N) return EGNN_ERR_SHAPE;
   if (dtype == EGNN_DTYPE_F64)
-    return launch_select<double>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, st);
-  return launch_select<float>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, st);
+    return box ? launch_select<double, true>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st)
+               : launch_select<double, false>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
+  return box ? launch_select<float, true>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st)
+             : launch_select<float, false>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
 }
 
 // only_sparse_neighbors WITH a node mask (egnn_pytorch.py:249-260, :296): valid_radius is 0, so the only slots whose
@@ -354,7 +382,8 @@ int adj_neighbors_dispatch(int B, int N, int k, const uint8_t* adj, int adj_batc
   return EGNN_OK;
 }
 
-int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st) {
+int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
+                     const void* box) {
   if (io.nbr_idx) {                                  // edge-list mode: the caller's lists, no ranking
     *nbr_idx = const_cast<int32_t*>(io.nbr_idx);
     *nbr_ok = nullptr;
@@ -368,7 +397,7 @@ int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nb
   const double vr = (d.flags & EGNN_FLAG_ONLY_SPARSE) ? 0.0 : d.valid_radius;     // egnn_pytorch.py:250
   // coordinates are fp64 for the fp64 layer and fp32 otherwise (bf16 layers included)
   return knn_select_dispatch(d.dtype == EGNN_DTYPE_F64 ? EGNN_DTYPE_F64 : EGNN_DTYPE_F32, d.B, d.N, d.C, d.k, io.coors,
-                             io.mask, io.adj, adj_batched, vr, *nbr_idx, *nbr_ok, st);
+                             io.mask, io.adj, adj_batched, vr, *nbr_idx, *nbr_ok, st, box);
 }
 
 }  // namespace egnn

@@ -68,6 +68,7 @@ struct BwdArgs {
   T* g_coors;                     // [B,N,C], pre-loaded with g_coors_out
   T* g_edges;                     // [B,N,N,edge_dim], [B,N,k,edge_dim] under EGNN_FLAG_EDGES_PER_SLOT, | null
   DropCfg drop;                   // the forward's dropout configuration (masks are regenerated, never stored)
+  const T* box;                   // [B,C] the forward's periodic box lengths (PBC instantiations only)
 };
 
 template <typename T> __device__ __forceinline__ T dsilu_from(T x, T sg) { return sg * (T(1) + x * (T(1) - sg)); }
@@ -117,7 +118,7 @@ inline size_t bwd1_smem_bytes(const Dims& s, const SimtPackLayout& L, bool soft)
   return round_up(n * sizeof(T), 16) + 16;
 }
 
-template <typename T, int MP, bool KNN, bool BLK>
+template <typename T, int MP, bool KNN, bool BLK, bool PBC = false>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd1_kernel(const BwdArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -126,6 +127,12 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
   const int TS = a.TS, TI = PAIR_THREADS / TS;
   const int g = tid / TS, sl = tid % TS;
   const int b = blockIdx.y;
+  T* pb = nullptr;
+  if constexpr (PBC) {
+    __shared__ T box_s[2 * PAIR_CMAX];
+    pb = box_s;
+    stage_box<T>(pb, a.box, b, s.C);
+  }
   const int i_raw = rows_begin<BLK>(s) + blockIdx.x * TI + g;
   const bool row_valid = i_raw < rows_end<BLK>(s);
   const int i = row_valid ? i_raw : rows_begin<BLK>(s);
@@ -200,7 +207,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
     const bool pair_valid = ps.valid;
     const size_t pair = node_i * s.N + j;
     T rel[PAIR_CMAX];
-    const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
+    const T d = pair_geometry<T, PBC>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel, pb);
     if (pair_exists) {
       T* r = a.rec + rec_index<KNN, BLK>(s, b, s.N, J, i, sidx) * a.rl.R;
       const T* erow = edge_row(a.edges, KNN && (a.flags & EGNN_FLAG_EDGES_PER_SLOT), node_i, sidx, j, s.N, s.k, s.edge_dim);
@@ -835,9 +842,10 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
 }
 
 // =====================================================================================
-// bwd3: dL/d(dist) -> coordinates and edges.  Same thread <-> pair mapping as bwd1.
+// bwd3: dL/d(dist) -> coordinates and edges.  Same thread <-> pair mapping as bwd1.  PBC: the minimum image has the
+// derivative of x_i - x_j (rint is piecewise constant), so only rel changes.
 // =====================================================================================
-template <typename T, bool KNN, bool BLK>
+template <typename T, bool KNN, bool BLK, bool PBC = false>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd3_kernel(const BwdArgs<T> a) {
   const Dims& s = a.s;
@@ -845,6 +853,12 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
   const int TS = a.TS, TI = PAIR_THREADS / TS;
   const int g = tid / TS, sl = tid % TS;
   const int b = blockIdx.y;
+  T* pb = nullptr;
+  if constexpr (PBC) {
+    __shared__ T box_s[2 * PAIR_CMAX];
+    pb = box_s;
+    stage_box<T>(pb, a.box, b, s.C);
+  }
   const int i_raw = rows_begin<BLK>(s) + blockIdx.x * TI + g;
   const bool row_valid = i_raw < rows_end<BLK>(s);
   const int i = row_valid ? i_raw : rows_begin<BLK>(s);
@@ -866,7 +880,7 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
     const int j = ps.j;
     const T* r = a.rec + rec_index<KNN, BLK>(s, b, s.N, J, i, sidx) * a.rl.R;
     T rel[PAIR_CMAX];
-    const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
+    const T d = pair_geometry<T, PBC>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel, pb);
     T gd = r[a.rl.gf + qd] + r[a.rl.gdn];
     for (int q = 0; q < s.F; ++q) {                        // fourier_encode_dist :34-41 reversed
       const T sc = T(1 << q);

@@ -76,16 +76,16 @@ static int launch_simt(void (*kernel)(Arg), dim3 grid, int threads, size_t smem,
   return EGNN_OK;
 }
 
-// The edge step over neighbour lists.
-template <typename T, int MP>
+// The edge step over neighbour lists.  PBC: the periodic instantiations (a.box set).
+template <typename T, int MP, bool PBC = false>
 static int launch_pair(const PairArgs<T>& a, cudaStream_t st) {
   dim3 grid(ceil_div(a.s.row1 - a.s.row0, PAIR_THREADS / a.TS), a.s.B);
-  void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_kernel<T, MP, true> : pair_kernel<T, MP, false>;
+  void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_kernel<T, MP, true, PBC> : pair_kernel<T, MP, false, PBC>;
   return launch_simt(kernel, grid, PAIR_THREADS, pair_smem_bytes<T>(a.s, a.L), st, a);
 }
 
 // The dense edge step at PP rows per thread; a.hsplit > 1 runs it as two phases over a split hidden axis.
-template <typename T, int MP, int PP>
+template <typename T, int MP, int PP, bool PBC>
 static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
   const size_t smem = pair_tiled_smem_bytes<T>(a.s, a.L, PP);
   dim3 grid(ceil_div(a.s.row1 - a.s.row0, 4 * PP), a.s.B);
@@ -93,21 +93,22 @@ static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
     PairArgs<T> a1 = a, a2 = a;
     a1.phase = 1; a2.phase = 2;
     a1.pre2_out = nullptr;                            // partial sums; phase 2 holds the full ones
-    EGNN_TRY(launch_simt(pair_dense_tiled_kernel<T, MP, PP, false>, dim3(grid.x, grid.y, a.hsplit), PAIR_THREADS, smem, st, a1));
-    return launch_simt(pair_dense_tiled_kernel<T, MP, PP, false>, grid, PAIR_THREADS, smem, st, a2);
+    EGNN_TRY(launch_simt(pair_dense_tiled_kernel<T, MP, PP, false, PBC>, dim3(grid.x, grid.y, a.hsplit), PAIR_THREADS, smem, st, a1));
+    return launch_simt(pair_dense_tiled_kernel<T, MP, PP, false, PBC>, grid, PAIR_THREADS, smem, st, a2);
   }
-  void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_dense_tiled_kernel<T, MP, PP, true> : pair_dense_tiled_kernel<T, MP, PP, false>;
+  void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_dense_tiled_kernel<T, MP, PP, true, PBC>
+                                                        : pair_dense_tiled_kernel<T, MP, PP, false, PBC>;
   return launch_simt(kernel, grid, PAIR_THREADS, smem, st, a);
 }
 
 // The dense edge step at two rows per thread where its shared memory fits, else at one (fp64 with m_dim > 16:
 // one always).
-template <typename T, int MP>
+template <typename T, int MP, bool PBC = false>
 static int launch_pair_dense(const PairArgs<T>& a, cudaStream_t st) {
   constexpr int PP = (MP == 32 && sizeof(T) == 8) ? 1 : 2;
-  const int rc = launch_pair_tiled<T, MP, PP>(a, st);
+  const int rc = launch_pair_tiled<T, MP, PP, PBC>(a, st);
   if (PP == 1 || rc != EGNN_ERR_UNSUPPORTED) return rc;
-  return launch_pair_tiled<T, MP, 1>(a, st);
+  return launch_pair_tiled<T, MP, 1, PBC>(a, st);
 }
 
 template <typename T, int ACT, bool RES>

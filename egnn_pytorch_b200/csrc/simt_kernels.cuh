@@ -304,6 +304,7 @@ struct PairArgs {
   T* pre2_out;                          // optional: [B,N,J][MP] W2 silu(pre1) per pair (J = N dense, k lists), kept for backward;
                                         // rows by pair_row ([B,R,J][MP] for a row block under EGNN_FLAG_ROW_PARTIAL_GRADS)
   DropCfg drop;                         // training-mode dropout of edge_mlp / coors_mlp hidden pre-activations (thr 0 = off)
+  const T* box;                         // [B,C] periodic box lengths (read by the PBC instantiations only)
 };
 
 // Slot `sidx` of row node_i -> neighbour j.  Dense: j = sidx.  Lists: j and its ok flag from the list; a -1 entry
@@ -326,16 +327,29 @@ __device__ __forceinline__ PairSlot pair_slot(const int32_t* nbr_idx, const uint
   return p;
 }
 
-// rel = x_i - x_j (zero beyond C) and the squared distance d (egnn_pytorch.py:232-233)
-template <typename T>
-__device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&rel)[PAIR_CMAX]) {
+// rel = x_i - x_j (zero beyond C) and the squared distance d (egnn_pytorch.py:232-233).  PBC: rel is the minimum image
+// under the box `pb` staged by stage_box.
+template <typename T, bool PBC = false>
+__device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&rel)[PAIR_CMAX], const T* pb = nullptr) {
   T d = T(0);
 #pragma unroll
   for (int c = 0; c < PAIR_CMAX; ++c) {
     rel[c] = T(0);
-    if (c < C) { rel[c] = xi[c] - xj[c]; d = sq_acc<T>(rel[c], d); }
+    if (c < C) {
+      rel[c] = xi[c] - xj[c];
+      if constexpr (PBC) rel[c] = min_image<T>(rel[c], pb[c], pb[PAIR_CMAX + c]);
+      d = sq_acc<T>(rel[c], d);
+    }
   }
   return d;
+}
+
+// Graph b's box in shared memory for pair_geometry: L[PAIR_CMAX] | 1/L[PAIR_CMAX] (box_axis), staged once per CTA
+// (every CTA of the pair kernels works on one graph).  Ends with a barrier, so all threads of the CTA must call it.
+template <typename T>
+__device__ __forceinline__ void stage_box(T* pb, const T* box, int b, int C) {
+  if (threadIdx.x < PAIR_CMAX) box_axis<T>(box, b, C, threadIdx.x, pb[threadIdx.x], pb[PAIR_CMAX + threadIdx.x]);
+  __syncthreads();
 }
 
 // Scalar channel q of a pair: fourier_encode_dist (egnn_pytorch.py:34-41), the squared distance, then the continuous
@@ -407,8 +421,8 @@ inline size_t pair_smem_bytes(const Dims& s, const SimtPackLayout& L) {
 }
 
 // Neighbour lists: 128 threads per CTA arranged as TI row-groups x TS slots (TS lanes of one warp).
-// BLK: pre2_out is block-relative (pair_row).
-template <typename T, int MP, bool BLK>
+// BLK: pre2_out is block-relative (pair_row).  PBC: minimum-image geometry under a.box.
+template <typename T, int MP, bool BLK, bool PBC = false>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -417,6 +431,12 @@ pair_kernel(const PairArgs<T> a) {
   const int TS = a.TS, TI = PAIR_THREADS / TS;
   const int g = tid / TS, sl = tid % TS;
   const int b = blockIdx.y;
+  T* pb = nullptr;
+  if constexpr (PBC) {
+    __shared__ T box_s[2 * PAIR_CMAX];
+    pb = box_s;
+    stage_box<T>(pb, a.box, b, s.C);
+  }
   const int i_raw = s.row0 + blockIdx.x * TI + g;
   const bool row_valid = i_raw < s.row1;
   const int i = row_valid ? i_raw : s.row0;
@@ -463,7 +483,7 @@ pair_kernel(const PairArgs<T> a) {
     const bool pair_valid = ps.valid;
     const size_t pair = node_i * s.N + j;
     T rel[PAIR_CMAX];
-    const T d = pair_geometry<T>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel);
+    const T d = pair_geometry<T, PBC>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel, pb);
     // ---- per-pair scalar channels other than d go through shared memory
     if (s.Q > 1) {
       const T* erow = edge_row(a.edges, a.flags & EGNN_FLAG_EDGES_PER_SLOT, node_i, sidx, j, s.N, s.k, s.edge_dim);
@@ -601,13 +621,20 @@ inline size_t pair_tiled_smem_bytes(const Dims& s, const SimtPackLayout& L, int 
   return round_up(n * sizeof(T), 16) + 16;
 }
 
-template <typename T, int MP, int PP, bool BLK>     // BLK: pre2_out / hpart are block-relative (pair_row)
+// BLK: pre2_out / hpart are block-relative (pair_row).  PBC: minimum-image geometry under a.box.
+template <typename T, int MP, int PP, bool BLK, bool PBC = false>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_dense_tiled_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
   const Dims& s = a.s;
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int b = blockIdx.y;
+  T* pb = nullptr;
+  if constexpr (PBC) {
+    __shared__ T box_s[2 * PAIR_CMAX];
+    pb = box_s;
+    stage_box<T>(pb, a.box, b, s.C);
+  }
   const int U = 4 * s.m;
   const int qd = 2 * s.F;
   constexpr int RS = MP + PAIR_CMAX + 4;          // row-sum record: m[MP] | csum[CMAX] | cnt | pad
@@ -660,7 +687,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
     for (int p = 0; p < PP; ++p) {
       const size_t pair = ((size_t)b * s.N + irow[p]) * s.N + j;
       T rel[PAIR_CMAX];
-      d[p] = pair_geometry<T>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel);
+      d[p] = pair_geometry<T, PBC>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel, pb);
       lab[p] = a.labels ? a.labels[pair] : 0;
       if (s.Q > 1)
         for (int q = 0; q < s.Q; ++q)
@@ -802,7 +829,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
         const size_t pair = ((size_t)b * s.N + irow[p]) * s.N + j;
         const T w = pair_coord_weight<T, MP>(a, mm, w3s, b3s, w4s, misc, pair, pm, pair_valid, d[p]);
         T rel[PAIR_CMAX];
-        pair_geometry<T>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel);
+        pair_geometry<T, PBC>(a.coors + ((size_t)b * s.N + irow[p]) * s.C, xj, s.C, rel, pb);
 #pragma unroll
         for (int c = 0; c < PAIR_CMAX; ++c)
           if (c < s.C) rec[MP + c] = w * rel[c];

@@ -80,6 +80,7 @@ struct TcPairArgs {
   const uint8_t* mask;             // [B][N] | null
   __nv_bfloat16* m_out;            // node_in + dim (stride ldn) | null
   float* coors_out;                // [B][N][C] | null
+  const float* box;                // [B][C] periodic box lengths (PBC instantiations only)
 };
 
 template <bool GEN> struct TpCfg {
@@ -107,7 +108,10 @@ inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
   (void)Q;
   if (GEN) n += tc_pair_gen_scalar_bytes(Qf, Q - Qf);
   n += 8 * 8;                                               // mbarriers
-  return n + 256;
+  n += (size_t)2 * 2 * TP_CMAX * 4;                         // periodic box per ring slot, first in the carve-up (PBC only)
+  return n + 128;                                           // (the box took 128 of the 256 bytes of headroom: every
+                                                            //  instantiation keeps its size, so a periodic layer fits
+                                                            //  wherever the plain one does)
 }
 
 // named barrier over one warpgroup (ids 1..WG; id 0 is __syncthreads)
@@ -181,7 +185,8 @@ __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* 
         }
 }
 
-template <bool GEN, int WG, int PPW>
+// PBC: the pair geometry is the minimum image under a.box, at the distance and at the coordinate sum
+template <bool GEN, int WG, int PPW, bool PBC = false>
 __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a) {
   static_assert(WG * 4 * PPW == TP_JB && (PPW == 16 || PPW == 32), "a j-block is WG warpgroups x 4 warps x PPW pairs");
   static_assert(!GEN || WG == 2, "the generic chunk loop needs more than the 128 registers of 4 warpgroups");
@@ -195,7 +200,10 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
   extern __shared__ __align__(128) unsigned char sm[];
   const int Hp = a.Hp, N = a.N;
   const int Q = GEN ? a.Q : 1, C = GEN ? a.C : 3;
-  unsigned char* w2s = sm;                                                    // Hp*32 bytes
+  // PBC: the box of each ring slot's graph, [2][L[TP_CMAX] | 1/L[TP_CMAX]], first (a constant address); everything else
+  // moves up by its 128 bytes, which keeps the 128-byte alignment of the TMA destinations
+  float* boxs = reinterpret_cast<float*>(sm);
+  unsigned char* w2s = sm + (PBC ? 2 * 2 * TP_CMAX * 4 : 0);                  // Hp*32 bytes
   float* wqs = reinterpret_cast<float*>(w2s + (size_t)Hp * 32);               // [Q][Hp]
   float* As = wqs + (size_t)Q * Hp;                                           // [2][TI][Hp]
   float* epi = As + (size_t)2 * TP_TI * Hp;                                   // constants
@@ -248,6 +256,9 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
       const int r = t - TP_TI * XC;
       const size_t node = (size_t)b * N + (r < rows_valid ? i0 + r : i0);
       mki[buf * TP_TI + r] = (r < rows_valid) && (a.has_mask ? a.mask[node] != 0 : true);
+    } else if (PBC && t < TP_TI * XC + TP_TI + TP_CMAX) {
+      const int c = t - TP_TI * XC - TP_TI;
+      box_axis<float>(a.box, b, C, c, boxs[buf * 2 * TP_CMAX + c], boxs[buf * 2 * TP_CMAX + TP_CMAX + c]);
     }
     sync();
     if (t == 0) {
@@ -316,6 +327,13 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
       const float* Ab = As + (size_t)buf * TP_TI * Hp;
       const float* xi = xis + buf * TP_TI * XC;
       const uint32_t* mk = mki + buf * TP_TI;
+      const float* bx = PBC ? boxs + buf * 2 * TP_CMAX : nullptr;      // L | 1/L of graph b
+      // x_i - x_j, the minimum image under PBC
+      auto rel_c = [&](int i, int c, float xjc) {
+        const float r = xi[i * XC + c] - xjc;
+        if constexpr (PBC) return min_image<float>(r, bx[c], bx[TP_CMAX + c]);
+        return r;
+      };
       double* mypart = part + ((size_t)buf * CWARPS + warp) * TP_TI * PW;
       for (int x = lane; x < TP_TI * PW; x += 32) mypart[x] = 0.0;
       __syncwarp();
@@ -341,7 +359,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
           const int i = rb + r;
           float d = 0.f;
 #pragma unroll
-          for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float rc = xi[i * XC + c] - xj[c]; d = fmaf(rc, rc, d); }
+          for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float rc = rel_c(i, c, xj[c]); d = fmaf(rc, rc, d); }
           swg[i * TW + pp] = d;
           if (GEN) {
             int q = 1;
@@ -612,7 +630,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
 #pragma unroll
           for (int c = 0; c < PW - 17; ++c) {
             constexpr int NX = GEN ? TP_CMAX : 3;
-            v[16 + c] = (c < NX && (!GEN || c < C)) ? w * (xi[i * XC + (c < NX ? c : 0)] - xj[c < NX ? c : 0]) : 0.f;
+            v[16 + c] = (c < NX && (!GEN || c < C)) ? w * rel_c(i, c < NX ? c : 0, xj[c < NX ? c : 0]) : 0.f;
           }
           v[PW - 1] = pm ? 1.f : 0.f;
           // sum over the warp's pairs: the PPW lanes that hold row i (the whole warp, or one half of it)

@@ -29,6 +29,7 @@ import contextlib
 import ctypes as C
 import os
 import warnings
+import weakref
 
 import torch
 from torch import nn
@@ -164,9 +165,15 @@ class _EGNNLayerFunction(torch.autograd.Function):
             nat.check("egnn_layer_backward_workspace_bytes",
                       lib.egnn_layer_backward_workspace_bytes(C.byref(sv["desc"]), C.byref(nb)))
             ws = _workspace(dev, nb.value)
-            nat.check("egnn_layer_backward",
-                      lib.egnn_layer_backward(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]), C.byref(sv["io"]),
-                                              _ptr(sv["ws"]), C.byref(grads), _ptr(ws), ws.numel(), stream))
+            if sv["box"] is None:
+                nat.check("egnn_layer_backward",
+                          lib.egnn_layer_backward(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]), C.byref(sv["io"]),
+                                                  _ptr(sv["ws"]), C.byref(grads), _ptr(ws), ws.numel(), stream))
+            else:
+                nat.check("egnn_layer_backward_periodic",
+                          lib.egnn_layer_backward_periodic(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]),
+                                                           C.byref(sv["io"]), _ptr(sv["box"]), _ptr(sv["ws"]), C.byref(grads),
+                                                           _ptr(ws), ws.numel(), stream))
             if sv["rows"] is not None:
                 # a row block returns its inputs unchanged outside [r0, r1): the identity's gradient for those rows (the
                 # library's partial gradients cover the block's own outputs only)
@@ -291,7 +298,7 @@ class EGNN(nn.Module):
         return torch.float32
 
     # -------------------------------------------------------------- forward
-    def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, neighbor_edges=None,
+    def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, neighbor_edges=None, box=None,
                 _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
         """Reference signature `forward(feats, coors, edges=None, mask=None, adj_mat=None)` (egnn_pytorch.py:224).
 
@@ -302,20 +309,28 @@ class EGNN(nn.Module):
         `neighbor_edges` (additive, keyword-only, needs `neighbors`, replaces `edges`): float tensor
         [B, N, k, edge_dim] of edge features per neighbour slot -- slot s of node i holds the features of the edge
         neighbors[b, i, s] -> i -- so a sparse graph needs no [B, N, N, edge_dim] tensor.  Its gradient has the same
-        shape (0 in empty slots)."""
+        shape (0 in empty slots).
+
+        `box` (additive, keyword-only): periodic boundaries.  Float tensor of box lengths, [C] (shared by the batch) or
+        [B, C], on any device; every pair geometry x_i - x_j becomes its minimum image rel - L rint(rel / L) on the axes
+        with a finite L > 0 (L = 0 or inf: not periodic).  Distances, neighbour ranking, CoorsNorm and the coordinate
+        update follow; the output coordinates are not wrapped back into the box.  Orthorhombic boxes, one image per
+        neighbour, no gradient with respect to the box (a box that requires grad is rejected)."""
         if neighbor_edges is not None:
             edges = self._check_neighbor_edges(feats, edges, neighbors, neighbor_edges, _label_emb)
+        if box is not None:
+            _check_box(box, feats.shape[0], coors.shape[-1], self.__dict__)
         if torch.is_grad_enabled():             # (the parameter scan is skipped entirely under torch.no_grad())
             fields = self._state_fields()
             if (feats.requires_grad or coors.requires_grad or (edges is not None and edges.requires_grad) or
                     (_label_emb is not None and _label_emb.requires_grad) or any(p.requires_grad for _, _, _, p in fields)):
                 return self._forward_train(fields, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb,
-                                           _k_hint, _rows, neighbor_edges is not None)
+                                           _k_hint, _rows, neighbor_edges is not None, box)
             with torch.no_grad():
                 return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint,
-                                          _rows, slot_edges=neighbor_edges is not None)
+                                          _rows, slot_edges=neighbor_edges is not None, box=box)
         return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
-                                  slot_edges=neighbor_edges is not None)
+                                  slot_edges=neighbor_edges is not None, box=box)
 
     def _check_neighbor_edges(self, feats, edges, neighbors, neighbor_edges, label_emb):
         """Misuse of `neighbor_edges` raises here, before anything is staged or launched; -> the tensor to run with."""
@@ -333,7 +348,7 @@ class EGNN(nn.Module):
         return neighbor_edges
 
     def _forward_train(self, fields, feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
-                       slot_edges=False):
+                       slot_edges=False, box=None):
         """With a row range (`_rows=(r0, r1)`) the layer is differentiated as the function it returns: rows r0:r1 are the
         layer's output, every other row is its input unchanged.  The library's backward then yields this block's share
         of every gradient (EGNN_FLAG_ROW_PARTIAL_GRADS): the blocks of a partition of the rows sum to the full gradient."""
@@ -341,12 +356,12 @@ class EGNN(nn.Module):
 
         def run():
             return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
-                                      train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges)
+                                      train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges, box=box)
 
         return _EGNNLayerFunction.apply(run, feats, coors, edges, label_emb, *params)
 
     def _forward_impl(self, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
-                      train=False, param_fields=None, slot_edges=False):
+                      train=False, param_fields=None, slot_edges=False, box=None):
         """`slot_edges`: `edges` holds features per neighbour slot, [B, N, k, edge_dim] (forward's `neighbor_edges`)."""
         lib = nat.load()
         dev = _compute_device(feats)
@@ -397,7 +412,7 @@ class EGNN(nn.Module):
             kdt = torch.float32
         try:
             return self._run(lib, dev, kdt, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
-                             b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, train, param_fields, drop_p)
+                             b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, train, param_fields, drop_p, box)
         except nat.EgnnNativeError as e:
             if e.code != nat.ERR_UNSUPPORTED or kdt != torch.bfloat16:
                 raise
@@ -408,10 +423,10 @@ class EGNN(nn.Module):
                       f"running the fp32 SIMT kernels instead (about 5x slower, same results to fp32 accuracy)", UserWarning,
                       stacklevel=3)
         return self._run(lib, dev, torch.float32, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
-                         b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr)
+                         b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, box=box)
 
     def _run(self, lib, dev, kdt, feats, coors, edges, mask, adj_u8, labels, label_emb, b, n, c, k, flags,
-             cont_edge_dim, label_dim, rows, nbr=None, train=False, param_fields=None, drop_p=0.0):
+             cont_edge_dim, label_dim, rows, nbr=None, train=False, param_fields=None, drop_p=0.0, box=None):
         cdt = torch.float64 if kdt == torch.float64 else torch.float32
         st = self._staged(dev, kdt)
         T = dict(st["tensors"])
@@ -475,6 +490,9 @@ class EGNN(nn.Module):
                 st["packed"] = {pkey: packed}
 
             f_in, x_in, e_in = _as(feats, dev, kdt), _as(coors, dev, cdt), _as(edges, dev, kdt)
+            bx = None if box is None else _as(box, dev, cdt).expand(b, c).contiguous()     # [B, C], like coors
+            if train and bx is not None and bx.data_ptr() == box.data_ptr():
+                bx = bx.clone()                  # the backward must see the forward's box, whatever the caller does to it
             m_in, l_in = _as_u8(mask, dev), _as_u8(labels, dev)
             f_out = torch.empty_like(f_in)
             x_out = torch.empty_like(x_in)
@@ -510,18 +528,46 @@ class EGNN(nn.Module):
             # training keeps the workspace (per-node tables, pooled messages, neighbour lists) for backward
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if train else _workspace(dev, ws_bytes, stream_handle)
             if train or rows is None or rows[0] != rows[1]:      # an empty row block computes nothing in inference
-                nat.check("egnn_layer_forward",
-                          lib.egnn_layer_forward(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io), _ptr(ws),
-                                                 ws.numel(), stream))
+                if bx is None:
+                    nat.check("egnn_layer_forward",
+                              lib.egnn_layer_forward(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io), _ptr(ws),
+                                                     ws.numel(), stream))
+                else:
+                    nat.check("egnn_layer_forward_periodic",
+                              lib.egnn_layer_forward_periodic(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io), _ptr(bx),
+                                                              _ptr(ws), ws.numel(), stream))
         object.__setattr__(self, "last_path", _PATH_NAME[kdt])
         outs = (f_out if (f_out.dtype == feats.dtype and f_out.device == feats.device) else f_out.to(device=feats.device, dtype=feats.dtype),
                 x_out if (x_out.dtype == coors.dtype and x_out.device == coors.device) else x_out.to(device=coors.device, dtype=coors.dtype))
         if not train:
             return outs
         saved = dict(dev=dev, kdt=kdt, cdt=cdt, desc=desc, w=w, packed=packed, io=io, ws=ws, tensors=T,
-                     f_in=f_in, x_in=x_in, e_in=e_in, param_fields=param_fields, rows=rows,
+                     f_in=f_in, x_in=x_in, e_in=e_in, param_fields=param_fields, rows=rows, box=bx,
                      keep=(m_in, l_in, adj_u8, nbr, lab_w, pre2))      # everything io points at stays alive
         return outs + (saved,)
+
+
+def _check_box(box, b, c, cache):
+    """Misuse of `box=` raises ValueError here, before anything launches.  The value check (no negative or NaN length)
+    reads the box on the host.  It is skipped for the very tensor object this module checked last, unchanged since (the
+    same object alive and the same version counter: an in-place write bumps it, a write through `.data` does not), and
+    while a CUDA graph is being captured (GraphedForward checks the box in its warm-up calls)."""
+    if not torch.is_tensor(box) or not box.is_floating_point():
+        raise ValueError(f"box must be a float tensor of box lengths, got {type(box).__name__}"
+                         f"{'' if not torch.is_tensor(box) else ' ' + str(box.dtype)}")
+    if tuple(box.shape) not in ((c,), (b, c)):
+        raise ValueError(f"box must have shape (C,) = ({c},) or (B, C) = ({b}, {c}), got {tuple(box.shape)}")
+    if box.requires_grad:
+        raise ValueError("box.requires_grad is set, but the layer has no gradient with respect to the box "
+                         "(stress / virial are not computed): pass box.detach()")
+    last = cache.get("_box_checked")
+    if last is not None and last[0]() is box and last[1] == box._version:
+        return
+    if box.is_cuda and torch.cuda.is_current_stream_capturing():
+        return
+    if bool(((box < 0) | torch.isnan(box)).any()):
+        raise ValueError("box lengths must be >= 0 or +inf (0 or inf: the axis is not periodic), got negative or NaN values")
+    cache["_box_checked"] = (weakref.ref(box), box._version)
 
 
 def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
@@ -687,7 +733,10 @@ class EGNN_Network(nn.Module):
                 EGNN(dim=dim, edge_dim=edge_dim + adj_dim, norm_feats=True, **kwargs),
             ]))
 
-    def forward(self, feats, coors, adj_mat=None, edges=None, mask=None, return_coor_changes=False):
+    def forward(self, feats, coors, adj_mat=None, edges=None, mask=None, return_coor_changes=False, *, box=None):
+        """`box` (additive, keyword-only): periodic box lengths [C] or [B, C], passed to every layer (EGNN.forward)."""
+        if box is not None:
+            _check_box(box, feats.shape[0], coors.shape[-1], self.__dict__)
         lib = nat.load()
         out_dev = coors.device
         dev = _compute_device(coors)
@@ -770,7 +819,7 @@ class EGNN_Network(nn.Module):
             if exists(global_attn):
                 feats, global_tokens = global_attn(feats, global_tokens, mask=mask)
             feats, coors = egnn(feats, coors, edges, mask, adj_mat, _edge_labels=labels, _label_emb=label_emb,
-                                _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None)
+                                _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None, box=box)
             coor_changes.append(coors)
 
         if out_dev != dev:

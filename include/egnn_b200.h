@@ -177,6 +177,17 @@ int egnn_layer_forward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, con
                        const EgnnLayerIO* io, void* workspace, size_t workspace_bytes,
                        void* stream);
 
+/* Periodic boundaries: egnn_layer_forward with every pair geometry x_i - x_j replaced by its minimum image
+ *   rel_c - L_c * rint(rel_c / L_c)   (rounding half to even; 1/L_c is formed once per row or CTA)
+ * on each axis c with a finite box length L_c > 0; an axis with L_c = 0 or +inf is not periodic.  The distance, its
+ * fourier features, the neighbour ranking (valid_radius, adjacency ranks unchanged), CoorsNorm and the coordinate update
+ * x_i + sum_j w_ij rel_ij all use the wrapped rel; the output coordinates are not wrapped back into the box.
+ * `box`: device [B, C] in the coordinates' type (float64 for EGNN_DTYPE_F64, else float32), lengths >= 0 or +inf;
+ * NULL = egnn_layer_forward.  Orthorhombic boxes only, one image per neighbour. */
+int egnn_layer_forward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                const EgnnLayerIO* io, const void* box, void* workspace, size_t workspace_bytes,
+                                void* stream);
+
 /* Same call with HOST buffers for io.* (pinned or pageable): allocates device staging,
  * copies in, runs, copies feats_out / coors_out back and synchronises.  Parameters (`w`,
  * `packed`) stay device-resident.  This is the end-to-end entry `bench.py` times as `e2e`. */
@@ -221,6 +232,11 @@ int egnn_layer_backward_workspace_bytes(const EgnnLayerDesc* desc, size_t* out_b
 int egnn_layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
                         const EgnnLayerIO* io, const void* fwd_workspace, const EgnnLayerGrads* grads,
                         void* workspace, size_t workspace_bytes, void* stream);
+/* Backward of egnn_layer_forward_periodic: pass the SAME `box` as the forward (NULL = egnn_layer_backward).  The wrap's
+ * derivative with respect to the coordinates is the identity; there is no gradient with respect to the box. */
+int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                 const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
+                                 const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Neighbour selection alone == ranking + topk of egnn_pytorch.py:237-260: for every node the k
  * lowest-ranked nodes (rank = squared distance; 1e5 if either end is masked out; -1 self and 0

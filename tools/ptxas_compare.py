@@ -1,0 +1,50 @@
+"""Compare two `nvcc -Xptxas -v` logs of the library kernel by kernel.
+
+    python tools/ptxas_compare.py parent.log this.log
+
+Each log holds the output of compiling every csrc/*.cu with the library's flags plus `-Xptxas -v`
+(`nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v -c ...`).  Every kernel
+entry becomes one line `demangled name | registers, barriers, stack, static shared memory | stack frame, spills`,
+sorted.  In the second log the trailing `PBC = false` template argument of the kernels that have one (the
+periodic-boundary switch, which the parent lacks) is dropped, so a kernel that existing calls run keeps its parent's
+name.  Prints a unified diff of the two listings: a line present in both is an instantiation whose registers, spills,
+stack and shared memory are unchanged."""
+import difflib
+import re
+import subprocess
+import sys
+
+PBC_KERNELS = ("pair_kernel<", "pair_dense_tiled_kernel<", "pair_bwd1_kernel<", "pair_bwd3_kernel<",
+               "knn_warp_select_kernel<", "knn_block_sort_kernel<", "tc_knn_kernel<", "tc_pair_kernel<")
+
+
+def entries(path, strip_pbc):
+    out, cur = [], None
+    for line in open(path):
+        m = re.search(r"Compiling entry function '(_Z\w+)'", line)
+        if m:
+            cur = [m.group(1), "", ""]
+            out.append(cur)
+        elif cur is not None and "bytes stack frame" in line:
+            cur[2] = line.split(":", 1)[-1].strip()
+        elif cur is not None and "Used" in line and "registers" in line:
+            cur[1] = line.split(":", 1)[-1].strip()
+    names = subprocess.run(["cu++filt"], input="\n".join(e[0] for e in out), capture_output=True, text=True,
+                           check=True).stdout.splitlines()
+    lines = []
+    for (_, regs, frame), name in zip(out, names):
+        if strip_pbc and any(k in name for k in PBC_KERNELS):
+            name = name.replace(", (bool)0>(", ">(", 1)
+        lines.append(f"{name} | {regs} | {frame}\n")
+    return sorted(lines)
+
+
+def main():
+    a, b = entries(sys.argv[1], False), entries(sys.argv[2], True)
+    sys.stdout.writelines(difflib.unified_diff(a, b, sys.argv[1], sys.argv[2], n=0))
+    print(f"# {len(a)} kernel entries before ({len(set(a))} distinct), {len(b)} after ({len(set(b))} distinct); "
+          f"{sum(1 for x in a if x not in set(b))} of the entries before are missing or changed after")
+
+
+if __name__ == "__main__":
+    main()
