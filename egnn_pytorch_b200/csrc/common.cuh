@@ -75,8 +75,20 @@ inline int sm_count(int* out) {
 // Neighbour lists of a layer with k > 0 (egnn_pytorch.py:237-260), ranked into *nbr_idx / *nbr_ok (workspace arrays
 // of [B,N,k]); in edge-list mode (io.nbr_idx set) the pointers are redirected to the caller's lists and *nbr_ok to null.
 // box: [B,C] periodic box lengths in the coordinates' type (distances are minimum-image distances), or null.
+// cell_ws: the layer's cell-grid scratch (cell_select_layer_ws_bytes(d) bytes), or null when it has none.
 int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
-                     const void* box = nullptr);
+                     const void* box = nullptr, void* cell_ws = nullptr);
+
+// The cell-grid radius select (radius_select.cu).  A layer is eligible from its descriptor alone (1 <= k <= 32, C <= 3,
+// 0 < (T)valid_radius < 1e5, no only_sparse / batched adjacency / per-slot edges); its forward workspace then carries
+// cell_select_layer_ws_bytes(d) bytes of scratch (0 for a layer that is not eligible), whatever the size threshold.
+// cell_select_runs adds what the call decides: a mask, no adjacency, no caller lists and N >= the threshold.
+bool cell_select_eligible(const EgnnLayerDesc& d);
+size_t cell_select_layer_ws_bytes(const EgnnLayerDesc& d);
+bool cell_select_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io);
+int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
+                         const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
+                         cudaStream_t st);
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {

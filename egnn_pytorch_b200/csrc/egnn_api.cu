@@ -15,7 +15,7 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
                         const EgnnLayerIO& io, const void* box, void* ws, size_t ws_bytes, cudaStream_t st) {
   const Dims s = make_dims(d);
   const SimtPackLayout L = simt_pack_layout(s);
-  const SimtWs wl = simt_ws_layout(s, sizeof(T), d.flags);
+  const SimtWs wl = simt_ws_layout(s, sizeof(T), d.flags, cell_select_layer_ws_bytes(d));
   if (ws_bytes < wl.total) return EGNN_ERR_WORKSPACE;
   if (s.row1 <= s.row0) return EGNN_OK;
   char* base = static_cast<char*>(ws);
@@ -30,7 +30,7 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
   const RowMap ident{s.N, s.N, 0};
 
   // 1. neighbour lists (egnn_pytorch.py:237-260)
-  if (s.k > 0) EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box));
+  if (s.k > 0) EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box, wl.cell_bytes ? base + wl.cell : nullptr));
   // 2. per-node tables  A = h W1[:, :dim]^T + b1,  B = h W1[:, dim:2dim]^T   (split of :287's Linear-1)
   {
     StageTimer tm(st, STAGE_NODE_PRE);
@@ -184,7 +184,7 @@ extern "C" int egnn_layer_workspace_bytes(const EgnnLayerDesc* desc, size_t* out
   EGNN_TRY(validate_desc(desc));
   const Dims s = make_dims(*desc);
   if (desc->dtype == EGNN_DTYPE_BF16) return fast_workspace_bytes(*desc, out_bytes);
-  *out_bytes = simt_ws_layout(s, elem_size(desc->dtype), desc->flags).total + 256;
+  *out_bytes = simt_ws_layout(s, elem_size(desc->dtype), desc->flags, cell_select_layer_ws_bytes(*desc)).total + 256;
   return EGNN_OK;
 }
 

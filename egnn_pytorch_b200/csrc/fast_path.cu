@@ -197,9 +197,10 @@ __global__ void ln_concat_bf16_kernel(const __nv_bfloat16* __restrict__ h, const
   for (int c = lane; c < dim; c += 32) y[c] = __float2bfloat16((__bfloat162float(x[c]) - mu) * rstd * g[c] + bta[c]);
 }
 
-struct FastWs { size_t Atab, Btab, node_in, h1, nbr_idx, nbr_ok, gpart, gcount, total; };
+struct FastWs { size_t Atab, Btab, node_in, h1, nbr_idx, nbr_ok, gpart, gcount, cell, cell_bytes, total; };
 constexpr int TP_JSPLIT_MAX = 8;
-FastWs fast_ws_layout(const FastDims& f, uint32_t flags) {
+// cell_bytes: the cell-grid select's scratch (cell_select_layer_ws_bytes), last, so every other offset stays put
+FastWs fast_ws_layout(const FastDims& f, uint32_t flags, size_t cell_bytes) {
   FastWs w;
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
@@ -214,6 +215,8 @@ FastWs fast_ws_layout(const FastDims& f, uint32_t flags) {
   const size_t rgs = f.s.k == 0 ? (size_t)f.s.B * ceil_div(f.s.row1 - f.s.row0, TP_TI) : 0;
   w.gpart = take(rgs * TP_JSPLIT_MAX * TP_TI * TpCfg<true>::PW * 8);
   w.gcount = take(rgs * 4);
+  w.cell = take(cell_bytes);
+  w.cell_bytes = cell_bytes;
   w.total = o;
   return w;
 }
@@ -295,7 +298,7 @@ int fast_pack_weights(const EgnnLayerDesc& d, const EgnnLayerWeights& w, void* p
 
 int fast_workspace_bytes(const EgnnLayerDesc& d, size_t* out) {
   EGNN_TRY(fast_supported(d));
-  *out = fast_ws_layout(fast_dims(d), d.flags).total + 256;
+  *out = fast_ws_layout(fast_dims(d), d.flags, cell_select_layer_ws_bytes(d)).total + 256;
   return EGNN_OK;
 }
 
@@ -306,7 +309,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
   const FastDims f = fast_dims(d);
   const Dims& s = f.s;
   const FastPack L = fast_pack_layout(f);
-  const FastWs wl = fast_ws_layout(f, d.flags);
+  const FastWs wl = fast_ws_layout(f, d.flags, cell_select_layer_ws_bytes(d));
   if (ws_bytes < wl.total) return EGNN_ERR_WORKSPACE;
   const unsigned char* pk = static_cast<const unsigned char*>(packed);
   unsigned char* base = static_cast<unsigned char*>(ws);
@@ -420,7 +423,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
   } else {         // neighbour lists: distance + top-k select, then the gathered fused edge kernel
     int32_t* nbr_idx = reinterpret_cast<int32_t*>(base + wl.nbr_idx);
     uint8_t* nbr_ok = base + wl.nbr_ok;
-    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box));
+    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box, wl.cell_bytes ? base + wl.cell : nullptr));
     StageTimer tm(st, STAGE_PAIR);
     TcKnnArgs a{};
     a.B = s.B; a.N = s.N; a.Hp = f.Hp; a.ldn = f.Kn; a.dim = s.dim; a.k = s.k; a.edge_dim = s.edge_dim;

@@ -14,6 +14,7 @@
 // k  > 32: one block per row sorts all N (rank, j) pairs in shared memory (bitonic).
 #include "common.cuh"
 #include "profile.h"
+#include "warp_select.cuh"
 
 namespace egnn {
 
@@ -46,46 +47,6 @@ __device__ __forceinline__ T rank_of(const SelArgs<T>& a, int b, int i, int j, c
     else if (a.adj[((size_t)(a.adj_batched ? b : 0) * a.N + i) * a.N + j]) d = T(0);
   }
   return d;
-}
-
-template <typename T>
-__device__ __forceinline__ bool lex_less(T ka, int ia, T kb, int ib) {
-  return ka < kb || (ka == kb && ia < ib);
-}
-
-// One compare-exchange step of a warp bitonic network on (key, idx) pairs.
-template <typename T>
-__device__ __forceinline__ void cmpex(T& key, int& idx, int lane, int partner_xor, bool ascending_block) {
-  T ok = shfl_xor_t<T>(key, partner_xor);
-  int oi = __shfl_xor_sync(0xffffffffu, idx, partner_xor);
-  const bool lower = (lane & partner_xor) == 0;
-  const bool other_less = lex_less<T>(ok, oi, key, idx);
-  // in an ascending block the lower lane keeps the min
-  const bool take_other = (lower == ascending_block) ? other_less : !other_less && !(ok == key && oi == idx);
-  if (take_other) { key = ok; idx = oi; }
-}
-
-template <typename T>
-__device__ __forceinline__ void warp_sort_asc(T& key, int& idx, int lane) {
-#pragma unroll
-  for (int size = 2; size <= 32; size <<= 1) {
-    const bool asc = (lane & size) == 0 || size == 32;
-#pragma unroll
-    for (int stride = size >> 1; stride > 0; stride >>= 1) cmpex<T>(key, idx, lane, stride, asc);
-  }
-}
-
-// best (sorted ascending across lanes) <- the 32 smallest of best U cand.
-template <typename T>
-__device__ __forceinline__ void warp_merge(T& bkey, int& bidx, T ckey, int cidx, int lane) {
-  warp_sort_asc<T>(ckey, cidx, lane);
-  // reverse the candidates so that best ++ reversed(cand) is bitonic; lane l meets cand[31-l]
-  T rk = shfl_idx_t<T>(ckey, 31 - lane);
-  int ri = __shfl_sync(0xffffffffu, cidx, 31 - lane);
-  if (lex_less<T>(rk, ri, bkey, bidx)) { bkey = rk; bidx = ri; }
-  // the kept 32 form a bitonic sequence: finish with the 5 merge steps
-#pragma unroll
-  for (int stride = 16; stride > 0; stride >>= 1) cmpex<T>(bkey, bidx, lane, stride, true);
 }
 
 constexpr int SEL_WARPS_MAX = 16;   // rows per CTA (one warp each, all of the same graph): 16, or 8 for grids that would not fill the GPU
@@ -383,21 +344,25 @@ int adj_neighbors_dispatch(int B, int N, int k, const uint8_t* adj, int adj_batc
 }
 
 int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
-                     const void* box) {
+                     const void* box, void* cell_ws) {
   if (io.nbr_idx) {                                  // edge-list mode: the caller's lists, no ranking
     *nbr_idx = const_cast<int32_t*>(io.nbr_idx);
     *nbr_ok = nullptr;
     return EGNN_OK;
   }
   StageTimer tm(st, STAGE_SELECT);
+  // coordinates are fp64 for the fp64 layer and fp32 otherwise (bf16 layers included)
+  const int32_t cdt = d.dtype == EGNN_DTYPE_F64 ? EGNN_DTYPE_F64 : EGNN_DTYPE_F32;
+  if (cell_ws && cell_select_runs(d, io))            // a radius graph with a mask: the same kept slots from a cell grid
+    return cell_select_dispatch(cdt, d.B, d.N, d.C, d.k, io.coors, io.mask, box, d.valid_radius, *nbr_idx, *nbr_ok,
+                                nullptr, cell_ws, st);
   count_launch();
   const int adj_batched = (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0;
   if ((d.flags & EGNN_FLAG_ONLY_SPARSE) && io.mask && io.adj)      // every slot top-k could add is masked out: row scan
     return adj_neighbors_dispatch(d.B, d.N, d.k, io.adj, adj_batched, *nbr_idx, *nbr_ok, st);
   const double vr = (d.flags & EGNN_FLAG_ONLY_SPARSE) ? 0.0 : d.valid_radius;     // egnn_pytorch.py:250
-  // coordinates are fp64 for the fp64 layer and fp32 otherwise (bf16 layers included)
-  return knn_select_dispatch(d.dtype == EGNN_DTYPE_F64 ? EGNN_DTYPE_F64 : EGNN_DTYPE_F32, d.B, d.N, d.C, d.k, io.coors,
-                             io.mask, io.adj, adj_batched, vr, *nbr_idx, *nbr_ok, st, box);
+  return knn_select_dispatch(cdt, d.B, d.N, d.C, d.k, io.coors, io.mask, io.adj, adj_batched, vr, *nbr_idx, *nbr_ok, st,
+                             box);
 }
 
 }  // namespace egnn

@@ -37,16 +37,18 @@ static inline size_t elem_size(int dtype) { return dtype == EGNN_DTYPE_F64 ? 8 :
 
 // ------------------------------------------------------------------ SIMT workspace
 struct SimtWs {
-  size_t P, node_in, h1, nbr_idx, nbr_ok, hpart, total;
+  size_t P, node_in, h1, nbr_idx, nbr_ok, hpart, cell, cell_bytes, total;
   int hsplit;
 };
 // Tiny dense graphs (the README example, BASELINE config 1): too few (row, neighbour) tiles to fill the GPU, so the
 // hidden axis is split over CTAs and the partial sums take one trip through the workspace.
+// cell_bytes: the cell-grid select's scratch (cell_select_layer_ws_bytes), placed last so that every other offset is
+// the same with and without it (the backward reads the forward's regions at these offsets).
 static int simt_hsplit(const Dims& s) {
   if (s.k != 0 || (long long)s.B * s.N * s.N > 4096 || s.Hp < 512 || s.row0 != 0 || s.row1 != s.N) return 1;
   return std::min(32, ceil_div(s.Hp, PAIR_CH));
 }
-static SimtWs simt_ws_layout(const Dims& s, size_t es, uint32_t flags) {
+static SimtWs simt_ws_layout(const Dims& s, size_t es, uint32_t flags, size_t cell_bytes = 0) {
   SimtWs w;
   size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
@@ -58,6 +60,8 @@ static SimtWs simt_ws_layout(const Dims& s, size_t es, uint32_t flags) {
   w.nbr_ok = take((size_t)s.M * s.k);
   w.hsplit = simt_hsplit(s);
   w.hpart = take(w.hsplit > 1 ? (size_t)w.hsplit * s.B * s.N * s.N * 32 * es : 0);
+  w.cell = take(cell_bytes);
+  w.cell_bytes = cell_bytes;
   w.total = o;
   return w;
 }

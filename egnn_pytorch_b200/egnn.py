@@ -27,6 +27,7 @@ from __future__ import annotations
 
 import contextlib
 import ctypes as C
+import math
 import os
 import warnings
 import weakref
@@ -37,7 +38,7 @@ import torch.nn.functional as F
 
 from . import _native as nat
 
-__all__ = ["EGNN", "EGNN_Network", "CoorsNorm", "GlobalLinearAttention", "edge_index_to_neighbors"]
+__all__ = ["EGNN", "EGNN_Network", "CoorsNorm", "GlobalLinearAttention", "edge_index_to_neighbors", "radius_neighbors"]
 
 
 def exists(v):
@@ -596,6 +597,71 @@ def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
     slot_attr = edge_attr.new_zeros((num_nodes, kmax, edge_attr.shape[1])).index_put(
         (dst[keep], slot[keep]), edge_attr[keep_idx])
     return out.unsqueeze(0), slot_attr.unsqueeze(0)
+
+
+_RADIUS_BOX_CHECKED: dict = {}
+
+
+def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, return_counts=False):
+    """Radius graph of a point cloud: for every node the (at most) `k` nearest nodes within distance `cutoff`, as int32
+    neighbour lists [B, N, k] for `EGNN.forward(..., neighbors=...)`, nearest first, ties to the lower index, -1 in the
+    slots left empty.  A node counts as its own neighbour (distance 0).  Computed on a cell grid (`egnn_radius_select`)
+    in O(N) per graph instead of the O(N^2) ranking of the layer's kNN select, whose kept slots it equals exactly.
+
+    `coors` float32 or float64 [B, N, C] with C <= 3, on any device (CPU tensors are staged to the current CUDA
+    device; the results come back on `coors`'s device).  `cutoff` is a distance: the squared distance computed in the
+    coordinates' type is compared with `float(cutoff) ** 2` cast to that type.  (The layer's `valid_radius`, as in the
+    reference, is a *squared* distance.)  `k` in [1, min(32, N)].  `mask` [B, N] bool / 0-1: a padded node is never a
+    neighbour and its own list is empty.  `box` [C] or [B, C]: periodic box lengths as `EGNN.forward(box=)` takes them
+    (minimum-image distances; 0 or inf: the axis is not periodic).  A node with a non-finite coordinate is never a
+    neighbour and its own list is empty.
+
+    With `return_counts=True` it returns `(neighbors, counts)`: counts int32 [B, N] is the number of nodes within the
+    cutoff before the truncation at k (the node itself included), so `counts > k` shows where k cut the list short.
+    Nothing synchronises with the host: the call can be captured in a CUDA graph."""
+    if not torch.is_tensor(coors) or coors.dim() != 3:
+        raise ValueError(f"coors must be a [B, N, C] tensor, got {type(coors).__name__}"
+                         f"{' of shape ' + str(tuple(coors.shape)) if torch.is_tensor(coors) else ''}")
+    if coors.dtype not in (torch.float32, torch.float64):
+        raise ValueError(f"coors must be float32 or float64, got {coors.dtype}")
+    b, n, c = coors.shape
+    if b < 1 or n < 1:
+        raise ValueError(f"coors must hold at least one node in at least one graph, got shape {tuple(coors.shape)}")
+    if not 1 <= c <= 3:
+        raise ValueError(f"radius_neighbors supports C <= 3 coordinates, got C={c}")
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, n):
+        raise ValueError(f"k must be an int in [1, min(32, N)] = [1, {min(32, n)}], got {k!r}")
+    cutoff = float(cutoff)
+    if not (cutoff > 0.0 and math.isfinite(cutoff)):
+        raise ValueError(f"cutoff must be a finite distance > 0, got {cutoff}")
+    r2 = cutoff * cutoff
+    if not torch.tensor(r2, dtype=coors.dtype).item() > 0.0:
+        raise ValueError(f"cutoff {cutoff} squared is 0 in {coors.dtype}")
+    if mask is not None and (not torch.is_tensor(mask) or tuple(mask.shape) != (b, n)):
+        raise ValueError(f"mask must be a [B, N] = [{b}, {n}] tensor, got "
+                         f"{tuple(mask.shape) if torch.is_tensor(mask) else type(mask).__name__}")
+    if box is not None:
+        _check_box(box, b, c, _RADIUS_BOX_CHECKED)
+    lib = nat.load()
+    dev = _compute_device(coors)
+    ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)
+    with ctx:
+        x = _as(coors, dev, coors.dtype)
+        m = _as_u8(mask, dev)
+        bx = None if box is None else _as(box, dev, coors.dtype).expand(b, c).contiguous()
+        out = torch.empty((b, n, k), dtype=torch.int32, device=dev)
+        counts = torch.empty((b, n), dtype=torch.int32, device=dev) if return_counts else None
+        nb = C.c_size_t()
+        nat.check("egnn_radius_select_workspace_bytes", lib.egnn_radius_select_workspace_bytes(b, n, c, k, C.byref(nb)))
+        stream_handle = torch.cuda.current_stream(dev).cuda_stream
+        ws = _workspace(dev, nb.value, stream_handle)
+        nat.check("egnn_radius_select", lib.egnn_radius_select(
+            _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(bx), r2, _ptr(out), _ptr(counts), _ptr(ws),
+            ws.numel(), C.c_void_p(stream_handle)))
+    if out.device != coors.device:
+        out = out.to(coors.device)
+        counts = None if counts is None else counts.to(coors.device)
+    return (out, counts) if return_counts else out
 
 
 # ----------------------------------------------------------------------------- global attention

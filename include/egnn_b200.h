@@ -256,6 +256,24 @@ int egnn_knn_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k,
 int egnn_adj_neighbors(int32_t B, int32_t N, int32_t k, const uint8_t* adj, int32_t adj_batched, int32_t* out_idx,
                        uint8_t* out_ok, void* stream);
 
+/* Radius graph from a cell grid, O(N) instead of egnn_knn_select's O(N^2): for every node the k lowest-ranked nodes
+ * with rank <= r2, ascending, ties to the lowest index -- exactly the ok = 1 slots of egnn_knn_select with the same
+ * coordinates, mask and valid_radius = r2 (rank = squared distance computed in the coordinates' type; minimum image
+ * under `box`).  A padded node (mask 0) or one with a non-finite coordinate is never a neighbour, and its own row is
+ * empty.  egnn_layer_forward runs the same search for an eligible layer (k <= 32, C <= 3, a mask, a finite
+ * valid_radius, no adjacency; DESIGN.md section 5) once N reaches a size threshold (EGNN_B200_CELL_SELECT_MIN_N).
+ * coors [B,N,C] (float32, or float64 when dtype == EGNN_DTYPE_F64); mask [B,N] 0/1 or NULL (all valid); box [B,C] in
+ * the coordinates' type or NULL, as egnn_layer_forward_periodic takes it; r2 > 0 (EGNN_ERR_SHAPE otherwise), a squared
+ * distance, compared as (float)r2 for float32 coordinates.  out_idx int32 [B,N,k]: the kept neighbours, then -1 in every
+ * remaining slot (the edge-list convention of EgnnLayerIO.nbr_idx); out_count int32 [B,N] or NULL: the number of nodes
+ * with rank <= r2 before the truncation at k (the node itself included).  k <= 32 and C <= 3, else EGNN_ERR_UNSUPPORTED.
+ * workspace: egnn_radius_select_workspace_bytes(B, N, C, k) bytes (O(B N), enough for either coordinate type),
+ * 256-byte aligned.  Enqueued on `stream`, no host synchronisation (CUDA-graph capturable). */
+int egnn_radius_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes);
+int egnn_radius_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors, const uint8_t* mask,
+                       const void* box, double r2, int32_t* out_idx, int32_t* out_count, void* workspace,
+                       size_t workspace_bytes, void* stream);
+
 /* N-th degree adjacency of EGNN_Network (egnn_pytorch.py:414-428) without the dense A@A:
  * adj_in [N,N] or [B,N,N] 0/1; writes the expanded adjacency adj_out [B,N,N] 0/1, the degree
  * labels labels_out [B,N,N] (0 = not connected, d = first reached in round d) and
