@@ -147,7 +147,6 @@ SYMBOLS = {
     "egnn_comm_destroy": (C.c_int, [C.c_void_p]),
     "egnn_profile_enable": (C.c_int, [C.c_int]),
     "egnn_profile_read": (C.c_int, [_P(C.c_float), _P(C.c_int32), _P(C.c_int64), C.c_int]),
-    "egnn_profile_pair_layouts": (C.c_int, [_P(C.c_int64), _P(C.c_int64)]),
 }
 
 _lib = None

@@ -301,15 +301,6 @@ extern "C" int egnn_profile_read(float* ms_out, int32_t* spans_out, int64_t* lau
     for (auto& sp : p.spans) { cudaEventDestroy(sp.a); cudaEventDestroy(sp.b); }
     p.spans.clear();
     p.launches = 0;
-    p.pair_layouts[0] = p.pair_layouts[1] = 0;
   }
-  return EGNN_OK;
-}
-
-extern "C" int egnn_profile_pair_layouts(int64_t* wg2_out, int64_t* wg4_out) {
-  Profiler& p = Profiler::get();
-  std::lock_guard<std::mutex> g(p.mu);
-  if (wg2_out) *wg2_out = p.pair_layouts[0];
-  if (wg4_out) *wg4_out = p.pair_layouts[1];
   return EGNN_OK;
 }

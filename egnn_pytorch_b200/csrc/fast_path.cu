@@ -77,8 +77,7 @@ int fast_supported(const EgnnLayerDesc& d) {
   if (d.C < 1 || d.C > TP_CMAX) return EGNN_ERR_UNSUPPORTED;
   if (d.k == 0) {                                                  // dense all-pairs: tc_pair_kernel<lean | generic>
     if (f.QT > TP_QMAX) return EGNN_ERR_UNSUPPORTED;
-    // (the 2-warpgroup layout, the default, needs the least shared memory; 4 warpgroups run only where they fit)
-    const size_t smem = pair_is_lean(f) ? tc_pair_smem_bytes<false, 2>(f.Hp, 1) : tc_pair_smem_bytes<true, 2>(f.Hp, f.QT, 1 + 2 * f.s.F);
+    const size_t smem = pair_is_lean(f) ? tc_pair_smem_bytes<false>(f.Hp, 1) : tc_pair_smem_bytes<true>(f.Hp, f.QT, 1 + 2 * f.s.F);
     if (smem > 227 * 1024) return EGNN_ERR_UNSUPPORTED;
   } else {                                                         // neighbour lists: tc_knn_kernel<lean | edges | generic>
     if (d.k > 32) return EGNN_ERR_UNSUPPORTED;
@@ -221,31 +220,10 @@ FastWs fast_ws_layout(const FastDims& f, uint32_t flags, size_t cell_bytes) {
   return w;
 }
 
-// Optional start-up delay between the warpgroups of the persistent dense kernel (tc_pair.cuh), EGNN_B200_SKEW_NS.
-// Default 0 (no de-phasing).
-uint32_t pair_skew_ns() {
-  static const uint32_t v = [] {
-    const char* e = getenv("EGNN_B200_SKEW_NS");
-    return e ? (uint32_t)strtoul(e, nullptr, 10) : 0u;
-  }();
-  return v;
-}
-
-// Compute warpgroups of the dense kernel's lean instantiation (tc_pair.cuh), EGNN_B200_TC_PAIR_WG = 2 | 4: 2 (the default,
-// 32 pairs per warp) or 4 (16 pairs per warp, taken where its shared memory fits; measured no faster on the H100,
-// DESIGN.md section 6).
-// Read at every launch, so that one process can time both layouts.
-int pair_wg() {
-  const char* e = getenv("EGNN_B200_TC_PAIR_WG");
-  return e && strtol(e, nullptr, 10) == 4 ? 4 : 2;
-}
-
-template <bool GEN, int WG, bool PBC = false>
+template <bool GEN, bool PBC = false>
 int launch_tc_pair(const TcPairArgs& a, int grid, size_t smem, cudaStream_t st) {
-  constexpr int PPW = TP_JB / (4 * WG);
-  EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<GEN, WG, PPW, PBC>, smem)));
-  tc_pair_kernel<GEN, WG, PPW, PBC><<<grid, WG * 128, smem, st>>>(a);
-  count_pair_layout(WG);
+  EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<GEN, PBC>, smem)));
+  tc_pair_kernel<GEN, PBC><<<grid, TP_THREADS, smem, st>>>(a);
   return EGNN_OK;
 }
 
@@ -371,7 +349,6 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     a.C = s.C; a.Q = f.QT; a.F = s.F; a.edge_dim = s.edge_dim; a.num_labels = f.L;
     a.row0 = r0; a.row1 = r1;
     a.flags = d.flags; a.has_mask = io.mask != nullptr; a.clamp = (float)d.clamp;
-    a.skew_ns = pair_skew_ns();
     a.Atab = Atab; a.Btab = Btab;
     a.wq = reinterpret_cast<const float*>(pk + L.wq);
     a.w2p = reinterpret_cast<const __nv_bfloat16*>(pk + L.w2p);
@@ -403,19 +380,14 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
         items *= js;
       }
       const int grid = items < sms ? items : sms;
-      if (items < 2 * sms) a.skew_ns = 0;                      // too few row groups per CTA for the de-phasing to pay
-      // 2 warpgroups (2 warps per SM sub-partition); the lean instantiation runs 4 when asked for and the shared memory
-      // allows.  The generic one always runs 2: its row-outermost chunk loop holds the pre-activations of a whole chunk
-      // and does not fit 128 registers.  A periodic layer runs the 2-warpgroup periodic instantiations (DESIGN section 5).
+      const bool lean = pair_is_lean(f);
+      const size_t smem = lean ? tc_pair_smem_bytes<false>(f.Hp, 1) : tc_pair_smem_bytes<true>(f.Hp, f.QT, 1 + 2 * f.s.F);
       if (box) {
-        if (pair_is_lean(f)) EGNN_TRY((launch_tc_pair<false, 2, true>(a, grid, tc_pair_smem_bytes<false, 2>(f.Hp, 1), st)));
-        else EGNN_TRY((launch_tc_pair<true, 2, true>(a, grid, tc_pair_smem_bytes<true, 2>(f.Hp, f.QT, 1 + 2 * f.s.F), st)));
-      } else if (pair_is_lean(f)) {
-        const size_t smem4 = tc_pair_smem_bytes<false, 4>(f.Hp, 1);
-        if (pair_wg() == 4 && smem4 <= 227 * 1024) EGNN_TRY((launch_tc_pair<false, 4>(a, grid, smem4, st)));
-        else EGNN_TRY((launch_tc_pair<false, 2>(a, grid, tc_pair_smem_bytes<false, 2>(f.Hp, 1), st)));
+        if (lean) EGNN_TRY((launch_tc_pair<false, true>(a, grid, smem, st)));
+        else EGNN_TRY((launch_tc_pair<true, true>(a, grid, smem, st)));
       } else {
-        EGNN_TRY((launch_tc_pair<true, 2>(a, grid, tc_pair_smem_bytes<true, 2>(f.Hp, f.QT, 1 + 2 * f.s.F), st)));
+        if (lean) EGNN_TRY((launch_tc_pair<false>(a, grid, smem, st)));
+        else EGNN_TRY((launch_tc_pair<true>(a, grid, smem, st)));
       }
       EGNN_LAUNCH_CHECK();
       count_launch();

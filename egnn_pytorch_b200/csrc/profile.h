@@ -15,7 +15,6 @@ struct Profiler {
   struct Span { cudaEvent_t a, b; int stage; };
   std::vector<Span> spans;
   long long launches = 0;
-  long long pair_layouts[2] = {0, 0};   // dense tensor-core edge kernel launches with 2 / 4 warpgroups
   static Profiler& get() { static Profiler p; return p; }
 };
 
@@ -39,12 +38,6 @@ struct StageTimer {
 inline void count_launch(int n = 1) {
   Profiler& p = Profiler::get();
   if (p.on) { std::lock_guard<std::mutex> g(p.mu); p.launches += n; }
-}
-
-// which warpgroup layout (2 or 4) a launch of the dense tensor-core edge kernel used
-inline void count_pair_layout(int wg) {
-  Profiler& p = Profiler::get();
-  if (p.on) { std::lock_guard<std::mutex> g(p.mu); p.pair_layouts[wg == 4 ? 1 : 0] += 1; }
 }
 
 }  // namespace egnn

@@ -11,21 +11,16 @@
 //
 // PERSISTENT kernel: one CTA per SM walks "row groups" (TI = 4 query rows i of one graph) with a static stride.
 // W2 (core-matrix order) and Wq are staged ONCE per CTA with TMA bulk copies; the A' rows of row group it+2 are
-// prefetched into a two-deep ring while it / it+1 are being computed.  The WG compute warpgroups (128 threads each)
-// are independent pipelines: warpgroup g owns the j-tile [256*jb + TW*g, +TW) of every j-block (TW = 256 / WG pairs),
-// has its own pair-scalar tile, and never waits for another warpgroup.  Two layouts (template parameters WG, PPW):
-//   WG = 2, PPW = 32 pairs per warp: 256 threads, 2 warps per SM sub-partition, up to 255 registers (the default);
-//   WG = 4, PPW = 16 pairs per warp: 512 threads, 4 warps per SM sub-partition, at most 128 registers (lean
-//     instantiation only, on request, EGNN_B200_TC_PAIR_WG=4, where its shared memory fits; measured no faster on
-//     the H100, DESIGN.md section 6).
-// (An optional start-up skew, skew_ns, can de-phase the warpgroups so that their MUFU-idle epilogues fall into
-// different time windows; off by default.)
-//   * For each hidden chunk of 64 channels and each row i a warp produces the 64 bf16 hidden values of its PPW
+// prefetched into a two-deep ring while it / it+1 are being computed.  The two compute warpgroups (256 threads: 2 warps
+// per SM sub-partition, up to 255 registers per thread) are independent pipelines: warpgroup g owns the j-tile
+// [256*jb + 128*g, +128) of every j-block (4 warps x 32 pairs), has its own pair-scalar tile, and never waits for the
+// other warpgroup.
+//   * For each hidden chunk of 64 channels and each row i a warp produces the 64 bf16 hidden values of its 32
 //     pairs in registers (fp32 math, one MUFU.TANH per value), packed directly in the mma.sync A-fragment layout,
 //     and multiplies each 16-channel slab with the W2 slab in shared memory right away (mma.sync m16n8k16, fp32
 //     accumulators in registers): the O(N^2 H) hidden tensor never leaves the registers.  H is padded to 16 (one
-//     K step), not 64: the last chunk runs 1..4 slabs.  The accumulators of the TI rows (m_pre[i], PPW pairs x 16
-//     per warp) stay in registers across all chunks: 2 * PPW per thread (32 at PPW = 16, 64 at PPW = 32).
+//     K step), not 64: the last chunk runs 1..4 slabs.  The accumulators of the TI rows (m_pre[i], 32 pairs x 16
+//     per warp) stay in registers across all chunks: 64 per thread.
 //   * After the last chunk each lane applies the message SiLU to its accumulators in the fragment mapping, and the
 //     messages go through a per-warp shared-memory tile (one row at a time) to the lane that owns the pair, which
 //     applies gate / coors MLP / mask / clamp in fp32; the warp reduces over j with shuffles into per-warp partial
@@ -33,11 +28,10 @@
 //     a fixed order (deterministic), writes m_i and x_i' once per row, and issues the TMA prefetch of row group it+2
 //     into the ring slot that just became free.
 //
-// Thread <-> data mappings inside a compute warp (its pairs are PPW*wq .. PPW*wq + PPW-1 of the warpgroup tile):
-//   "pair" mapping     (geometry, epilogue): lane l owns pair l % PPW of the warp and the RPL = TI*PPW/32 rows
-//     RPL*(l / PPW) .. +RPL-1 (PPW = 32: all 4 rows; PPW = 16: rows 2*(l/16), 2*(l/16)+1);
+// Thread <-> data mappings inside a compute warp (its pairs are 32*wq .. 32*wq + 31 of the warpgroup tile):
+//   "pair" mapping     (geometry, epilogue): lane l owns pair l of the warp, for all TI rows;
 //   "fragment" mapping (hidden production, mma.sync A / D fragments): lane (lr = l/4, lq = l%4) owns pairs
-//     lr + 8*rho (rho < PPW/8) of the warp and, in every 16-channel K-slab, channels 4*lq .. 4*lq+3.  Lanes sharing
+//     lr + 8*rho (rho < 4) of the warp and, in every 16-channel K-slab, channels 4*lq .. 4*lq+3.  Lanes sharing
 //     lq read the same A'/Wq words (4 distinct addresses per warp instead of a 32-way broadcast, which cost one
 //     shared-memory wavefront per 4 bytes in the first version).
 #pragma once
@@ -48,13 +42,14 @@
 
 namespace egnn {
 
-#ifndef EPI_UNROLL
-#define EPI_UNROLL 2
-#endif
-constexpr int TP_EPI_UNROLL = EPI_UNROLL;
 constexpr int TP_TI = 4;          // query rows per row group
 constexpr int TP_KC = 64;         // hidden channels per chunk (4 K slabs)
-constexpr int TP_JB = 256;            // neighbours per block: WG warpgroups x 4 warps x PPW pairs in both layouts
+constexpr int TP_JB = 256;            // neighbours per block: 2 warpgroups x 4 warps x 32 pairs (one per lane)
+constexpr int TP_WG = 2;              // compute warpgroups per CTA
+constexpr int TP_WARPS = 4 * TP_WG;   // compute warps per CTA
+constexpr int TP_THREADS = 32 * TP_WARPS;
+constexpr int TP_TW = TP_JB / TP_WG;  // pairs of a warpgroup's j-tile
+constexpr int TP_NH = 2;              // m16 halves of a warp's 32 pairs (fragment mapping)
 constexpr int TP_ACC_LD = 18;         // floats per pair row of the per-warp message transpose tile
 constexpr int TP_EPI_FLOATS = 64 * 16 + 64 + 64 + 16 + 16 + 4;   // W3 | b3 | w4 | b2 | gate_w | gate_b, b4, scale, 0
 constexpr int TP_QMAX = 12;           // per-pair scalar channels of the generic instantiation
@@ -65,7 +60,6 @@ struct TcPairArgs {
   int C, Q, F, edge_dim, num_labels;   // Q = 1 + 2F + edge_dim + num_labels  (lean kernel: C = 3, Q = 1)
   int row0, row1;                  // i-rows [row0, row1) of every graph are evaluated (row-sharded multi-GPU)
   uint32_t flags; int has_mask; float clamp;
-  uint32_t skew_ns;                // start-up delay between consecutive warpgroups
   int jsplit;                      // j-blocks of a row group are dealt to `jsplit` work items (1 = one item per row group)
   double* gpart;                   // [B * row groups][jsplit][TI][PW] partial sums of the items (jsplit > 1)
   unsigned int* gcount;            // [B * row groups] arrival counters, zero on entry and on exit (jsplit > 1)
@@ -92,17 +86,16 @@ template <bool GEN> struct TpCfg {
 // continuous edge channels / one-hot labels in bf16 (Qh planes; both are exactly representable: edges arrive as bf16).
 inline size_t tc_pair_gen_scalar_bytes(int Qf, int Qh) { return (size_t)TP_TI * TP_JB * (Qf * 4 + Qh * 2); }
 
-// shared memory of the kernel with WG compute warpgroups (the 2-warpgroup layout needs the least)
-template <bool GEN, int WG>
+// dynamic shared memory of tc_pair_kernel<GEN, PBC>
+template <bool GEN>
 inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
-  constexpr int CWARPS = WG * 4, PPW = TP_JB / CWARPS;
   size_t n = 0;
   n += (size_t)Hp * 32;                                     // W2 slabs
   n += (size_t)Q * Hp * 4;                                  // Wq
   n += (size_t)2 * TP_TI * Hp * 4;                          // A' rows, two-deep ring
   n += (size_t)TP_EPI_FLOATS * 4;                           // epilogue constants
-  n += (size_t)2 * CWARPS * TP_TI * TpCfg<GEN>::PW * 8;     // per-warp partial sums (fp64), per ring slot
-  n += (size_t)CWARPS * PPW * TP_ACC_LD * 4;                // per-warp message transpose tile (one row)
+  n += (size_t)2 * TP_WARPS * TP_TI * TpCfg<GEN>::PW * 8;   // per-warp partial sums (fp64), per ring slot
+  n += (size_t)TP_WARPS * 32 * TP_ACC_LD * 4;               // per-warp message transpose tile (one row)
   n += (size_t)2 * TP_TI * TpCfg<GEN>::XC * 4 + 2 * TP_TI * 4 + 64;   // x_i, mask_i per ring slot; counters, flags
   n += (size_t)(GEN ? 0 : 1) * TP_TI * TP_JB * 4;           // lean: d_ij of the current tiles
   (void)Q;
@@ -114,7 +107,7 @@ inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
                                                             //  wherever the plain one does)
 }
 
-// named barrier over one warpgroup (ids 1..WG; id 0 is __syncthreads)
+// named barrier over one warpgroup (ids 1..TP_WG; id 0 is __syncthreads)
 __device__ __forceinline__ void tp_wg_sync(int g) { asm volatile("bar.sync %0, 128;" ::"r"(g + 1) : "memory"); }
 
 // End of a work item, run by the LAST warpgroup of the CTA to finish it (kept out of line: its registers must not add to the
@@ -125,7 +118,7 @@ struct TpFinishArgs {               // the fields of TcPairArgs the finish needs
   uint32_t flags;
   double* gpart; unsigned int* gcount; __nv_bfloat16* m_out; float* coors_out;
 };
-template <bool GEN, int CWARPS>
+template <bool GEN>
 __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* partb, uint32_t* misc, const float* xi, int item, int b,
                                             int i0, int rows_valid, int active_wgs, int g, int t128) {
   constexpr int PW = TpCfg<GEN>::PW, XC = TpCfg<GEN>::XC;
@@ -167,7 +160,7 @@ __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* 
               }
             } else {
 #pragma unroll
-              for (int wv = 0; wv < CWARPS; ++wv)
+              for (int wv = 0; wv < TP_WARPS; ++wv)
                 if (wv < active_wgs * 4) s += pb[(size_t)wv * TP_TI * PW + o];      // idle warpgroups never wrote theirs
               for (int wv = 0; wv < active_wgs * 4; ++wv) cnt += pb[(size_t)wv * TP_TI * PW + PW - 1];
             }
@@ -186,15 +179,9 @@ __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* 
 }
 
 // PBC: the pair geometry is the minimum image under a.box, at the distance and at the coordinate sum
-template <bool GEN, int WG, int PPW, bool PBC = false>
-__global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a) {
-  static_assert(WG * 4 * PPW == TP_JB && (PPW == 16 || PPW == 32), "a j-block is WG warpgroups x 4 warps x PPW pairs");
-  static_assert(!GEN || WG == 2, "the generic chunk loop needs more than the 128 registers of 4 warpgroups");
+template <bool GEN, bool PBC = false>
+__global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs a) {
   constexpr int PW = TpCfg<GEN>::PW, XC = TpCfg<GEN>::XC;
-  constexpr int CWARPS = WG * 4, THREADS = WG * 128;
-  constexpr int TW = 4 * PPW;              // pairs of a warpgroup's j-tile
-  constexpr int NH = PPW / 16;             // m16 halves of a warp's pairs (fragment mapping)
-  constexpr int RPL = TP_TI * PPW / 32;    // rows of a lane's pair (pair mapping)
   // carve the dynamic shared memory directly (no integer round trip) so every access stays in the
   // shared state space (LDS/STS, not generic LD/ST); nothing here needs more than 128-byte alignment
   extern __shared__ __align__(128) unsigned char sm[];
@@ -210,15 +197,15 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
   // Sums ACROSS tiles are kept in fp64: the per-tile sums are fp32 (fixed shuffle tree), and adding a few hundred
   // fp32 numbers in fp64 is exact, so the result does not depend on how the tiles were dealt to warps, work items or
   // ranks (row-sharded == single GPU, bit for bit, whatever jsplit is).
-  double* part = reinterpret_cast<double*>(epi + TP_EPI_FLOATS);              // [2][CWARPS][TI][PW]
-  float* xis = reinterpret_cast<float*>(part + 2 * CWARPS * TP_TI * PW);      // [2][TI][XC]
+  double* part = reinterpret_cast<double*>(epi + TP_EPI_FLOATS);              // [2][TP_WARPS][TI][PW]
+  float* xis = reinterpret_cast<float*>(part + 2 * TP_WARPS * TP_TI * PW);    // [2][TI][XC]
   uint32_t* mki = reinterpret_cast<uint32_t*>(xis + 2 * TP_TI * XC);          // [2][TI]
   uint32_t* misc = mki + 2 * TP_TI;        // [0..1] done counters, [4 + g] / [8 + g] last-warpgroup / last-item flags
   const int Qf = GEN ? 1 + 2 * a.F : 1, Qh = Q - Qf;
-  float* ssm = reinterpret_cast<float*>(misc + 16);                           // [WG][Qf][TI][TW] fp32
-  __nv_bfloat16* ssh = reinterpret_cast<__nv_bfloat16*>(ssm + (size_t)Qf * TP_TI * TP_JB);   // [WG][Qh][TI][TW] bf16
-  float* accs = reinterpret_cast<float*>(ssh + (size_t)Qh * TP_TI * TP_JB);    // [CWARPS][PPW][TP_ACC_LD]
-  uint64_t* bars = reinterpret_cast<uint64_t*>(accs + CWARPS * PPW * TP_ACC_LD);
+  float* ssm = reinterpret_cast<float*>(misc + 16);                           // [TP_WG][Qf][TI][TP_TW] fp32
+  __nv_bfloat16* ssh = reinterpret_cast<__nv_bfloat16*>(ssm + (size_t)Qf * TP_TI * TP_JB);   // [TP_WG][Qh][TI][TP_TW] bf16
+  float* accs = reinterpret_cast<float*>(ssh + (size_t)Qh * TP_TI * TP_JB);    // [TP_WARPS][32][TP_ACC_LD]
+  uint64_t* bars = reinterpret_cast<uint64_t*>(accs + TP_WARPS * 32 * TP_ACC_LD);
   uint64_t* ldbar = bars;                         // W2 / Wq staging
   uint64_t* rowfull = ldbar + 1;                  // [2] A' ring
 
@@ -276,8 +263,8 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
     tc::mbar_init(&rowfull[0], 1); tc::mbar_init(&rowfull[1], 1);
     tc::mbar_fence_init();
   }
-  for (int x = tid; x < TP_EPI_FLOATS; x += THREADS) epi[x] = a.epi[x];
-  for (int x = tid; x < 2 * TP_TI * Hp; x += THREADS) As[x] = 0.f;         // rows beyond a graph's end stay finite
+  for (int x = tid; x < TP_EPI_FLOATS; x += TP_THREADS) epi[x] = a.epi[x];
+  for (int x = tid; x < 2 * TP_TI * Hp; x += TP_THREADS) As[x] = 0.f;        // rows beyond a graph's end stay finite
   if (tid < 2) misc[tid] = 0;
   tc::fence_proxy_async_smem();                    // the zero fill above precedes TMA writes to the same buffers
   __syncthreads();
@@ -302,20 +289,13 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
     // =========================================================== compute warpgroups (independent pipelines)
     const int g = warp >> 2, wq = warp & 3, t128 = tid & 127;
     const int lr = lane >> 2, lq = lane & 3;
-    const int pp = wq * PPW + lane % PPW;            // pair mapping: this lane's pair in the warpgroup tile ...
-    const int rb = lane / PPW * RPL;                 // ... and its first row
-    float* swg = ssm + (size_t)g * Qf * TP_TI * TW;  // pair scalars of this warpgroup's tile: swg[(q*TI + i)*TW + pair]
-    __nv_bfloat16* shg = ssh + (size_t)g * Qh * TP_TI * TW;
-    float* myacc = accs + (size_t)warp * PPW * TP_ACC_LD;
-    if (a.skew_ns && g > 0) {                         // de-phase the warpgroups (see the header)
-      uint64_t t0, t1;
-      asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t0));
-      const uint64_t until = t0 + (uint64_t)a.skew_ns * g;
-      do { __nanosleep(1000); asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t1)); } while (t1 < until);
-    }
-    // warpgroups whose j-tiles all lie beyond the graph (N <= TW g) have nothing to do in ANY row group: they leave
+    const int pp = wq * 32 + lane;                   // pair mapping: this lane's pair in the warpgroup tile
+    float* swg = ssm + (size_t)g * Qf * TP_TI * TP_TW;   // pair scalars of this warpgroup's tile: swg[(q*TI + i)*TP_TW + pair]
+    __nv_bfloat16* shg = ssh + (size_t)g * Qh * TP_TI * TP_TW;
+    float* myacc = accs + (size_t)warp * 32 * TP_ACC_LD;
+    // warpgroups whose j-tiles all lie beyond the graph (N <= TP_TW g) have nothing to do in ANY row group: they leave
     // now instead of spinning on the ring barriers next to the working warps of their SM sub-partitions
-    const int active_wgs = min(WG, (N + TW - 1) / TW);
+    const int active_wgs = min(TP_WG, (N + TP_TW - 1) / TP_TW);
     const bool wg_active = g < active_wgs;
     if (wg_active) tc::mbar_wait(ldbar, 0);
     int it = 0;
@@ -334,16 +314,16 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
         if constexpr (PBC) return min_image<float>(r, bx[c], bx[TP_CMAX + c]);
         return r;
       };
-      double* mypart = part + ((size_t)buf * CWARPS + warp) * TP_TI * PW;
+      double* mypart = part + ((size_t)buf * TP_WARPS + warp) * TP_TI * PW;
       for (int x = lane; x < TP_TI * PW; x += 32) mypart[x] = 0.0;
       __syncwarp();
 
       for (int jb = item % a.jsplit; jb < njb; jb += a.jsplit) {
-        if (jb * TP_JB + g * TW >= N) break;            // this warpgroup's tile lies beyond the graph
-        // ---- pair mapping: geometry (and the other per-pair scalar channels) of (i, j) for this lane's rows i
-        // (lean: x_j and mask_j are read here and again in the epilogue rather than held across the chunk loop, which
-        //  the 128 registers of the 4-warpgroup layout need; the generic instantiation holds them)
-        const int j = jb * TP_JB + g * TW + pp;
+        if (jb * TP_JB + g * TP_TW >= N) break;         // this warpgroup's tile lies beyond the graph
+        // ---- pair mapping: geometry (and the other per-pair scalar channels) of (i, j) for the TI rows i
+        // (lean: x_j and mask_j are read here and again in the epilogue, so that they hold no registers across the
+        //  chunk loop; the generic instantiation holds them)
+        const int j = jb * TP_JB + g * TP_TW + pp;
         const bool jv = j < N;
         auto load_xj = [&](float (&xj)[GEN ? TP_CMAX : 3]) {
           const size_t nodej = (size_t)b * N + (jv ? j : N - 1);
@@ -355,62 +335,61 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
         float xj[GEN ? TP_CMAX : 3];
         const bool mask_j0 = load_xj(xj);
 #pragma unroll
-        for (int r = 0; r < RPL; ++r) {
-          const int i = rb + r;
+        for (int i = 0; i < TP_TI; ++i) {
           float d = 0.f;
 #pragma unroll
           for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float rc = rel_c(i, c, xj[c]); d = fmaf(rc, rc, d); }
-          swg[i * TW + pp] = d;
+          swg[i * TP_TW + pp] = d;
           if (GEN) {
             int q = 1;
             for (int f = 0; f < a.F; ++f) {                                                       // :34-41
               const float sc = d * exp2f(-(float)f);
-              swg[((q + f) * TP_TI + i) * TW + pp] = sinf(sc);
-              swg[((q + a.F + f) * TP_TI + i) * TW + pp] = cosf(sc);
+              swg[((q + f) * TP_TI + i) * TP_TW + pp] = sinf(sc);
+              swg[((q + a.F + f) * TP_TI + i) * TP_TW + pp] = cosf(sc);
             }
             const size_t pij = ((size_t)b * N + min(i0 + i, N - 1)) * N + (jv ? j : N - 1);
-            for (int e = 0; e < a.edge_dim; ++e) shg[(e * TP_TI + i) * TW + pp] = a.edges[pij * a.edge_dim + e];
+            for (int e = 0; e < a.edge_dim; ++e) shg[(e * TP_TI + i) * TP_TW + pp] = a.edges[pij * a.edge_dim + e];
             if (a.num_labels > 0) {
               const int lab = a.labels[pij];
               for (int l = 0; l < a.num_labels; ++l)
-                shg[((a.edge_dim + l) * TP_TI + i) * TW + pp] = __float2bfloat16((l == lab) ? 1.f : 0.f);
+                shg[((a.edge_dim + l) * TP_TI + i) * TP_TW + pp] = __float2bfloat16((l == lab) ? 1.f : 0.f);
             }
           }
         }
         __syncwarp();
-        // ---- fragment mapping: B' rows of this lane's 2 * NH pairs
+        // ---- fragment mapping: B' rows of this lane's 2 * TP_NH pairs
         // (rows lr + 8 rho of the tile are 8 table rows apart: one base pointer + a stride instead of four pointers.  Rows
         //  beyond the graph are NOT clamped: they read the next graph's rows or the 128 padding rows of the table, and
         //  their pairs are discarded by `jv` -- NaN-safe, every use is a select)
-        const uint2* Bp0 = reinterpret_cast<const uint2*>(a.Btab + ((size_t)b * N + jb * TP_JB + g * TW + wq * PPW + lr) * Hp + 4 * lq);
+        const uint2* Bp0 = reinterpret_cast<const uint2*>(a.Btab + ((size_t)b * N + jb * TP_JB + g * TP_TW + wq * 32 + lr) * Hp + 4 * lq);
         const int Bstride = 8 * Hp / 4;                 // uint2 units between rows lr + 8 rho and lr + 8 (rho + 1)
 #define Bp_(rho) (Bp0 + (rho) * Bstride)
         // lean: a two-slab ring of B' (see the lean chunk below); generic: B' of the whole chunk
         constexpr int BCS = GEN ? 4 : 2;
-        uint2 Bc[2 * NH][BCS];                          // [rho][slab % BCS] B' (bf16 x4 each)
+        uint2 Bc[2 * TP_NH][BCS];                       // [rho][slab % BCS] B' (bf16 x4 each)
         {
           const int nsl0 = nchunks == 1 ? nsl_last : 4;
 #pragma unroll
-          for (int rho = 0; rho < 2 * NH; ++rho)
+          for (int rho = 0; rho < 2 * TP_NH; ++rho)
 #pragma unroll
             for (int sl = 0; sl < BCS; ++sl) Bc[rho][sl] = sl < nsl0 ? __ldg(Bp_(rho) + sl * 4) : make_uint2(0u, 0u);
         }
 
-        float acc[TP_TI][NH][2][4];                     // m_pre[i] of pairs [16 half, +16) x channels [8 nt, +8) (D fragments)
+        float acc[TP_TI][TP_NH][2][4];                  // m_pre[i] of pairs [16 half, +16) x channels [8 nt, +8) (D fragments)
 #pragma unroll
         for (int i = 0; i < TP_TI; ++i)
 #pragma unroll
-          for (int h = 0; h < NH; ++h)
+          for (int h = 0; h < TP_NH; ++h)
 #pragma unroll
             for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
               for (int e = 0; e < 4; ++e) acc[i][h][nt][e] = 0.f;
-        float dr[GEN ? 1 : TP_TI][2 * NH];              // lean: d_ij of this lane's fragment pairs, for the whole tile
+        float dr[GEN ? 1 : TP_TI][2 * TP_NH];           // lean: d_ij of this lane's fragment pairs, for the whole tile
         if (!GEN) {
 #pragma unroll
           for (int i = 0; i < TP_TI; ++i)
 #pragma unroll
-            for (int rho = 0; rho < 2 * NH; ++rho) dr[GEN ? 0 : i][rho] = swg[i * TW + wq * PPW + lr + 8 * rho];
+            for (int rho = 0; rho < 2 * TP_NH; ++rho) dr[GEN ? 0 : i][rho] = swg[i * TP_TW + wq * 32 + lr + 8 * rho];
         }
         // 8 hidden values (2 pairs x 4 channels of one K slab) from their pre-activation / 2 without B' (z), + B', SiLU,
         // packed as the mma.sync A fragment: regs {0,1} -> pair lr (+16), regs {2,3} -> pair lr+8 (+24); even k low
@@ -449,7 +428,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
             for (int i = 0; i < TP_TI; ++i) {
               const float4 av = *reinterpret_cast<const float4*>(Ab + (size_t)i * Hp + s * 16 + lq * 4);
 #pragma unroll
-              for (int half = 0; half < NH; ++half) {    // pairs (lr, lr+8), then (lr+16, lr+24)
+              for (int half = 0; half < TP_NH; ++half) { // pairs (lr, lr+8), then (lr+16, lr+24)
                 float2 z[2][2];                          // [r2][channel pair]: wd*d + A'
 #pragma unroll
                 for (int r2 = 0; r2 < 2; ++r2) {
@@ -467,7 +446,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
             // B' of slab sl + 2 into the ring slot slab sl just freed
             if (sl + 2 < 4 ? sl + 2 < nsl : more && sl - 2 < nsl_next) {
 #pragma unroll
-              for (int rho = 0; rho < 2 * NH; ++rho) Bc[rho][sl % BCS] = __ldg(Bp_(rho) + (s + 2) * 4);
+              for (int rho = 0; rho < 2 * TP_NH; ++rho) Bc[rho][sl % BCS] = __ldg(Bp_(rho) + (s + 2) * 4);
             }
           }
         };
@@ -483,7 +462,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
             constexpr bool reload = decltype(reload_tag)::value != 0;
             const float* Ai = Ab + (size_t)i * Hp + c * TP_KC + lq * 4;
 #pragma unroll
-            for (int half = 0; half < NH; ++half) {
+            for (int half = 0; half < TP_NH; ++half) {
               float2 z[4][2][2];                         // [slab][r2][channel pair]: A' + sum_q Wq s_q
 #pragma unroll
               for (int sl = 0; sl < 4; ++sl) {
@@ -498,10 +477,10 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
               for (int q = 0; q < Q; ++q) {
                 float s0, s1;
                 if (q < Qf) {
-                  const float* sq = swg + (q * TP_TI + i) * TW + wq * PPW + lr + 16 * half;
+                  const float* sq = swg + (q * TP_TI + i) * TP_TW + wq * 32 + lr + 16 * half;
                   s0 = sq[0]; s1 = sq[8];
                 } else {
-                  const __nv_bfloat16* sq = shg + ((q - Qf) * TP_TI + i) * TW + wq * PPW + lr + 16 * half;
+                  const __nv_bfloat16* sq = shg + ((q - Qf) * TP_TI + i) * TP_TW + wq * 32 + lr + 16 * half;
                   s0 = __bfloat162float(sq[0]); s1 = __bfloat162float(sq[8]);
                 }
                 const float2 ss0 = make_float2(s0, s0), ss1 = make_float2(s1, s1);
@@ -554,7 +533,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
         //      messages through the per-warp tile, one row at a time, to the lanes that own the pair (pair mapping)
         const float* W3 = epi; const float* b3 = epi + 1024; const float* w4 = b3 + 64;
         const float* b2 = w4 + 64; const float* gw = b2 + 16; const float* sc = gw + 16;   // sc: gate_b, b4, scale
-        float m[RPL][16];                                // m_ij of this lane's pair for its RPL rows
+        float m[TP_TI][16];                              // m_ij of this lane's pair for the TI rows
         {
           float b2f[2][2];                               // b2 of this lane's D-fragment channels 8 nt + 2 lq + e
 #pragma unroll
@@ -562,7 +541,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
 #pragma unroll
           for (int i = 0; i < TP_TI; ++i) {
 #pragma unroll
-            for (int h = 0; h < NH; ++h)
+            for (int h = 0; h < TP_NH; ++h)
 #pragma unroll
               for (int nt = 0; nt < 2; ++nt)
 #pragma unroll
@@ -571,17 +550,15 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
                       make_float2(tc::silu_half_arg(0.5f * (acc[i][h][nt][2 * r2] + b2f[nt][0])),
                                   tc::silu_half_arg(0.5f * (acc[i][h][nt][2 * r2 + 1] + b2f[nt][1])));
             __syncwarp();
-            if (i / RPL == lane / PPW) {                 // (always, at PPW = 32)
 #pragma unroll
-              for (int o = 0; o < 16; ++o) m[i % RPL][o] = myacc[(lane % PPW) * TP_ACC_LD + o];
-            }
+            for (int o = 0; o < 16; ++o) m[i][o] = myacc[lane * TP_ACC_LD + o];
             __syncwarp();
           }
         }
         const bool mask_j = GEN ? mask_j0 : load_xj(xj);
         if (a.flags & EGNN_FLAG_SOFT_EDGES) {                                                                 // :289-290
 #pragma unroll
-          for (int r = 0; r < RPL; ++r) {
+          for (int r = 0; r < TP_TI; ++r) {
             float z = sc[0];
 #pragma unroll
             for (int o = 0; o < 16; ++o) z = fmaf(gw[o], m[r][o], z);
@@ -590,19 +567,19 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
             for (int o = 0; o < 16; ++o) m[r][o] *= gate;
           }
         }
-        float wgt[RPL];
+        float wgt[TP_TI];
 #pragma unroll
-        for (int r = 0; r < RPL; ++r) wgt[r] = 0.f;
+        for (int r = 0; r < TP_TI; ++r) wgt[r] = 0.f;
         if (upd_coors) {                                                                                      // :302-315
-          // hidden unit u outermost: one W3 row (4 x LDS.128) serves all RPL rows of this pair; the rows are
+          // hidden unit u outermost: one W3 row (4 x LDS.128) serves all TI rows of this pair; the rows are
           // independent FMA chains
-#pragma unroll TP_EPI_UNROLL
+#pragma unroll 2
           for (int u = 0; u < 64; ++u) {
             const float4* w3 = reinterpret_cast<const float4*>(W3 + u * 16);
             const float4 wa = w3[0], wb = w3[1], wc = w3[2], wd4 = w3[3];
             const float bu = b3[u], w4u = w4[u];
 #pragma unroll
-            for (int r = 0; r < RPL; ++r) {
+            for (int r = 0; r < TP_TI; ++r) {
               float tt = bu;
               tt = fmaf(wa.x, m[r][0], tt); tt = fmaf(wa.y, m[r][1], tt); tt = fmaf(wa.z, m[r][2], tt); tt = fmaf(wa.w, m[r][3], tt);
               tt = fmaf(wb.x, m[r][4], tt); tt = fmaf(wb.y, m[r][5], tt); tt = fmaf(wb.z, m[r][6], tt); tt = fmaf(wb.w, m[r][7], tt);
@@ -613,39 +590,38 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
           }
         }
 #pragma unroll
-        for (int r = 0; r < RPL; ++r) {
-          const int i = rb + r;
+        for (int i = 0; i < TP_TI; ++i) {
           const bool pm = jv && (mk[i] != 0) && (a.has_mask ? mask_j : true);
-          float w = wgt[r] + sc[1];
+          float w = wgt[i] + sc[1];
           if (upd_coors) {
             if (!pm) w = 0.f;                                                                                 // :309
             if (a.flags & EGNN_FLAG_CLAMP) w = fminf(fmaxf(w, -a.clamp), a.clamp);                            // :313
-            if (a.flags & EGNN_FLAG_NORM_COORS) w *= sc[2] / fmaxf(sqrtf(swg[i * TW + pp]), 1e-8f);           // :74-77
+            if (a.flags & EGNN_FLAG_NORM_COORS) w *= sc[2] / fmaxf(sqrtf(swg[i * TP_TW + pp]), 1e-8f);        // :74-77
           } else {
             w = 0.f;
           }
           float v[PW];
 #pragma unroll
-          for (int o = 0; o < 16; ++o) v[o] = pm ? m[r][o] : 0.f;                                             // :322
+          for (int o = 0; o < 16; ++o) v[o] = pm ? m[i][o] : 0.f;                                             // :322
 #pragma unroll
           for (int c = 0; c < PW - 17; ++c) {
             constexpr int NX = GEN ? TP_CMAX : 3;
             v[16 + c] = (c < NX && (!GEN || c < C)) ? w * rel_c(i, c < NX ? c : 0, xj[c < NX ? c : 0]) : 0.f;
           }
           v[PW - 1] = pm ? 1.f : 0.f;
-          // sum over the warp's pairs: the PPW lanes that hold row i (the whole warp, or one half of it)
+          // sum over the warp's 32 pairs
 #pragma unroll
-          for (int off = PPW / 2; off > 0; off >>= 1)
+          for (int off = 16; off > 0; off >>= 1)
 #pragma unroll
             for (int o = 0; o < PW; ++o) v[o] += __shfl_xor_sync(0xffffffffu, v[o], off);
-          if (lane % PPW == 0) {
+          if (lane == 0) {
 #pragma unroll
             for (int o = 0; o < PW; ++o) mypart[i * PW + o] += (double)v[o];
           }
         }
       }
 
-      // ---- this warpgroup is done with the row group: the last of the WG finishes it
+      // ---- this warpgroup is done with the row group: the last of the warpgroups finishes it
       __syncwarp();
       tp_wg_sync(g);                                       // all partial sums of this warpgroup are in shared memory
       if (t128 == 0) {
@@ -660,7 +636,7 @@ __global__ void __launch_bounds__(WG * 128, 1) tc_pair_kernel(const TcPairArgs a
         TpFinishArgs fa;
         fa.jsplit = a.jsplit; fa.N = N; fa.C = C; fa.ldn = a.ldn; fa.has_mask = a.has_mask; fa.flags = a.flags;
         fa.gpart = a.gpart; fa.gcount = a.gcount; fa.m_out = a.m_out; fa.coors_out = a.coors_out;
-        tp_finish_item<GEN, CWARPS>(fa, part + (size_t)buf * CWARPS * TP_TI * PW, misc, xi, item, b, i0, rows_valid, active_wgs, g, t128);
+        tp_finish_item<GEN>(fa, part + (size_t)buf * TP_WARPS * TP_TI * PW, misc, xi, item, b, i0, rows_valid, active_wgs, g, t128);
         tp_wg_sync(g);                                     // every reader of ring slot `buf` is done
         const int nxt = item + 2 * gridDim.x;
         if (nxt < n_items) stage_item(nxt, buf, t128, [&]() { tp_wg_sync(g); });

@@ -362,9 +362,6 @@ int egnn_comm_destroy(void* comm);
  * count.  Off by default; the only mutable global state in the library. */
 int egnn_profile_enable(int on);
 int egnn_profile_read(float* ms_out, int32_t* spans_out, int64_t* launches_out, int reset);
-/* Launches of the dense tensor-core edge kernel with 2 and with 4 warpgroups (EGNN_B200_TC_PAIR_WG) counted while
- * profiling is enabled, since the last egnn_profile_read with reset. */
-int egnn_profile_pair_layouts(int64_t* wg2_out, int64_t* wg4_out);
 
 #ifdef __cplusplus
 }

@@ -19,13 +19,16 @@ PBC_KERNELS = ("pair_kernel<", "pair_dense_tiled_kernel<", "pair_bwd1_kernel<", 
 
 
 def entries(path, strip_pbc):
-    out, cur = [], None
+    out, cur, owner = [], None, None
     for line in open(path):
         m = re.search(r"Compiling entry function '(_Z\w+)'", line)
+        p = re.search(r"Function properties for (\w+)", line)
         if m:
             cur = [m.group(1), "", ""]
             out.append(cur)
-        elif cur is not None and "bytes stack frame" in line:
+        elif p:
+            owner = p.group(1)      # a non-inlined device function's properties can follow the entry's own
+        elif cur is not None and owner == cur[0] and "bytes stack frame" in line:
             cur[2] = line.split(":", 1)[-1].strip()
         elif cur is not None and "Used" in line and "registers" in line:
             cur[1] = line.split(":", 1)[-1].strip()
