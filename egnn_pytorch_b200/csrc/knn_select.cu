@@ -7,6 +7,10 @@
 //             = 0     if an adjacency is given and adj[i,j], i != j            (:256)
 //   keep the k smallest (rank, j) pairs in ascending lexicographic order -> deterministic
 //   "lowest index wins" tie rule (torch.topk leaves ties unspecified).
+//   A NaN rank (a NaN coordinate, or inf - inf) is ordered as (+inf, j + N): after every +inf rank, ties to the lower
+//   index, as a stable sort puts NaN last.  Such a slot is written as j with ok = 0, so every index is in [0, N).  The
+//   sort never compares a NaN (its network needs a total order); the warp select never queues one and fills the slots
+//   its list leaves empty after the scan.
 //
 // k <= 32: one warp per row keeps the running top-32 sorted across its lanes; candidates that
 // beat the current k-th entry are queued in shared memory and merged 32 at a time with a
@@ -132,7 +136,7 @@ knn_warp_select_kernel(const SelArgs<T> a) {
           }
           key[u] = d;
         }
-        pass[u] = jvalid && lex_less<T>(key[u], j, thr_key, thr_idx);
+        pass[u] = jvalid && lex_less<T>(key[u], j, thr_key, thr_idx);     // false for a NaN key: see the fill-in below
       }
       if (!__any_sync(0xffffffffu, pass[0] || pass[1])) continue;
 #pragma unroll
@@ -168,10 +172,42 @@ knn_warp_select_kernel(const SelArgs<T> a) {
     int cidx = lane < count ? myqi[lane] : IMAX;
     warp_merge<T>(bkey, bidx, ckey, cidx, lane);
   }
-  if (rv && lane < a.k) {
+  // A NaN key never passes the filter, so the list holds the k smallest non-NaN ranks and ends in empty (INF, IMAX)
+  // entries when there are fewer than k of them.  Those slots take the NaN ranks in index order (the order (+inf, j + N)
+  // gives them): a cold rescan of the row, off the per-candidate path, written with ok = 0.
+  int filled = __popc(__ballot_sync(0xffffffffu, bidx != IMAX));
+  if (rv && lane < a.k && bidx != IMAX) {
     const size_t o = row * a.k + lane;
     a.out_idx[o] = bidx;
     if (a.out_ok) a.out_ok[o] = bkey <= a.valid_radius ? 1 : 0;
+  }
+  for (int j0 = 0; j0 < a.N && filled < a.k; j0 += 32) {           // warp-uniform
+    const int j = j0 + lane;
+    bool nan_rank = false;
+    if (j < a.N) {                     // the rank of the scan above, read from global memory
+      const T* xj = a.coors + ((size_t)b * a.N + j) * a.C;
+      T d = T(0);
+#pragma unroll
+      for (int c = 0; c < NC; ++c)
+        if (CDIM || c < a.C) {
+          T r = xi[c] - xj[c];
+          if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
+          d = sq_acc<T>(r, d);
+        }
+      if (a.mask && !(mask_i && a.mask[(size_t)b * a.N + j])) d = T(1e5);
+      if (adjrow) {
+        if (i == j) d = T(-1);
+        else if (adjrow[j]) d = T(0);
+      }
+      nan_rank = d != d;
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, nan_rank);
+    const int pos = filled + __popc(bal & ((1u << lane) - 1));
+    if (rv && nan_rank && pos < a.k) {
+      a.out_idx[row * a.k + pos] = j;
+      if (a.out_ok) a.out_ok[row * a.k + pos] = 0;
+    }
+    filled += __popc(bal);
   }
 }
 
@@ -194,8 +230,11 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
     __syncthreads();
   }
   for (int j = threadIdx.x; j < Npad; j += blockDim.x) {
-    keys[j] = j < a.N ? rank_of<T, PBC>(a, b, i, j, xi, mask_i, pb) : T(INFINITY);
-    idxs[j] = j < a.N ? j : 0x7fffffff;
+    T d = j < a.N ? rank_of<T, PBC>(a, b, i, j, xi, mask_i, pb) : T(INFINITY);
+    int jk = j < a.N ? j : 0x7fffffff;
+    if (d != d) { d = T(INFINITY); jk = j + a.N; }        // NaN rank: after every +inf (see the top of the file)
+    keys[j] = d;
+    idxs[j] = jk;
   }
   __syncthreads();
   for (int size = 2; size <= Npad; size <<= 1) {
@@ -215,8 +254,9 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   }
   for (int s = threadIdx.x; s < a.k; s += blockDim.x) {
     const size_t o = (size_t)row * a.k + s;
-    a.out_idx[o] = idxs[s];
-    if (a.out_ok) a.out_ok[o] = keys[s] <= a.valid_radius ? 1 : 0;
+    const bool nan_rank = idxs[s] >= a.N;
+    a.out_idx[o] = nan_rank ? idxs[s] - a.N : idxs[s];
+    if (a.out_ok) a.out_ok[o] = !nan_rank && keys[s] <= a.valid_radius ? 1 : 0;
   }
 }
 

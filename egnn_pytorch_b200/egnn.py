@@ -71,6 +71,8 @@ def _compute_device(t: torch.Tensor) -> torch.device:
 
 _KERNEL_DTYPE = {torch.float32: nat.DTYPE_F32, torch.float64: nat.DTYPE_F64, torch.bfloat16: nat.DTYPE_BF16}
 _PATH_NAME = {torch.float64: "fp64-simt", torch.float32: "fp32-simt", torch.bfloat16: "bf16-tc"}
+# k > 32: knn_block_sort_kernel sorts a row's next_pow2(N) (rank, index) pairs in at most 200 KiB of shared memory
+SELECT_SORT_MAX_N = 16384
 
 
 def _ptr(t):
@@ -407,6 +409,11 @@ class EGNN(nn.Module):
                     k = int(_k_hint) if _k_hint is not None else int(adj_u8.sum(dim=-1, dtype=torch.int32).max().item())
             if not (0 < k <= n):
                 raise RuntimeError(f"number of neighbours k={k} must satisfy 0 < k <= N={n} (torch.topk would raise)")
+            row_scan = self.only_sparse_neighbors and exists(mask) and adj_u8 is not None     # no ranking (select_neighbors)
+            if k > 32 and n > SELECT_SORT_MAX_N and not row_scan:
+                raise RuntimeError(f"num_nearest_neighbors={k} > 32 ranks each node with a shared-memory sort of all N nodes, "
+                                   f"which holds at most N={SELECT_SORT_MAX_N}, got N={n}: use k <= 32, or pass "
+                                   f"neighbors= (e.g. from radius_neighbors)")
 
         cfg_key = (c, k > 0, min(k, 33), cont_edge_dim, label_dim, _rows is None)
         if kdt == torch.bfloat16 and cfg_key in self._tc_unsupported:

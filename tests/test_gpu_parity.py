@@ -84,40 +84,6 @@ def test_inputs_not_mutated_and_param_update_is_seen():
     util.assert_close(o2[0], want[0], atol=2e-5, rtol=1e-4)
 
 
-@pytest.mark.parametrize("dtype", [torch.float64, torch.float32], ids=["fp64", "fp32"])
-@pytest.mark.parametrize("k,n,masked,adj", [(1, 5, False, False), (8, 300, True, False), (32, 1000, False, False),
-                                            (7, 64, True, True), (40, 333, True, False), (64, 64, False, False)])
-def test_knn_select_kernel(k, n, masked, adj, dtype):
-    """egnn_knn_select alone vs the oracle's ranking + stable smallest-k (egnn_pytorch.py:237-260)."""
-    import ctypes as C
-    from egnn_pytorch_b200 import _native as nat
-    lib = nat.load()
-    rs = np.random.RandomState(k * 1000 + n)
-    B, Cd = 2, 3
-    # coordinates on a 1/8 grid: squared distances are exact in fp32 and fp64, so the ranking is
-    # independent of FMA contraction, and ties (incl. coincident nodes) are frequent -> this pins
-    # the lowest-index tie rule
-    coors = np.round(rs.standard_normal((B, n, Cd)) * 8) / 8
-    mask = (rs.uniform(size=(B, n)) < 0.85) if masked else None
-    adjm = cases.chain_adjacency(n, True) if adj else None
-    cfg = cases.O.layer_cfg(dim=4, num_nearest_neighbors=k, valid_radius=1.0)
-    idx, ok, _ = cases.O.neighbour_selection(cfg, coors.astype(np.float32 if dtype == torch.float32 else np.float64),
-                                             mask, adjm)
-    tc = torch.from_numpy(coors).to("cuda", dtype).contiguous()
-    tm = None if mask is None else torch.from_numpy(mask).to("cuda", torch.uint8).contiguous()
-    ta = None if adjm is None else torch.from_numpy(adjm).to("cuda", torch.uint8).contiguous()
-    oi = torch.empty((B, n, k), dtype=torch.int32, device="cuda")
-    oo = torch.empty((B, n, k), dtype=torch.uint8, device="cuda")
-    p = lambda t: None if t is None else C.c_void_p(t.data_ptr())
-    rc = lib.egnn_knn_select(nat.DTYPE_F64 if dtype == torch.float64 else nat.DTYPE_F32, B, n, Cd, k, p(tc), p(tm), p(ta),
-                             0, 1.0, p(oi), p(oo), None)
-    assert rc == 0, nat.strerror(rc)
-    torch.cuda.synchronize()
-    got = oi.cpu().numpy()
-    np.testing.assert_array_equal(got, idx)
-    np.testing.assert_array_equal(oo.cpu().numpy().astype(bool), ok)
-
-
 @pytest.mark.parametrize("n,deg,batched", [(40, 3, False), (70, 2, True), (33, 4, False), (257, 3, False)])
 def test_adj_expand_kernel(n, deg, batched):
     import ctypes as C
