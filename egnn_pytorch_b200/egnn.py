@@ -705,8 +705,9 @@ class GlobalLinearAttention(nn.Module):
     """Induced-set attention between the nodes and a few global tokens (reference egnn_pytorch.py:112-144).
 
     Inference (no autograd recording): ONE call of `egnn_global_attn_forward` (csrc/global_attn.cu) on staged fp32 / fp64
-    copies of the parameters -- the module itself is never moved.  When a gradient is required the same arithmetic runs
-    through PyTorch autograd (the hand-written backward of SURVEY.md section 8(f) covers the EGNN layers only)."""
+    copies of the parameters -- the module itself is never moved.  When a gradient is required, or there are more than 32
+    global tokens, the same arithmetic runs through PyTorch (the hand-written backward of SURVEY.md section 8(f) covers
+    the EGNN layers only).  A size-1 batch of `x`, `queries` or `mask` is broadcast, as in the reference."""
 
     def __init__(self, *, dim, heads=8, dim_head=64):
         super().__init__()
@@ -740,20 +741,43 @@ class GlobalLinearAttention(nn.Module):
     def invalidate_cache(self):
         self._stage = {}
 
+    def _batch(self, x, queries, mask):
+        """Shape check -> the common batch B.  x [Bx, N, dim], queries [Bq, T, dim], mask [Bm, N]; each of Bx, Bq, Bm is 1
+        or B, as the reference's einsum and masked_fill broadcast a size-1 batch."""
+        def shape(t):
+            return tuple(t.shape) if torch.is_tensor(t) else type(t).__name__
+        if not (torch.is_tensor(x) and x.dim() == 3 and x.shape[2] == self.dim):
+            raise ValueError(f"x must be [B, N, dim={self.dim}], got {shape(x)}")
+        if not (torch.is_tensor(queries) and queries.dim() == 3 and queries.shape[2] == self.dim):
+            raise ValueError(f"queries must be [B, T, dim={self.dim}], got {shape(queries)}")
+        batches = [x.shape[0], queries.shape[0]]
+        if mask is not None:
+            if not (torch.is_tensor(mask) and mask.dim() == 2 and mask.shape[1] == x.shape[1]):
+                raise ValueError(f"mask must be [B, N={x.shape[1]}], got {shape(mask)}")
+            batches.append(mask.shape[0])
+        b = max(batches)
+        if any(v not in (1, b) for v in batches):
+            raise ValueError(f"batch sizes of x, queries and mask must each be 1 or the same B, got {batches}")
+        return b
+
     def forward(self, x, queries, mask=None):
+        b = self._batch(x, queries, mask)
         needs_grad = torch.is_grad_enabled() and (x.requires_grad or queries.requires_grad or
                                                   any(p.requires_grad for p in self.parameters()))
-        if needs_grad:
+        # T > 32: ga_attn2_kernel keeps a node's T scores in registers, so more tokens take the autograd path's arithmetic
+        if needs_grad or queries.shape[1] > 32:
             dev = x.device
             if any(p.device != dev for p in self.parameters()):
-                raise RuntimeError("training GlobalLinearAttention needs the module on the device of its inputs")
+                raise RuntimeError("training GlobalLinearAttention, or running it with more than 32 global tokens, needs "
+                                   "the module on the device of its inputs")
             return self._forward_autograd(x, queries, mask)
         lib = nat.load()
         dev = _compute_device(x)
         kdt = torch.float64 if x.dtype == torch.float64 else torch.float32
         _, _, w = self._staged(dev, kdt)
-        b, n, d = x.shape
-        t = queries.shape[1]
+        n, d, t = x.shape[1], x.shape[2], queries.shape[1]
+        x, queries = x.expand(b, -1, -1), queries.expand(b, -1, -1)
+        mask = None if mask is None else mask.expand(b, -1)
         x_in, q_in, m_in = _as(x, dev, kdt), _as(queries, dev, kdt), _as_u8(mask, dev)
         x_out, q_out = torch.empty_like(x_in), torch.empty_like(q_in)
         desc = nat.GlobalAttnDesc(abi_version=nat.ABI_VERSION, dtype=_KERNEL_DTYPE[kdt], B=b, N=n, T=t, dim=d, heads=self.heads,

@@ -304,7 +304,8 @@ int egnn_gemm_bf16(int32_t M, int32_t N, int32_t K, const void* A, const void* W
 typedef struct EgnnGlobalAttnDesc {
   int32_t abi_version;    /* EGNN_ABI_VERSION */
   int32_t dtype;          /* EGNN_DTYPE_F32 | EGNN_DTYPE_F64 */
-  int32_t B, N, T;        /* graphs, nodes, global tokens (T <= 32) */
+  int32_t B, N, T;        /* graphs, nodes, global tokens (T <= 32, else EGNN_ERR_UNSUPPORTED; the Python module
+                             GlobalLinearAttention falls back to its PyTorch arithmetic above 32) */
   int32_t dim, heads, dim_head;
 } EgnnGlobalAttnDesc;
 
