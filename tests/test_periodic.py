@@ -2,8 +2,8 @@
 rel = x_i - x_j - L rint((x_i - x_j) / L) on every axis with a finite L > 0 (egnn_layer_forward_periodic /
 egnn_layer_backward_periodic).
 
-The periodic restatement below is the reference layer (egnn_pytorch.py:224-341) in float64 torch on the CPU with the
-wrapped rel in place of rel_coors, so gradients come from autograd.  It is pinned three ways without trusting its own
+The periodic restatement (tests/torch_reference.py) is the reference layer (egnn_pytorch.py:224-341) in float64 torch
+with the wrapped rel in place of rel_coors, so gradients come from autograd.  It is pinned three ways without trusting its own
 wrap: with no box and with a 2^20 box it equals the golden-pinned numpy oracle; on a 3^C supercell of images, where
 every central node lists the nearest image of each partner, the existing edge-list oracles (forward and gradient) give
 its outputs and gradients; its kNN selection equals a stable argsort of brute-force wrapped distances.
@@ -23,7 +23,6 @@ import os
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as TF
 
 import cases
 import util
@@ -33,144 +32,8 @@ from oracle import egnn_oracle_grad as G
 HUGE = 2.0 ** 20
 
 
-# ----------------------------------------------------------------------------- the periodic restatement
-
-
-def _t(x):
-    return x if torch.is_tensor(x) else torch.as_tensor(np.array(x, np.float64))
-
-
-def wrap(rel, box):
-    """Minimum image of rel [..., C] under box lengths broadcastable to it (0 or inf: the axis is not periodic)."""
-    box = _t(box)
-    per = (box > 0) & torch.isfinite(box)
-    L = torch.where(per, box, torch.zeros_like(box))
-    inv = torch.where(per, 1.0 / torch.where(per, box, torch.ones_like(box)), torch.zeros_like(box))
-    return rel - L * torch.round(rel * inv)
-
-
-def box_bc(box, b, c):
-    return None if box is None else _t(box).expand(b, c)
-
-
-def select(cfg, rel_dist, mask, adj):
-    """Neighbour ranking + top-k of egnn_pytorch.py:237-260, ties to the lowest index -> (idx [B,N,k], nbhd_mask)."""
-    b, n, _ = rel_dist.shape
-    ranking = rel_dist.clone()
-    k = cfg["num_nearest_neighbors"]
-    vr = cfg["valid_radius"]
-    if mask is not None:
-        mk = torch.as_tensor(np.asarray(mask)).bool()
-        ranking = ranking.masked_fill(~(mk[:, :, None] & mk[:, None, :]), 1e5)
-    if adj is not None:
-        a = torch.as_tensor(np.asarray(adj)).bool()
-        if a.dim() == 2:
-            a = a.expand(b, n, n)
-        if cfg["only_sparse_neighbors"]:
-            k = int(a.float().sum(-1).max())
-            vr = 0.0
-        eye = torch.eye(n, dtype=torch.bool)[None]
-        a = a & ~eye
-        ranking = ranking.masked_fill(eye, -1.0).masked_fill(a, 0.0)
-    order = torch.sort(ranking, dim=-1, stable=True).indices[..., :k]
-    return order, torch.gather(ranking, -1, order) <= vr
-
-
-def layer(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neighbors=None, slot_edges=None):
-    """One EGNN layer with periodic geometry, float64.  `neighbors` [B,N,k] (-1 = empty slot) runs edge-list mode;
-    `slot_edges` [B,N,k,e] are its per-slot edge features."""
-    P = {k: _t(v) for k, v in P.items()}
-    feats, coors = _t(feats), _t(coors)
-    b, n, d = feats.shape
-    c = coors.shape[-1]
-    rel = coors[:, :, None] - coors[:, None]
-    if box is not None:
-        rel = wrap(rel, box_bc(box, b, c)[:, None, None, :])
-    dist = (rel ** 2).sum(-1)
-    use_nearest = cfg["num_nearest_neighbors"] > 0 or cfg["only_sparse_neighbors"] or neighbors is not None
-    bi = torch.arange(b)[:, None, None]
-    ii = torch.arange(n)[None, :, None]
-    valid = None
-    if neighbors is not None:
-        nb = torch.as_tensor(np.asarray(neighbors)).long()
-        valid = nb >= 0
-        idx = nb.clamp_min(0)
-        nbhd = valid
-    elif use_nearest:
-        idx, nbhd = select(cfg, dist, mask, adj)
-    if use_nearest:
-        rel, dist = rel[bi, ii, idx], dist[bi, ii, idx]
-        if slot_edges is not None:
-            edges = _t(slot_edges)
-        elif edges is not None:
-            edges = _t(edges)[bi, ii, idx]
-        feats_j = feats[bi, idx]
-    else:
-        feats_j = feats[:, None].expand(b, n, n, d)
-        edges = None if edges is None else _t(edges)
-    j = feats_j.shape[2]
-    F = cfg["fourier_features"]
-    dfeat = dist[..., None]
-    if F > 0:
-        sc = dist[..., None] / (2.0 ** torch.arange(F, dtype=torch.float64))
-        dfeat = torch.cat([torch.sin(sc), torch.cos(sc), dist[..., None]], -1)
-    edge_in = torch.cat([feats[:, :, None].expand(b, n, j, d), feats_j, dfeat] + ([edges] if edges is not None else []), -1)
-    lin = lambda x, key: x @ P[key + ".weight"].T + P[key + ".bias"]
-    m = TF.silu(lin(TF.silu(lin(edge_in, "edge_mlp.0")), "edge_mlp.3"))
-    if cfg["soft_edges"]:
-        m = m * torch.sigmoid(lin(m, "edge_gate.0"))
-    live = valid
-    if mask is not None:
-        mk = torch.as_tensor(np.asarray(mask)).bool()
-        mj = mk[bi, idx] if use_nearest else mk[:, None, :].expand(b, n, n)
-        live = mk[:, :, None] & mj
-        if use_nearest:
-            live = live & nbhd
-    coors_out = coors
-    if cfg["update_coors"]:
-        w = lin(TF.silu(lin(m, "coors_mlp.0")), "coors_mlp.3")[..., 0]
-        if live is not None:
-            w = torch.where(live, w, torch.zeros_like(w))
-        cv = cfg["coor_weights_clamp_value"]
-        if cv is not None:
-            w = w.clamp(-cv, cv)
-        if valid is not None:
-            w = torch.where(valid, w, torch.zeros_like(w))
-        r = rel
-        if cfg["norm_coors"]:
-            r = rel / torch.linalg.vector_norm(rel, dim=-1, keepdim=True).clamp_min(1e-8) * P["coors_norm.scale"]
-        coors_out = coors + (w[..., None] * r).sum(2)
-    feats_out = feats
-    if cfg["update_feats"]:
-        mm = m if live is None else torch.where(live[..., None], m, torch.zeros_like(m))
-        m_i = mm.sum(2)
-        if cfg["m_pool_method"] == "mean":
-            if mask is not None:
-                cnt = live.double().sum(-1, keepdim=True)
-                m_i = torch.where(cnt == 0, torch.zeros_like(m_i), m_i / cnt.clamp_min(1e-8))
-            else:
-                m_i = m_i / j
-        normed = TF.layer_norm(feats, (d,), P["node_norm.weight"], P["node_norm.bias"], 1e-5) if cfg["norm_feats"] else feats
-        feats_out = lin(TF.silu(lin(torch.cat([normed, m_i], -1), "node_mlp.0")), "node_mlp.3") + feats
-    return feats_out, coors_out
-
-
-def layer_grads(case, box, gf, gx, neighbors=None, slot_edges=None):
-    """Gradients of sum(fo * gf) + sum(xo * gx) through the restatement: 'in.feats', 'in.coors', ['in.edges'], 'p.*'."""
-    ins = case["inputs"]
-    leaves = {"in.feats": _t(ins["feats"]).clone().requires_grad_(True), "in.coors": _t(ins["coors"]).clone().requires_grad_(True)}
-    e = slot_edges if slot_edges is not None else ins.get("edges")
-    if e is not None:
-        leaves["in.edges"] = _t(e).clone().requires_grad_(True)
-    P = {k: _t(v).clone().requires_grad_(True) for k, v in case["params"].items()}
-    with torch.enable_grad():
-        fo, xo = layer(P, case["cfg"], leaves["in.feats"], leaves["in.coors"],
-                       None if slot_edges is not None else leaves.get("in.edges"), ins.get("mask"), ins.get("adj_mat"),
-                       box, neighbors, leaves.get("in.edges") if slot_edges is not None else None)
-        ((fo * _t(gf)).sum() + (xo * _t(gx)).sum()).backward()
-    out = {k: v.grad.numpy() for k, v in leaves.items()}
-    out.update({f"p.{k}": v.grad.numpy() for k, v in P.items()})
-    return out
+# the periodic restatement: tests/torch_reference.py
+from torch_reference import _t, box_bc, layer, layer_grads, select, wrap  # noqa: E402
 
 
 # ----------------------------------------------------------------------------- inputs
