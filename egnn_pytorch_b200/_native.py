@@ -117,18 +117,25 @@ SYMBOLS = {
                                      C.c_size_t, C.c_void_p]),
     "egnn_layer_forward_periodic": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
                                               C.c_void_p, C.c_size_t, C.c_void_p]),
+    "egnn_layer_forward_triclinic": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
+                                               C.c_void_p, C.c_size_t, C.c_void_p]),
     "egnn_layer_forward_host": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p]),
     "egnn_layer_backward_workspace_bytes": (C.c_int, [_P(LayerDesc), _P(C.c_size_t)]),
     "egnn_layer_backward": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
                                       _P(LayerGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
     "egnn_layer_backward_periodic": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
                                                C.c_void_p, _P(LayerGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "egnn_layer_backward_triclinic": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
+                                                C.c_void_p, _P(LayerGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
     "egnn_knn_select": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "egnn_adj_neighbors": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),
     "egnn_radius_select_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P(C.c_size_t)]),
     "egnn_radius_select": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                      C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "egnn_radius_select_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                               C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
+                                               C.c_size_t, C.c_void_p]),
     "egnn_adj_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_size_t)]),
     "egnn_adj_expand": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

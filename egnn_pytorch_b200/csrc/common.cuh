@@ -74,10 +74,11 @@ inline int sm_count(int* out) {
 
 // Neighbour lists of a layer with k > 0 (egnn_pytorch.py:237-260), ranked into *nbr_idx / *nbr_ok (workspace arrays
 // of [B,N,k]); in edge-list mode (io.nbr_idx set) the pointers are redirected to the caller's lists and *nbr_ok to null.
-// box: [B,C] periodic box lengths in the coordinates' type (distances are minimum-image distances), or null.
+// box: [B,C] periodic box lengths (pbc = PBC_BOX) or a [B,C,C] lower-triangular cell (pbc = PBC_CELL) in the
+// coordinates' type, distances then being those of the wrapped pair vector; null with PBC_NONE.
 // cell_ws: the layer's cell-grid scratch (cell_select_layer_ws_bytes(d) bytes), or null when it has none.
 int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
-                     const void* box = nullptr, void* cell_ws = nullptr);
+                     const void* box = nullptr, void* cell_ws = nullptr, int pbc = 0);
 
 // The cell-grid radius select (radius_select.cu).  A layer is eligible from its descriptor alone (1 <= k <= 32, C <= 3,
 // 0 < (T)valid_radius < 1e5, no only_sparse / batched adjacency / per-slot edges); its forward workspace then carries
@@ -88,7 +89,7 @@ size_t cell_select_layer_ws_bytes(const EgnnLayerDesc& d);
 bool cell_select_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io);
 int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
                          const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
-                         cudaStream_t st);
+                         cudaStream_t st, int pbc);
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {
@@ -208,6 +209,38 @@ __device__ __forceinline__ void box_axis(const T* box, int b, int C, int c, T& L
 template <typename T> __device__ __forceinline__ T min_image(T r, T L, T inv);
 template <> __device__ __forceinline__ float min_image<float>(float r, float L, float inv) { return fmaf(-L, rintf(r * inv), r); }
 template <> __device__ __forceinline__ double min_image<double>(double r, double L, double inv) { return fma(-L, rint(r * inv), r); }
+
+// ------------------------------------------------------------------ periodic boundaries (triclinic cells)
+// The PBC template parameter of every kernel that forms x_i - x_j: no wrap, an orthorhombic box ([B,C] lengths), or a
+// lower-triangular cell ([B,C,C], row k = lattice vector a_k, C in {2, 3}; DESIGN.md section 4).
+constexpr int PBC_NONE = 0, PBC_BOX = 1, PBC_CELL = 2;
+// A cell as the kernels stage it, once per CTA, row or ring slot: the diagonal L[3] and 1/L[3] exactly as box_axis
+// forms them (0 on an aperiodic axis and beyond C), then the off-diagonals a_1x, a_2x, a_2y (0 beyond C).
+constexpr int CELL_STAGED = 9;
+template <typename T>
+__device__ __forceinline__ T cell_staged(const T* cell, int b, int C, int t) {
+  const T* m = cell + (size_t)b * C * C;
+  if (t < 6) {
+    const int c = t % 3;
+    const T l = c < C ? m[c * C + c] : T(0);
+    const bool periodic = l > T(0) && l < T(INFINITY);
+    return !periodic ? T(0) : (t < 3 ? l : T(1) / l);
+  }
+  const int r = t == 6 ? 1 : 2, c = t == 8 ? 1 : 0;
+  return r < C ? m[r * C + c] : T(0);
+}
+// The sequential wrap under a staged cell pc, from the last axis to the first: n = rint(r_c / L_c), then
+// r_d -= cell[c][d] n for every d <= c.  Afterwards |r_c| <= L_c / 2 on every periodic axis.  With a diagonal cell
+// the off-diagonal steps subtract exact zeros, so the result is min_image's bit for bit.
+template <typename T>
+__device__ __forceinline__ void cell_wrap(T& r0, T& r1, T& r2, const T* pc) {
+  const T n2 = rint(r2 * pc[5]);
+  r0 = fma_t<T>(-pc[7], n2, r0); r1 = fma_t<T>(-pc[8], n2, r1); r2 = fma_t<T>(-pc[2], n2, r2);
+  const T n1 = rint(r1 * pc[4]);
+  r0 = fma_t<T>(-pc[6], n1, r0); r1 = fma_t<T>(-pc[1], n1, r1);
+  const T n0 = rint(r0 * pc[3]);
+  r0 = fma_t<T>(-pc[0], n0, r0);
+}
 
 // 4 consecutive elements, 4-element aligned.
 template <typename T> struct Vec4;

@@ -12,7 +12,7 @@ namespace egnn {
 
 template <typename T>
 static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed,
-                        const EgnnLayerIO& io, const void* box, void* ws, size_t ws_bytes, cudaStream_t st) {
+                        const EgnnLayerIO& io, const void* box, int pbc, void* ws, size_t ws_bytes, cudaStream_t st) {
   const Dims s = make_dims(d);
   const SimtPackLayout L = simt_pack_layout(s);
   const SimtWs wl = simt_ws_layout(s, sizeof(T), d.flags, cell_select_layer_ws_bytes(d));
@@ -30,7 +30,7 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
   const RowMap ident{s.N, s.N, 0};
 
   // 1. neighbour lists (egnn_pytorch.py:237-260)
-  if (s.k > 0) EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box, wl.cell_bytes ? base + wl.cell : nullptr));
+  if (s.k > 0) EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box, wl.cell_bytes ? base + wl.cell : nullptr, pbc));
   // 2. per-node tables  A = h W1[:, :dim]^T + b1,  B = h W1[:, dim:2dim]^T   (split of :287's Linear-1)
   {
     StageTimer tm(st, STAGE_NODE_PRE);
@@ -76,11 +76,13 @@ static int simt_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const
       int TS = 1;
       while (TS < s.k && TS < 32) TS <<= 1;
       a.TS = TS;
-      if (box) EGNN_TRY((L.MP == 16 ? launch_pair<T, 16, true>(a, st) : launch_pair<T, 32, true>(a, st)));
+      if (pbc == PBC_CELL) EGNN_TRY((L.MP == 16 ? launch_pair<T, 16, PBC_CELL>(a, st) : launch_pair<T, 32, PBC_CELL>(a, st)));
+      else if (pbc == PBC_BOX) EGNN_TRY((L.MP == 16 ? launch_pair<T, 16, PBC_BOX>(a, st) : launch_pair<T, 32, PBC_BOX>(a, st)));
       else EGNN_TRY((L.MP == 16 ? launch_pair<T, 16>(a, st) : launch_pair<T, 32>(a, st)));
       count_launch();
     } else {
-      if (box) EGNN_TRY((L.MP == 16 ? launch_pair_dense<T, 16, true>(a, st) : launch_pair_dense<T, 32, true>(a, st)));
+      if (pbc == PBC_CELL) EGNN_TRY((L.MP == 16 ? launch_pair_dense<T, 16, PBC_CELL>(a, st) : launch_pair_dense<T, 32, PBC_CELL>(a, st)));
+      else if (pbc == PBC_BOX) EGNN_TRY((L.MP == 16 ? launch_pair_dense<T, 16, PBC_BOX>(a, st) : launch_pair_dense<T, 32, PBC_BOX>(a, st)));
       else EGNN_TRY((L.MP == 16 ? launch_pair_dense<T, 16>(a, st) : launch_pair_dense<T, 32>(a, st)));
       count_launch(wl.hsplit > 1 ? 2 : 1);
     }
@@ -188,21 +190,36 @@ extern "C" int egnn_layer_workspace_bytes(const EgnnLayerDesc* desc, size_t* out
   return EGNN_OK;
 }
 
-extern "C" int egnn_layer_forward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
-                                           const EgnnLayerIO* io, const void* box, void* workspace, size_t workspace_bytes,
-                                           void* stream) {
+// box: [B,C] lengths (pbc = PBC_BOX), a [B,C,C] lower-triangular cell (PBC_CELL), or null
+static int layer_forward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed, const EgnnLayerIO* io,
+                         const void* box, int pbc, void* workspace, size_t workspace_bytes, void* stream) {
   EGNN_TRY(validate_desc(desc));
+  if (!box) pbc = PBC_NONE;
+  if (pbc == PBC_CELL && (desc->C < 2 || desc->C > 3)) return EGNN_ERR_SHAPE;
   if (!io || !packed || !workspace) return EGNN_ERR_NULL;
   EGNN_TRY(check_ptrs(*desc, w, io));
   if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
   if ((uintptr_t)packed & 0xF) return EGNN_ERR_ALIGN;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   switch (desc->dtype) {
-    case EGNN_DTYPE_F64: return simt_forward<double>(*desc, *w, packed, *io, box, workspace, workspace_bytes, st);
-    case EGNN_DTYPE_F32: return simt_forward<float>(*desc, *w, packed, *io, box, workspace, workspace_bytes, st);
-    case EGNN_DTYPE_BF16: return fast_forward(*desc, *w, packed, *io, box, workspace, workspace_bytes, st);
+    case EGNN_DTYPE_F64: return simt_forward<double>(*desc, *w, packed, *io, box, pbc, workspace, workspace_bytes, st);
+    case EGNN_DTYPE_F32: return simt_forward<float>(*desc, *w, packed, *io, box, pbc, workspace, workspace_bytes, st);
+    case EGNN_DTYPE_BF16: return fast_forward(*desc, *w, packed, *io, box, pbc, workspace, workspace_bytes, st);
     default: return EGNN_ERR_UNSUPPORTED;
   }
+}
+
+extern "C" int egnn_layer_forward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                           const EgnnLayerIO* io, const void* box, void* workspace, size_t workspace_bytes,
+                                           void* stream) {
+  return layer_forward(desc, w, packed, io, box, PBC_BOX, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_layer_forward_triclinic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                            const EgnnLayerIO* io, const void* cell, void* workspace,
+                                            size_t workspace_bytes, void* stream) {
+  if (!cell) return EGNN_ERR_NULL;
+  return layer_forward(desc, w, packed, io, cell, PBC_CELL, workspace, workspace_bytes, stream);
 }
 
 extern "C" int egnn_layer_forward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,

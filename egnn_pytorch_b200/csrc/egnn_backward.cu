@@ -3,9 +3,9 @@
 
 namespace egnn {
 
-template int simt_backward<float>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, const void*,
+template int simt_backward<float>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, int, const void*,
                                   const EgnnLayerGrads&, void*, size_t, cudaStream_t);
-extern template int simt_backward<double>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, const void*,
+extern template int simt_backward<double>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, int, const void*,
                                           const EgnnLayerGrads&, void*, size_t, cudaStream_t);   // egnn_backward_f64.cu
 
 static int check_grad_ptrs(const EgnnLayerDesc& d, const EgnnLayerGrads* g) {
@@ -34,10 +34,12 @@ extern "C" int egnn_layer_backward_workspace_bytes(const EgnnLayerDesc* desc, si
   return EGNN_OK;
 }
 
-extern "C" int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
-                                            const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
-                                            const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+// box: [B,C] lengths (pbc = PBC_BOX), a [B,C,C] lower-triangular cell (PBC_CELL), or null
+static int layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed, const EgnnLayerIO* io,
+                          const void* box, int pbc, const void* fwd_workspace, const EgnnLayerGrads* grads, void* workspace,
+                          size_t workspace_bytes, void* stream) {
   EGNN_TRY(validate_desc(desc));
+  if (pbc == PBC_CELL && (desc->C < 2 || desc->C > 3)) return EGNN_ERR_SHAPE;
   EGNN_TRY(backward_supported(*desc));
   if (!io || !packed || !workspace || !fwd_workspace) return EGNN_ERR_NULL;
   EGNN_TRY(check_ptrs(*desc, w, nullptr));
@@ -49,8 +51,22 @@ extern "C" int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const Egn
   if (((uintptr_t)workspace | (uintptr_t)fwd_workspace) & 0xFF) return EGNN_ERR_ALIGN;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (desc->dtype == EGNN_DTYPE_F64)
-    return simt_backward<double>(*desc, *w, packed, *io, box, fwd_workspace, *grads, workspace, workspace_bytes, st);
-  return simt_backward<float>(*desc, *w, packed, *io, box, fwd_workspace, *grads, workspace, workspace_bytes, st);
+    return simt_backward<double>(*desc, *w, packed, *io, box, pbc, fwd_workspace, *grads, workspace, workspace_bytes, st);
+  return simt_backward<float>(*desc, *w, packed, *io, box, pbc, fwd_workspace, *grads, workspace, workspace_bytes, st);
+}
+
+extern "C" int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                            const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
+                                            const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
+  return layer_backward(desc, w, packed, io, box, PBC_BOX, fwd_workspace, grads, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_layer_backward_triclinic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                             const EgnnLayerIO* io, const void* cell, const void* fwd_workspace,
+                                             const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes,
+                                             void* stream) {
+  if (!cell) return EGNN_ERR_NULL;
+  return layer_backward(desc, w, packed, io, cell, PBC_CELL, fwd_workspace, grads, workspace, workspace_bytes, stream);
 }
 
 extern "C" int egnn_layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,

@@ -2,6 +2,6 @@
 #include "egnn_backward_impl.cuh"
 
 namespace egnn {
-template int simt_backward<double>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, const void*,
+template int simt_backward<double>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, int, const void*,
                                    const EgnnLayerGrads&, void*, size_t, cudaStream_t);
 }  // namespace egnn

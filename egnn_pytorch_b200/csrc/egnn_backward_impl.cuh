@@ -94,7 +94,7 @@ static int launch_colsum(const T* X, long ld, int rows, int cols, T* out, cudaSt
 // W2 silu(pre1) of every pair into pre2 when the forward did not keep it, by the forward's own edge kernels (with
 // the forward's dropout masks): for dense graphs the register-tiled kernel's split-H phase 1 over one split, which
 // stores exactly that; for neighbour lists pair_kernel with no node or coordinate update.
-template <typename T, int MP, bool PBC>
+template <typename T, int MP, int PBC>
 static int recompute_pre2(const BwdArgs<T>& a, T* pre2, cudaStream_t st) {
   PairArgs<T> f;
   f.s = a.s; f.L = a.L; f.flags = a.flags; f.has_mask = a.has_mask; f.TS = a.TS; f.clamp = a.clamp;
@@ -116,7 +116,7 @@ static int recompute_pre2(const BwdArgs<T>& a, T* pre2, cudaStream_t st) {
 
 // BLK: a row block (its own instantiations, so that the whole-graph kernels keep their plain row arithmetic).
 // PBC: periodic geometry in bwd1 / bwd3 (bwd2 reads the pair records only).
-template <typename T, int MP, bool KNN, bool BLK, bool PBC>
+template <typename T, int MP, bool KNN, bool BLK, int PBC>
 static int launch_pair_bwd(const BwdArgs<T>& a, cudaStream_t st) {
   const Dims& s = a.s;
   const int rows = s.row1 - s.row0;                 // the i-rows of the call (all N unless a row block); the last CTA
@@ -148,8 +148,8 @@ static int launch_pair_bwd(const BwdArgs<T>& a, cudaStream_t st) {
   return EGNN_OK;
 }
 
-// The edge step reversed for one choice of (row block, neighbour lists, periodic box).
-template <typename T, bool PBC>
+// The edge step reversed for one choice of (row block, neighbour lists, periodic box or cell).
+template <typename T, int PBC>
 static int launch_edge_bwd(const BwdArgs<T>& a, T* pre2, bool saved, bool part, cudaStream_t st) {
   const int MP = a.L.MP;
   if (!saved) EGNN_TRY((MP == 16 ? recompute_pre2<T, 16, PBC>(a, pre2, st) : recompute_pre2<T, 32, PBC>(a, pre2, st)));
@@ -163,7 +163,8 @@ static int launch_edge_bwd(const BwdArgs<T>& a, T* pre2, bool saved, bool part, 
 
 template <typename T>
 int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed, const EgnnLayerIO& io,
-                  const void* box, const void* fwd_ws, const EgnnLayerGrads& gr, void* ws, size_t ws_bytes, cudaStream_t st) {
+                  const void* box, int pbc, const void* fwd_ws, const EgnnLayerGrads& gr, void* ws, size_t ws_bytes,
+                  cudaStream_t st) {
   const Dims s = make_dims(d);
   const SimtPackLayout L = simt_pack_layout(s);
   const SimtWs fl = simt_ws_layout(s, sizeof(T), d.flags);
@@ -318,8 +319,9 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
     a.TS = 32; a.TI2 = 32;
   }
   a.box = static_cast<const T*>(box);
-  if (box) EGNN_TRY((launch_edge_bwd<T, true>(a, pre2, saved, part, st)));
-  else EGNN_TRY((launch_edge_bwd<T, false>(a, pre2, saved, part, st)));
+  if (box && pbc == PBC_CELL) EGNN_TRY((launch_edge_bwd<T, PBC_CELL>(a, pre2, saved, part, st)));
+  else if (box) EGNN_TRY((launch_edge_bwd<T, PBC_BOX>(a, pre2, saved, part, st)));
+  else EGNN_TRY((launch_edge_bwd<T, PBC_NONE>(a, pre2, saved, part, st)));
 
   // ---- per-node tables reversed: A = h W1[:, :dim]^T + b1, B = h W1[:, dim:2dim]^T.  dL/dA is 0 outside the row block,
   // so its terms run over the block's rows; dL/dB (every j) over all rows

@@ -220,7 +220,7 @@ FastWs fast_ws_layout(const FastDims& f, uint32_t flags, size_t cell_bytes) {
   return w;
 }
 
-template <bool GEN, bool PBC = false>
+template <bool GEN, int PBC = PBC_NONE>
 int launch_tc_pair(const TcPairArgs& a, int grid, size_t smem, cudaStream_t st) {
   EGNN_TRY((ensure_dynamic_smem(tc_pair_kernel<GEN, PBC>, smem)));
   tc_pair_kernel<GEN, PBC><<<grid, TP_THREADS, smem, st>>>(a);
@@ -281,7 +281,7 @@ int fast_workspace_bytes(const EgnnLayerDesc& d, size_t* out) {
 }
 
 int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed, const EgnnLayerIO& io,
-                 const void* box, void* ws, size_t ws_bytes, cudaStream_t st) {
+                 const void* box, int pbc, void* ws, size_t ws_bytes, cudaStream_t st) {
   (void)w;
   EGNN_TRY(fast_supported(d));
   const FastDims f = fast_dims(d);
@@ -382,9 +382,12 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
       const int grid = items < sms ? items : sms;
       const bool lean = pair_is_lean(f);
       const size_t smem = lean ? tc_pair_smem_bytes<false>(f.Hp, 1) : tc_pair_smem_bytes<true>(f.Hp, f.QT, 1 + 2 * f.s.F);
-      if (box) {
-        if (lean) EGNN_TRY((launch_tc_pair<false, true>(a, grid, smem, st)));
-        else EGNN_TRY((launch_tc_pair<true, true>(a, grid, smem, st)));
+      if (pbc == PBC_CELL) {
+        if (lean) EGNN_TRY((launch_tc_pair<false, PBC_CELL>(a, grid, smem, st)));
+        else EGNN_TRY((launch_tc_pair<true, PBC_CELL>(a, grid, smem, st)));
+      } else if (pbc == PBC_BOX) {
+        if (lean) EGNN_TRY((launch_tc_pair<false, PBC_BOX>(a, grid, smem, st)));
+        else EGNN_TRY((launch_tc_pair<true, PBC_BOX>(a, grid, smem, st)));
       } else {
         if (lean) EGNN_TRY((launch_tc_pair<false>(a, grid, smem, st)));
         else EGNN_TRY((launch_tc_pair<true>(a, grid, smem, st)));
@@ -395,7 +398,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
   } else {         // neighbour lists: distance + top-k select, then the gathered fused edge kernel
     int32_t* nbr_idx = reinterpret_cast<int32_t*>(base + wl.nbr_idx);
     uint8_t* nbr_ok = base + wl.nbr_ok;
-    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box, wl.cell_bytes ? base + wl.cell : nullptr));
+    EGNN_TRY(select_neighbors(d, io, &nbr_idx, &nbr_ok, st, box, wl.cell_bytes ? base + wl.cell : nullptr, pbc));
     StageTimer tm(st, STAGE_PAIR);
     TcKnnArgs a{};
     a.B = s.B; a.N = s.N; a.Hp = f.Hp; a.ldn = f.Kn; a.dim = s.dim; a.k = s.k; a.edge_dim = s.edge_dim;
@@ -423,9 +426,12 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     if (R > 0) {
 #define EGNN_TC_KNN_LAUNCH(MODE_, ROWS_)                                                  \
   do {                                                                              \
-    if (box) {                                                                      \
-      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, true>, smem)));     \
-      tc_knn_kernel<MODE_, ROWS_, true><<<grid, ROWS_ * 32, smem, st>>>(a);         \
+    if (pbc == PBC_CELL) {                                                          \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_CELL>, smem))); \
+      tc_knn_kernel<MODE_, ROWS_, PBC_CELL><<<grid, ROWS_ * 32, smem, st>>>(a);     \
+    } else if (pbc == PBC_BOX) {                                                    \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_BOX>, smem)));  \
+      tc_knn_kernel<MODE_, ROWS_, PBC_BOX><<<grid, ROWS_ * 32, smem, st>>>(a);      \
     } else {                                                                        \
       EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_>, smem)));           \
       tc_knn_kernel<MODE_, ROWS_><<<grid, ROWS_ * 32, smem, st>>>(a);               \

@@ -35,15 +35,22 @@ struct SelArgs {
   const T* box;              // [B,C] periodic box lengths (PBC instantiations only)
 };
 
-// pb (PBC only): the box of graph b as L[8] | 1/L[8] (box_axis)
-template <typename T, bool PBC>
+// pb: the box of graph b as L[8] | 1/L[8] (box_axis; PBC_BOX), or its staged cell (cell_staged; PBC_CELL)
+template <typename T, int PBC>
 __device__ __forceinline__ T rank_of(const SelArgs<T>& a, int b, int i, int j, const T* xi, bool mask_i, const T* pb) {
   const T* xj = a.coors + ((size_t)b * a.N + j) * a.C;
   T d = T(0);
-  for (int c = 0; c < a.C; ++c) {
-    T r = xi[c] - xj[c];
-    if constexpr (PBC) r = min_image<T>(r, pb[c], pb[8 + c]);
-    d = sq_acc<T>(r, d);
+  if constexpr (PBC == PBC_CELL) {
+    T r[3];
+    for (int c = 0; c < 3; ++c) r[c] = c < a.C ? xi[c] - xj[c] : T(0);
+    cell_wrap<T>(r[0], r[1], r[2], pb);
+    for (int c = 0; c < a.C; ++c) d = sq_acc<T>(r[c], d);
+  } else {
+    for (int c = 0; c < a.C; ++c) {
+      T r = xi[c] - xj[c];
+      if constexpr (PBC) r = min_image<T>(r, pb[c], pb[8 + c]);
+      d = sq_acc<T>(r, d);
+    }
   }
   if (a.mask && !(mask_i && a.mask[(size_t)b * a.N + j])) d = T(1e5);
   if (a.adj) {
@@ -64,7 +71,7 @@ inline size_t sel_smem_bytes(int C, int warps = SEL_WARPS_MAX) {
 // CDIM = 3: the coordinate loops are exactly three steps (the generic instantiation, CDIM = 0, issues all eight predicated
 // steps per candidate -- 125 instead of ~55 instructions per trip of the scan, which is 63 % of the kernel; ncu source page)
 // PBC: ranks by the minimum-image distance under a.box.
-template <typename T, int SEL_WARPS, int CDIM, bool PBC = false>
+template <typename T, int SEL_WARPS, int CDIM, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(SEL_WARPS * 32)
 knn_warp_select_kernel(const SelArgs<T> a) {
   constexpr int NC = CDIM ? CDIM : 8;
@@ -83,11 +90,37 @@ knn_warp_select_kernel(const SelArgs<T> a) {
 #pragma unroll
   for (int c = 0; c < NC; ++c) xi[c] = (CDIM || c < a.C) ? a.coors[row * a.C + c] : T(0);
   const bool mask_i = a.mask ? a.mask[row] != 0 : true;
-  T bl[PBC ? NC : 1], binv[PBC ? NC : 1];          // the box of graph b, once per row (box_axis)
-  if constexpr (PBC) {
+  T bl[PBC == PBC_BOX ? NC : 1], binv[PBC == PBC_BOX ? NC : 1];   // the box of graph b, once per row (box_axis)
+  T pc[PBC == PBC_CELL ? CELL_STAGED : 1];         // or its cell (cell_staged)
+  if constexpr (PBC == PBC_CELL) {
+#pragma unroll
+    for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, a.C, t);
+  } else if constexpr (PBC) {
 #pragma unroll
     for (int c = 0; c < NC; ++c) box_axis<T>(a.box, b, a.C, c, bl[c], binv[c]);
   }
+  // the rank of x_i - x_j(c) (xj(c) reads candidate coordinate c): the squared length of the wrapped pair vector
+  auto dist = [&](auto xj) {
+    T d = T(0);
+    if constexpr (PBC == PBC_CELL) {
+      T r[3];
+#pragma unroll
+      for (int c = 0; c < 3; ++c) r[c] = (c < NC && (CDIM || c < a.C)) ? xi[c < NC ? c : 0] - xj(c) : T(0);
+      cell_wrap<T>(r[0], r[1], r[2], pc);
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        if (c < NC && (CDIM || c < a.C)) d = sq_acc<T>(r[c], d);
+    } else {
+#pragma unroll
+      for (int c = 0; c < NC; ++c)
+        if (CDIM || c < a.C) {
+          T r = xi[c] - xj(c);
+          if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
+          d = sq_acc<T>(r, d);
+        }
+    }
+    return d;
+  };
   const uint8_t* adjrow = a.adj ? a.adj + ((size_t)(a.adj_batched ? b : 0) * a.N + i) * a.N : nullptr;
   const T INF = T(INFINITY);
   const int IMAX = 0x7fffffff;
@@ -121,14 +154,7 @@ knn_warp_select_kernel(const SelArgs<T> a) {
         const bool jvalid = jj < jn;
         key[u] = INF;
         if (jvalid) {
-          T d = T(0);
-#pragma unroll
-          for (int c = 0; c < NC; ++c)
-            if (CDIM || c < a.C) {
-              T r = xi[c] - xs[c * SEL_JC + jj];
-              if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-              d = sq_acc<T>(r, d);
-            }
+          T d = dist([&](int c) { return xs[c * SEL_JC + jj]; });
           if (a.mask && !(mask_i && ms[jj])) d = T(1e5);
           if (adjrow) {
             if (i == j) d = T(-1);
@@ -186,14 +212,7 @@ knn_warp_select_kernel(const SelArgs<T> a) {
     bool nan_rank = false;
     if (j < a.N) {                     // the rank of the scan above, read from global memory
       const T* xj = a.coors + ((size_t)b * a.N + j) * a.C;
-      T d = T(0);
-#pragma unroll
-      for (int c = 0; c < NC; ++c)
-        if (CDIM || c < a.C) {
-          T r = xi[c] - xj[c];
-          if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-          d = sq_acc<T>(r, d);
-        }
+      T d = dist([&](int c) { return xj[c]; });
       if (a.mask && !(mask_i && a.mask[(size_t)b * a.N + j])) d = T(1e5);
       if (adjrow) {
         if (i == j) d = T(-1);
@@ -212,7 +231,7 @@ knn_warp_select_kernel(const SelArgs<T> a) {
 }
 
 // k > 32: block-wide bitonic sort of all N candidates in shared memory.
-template <typename T, bool PBC = false>
+template <typename T, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(256)
 knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   extern __shared__ __align__(16) unsigned char sel_smem[];
@@ -226,7 +245,11 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   if constexpr (PBC) {
     __shared__ T box_s[16];
     pb = box_s;
-    if (threadIdx.x < 8) box_axis<T>(a.box, b, a.C, threadIdx.x, pb[threadIdx.x], pb[8 + threadIdx.x]);
+    if constexpr (PBC == PBC_CELL) {
+      if (threadIdx.x < CELL_STAGED) pb[threadIdx.x] = cell_staged<T>(a.box, b, a.C, threadIdx.x);
+    } else {
+      if (threadIdx.x < 8) box_axis<T>(a.box, b, a.C, threadIdx.x, pb[threadIdx.x], pb[8 + threadIdx.x]);
+    }
     __syncthreads();
   }
   for (int j = threadIdx.x; j < Npad; j += blockDim.x) {
@@ -260,7 +283,7 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
   }
 }
 
-template <typename T, bool PBC>
+template <typename T, int PBC>
 static int launch_select(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const uint8_t* adj,
                          int adj_batched, double valid_radius, int32_t* out_idx, uint8_t* out_ok, const void* box,
                          cudaStream_t st) {
@@ -308,17 +331,29 @@ static int launch_select(int B, int N, int C, int k, const void* coors, const ui
   return EGNN_OK;
 }
 
-// box: [B,C] periodic box lengths in the coordinates' type, or null (the layer's select only: egnn_knn_select has none)
+template <typename T>
+static int launch_select_pbc(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const uint8_t* adj,
+                             int adj_batched, double valid_radius, int32_t* out_idx, uint8_t* out_ok, const void* box,
+                             int pbc, cudaStream_t st) {
+  if (pbc == PBC_CELL)
+    return launch_select<T, PBC_CELL>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
+  if (pbc == PBC_BOX)
+    return launch_select<T, PBC_BOX>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
+  return launch_select<T, PBC_NONE>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
+}
+
+// box: [B,C] periodic box lengths (pbc = PBC_BOX) or a [B,C,C] cell (PBC_CELL, C in {2, 3}) in the coordinates' type,
+// or null (the layer's select only: egnn_knn_select has none)
 int knn_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
                         const uint8_t* adj, int adj_batched, double valid_radius, int32_t* out_idx,
-                        uint8_t* out_ok, cudaStream_t st, const void* box = nullptr) {
+                        uint8_t* out_ok, cudaStream_t st, const void* box = nullptr, int pbc = PBC_NONE) {
   if (!coors || !out_idx) return EGNN_ERR_NULL;
   if (B <= 0 || B > 65535 || N <= 0 || C <= 0 || C > 8 || k <= 0 || k > N) return EGNN_ERR_SHAPE;
+  if (!box) pbc = PBC_NONE;
+  if (pbc == PBC_CELL && (C < 2 || C > 3)) return EGNN_ERR_SHAPE;
   if (dtype == EGNN_DTYPE_F64)
-    return box ? launch_select<double, true>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st)
-               : launch_select<double, false>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
-  return box ? launch_select<float, true>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st)
-             : launch_select<float, false>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, st);
+    return launch_select_pbc<double>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, pbc, st);
+  return launch_select_pbc<float>(B, N, C, k, coors, mask, adj, adj_batched, valid_radius, out_idx, out_ok, box, pbc, st);
 }
 
 // only_sparse_neighbors WITH a node mask (egnn_pytorch.py:249-260, :296): valid_radius is 0, so the only slots whose
@@ -384,7 +419,7 @@ int adj_neighbors_dispatch(int B, int N, int k, const uint8_t* adj, int adj_batc
 }
 
 int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
-                     const void* box, void* cell_ws) {
+                     const void* box, void* cell_ws, int pbc) {
   if (io.nbr_idx) {                                  // edge-list mode: the caller's lists, no ranking
     *nbr_idx = const_cast<int32_t*>(io.nbr_idx);
     *nbr_ok = nullptr;
@@ -395,14 +430,14 @@ int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nb
   const int32_t cdt = d.dtype == EGNN_DTYPE_F64 ? EGNN_DTYPE_F64 : EGNN_DTYPE_F32;
   if (cell_ws && cell_select_runs(d, io))            // a radius graph with a mask: the same kept slots from a cell grid
     return cell_select_dispatch(cdt, d.B, d.N, d.C, d.k, io.coors, io.mask, box, d.valid_radius, *nbr_idx, *nbr_ok,
-                                nullptr, cell_ws, st);
+                                nullptr, cell_ws, st, pbc);
   count_launch();
   const int adj_batched = (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0;
   if ((d.flags & EGNN_FLAG_ONLY_SPARSE) && io.mask && io.adj)      // every slot top-k could add is masked out: row scan
     return adj_neighbors_dispatch(d.B, d.N, d.k, io.adj, adj_batched, *nbr_idx, *nbr_ok, st);
   const double vr = (d.flags & EGNN_FLAG_ONLY_SPARSE) ? 0.0 : d.valid_radius;     // egnn_pytorch.py:250
   return knn_select_dispatch(cdt, d.B, d.N, d.C, d.k, io.coors, io.mask, io.adj, adj_batched, vr, *nbr_idx, *nbr_ok, st,
-                             box);
+                             box, pbc);
 }
 
 }  // namespace egnn

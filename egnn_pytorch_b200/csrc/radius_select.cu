@@ -9,6 +9,7 @@
 //
 // Grid, per graph: cell edge cs = sqrt(r2) (1 + 2^-10).  A periodic axis (finite L > 0) has n = max(1, floor(L / cs))
 // cells of width L / n >= cs, positions wrapped into [0, L); an aperiodic axis uses floor(x / cs), clamped to +-2^30.
+// A triclinic cell bins its periodic axes in fractional coordinates instead (frac_cells).
 // Binning runs in double.  Cell coordinates hash into Tb = next_pow2(2N) buckets, so the scratch follows from N alone;
 // a collision only adds candidates that the exact rank filter removes.  DESIGN.md section 5 gives the argument that
 // no pair the filter keeps lies outside the 3^C cells around a node.
@@ -87,7 +88,7 @@ struct RadArgs {
   double cs;                       // cell edge
   const T* coors;                  // [B,N,C]
   const uint8_t* mask;             // [B,N] or null
-  const T* box;                    // [B,C] (PBC instantiations only)
+  const T* box;                    // [B,C] box (PBC_BOX) or [B,C,C] cell (PBC_CELL)
   int* cnt;                        // [B,Tb] bucket sizes
   int* end;                        // [B,Tb] bucket starts after the scan, bucket ends after the scatter
   T* xs;                           // [C][B*N] coordinates in cell order (graph b at b*N)
@@ -98,7 +99,7 @@ struct RadArgs {
 };
 
 // Axis c of graph b's grid: n[c] > 0 cells of width w[c] on a periodic axis of length L[c]; n[c] = 0 on an aperiodic one.
-template <typename T, int CD, bool PBC>
+template <typename T, int CD, int PBC>
 __device__ __forceinline__ void axis_grids(const RadArgs<T>& a, int b, double (&L)[CD], double (&w)[CD], int (&n)[CD]) {
 #pragma unroll
   for (int c = 0; c < CD; ++c) {
@@ -144,17 +145,59 @@ __device__ __forceinline__ bool load_node(const RadArgs<T>& a, size_t t, T (&x)[
   return ok;
 }
 
-template <typename T, int CD, bool PBC>
+// PBC_CELL: the cell coordinates cc of x in graph b's grid, and the cell count n of every axis (0: aperiodic).  A
+// periodic axis k is binned in the fractional coordinate s_k = sum_d x_d G[d][k], G = A^-1 of the lower-triangular cell
+// A with 1 in place of every aperiodic diagonal, wrapped into [0, 1) and cut into n_k = max(1, floor(w_k / cs)) cells,
+// w_k = 1 / |column k of G| being the cell's perpendicular width along a_k.  An aperiodic axis (its row and column of
+// A are zero but for the diagonal, so s_k = x_k) is binned as without a cell.  Double precision throughout.
+template <typename T, int CD>
+__device__ __forceinline__ void frac_cells(const RadArgs<T>& a, int b, const T (&x)[CD], int (&cc)[CD], int (&n)[CD]) {
+  const T* m = a.box + (size_t)b * CD * CD;
+  double A[CD][CD], G[CD][CD];
+  bool per[CD];
+#pragma unroll
+  for (int r = 0; r < CD; ++r) {
+#pragma unroll
+    for (int c = 0; c < CD; ++c) { A[r][c] = c <= r ? (double)m[r * CD + c] : 0.0; G[r][c] = 0.0; }
+    per[r] = A[r][r] > 0.0 && A[r][r] < INFINITY;
+    if (!per[r]) A[r][r] = 1.0;
+  }
+#pragma unroll
+  for (int k = 0; k < CD; ++k) {                       // column k of G: forward substitution down the rows
+    G[k][k] = 1.0 / A[k][k];
+#pragma unroll
+    for (int r = k + 1; r < CD; ++r) {
+      double acc = 0.0;
+#pragma unroll
+      for (int q = k; q < r; ++q) acc = fma(A[r][q], G[q][k], acc);
+      G[r][k] = -acc / A[r][r];
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < CD; ++k) {
+    double s = 0.0, g2 = 0.0;
+#pragma unroll
+    for (int d = k; d < CD; ++d) { s = fma((double)x[d], G[d][k], s); g2 = fma(G[d][k], G[d][k], g2); }
+    n[k] = per[k] ? (int)fmin(fmax(floor(1.0 / (sqrt(g2) * a.cs)), 1.0), RS_CLAMP) : 0;
+    cc[k] = n[k] > 0 ? cell_coord(s, a.cs, 1.0, 1.0 / n[k], n[k]) : cell_coord(s, a.cs, 0.0, a.cs, 0);
+  }
+}
+
+template <typename T, int CD, int PBC>
 __device__ __forceinline__ int node_bucket(const RadArgs<T>& a, int b, const T (&x)[CD]) {
   double L[CD], w[CD];
   int n[CD], cc[CD];
+  if constexpr (PBC == PBC_CELL) {
+    frac_cells<T, CD>(a, b, x, cc, n);
+    return cell_bucket<CD>(cc, a.Tb);
+  }
   axis_grids<T, CD, PBC>(a, b, L, w, n);
 #pragma unroll
   for (int c = 0; c < CD; ++c) cc[c] = cell_coord((double)x[c], a.cs, L[c], w[c], n[c]);
   return cell_bucket<CD>(cc, a.Tb);
 }
 
-template <typename T, int CD, bool PBC>
+template <typename T, int CD, int PBC>
 __global__ void __launch_bounds__(RS_THREADS) radius_count_kernel(const RadArgs<T> a) {
   const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
   if (t >= (size_t)a.B * a.N) return;
@@ -198,7 +241,7 @@ __global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_kernel(const int*
   }
 }
 
-template <typename T, int CD, bool PBC>
+template <typename T, int CD, int PBC>
 __global__ void __launch_bounds__(RS_THREADS) radius_scatter_kernel(const RadArgs<T> a) {
   const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
   if (t >= (size_t)a.B * a.N) return;
@@ -212,7 +255,7 @@ __global__ void __launch_bounds__(RS_THREADS) radius_scatter_kernel(const RadArg
   a.idx[g0 + pos] = i;
 }
 
-template <typename T, int CD, bool PBC>
+template <typename T, int CD, int PBC>
 __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadArgs<T> a) {
   constexpr int NB = CD == 1 ? 3 : (CD == 2 ? 9 : 27);           // neighbouring cells
   __shared__ T qkey[RS_WARPS][64];
@@ -231,8 +274,11 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
   T xi[CD];
 #pragma unroll
   for (int c = 0; c < CD; ++c) xi[c] = a.xs[c * BN + g0 + p];
-  T bl[CD], binv[CD];
-  if constexpr (PBC) {
+  T bl[CD], binv[CD], pc[PBC == PBC_CELL ? CELL_STAGED : 1];
+  if constexpr (PBC == PBC_CELL) {
+#pragma unroll
+    for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, CD, t);
+  } else if constexpr (PBC) {
 #pragma unroll
     for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);
   }
@@ -243,14 +289,25 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
   if (lane < NB) {
     double L[CD], w[CD];
     int n[CD], cc[CD];
-    axis_grids<T, CD, PBC>(a, b, L, w, n);
     int r = lane;
+    if constexpr (PBC == PBC_CELL) {
+      frac_cells<T, CD>(a, b, xi, cc, n);
 #pragma unroll
-    for (int c = 0; c < CD; ++c) {
-      int v = cell_coord((double)xi[c], a.cs, L[c], w[c], n[c]) + r % 3 - 1;
-      r /= 3;
-      if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
-      cc[c] = v;
+      for (int c = 0; c < CD; ++c) {
+        int v = cc[c] + r % 3 - 1;
+        r /= 3;
+        if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
+        cc[c] = v;
+      }
+    } else {
+      axis_grids<T, CD, PBC>(a, b, L, w, n);
+#pragma unroll
+      for (int c = 0; c < CD; ++c) {
+        int v = cell_coord((double)xi[c], a.cs, L[c], w[c], n[c]) + r % 3 - 1;
+        r /= 3;
+        if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
+        cc[c] = v;
+      }
     }
     bkt = cell_bucket<CD>(cc, a.Tb);
   }
@@ -287,11 +344,20 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
       const size_t pos = g0 + sdelta[warp][s] + t;
       j = a.idx[pos];
       T d = T(0);
+      if constexpr (PBC == PBC_CELL) {
+        T r[3];
 #pragma unroll
-      for (int c = 0; c < CD; ++c) {
-        T r = xi[c] - a.xs[c * BN + pos];
-        if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-        d = sq_acc<T>(r, d);
+        for (int c = 0; c < 3; ++c) r[c] = c < CD ? xi[c < CD ? c : 0] - a.xs[(c < CD ? c : 0) * BN + pos] : T(0);
+        cell_wrap<T>(r[0], r[1], r[2], pc);
+#pragma unroll
+        for (int c = 0; c < CD; ++c) d = sq_acc<T>(r[c], d);
+      } else {
+#pragma unroll
+        for (int c = 0; c < CD; ++c) {
+          T r = xi[c] - a.xs[c * BN + pos];
+          if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
+          d = sq_acc<T>(r, d);
+        }
       }
       const bool in = d <= a.r2;
       nin += in ? 1 : 0;
@@ -341,7 +407,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
   }
 }
 
-template <typename T, int CD, bool PBC>
+template <typename T, int CD, int PBC>
 static int launch_cell(const RadArgs<T>& a, cudaStream_t st) {
   const size_t nodes = (size_t)a.B * a.N;
   const unsigned gn = (unsigned)((nodes + RS_THREADS - 1) / RS_THREADS);
@@ -360,7 +426,7 @@ static int launch_cell(const RadArgs<T>& a, cudaStream_t st) {
 
 template <typename T>
 static int cell_select(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box, double r2,
-                       int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws, cudaStream_t st) {
+                       int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws, cudaStream_t st, int pbc) {
   const CellWs L = cell_ws_layout(B, N, C, sizeof(T));
   char* base = static_cast<char*>(ws);
   RadArgs<T> a;
@@ -373,13 +439,18 @@ static int cell_select(int B, int N, int C, int k, const void* coors, const uint
   a.xs = reinterpret_cast<T*>(base + L.xs);
   a.idx = reinterpret_cast<int*>(base + L.idx);
   a.out_idx = out_idx; a.out_ok = out_ok; a.out_count = out_count;
+  if (box && pbc == PBC_CELL) {
+    if (C == 2) return launch_cell<T, 2, PBC_CELL>(a, st);
+    if (C == 3) return launch_cell<T, 3, PBC_CELL>(a, st);
+    return EGNN_ERR_SHAPE;
+  }
   switch (C * 2 + (box ? 1 : 0)) {
-    case 2: return launch_cell<T, 1, false>(a, st);
-    case 3: return launch_cell<T, 1, true>(a, st);
-    case 4: return launch_cell<T, 2, false>(a, st);
-    case 5: return launch_cell<T, 2, true>(a, st);
-    case 6: return launch_cell<T, 3, false>(a, st);
-    case 7: return launch_cell<T, 3, true>(a, st);
+    case 2: return launch_cell<T, 1, PBC_NONE>(a, st);
+    case 3: return launch_cell<T, 1, PBC_BOX>(a, st);
+    case 4: return launch_cell<T, 2, PBC_NONE>(a, st);
+    case 5: return launch_cell<T, 2, PBC_BOX>(a, st);
+    case 6: return launch_cell<T, 3, PBC_NONE>(a, st);
+    case 7: return launch_cell<T, 3, PBC_BOX>(a, st);
     default: return EGNN_ERR_UNSUPPORTED;
   }
 }
@@ -394,16 +465,16 @@ static int radius_check(int B, int N, int C, int k) {
 // r2 is the radius as the caller passes it; the kernels compare against (T)r2.
 int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
                          const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
-                         cudaStream_t st) {
+                         cudaStream_t st, int pbc) {
   if (!coors || !out_idx || !ws) return EGNN_ERR_NULL;
   EGNN_TRY(radius_check(B, N, C, k));
   if (dtype == EGNN_DTYPE_F64) {
     if (!(r2 > 0.0)) return EGNN_ERR_SHAPE;
-    return cell_select<double>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st);
+    return cell_select<double>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
   }
   if (dtype != EGNN_DTYPE_F32) return EGNN_ERR_UNSUPPORTED;
   if (!((float)r2 > 0.f)) return EGNN_ERR_SHAPE;
-  return cell_select<float>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st);
+  return cell_select<float>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
 }
 
 }  // namespace egnn
@@ -423,5 +494,17 @@ extern "C" int egnn_radius_select(int32_t dtype, int32_t B, int32_t N, int32_t C
   if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
   if (workspace_bytes < egnn::cell_select_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
   return egnn::cell_select_dispatch(dtype, B, N, C, k, coors, mask, box, r2, out_idx, nullptr, out_count, workspace,
-                                    static_cast<cudaStream_t>(stream));
+                                    static_cast<cudaStream_t>(stream), egnn::PBC_BOX);
+}
+
+extern "C" int egnn_radius_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                                            const uint8_t* mask, const void* cell, double r2, int32_t* out_idx,
+                                            int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream) {
+  if (!workspace || !cell) return EGNN_ERR_NULL;
+  if (C < 2 || C > 3) return EGNN_ERR_SHAPE;               // a cell is 2-D or 3-D (before radius_check's C > 3)
+  EGNN_TRY(egnn::radius_check(B, N, C, k));
+  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
+  if (workspace_bytes < egnn::cell_select_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
+  return egnn::cell_select_dispatch(dtype, B, N, C, k, coors, mask, cell, r2, out_idx, nullptr, out_count, workspace,
+                                    static_cast<cudaStream_t>(stream), egnn::PBC_CELL);
 }

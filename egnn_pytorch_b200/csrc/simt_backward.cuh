@@ -118,7 +118,7 @@ inline size_t bwd1_smem_bytes(const Dims& s, const SimtPackLayout& L, bool soft)
   return round_up(n * sizeof(T), 16) + 16;
 }
 
-template <typename T, int MP, bool KNN, bool BLK, bool PBC = false>
+template <typename T, int MP, bool KNN, bool BLK, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd1_kernel(const BwdArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -131,7 +131,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
   if constexpr (PBC) {
     __shared__ T box_s[2 * PAIR_CMAX];
     pb = box_s;
-    stage_box<T>(pb, a.box, b, s.C);
+    stage_box<T, PBC>(pb, a.box, b, s.C);
   }
   const int i_raw = rows_begin<BLK>(s) + blockIdx.x * TI + g;
   const bool row_valid = i_raw < rows_end<BLK>(s);
@@ -845,7 +845,7 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
 // bwd3: dL/d(dist) -> coordinates and edges.  Same thread <-> pair mapping as bwd1.  PBC: the minimum image has the
 // derivative of x_i - x_j (rint is piecewise constant), so only rel changes.
 // =====================================================================================
-template <typename T, bool KNN, bool BLK, bool PBC = false>
+template <typename T, bool KNN, bool BLK, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd3_kernel(const BwdArgs<T> a) {
   const Dims& s = a.s;
@@ -857,7 +857,7 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
   if constexpr (PBC) {
     __shared__ T box_s[2 * PAIR_CMAX];
     pb = box_s;
-    stage_box<T>(pb, a.box, b, s.C);
+    stage_box<T, PBC>(pb, a.box, b, s.C);
   }
   const int i_raw = rows_begin<BLK>(s) + blockIdx.x * TI + g;
   const bool row_valid = i_raw < rows_end<BLK>(s);

@@ -81,7 +81,7 @@ static int launch_simt(void (*kernel)(Arg), dim3 grid, int threads, size_t smem,
 }
 
 // The edge step over neighbour lists.  PBC: the periodic instantiations (a.box set).
-template <typename T, int MP, bool PBC = false>
+template <typename T, int MP, int PBC = PBC_NONE>
 static int launch_pair(const PairArgs<T>& a, cudaStream_t st) {
   dim3 grid(ceil_div(a.s.row1 - a.s.row0, PAIR_THREADS / a.TS), a.s.B);
   void (*kernel)(PairArgs<T>) = row_block(a.s, a.flags) ? pair_kernel<T, MP, true, PBC> : pair_kernel<T, MP, false, PBC>;
@@ -89,7 +89,7 @@ static int launch_pair(const PairArgs<T>& a, cudaStream_t st) {
 }
 
 // The dense edge step at PP rows per thread; a.hsplit > 1 runs it as two phases over a split hidden axis.
-template <typename T, int MP, int PP, bool PBC>
+template <typename T, int MP, int PP, int PBC>
 static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
   const size_t smem = pair_tiled_smem_bytes<T>(a.s, a.L, PP);
   dim3 grid(ceil_div(a.s.row1 - a.s.row0, 4 * PP), a.s.B);
@@ -107,7 +107,7 @@ static int launch_pair_tiled(const PairArgs<T>& a, cudaStream_t st) {
 
 // The dense edge step at two rows per thread where its shared memory fits, else at one (fp64 with m_dim > 16:
 // one always).
-template <typename T, int MP, bool PBC = false>
+template <typename T, int MP, int PBC = PBC_NONE>
 static int launch_pair_dense(const PairArgs<T>& a, cudaStream_t st) {
   constexpr int PP = (MP == 32 && sizeof(T) == 8) ? 1 : 2;
   const int rc = launch_pair_tiled<T, MP, PP, PBC>(a, st);

@@ -328,27 +328,41 @@ __device__ __forceinline__ PairSlot pair_slot(const int32_t* nbr_idx, const uint
 }
 
 // rel = x_i - x_j (zero beyond C) and the squared distance d (egnn_pytorch.py:232-233).  PBC: rel is the minimum image
-// under the box `pb` staged by stage_box.
-template <typename T, bool PBC = false>
+// under the box `pb` staged by stage_box (PBC_BOX), or wrapped by the cell it staged (PBC_CELL, C <= 3).
+template <typename T, int PBC = PBC_NONE>
 __device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&rel)[PAIR_CMAX], const T* pb = nullptr) {
   T d = T(0);
+  if constexpr (PBC == PBC_CELL) {
 #pragma unroll
-  for (int c = 0; c < PAIR_CMAX; ++c) {
-    rel[c] = T(0);
-    if (c < C) {
-      rel[c] = xi[c] - xj[c];
-      if constexpr (PBC) rel[c] = min_image<T>(rel[c], pb[c], pb[PAIR_CMAX + c]);
-      d = sq_acc<T>(rel[c], d);
+    for (int c = 0; c < PAIR_CMAX; ++c) rel[c] = c < C ? xi[c] - xj[c] : T(0);
+    cell_wrap<T>(rel[0], rel[1], rel[2], pb);
+#pragma unroll
+    for (int c = 0; c < 3; ++c)
+      if (c < C) d = sq_acc<T>(rel[c], d);
+  } else {
+#pragma unroll
+    for (int c = 0; c < PAIR_CMAX; ++c) {
+      rel[c] = T(0);
+      if (c < C) {
+        rel[c] = xi[c] - xj[c];
+        if constexpr (PBC) rel[c] = min_image<T>(rel[c], pb[c], pb[PAIR_CMAX + c]);
+        d = sq_acc<T>(rel[c], d);
+      }
     }
   }
   return d;
 }
 
-// Graph b's box in shared memory for pair_geometry: L[PAIR_CMAX] | 1/L[PAIR_CMAX] (box_axis), staged once per CTA
-// (every CTA of the pair kernels works on one graph).  Ends with a barrier, so all threads of the CTA must call it.
-template <typename T>
+// Graph b's box in shared memory for pair_geometry: L[PAIR_CMAX] | 1/L[PAIR_CMAX] (box_axis), or its cell as
+// cell_staged lays it out (PBC_CELL), staged once per CTA (every CTA of the pair kernels works on one graph).  Ends
+// with a barrier, so all threads of the CTA must call it.
+template <typename T, int PBC = PBC_BOX>
 __device__ __forceinline__ void stage_box(T* pb, const T* box, int b, int C) {
-  if (threadIdx.x < PAIR_CMAX) box_axis<T>(box, b, C, threadIdx.x, pb[threadIdx.x], pb[PAIR_CMAX + threadIdx.x]);
+  if constexpr (PBC == PBC_CELL) {
+    if (threadIdx.x < CELL_STAGED) pb[threadIdx.x] = cell_staged<T>(box, b, C, threadIdx.x);
+  } else {
+    if (threadIdx.x < PAIR_CMAX) box_axis<T>(box, b, C, threadIdx.x, pb[threadIdx.x], pb[PAIR_CMAX + threadIdx.x]);
+  }
   __syncthreads();
 }
 
@@ -422,7 +436,7 @@ inline size_t pair_smem_bytes(const Dims& s, const SimtPackLayout& L) {
 
 // Neighbour lists: 128 threads per CTA arranged as TI row-groups x TS slots (TS lanes of one warp).
 // BLK: pre2_out is block-relative (pair_row).  PBC: minimum-image geometry under a.box.
-template <typename T, int MP, bool BLK, bool PBC = false>
+template <typename T, int MP, bool BLK, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -435,7 +449,7 @@ pair_kernel(const PairArgs<T> a) {
   if constexpr (PBC) {
     __shared__ T box_s[2 * PAIR_CMAX];
     pb = box_s;
-    stage_box<T>(pb, a.box, b, s.C);
+    stage_box<T, PBC>(pb, a.box, b, s.C);
   }
   const int i_raw = s.row0 + blockIdx.x * TI + g;
   const bool row_valid = i_raw < s.row1;
@@ -622,7 +636,7 @@ inline size_t pair_tiled_smem_bytes(const Dims& s, const SimtPackLayout& L, int 
 }
 
 // BLK: pre2_out / hpart are block-relative (pair_row).  PBC: minimum-image geometry under a.box.
-template <typename T, int MP, int PP, bool BLK, bool PBC = false>
+template <typename T, int MP, int PP, bool BLK, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_dense_tiled_kernel(const PairArgs<T> a) {
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -633,7 +647,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
   if constexpr (PBC) {
     __shared__ T box_s[2 * PAIR_CMAX];
     pb = box_s;
-    stage_box<T>(pb, a.box, b, s.C);
+    stage_box<T, PBC>(pb, a.box, b, s.C);
   }
   const int U = 4 * s.m;
   const int qd = 2 * s.F;

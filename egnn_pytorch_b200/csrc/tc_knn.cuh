@@ -52,7 +52,7 @@ struct TcKnnArgs {
   const uint8_t* nbr_ok;           // [B][N][k]
   __nv_bfloat16* m_out;            // node_in + dim (stride ldn) | null
   float* coors_out;                // [B][N][3] | null
-  const float* box;                // [B][C] periodic box lengths (PBC instantiations only)
+  const float* box;                // [B][C] periodic box lengths (PBC_BOX) or [B][C][C] cell (PBC_CELL)
 };
 
 // channels of the Wq table staged in shared memory: 1 (lean), 1 + TK_QE (edges), Q (generic)
@@ -77,8 +77,9 @@ inline size_t tc_knn_smem_bytes(int Hp, int mode, int Q = 1, int rows = TK_ROWS)
 // host takes ROWS = 8 whenever two CTAs fit in shared memory (rows_per_cta below).
 inline int tc_knn_rows_per_cta(int Hp, int mode, int Q) { return 2 * (tc_knn_smem_bytes(Hp, mode, Q, 8) + 1024) <= 227 * 1024 ? 8 : 16; }
 
-// PBC: rel is the minimum image under a.box (the distance and the coordinate sum both follow from it)
-template <int MODE, int ROWS, bool PBC = false>
+// PBC: rel is the minimum image under a.box (PBC_BOX) or wrapped by the cell a.box (PBC_CELL); the distance and the
+// coordinate sum both follow from it
+template <int MODE, int ROWS, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(const TcKnnArgs a) {
   constexpr int TK_THREADS = ROWS * 32;
   constexpr bool EDGES = MODE == TK_EDGES, GEN = MODE == TK_GEN;
@@ -147,15 +148,27 @@ __global__ void __launch_bounds__(ROWS * 32, ROWS == 8 ? 2 : 1) tc_knn_kernel(co
   }
   const size_t nodej = (size_t)b * N + j;
   float boxL = 0.f, boxinv = 0.f;                      // PBC: lane c holds axis c of this graph's box, once per row
-  if constexpr (PBC) box_axis<float>(a.box, b, C, lane < NX ? lane : NX, boxL, boxinv);
   float rel[NX];
   float dmine = 0.f;
+  if constexpr (PBC == PBC_CELL) {                     // lane t < 9 holds value t of this graph's staged cell
+    const float cv = cell_staged<float>(a.box, b, C, lane < CELL_STAGED ? lane : 0);
+    float pc[CELL_STAGED];
 #pragma unroll
-  for (int c = 0; c < NX; ++c) {
-    rel[c] = (!GEN || c < C) ? xi[c] - a.coors[nodej * C + c] : 0.f;
-    if constexpr (PBC)
-      rel[c] = min_image<float>(rel[c], __shfl_sync(0xffffffffu, boxL, c), __shfl_sync(0xffffffffu, boxinv, c));
-    dmine = fmaf(rel[c], rel[c], dmine);
+    for (int t = 0; t < CELL_STAGED; ++t) pc[t] = __shfl_sync(0xffffffffu, cv, t);
+#pragma unroll
+    for (int c = 0; c < NX; ++c) rel[c] = (!GEN || c < C) ? xi[c] - a.coors[nodej * C + c] : 0.f;
+    cell_wrap<float>(rel[0], rel[1], rel[2], pc);
+#pragma unroll
+    for (int c = 0; c < NX; ++c) dmine = fmaf(rel[c], rel[c], dmine);
+  } else {
+    if constexpr (PBC) box_axis<float>(a.box, b, C, lane < NX ? lane : NX, boxL, boxinv);
+#pragma unroll
+    for (int c = 0; c < NX; ++c) {
+      rel[c] = (!GEN || c < C) ? xi[c] - a.coors[nodej * C + c] : 0.f;
+      if constexpr (PBC)
+        rel[c] = min_image<float>(rel[c], __shfl_sync(0xffffffffu, boxL, c), __shfl_sync(0xffffffffu, boxinv, c));
+      dmine = fmaf(rel[c], rel[c], dmine);
+    }
   }
   float* myS = stile + (size_t)warp * Q * 32;          // generic: this warp's per-slot scalar channels
   if (GEN) {

@@ -74,7 +74,7 @@ struct TcPairArgs {
   const uint8_t* mask;             // [B][N] | null
   __nv_bfloat16* m_out;            // node_in + dim (stride ldn) | null
   float* coors_out;                // [B][N][C] | null
-  const float* box;                // [B][C] periodic box lengths (PBC instantiations only)
+  const float* box;                // [B][C] periodic box lengths (PBC_BOX) or [B][C][C] cell (PBC_CELL)
 };
 
 template <bool GEN> struct TpCfg {
@@ -101,7 +101,7 @@ inline size_t tc_pair_smem_bytes(int Hp, int Q, int Qf = 1) {
   (void)Q;
   if (GEN) n += tc_pair_gen_scalar_bytes(Qf, Q - Qf);
   n += 8 * 8;                                               // mbarriers
-  n += (size_t)2 * 2 * TP_CMAX * 4;                         // periodic box per ring slot, first in the carve-up (PBC only)
+  n += (size_t)2 * 2 * TP_CMAX * 4;                         // periodic box or cell per ring slot, first in the carve-up (PBC only)
   return n + 128;                                           // (the box took 128 of the 256 bytes of headroom: every
                                                             //  instantiation keeps its size, so a periodic layer fits
                                                             //  wherever the plain one does)
@@ -178,8 +178,9 @@ __device__ __noinline__ void tp_finish_item(const TpFinishArgs a, const double* 
         }
 }
 
-// PBC: the pair geometry is the minimum image under a.box, at the distance and at the coordinate sum
-template <bool GEN, bool PBC = false>
+// PBC: the pair geometry is the minimum image under the box a.box (PBC_BOX) or wrapped by the cell a.box (PBC_CELL),
+// at the distance and at the coordinate sum
+template <bool GEN, int PBC = PBC_NONE>
 __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs a) {
   constexpr int PW = TpCfg<GEN>::PW, XC = TpCfg<GEN>::XC;
   // carve the dynamic shared memory directly (no integer round trip) so every access stays in the
@@ -187,7 +188,8 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
   extern __shared__ __align__(128) unsigned char sm[];
   const int Hp = a.Hp, N = a.N;
   const int Q = GEN ? a.Q : 1, C = GEN ? a.C : 3;
-  // PBC: the box of each ring slot's graph, [2][L[TP_CMAX] | 1/L[TP_CMAX]], first (a constant address); everything else
+  // PBC: the box of each ring slot's graph, [2][L[TP_CMAX] | 1/L[TP_CMAX]], or its cell (cell_staged, 9 of the 16
+  // floats per slot), first (a constant address); everything else
   // moves up by its 128 bytes, which keeps the 128-byte alignment of the TMA destinations
   float* boxs = reinterpret_cast<float*>(sm);
   unsigned char* w2s = sm + (PBC ? 2 * 2 * TP_CMAX * 4 : 0);                  // Hp*32 bytes
@@ -243,9 +245,12 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
       const int r = t - TP_TI * XC;
       const size_t node = (size_t)b * N + (r < rows_valid ? i0 + r : i0);
       mki[buf * TP_TI + r] = (r < rows_valid) && (a.has_mask ? a.mask[node] != 0 : true);
-    } else if (PBC && t < TP_TI * XC + TP_TI + TP_CMAX) {
+    } else if (PBC == PBC_BOX && t < TP_TI * XC + TP_TI + TP_CMAX) {
       const int c = t - TP_TI * XC - TP_TI;
       box_axis<float>(a.box, b, C, c, boxs[buf * 2 * TP_CMAX + c], boxs[buf * 2 * TP_CMAX + TP_CMAX + c]);
+    } else if (PBC == PBC_CELL && t < TP_TI * XC + TP_TI + CELL_STAGED) {
+      const int v = t - TP_TI * XC - TP_TI;
+      boxs[buf * 2 * TP_CMAX + v] = cell_staged<float>(a.box, b, C, v);
     }
     sync();
     if (t == 0) {
@@ -307,12 +312,18 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
       const float* Ab = As + (size_t)buf * TP_TI * Hp;
       const float* xi = xis + buf * TP_TI * XC;
       const uint32_t* mk = mki + buf * TP_TI;
-      const float* bx = PBC ? boxs + buf * 2 * TP_CMAX : nullptr;      // L | 1/L of graph b
-      // x_i - x_j, the minimum image under PBC
+      const float* bx = PBC ? boxs + buf * 2 * TP_CMAX : nullptr;      // L | 1/L of graph b (or its staged cell)
+      // x_i - x_j, the minimum image under PBC_BOX
       auto rel_c = [&](int i, int c, float xjc) {
         const float r = xi[i * XC + c] - xjc;
-        if constexpr (PBC) return min_image<float>(r, bx[c], bx[TP_CMAX + c]);
+        if constexpr (PBC == PBC_BOX) return min_image<float>(r, bx[c], bx[TP_CMAX + c]);
         return r;
+      };
+      // PBC_CELL: the three axes of x_i - x_j wrapped together (C <= 3, so any further axis is zero)
+      auto rel_cell = [&](int i, const float* xjv, float (&r)[3]) {
+#pragma unroll
+        for (int c = 0; c < 3; ++c) r[c] = rel_c(i, c, xjv[c]);
+        cell_wrap<float>(r[0], r[1], r[2], bx);
       };
       double* mypart = part + ((size_t)buf * TP_WARPS + warp) * TP_TI * PW;
       for (int x = lane; x < TP_TI * PW; x += 32) mypart[x] = 0.0;
@@ -337,8 +348,15 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
 #pragma unroll
         for (int i = 0; i < TP_TI; ++i) {
           float d = 0.f;
+          if constexpr (PBC == PBC_CELL) {
+            float r[3];
+            rel_cell(i, xj, r);
 #pragma unroll
-          for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float rc = rel_c(i, c, xj[c]); d = fmaf(rc, rc, d); }
+            for (int c = 0; c < 3; ++c) d = fmaf(r[c], r[c], d);
+          } else {
+#pragma unroll
+            for (int c = 0; c < (GEN ? TP_CMAX : 3); ++c) { const float rc = rel_c(i, c, xj[c]); d = fmaf(rc, rc, d); }
+          }
           swg[i * TP_TW + pp] = d;
           if (GEN) {
             int q = 1;
@@ -603,10 +621,17 @@ __global__ void __launch_bounds__(TP_THREADS, 1) tc_pair_kernel(const TcPairArgs
           float v[PW];
 #pragma unroll
           for (int o = 0; o < 16; ++o) v[o] = pm ? m[i][o] : 0.f;                                             // :322
+          if constexpr (PBC == PBC_CELL) {
+            float r[3];
+            rel_cell(i, xj, r);
 #pragma unroll
-          for (int c = 0; c < PW - 17; ++c) {
-            constexpr int NX = GEN ? TP_CMAX : 3;
-            v[16 + c] = (c < NX && (!GEN || c < C)) ? w * rel_c(i, c < NX ? c : 0, xj[c < NX ? c : 0]) : 0.f;
+            for (int c = 0; c < PW - 17; ++c) v[16 + c] = (c < 3 && (!GEN || c < C)) ? w * r[c < 3 ? c : 0] : 0.f;
+          } else {
+#pragma unroll
+            for (int c = 0; c < PW - 17; ++c) {
+              constexpr int NX = GEN ? TP_CMAX : 3;
+              v[16 + c] = (c < NX && (!GEN || c < C)) ? w * rel_c(i, c < NX ? c : 0, xj[c < NX ? c : 0]) : 0.f;
+            }
           }
           v[PW - 1] = pm ? 1.f : 0.f;
           // sum over the warp's 32 pairs

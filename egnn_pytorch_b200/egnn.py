@@ -168,7 +168,12 @@ class _EGNNLayerFunction(torch.autograd.Function):
             nat.check("egnn_layer_backward_workspace_bytes",
                       lib.egnn_layer_backward_workspace_bytes(C.byref(sv["desc"]), C.byref(nb)))
             ws = _workspace(dev, nb.value)
-            if sv["box"] is None:
+            if sv["cell"] is not None:
+                nat.check("egnn_layer_backward_triclinic",
+                          lib.egnn_layer_backward_triclinic(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]),
+                                                            C.byref(sv["io"]), _ptr(sv["cell"]), _ptr(sv["ws"]),
+                                                            C.byref(grads), _ptr(ws), ws.numel(), stream))
+            elif sv["box"] is None:
                 nat.check("egnn_layer_backward",
                           lib.egnn_layer_backward(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]), C.byref(sv["io"]),
                                                   _ptr(sv["ws"]), C.byref(grads), _ptr(ws), ws.numel(), stream))
@@ -302,7 +307,7 @@ class EGNN(nn.Module):
 
     # -------------------------------------------------------------- forward
     def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, neighbor_edges=None, box=None,
-                _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
+                cell=None, _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
         """Reference signature `forward(feats, coors, edges=None, mask=None, adj_mat=None)` (egnn_pytorch.py:224).
 
         `neighbors` (additive, keyword-only): int tensor [B, N, k] of neighbour indices, -1 = empty slot.  When
@@ -318,22 +323,36 @@ class EGNN(nn.Module):
         [B, C], on any device; every pair geometry x_i - x_j becomes its minimum image rel - L rint(rel / L) on the axes
         with a finite L > 0 (L = 0 or inf: not periodic).  Distances, neighbour ranking, CoorsNorm and the coordinate
         update follow; the output coordinates are not wrapped back into the box.  Orthorhombic boxes, one image per
-        neighbour, no gradient with respect to the box (a box that requires grad is rejected)."""
+        neighbour, no gradient with respect to the box (a box that requires grad is rejected).
+
+        `cell` (additive, keyword-only, instead of `box`): periodic boundaries in a triclinic cell.  Float tensor [C, C]
+        (shared by the batch) or [B, C, C], C in {2, 3}, row k = lattice vector a_k, lower-triangular (the LAMMPS
+        restricted-triclinic form; README shows how to rotate any cell into it).  A diagonal entry of 0 or inf leaves
+        its axis aperiodic; that axis's row and column must be zero off the diagonal.  Every pair vector is wrapped
+        sequentially from the last axis to the first (n = rint(r_c / L_c), r_d -= cell[c, d] n for d <= c), after which
+        |r_c| <= L_c / 2 on every periodic axis: the result lies in the centred box of the diagonal entries, a
+        fundamental domain of the lattice, so it is the minimum image whenever the minimum image is shorter than
+        min_c L_c / 2; pairs farther apart get that centred-box image, one image per neighbour.  A diagonal cell gives
+        exactly the outputs of `box=` with the same lengths.  No gradient with respect to the cell."""
         if neighbor_edges is not None:
             edges = self._check_neighbor_edges(feats, edges, neighbors, neighbor_edges, _label_emb)
         if box is not None:
+            if cell is not None:
+                raise ValueError("pass either box= or cell=, not both")
             _check_box(box, feats.shape[0], coors.shape[-1], self.__dict__)
+        if cell is not None:
+            _check_cell(cell, feats.shape[0], coors.shape[-1], self.__dict__)
         if torch.is_grad_enabled():             # (the parameter scan is skipped entirely under torch.no_grad())
             fields = self._state_fields()
             if (feats.requires_grad or coors.requires_grad or (edges is not None and edges.requires_grad) or
                     (_label_emb is not None and _label_emb.requires_grad) or any(p.requires_grad for _, _, _, p in fields)):
                 return self._forward_train(fields, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb,
-                                           _k_hint, _rows, neighbor_edges is not None, box)
+                                           _k_hint, _rows, neighbor_edges is not None, box, cell)
             with torch.no_grad():
                 return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint,
-                                          _rows, slot_edges=neighbor_edges is not None, box=box)
+                                          _rows, slot_edges=neighbor_edges is not None, box=box, cell=cell)
         return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
-                                  slot_edges=neighbor_edges is not None, box=box)
+                                  slot_edges=neighbor_edges is not None, box=box, cell=cell)
 
     def _check_neighbor_edges(self, feats, edges, neighbors, neighbor_edges, label_emb):
         """Misuse of `neighbor_edges` raises here, before anything is staged or launched; -> the tensor to run with."""
@@ -351,7 +370,7 @@ class EGNN(nn.Module):
         return neighbor_edges
 
     def _forward_train(self, fields, feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
-                       slot_edges=False, box=None):
+                       slot_edges=False, box=None, cell=None):
         """With a row range (`_rows=(r0, r1)`) the layer is differentiated as the function it returns: rows r0:r1 are the
         layer's output, every other row is its input unchanged.  The library's backward then yields this block's share
         of every gradient (EGNN_FLAG_ROW_PARTIAL_GRADS): the blocks of a partition of the rows sum to the full gradient."""
@@ -359,12 +378,13 @@ class EGNN(nn.Module):
 
         def run():
             return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
-                                      train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges, box=box)
+                                      train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges, box=box,
+                                      cell=cell)
 
         return _EGNNLayerFunction.apply(run, feats, coors, edges, label_emb, *params)
 
     def _forward_impl(self, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
-                      train=False, param_fields=None, slot_edges=False, box=None):
+                      train=False, param_fields=None, slot_edges=False, box=None, cell=None):
         """`slot_edges`: `edges` holds features per neighbour slot, [B, N, k, edge_dim] (forward's `neighbor_edges`)."""
         lib = nat.load()
         dev = _compute_device(feats)
@@ -420,7 +440,7 @@ class EGNN(nn.Module):
             kdt = torch.float32
         try:
             return self._run(lib, dev, kdt, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
-                             b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, train, param_fields, drop_p, box)
+                             b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, train, param_fields, drop_p, box, cell)
         except nat.EgnnNativeError as e:
             if e.code != nat.ERR_UNSUPPORTED or kdt != torch.bfloat16:
                 raise
@@ -431,10 +451,10 @@ class EGNN(nn.Module):
                       f"running the fp32 SIMT kernels instead (about 5x slower, same results to fp32 accuracy)", UserWarning,
                       stacklevel=3)
         return self._run(lib, dev, torch.float32, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
-                         b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, box=box)
+                         b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, box=box, cell=cell)
 
     def _run(self, lib, dev, kdt, feats, coors, edges, mask, adj_u8, labels, label_emb, b, n, c, k, flags,
-             cont_edge_dim, label_dim, rows, nbr=None, train=False, param_fields=None, drop_p=0.0, box=None):
+             cont_edge_dim, label_dim, rows, nbr=None, train=False, param_fields=None, drop_p=0.0, box=None, cell=None):
         cdt = torch.float64 if kdt == torch.float64 else torch.float32
         st = self._staged(dev, kdt)
         T = dict(st["tensors"])
@@ -501,6 +521,9 @@ class EGNN(nn.Module):
             bx = None if box is None else _as(box, dev, cdt).expand(b, c).contiguous()     # [B, C], like coors
             if train and bx is not None and bx.data_ptr() == box.data_ptr():
                 bx = bx.clone()                  # the backward must see the forward's box, whatever the caller does to it
+            cl = None if cell is None else _as(cell, dev, cdt).expand(b, c, c).contiguous()    # [B, C, C]
+            if train and cl is not None and cl.data_ptr() == cell.data_ptr():
+                cl = cl.clone()                  # (the same for the cell)
             m_in, l_in = _as_u8(mask, dev), _as_u8(labels, dev)
             f_out = torch.empty_like(f_in)
             x_out = torch.empty_like(x_in)
@@ -536,7 +559,11 @@ class EGNN(nn.Module):
             # training keeps the workspace (per-node tables, pooled messages, neighbour lists) for backward
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=dev) if train else _workspace(dev, ws_bytes, stream_handle)
             if train or rows is None or rows[0] != rows[1]:      # an empty row block computes nothing in inference
-                if bx is None:
+                if cl is not None:
+                    nat.check("egnn_layer_forward_triclinic",
+                              lib.egnn_layer_forward_triclinic(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io),
+                                                               _ptr(cl), _ptr(ws), ws.numel(), stream))
+                elif bx is None:
                     nat.check("egnn_layer_forward",
                               lib.egnn_layer_forward(C.byref(desc), C.byref(w), _ptr(packed), C.byref(io), _ptr(ws),
                                                      ws.numel(), stream))
@@ -550,7 +577,7 @@ class EGNN(nn.Module):
         if not train:
             return outs
         saved = dict(dev=dev, kdt=kdt, cdt=cdt, desc=desc, w=w, packed=packed, io=io, ws=ws, tensors=T,
-                     f_in=f_in, x_in=x_in, e_in=e_in, param_fields=param_fields, rows=rows, box=bx,
+                     f_in=f_in, x_in=x_in, e_in=e_in, param_fields=param_fields, rows=rows, box=bx, cell=cl,
                      keep=(m_in, l_in, adj_u8, nbr, lab_w, pre2))      # everything io points at stays alive
         return outs + (saved,)
 
@@ -576,6 +603,43 @@ def _check_box(box, b, c, cache):
     if bool(((box < 0) | torch.isnan(box)).any()):
         raise ValueError("box lengths must be >= 0 or +inf (0 or inf: the axis is not periodic), got negative or NaN values")
     cache["_box_checked"] = (weakref.ref(box), box._version)
+
+
+def _check_cell(cell, b, c, cache):
+    """Misuse of `cell=` raises ValueError here, before anything launches, with the caching and capture rules of
+    _check_box: the value checks read the cell on the host, except for the very tensor object this module checked last,
+    unchanged since, and while a CUDA graph is being captured."""
+    if not torch.is_tensor(cell) or not cell.is_floating_point():
+        raise ValueError(f"cell must be a float tensor of lattice vectors, got {type(cell).__name__}"
+                         f"{'' if not torch.is_tensor(cell) else ' ' + str(cell.dtype)}")
+    if c not in (2, 3):
+        raise ValueError(f"cell= needs C = 2 or 3 coordinates, got C={c}")
+    if tuple(cell.shape) not in ((c, c), (b, c, c)):
+        raise ValueError(f"cell must have shape (C, C) = ({c}, {c}) or (B, C, C) = ({b}, {c}, {c}), got {tuple(cell.shape)}")
+    if cell.requires_grad:
+        raise ValueError("cell.requires_grad is set, but the layer has no gradient with respect to the cell "
+                         "(stress / virial are not computed): pass cell.detach()")
+    last = cache.get("_cell_checked")
+    if last is not None and last[0]() is cell and last[1] == cell._version:
+        return
+    if cell.is_cuda and torch.cuda.is_current_stream_capturing():
+        return
+    m = cell.detach().to("cpu", torch.float64).reshape(-1, c, c)
+    diag = torch.diagonal(m, dim1=-2, dim2=-1)
+    off = m.masked_fill(torch.eye(c, dtype=torch.bool), 0.0)
+    if bool((torch.triu(m, diagonal=1) != 0).any()):
+        raise ValueError("cell must be lower-triangular (row k = lattice vector a_k, cell[k, d] == 0 for d > k); "
+                         "rotate a general cell into that form (README, periodic boundaries)")
+    if not bool(torch.isfinite(off).all()):
+        raise ValueError("cell off-diagonal entries must be finite, got NaN or inf")
+    if bool(((diag < 0) | torch.isnan(diag)).any()):
+        raise ValueError("cell diagonal entries must be >= 0 or +inf (0 or inf: the axis is not periodic), "
+                         "got negative or NaN values")
+    aper = (diag == 0) | torch.isinf(diag)                       # [G, C]
+    if bool(((off != 0) & (aper.unsqueeze(-1) | aper.unsqueeze(-2))).any()):
+        raise ValueError("an aperiodic axis of the cell (diagonal 0 or inf) must have a zero row and column off the "
+                         "diagonal")
+    cache["_cell_checked"] = (weakref.ref(cell), cell._version)
 
 
 def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
@@ -609,7 +673,7 @@ def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
 _RADIUS_BOX_CHECKED: dict = {}
 
 
-def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, return_counts=False):
+def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return_counts=False):
     """Radius graph of a point cloud: for every node the (at most) `k` nearest nodes within distance `cutoff`, as int32
     neighbour lists [B, N, k] for `EGNN.forward(..., neighbors=...)`, nearest first, ties to the lower index, -1 in the
     slots left empty.  A node counts as its own neighbour (distance 0).  Computed on a cell grid (`egnn_radius_select`)
@@ -620,7 +684,9 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, return_counts=Fal
     coordinates' type is compared with `float(cutoff) ** 2` cast to that type.  (The layer's `valid_radius`, as in the
     reference, is a *squared* distance.)  `k` in [1, min(32, N)].  `mask` [B, N] bool / 0-1: a padded node is never a
     neighbour and its own list is empty.  `box` [C] or [B, C]: periodic box lengths as `EGNN.forward(box=)` takes them
-    (minimum-image distances; 0 or inf: the axis is not periodic).  A node with a non-finite coordinate is never a
+    (minimum-image distances; 0 or inf: the axis is not periodic).  `cell` [C, C] or [B, C, C] (C in {2, 3}), instead
+    of `box`: a lower-triangular triclinic cell as `EGNN.forward(cell=)` takes it (distances of the wrapped pair
+    vector; periodic axes are binned in fractional coordinates).  A node with a non-finite coordinate is never a
     neighbour and its own list is empty.
 
     With `return_counts=True` it returns `(neighbors, counts)`: counts int32 [B, N] is the number of nodes within the
@@ -648,7 +714,11 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, return_counts=Fal
         raise ValueError(f"mask must be a [B, N] = [{b}, {n}] tensor, got "
                          f"{tuple(mask.shape) if torch.is_tensor(mask) else type(mask).__name__}")
     if box is not None:
+        if cell is not None:
+            raise ValueError("pass either box= or cell=, not both")
         _check_box(box, b, c, _RADIUS_BOX_CHECKED)
+    if cell is not None:
+        _check_cell(cell, b, c, _RADIUS_BOX_CHECKED)
     lib = nat.load()
     dev = _compute_device(coors)
     ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)
@@ -656,15 +726,21 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, return_counts=Fal
         x = _as(coors, dev, coors.dtype)
         m = _as_u8(mask, dev)
         bx = None if box is None else _as(box, dev, coors.dtype).expand(b, c).contiguous()
+        cl = None if cell is None else _as(cell, dev, coors.dtype).expand(b, c, c).contiguous()
         out = torch.empty((b, n, k), dtype=torch.int32, device=dev)
         counts = torch.empty((b, n), dtype=torch.int32, device=dev) if return_counts else None
         nb = C.c_size_t()
         nat.check("egnn_radius_select_workspace_bytes", lib.egnn_radius_select_workspace_bytes(b, n, c, k, C.byref(nb)))
         stream_handle = torch.cuda.current_stream(dev).cuda_stream
         ws = _workspace(dev, nb.value, stream_handle)
-        nat.check("egnn_radius_select", lib.egnn_radius_select(
-            _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(bx), r2, _ptr(out), _ptr(counts), _ptr(ws),
-            ws.numel(), C.c_void_p(stream_handle)))
+        if cl is not None:
+            nat.check("egnn_radius_select_triclinic", lib.egnn_radius_select_triclinic(
+                _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(cl), r2, _ptr(out), _ptr(counts),
+                _ptr(ws), ws.numel(), C.c_void_p(stream_handle)))
+        else:
+            nat.check("egnn_radius_select", lib.egnn_radius_select(
+                _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(bx), r2, _ptr(out), _ptr(counts),
+                _ptr(ws), ws.numel(), C.c_void_p(stream_handle)))
     if out.device != coors.device:
         out = out.to(coors.device)
         counts = None if counts is None else counts.to(coors.device)
@@ -830,10 +906,17 @@ class EGNN_Network(nn.Module):
                 EGNN(dim=dim, edge_dim=edge_dim + adj_dim, norm_feats=True, **kwargs),
             ]))
 
-    def forward(self, feats, coors, adj_mat=None, edges=None, mask=None, return_coor_changes=False, *, box=None):
-        """`box` (additive, keyword-only): periodic box lengths [C] or [B, C], passed to every layer (EGNN.forward)."""
+    def forward(self, feats, coors, adj_mat=None, edges=None, mask=None, return_coor_changes=False, *, box=None,
+                cell=None):
+        """`box` (additive, keyword-only): periodic box lengths [C] or [B, C], passed to every layer (EGNN.forward).
+        `cell` (additive, keyword-only, instead of `box`): a lower-triangular triclinic cell [C, C] or [B, C, C], passed
+        to every layer (EGNN.forward)."""
         if box is not None:
+            if cell is not None:
+                raise ValueError("pass either box= or cell=, not both")
             _check_box(box, feats.shape[0], coors.shape[-1], self.__dict__)
+        if cell is not None:
+            _check_cell(cell, feats.shape[0], coors.shape[-1], self.__dict__)
         lib = nat.load()
         out_dev = coors.device
         dev = _compute_device(coors)
@@ -916,7 +999,7 @@ class EGNN_Network(nn.Module):
             if exists(global_attn):
                 feats, global_tokens = global_attn(feats, global_tokens, mask=mask)
             feats, coors = egnn(feats, coors, edges, mask, adj_mat, _edge_labels=labels, _label_emb=label_emb,
-                                _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None, box=box)
+                                _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None, box=box, cell=cell)
             coor_changes.append(coors)
 
         if out_dev != dev:

@@ -188,6 +188,20 @@ int egnn_layer_forward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeight
                                 const EgnnLayerIO* io, const void* box, void* workspace, size_t workspace_bytes,
                                 void* stream);
 
+/* Triclinic cells: egnn_layer_forward_periodic with a lattice in place of the box.  `cell`: device [B, C, C], row-major,
+ * in the coordinates' type, C in {2, 3} (EGNN_ERR_SHAPE otherwise); row k is lattice vector a_k and the cell is lower-
+ * triangular (cell[k][d] == 0 for d > k).  A diagonal entry of 0 or +inf marks axis k aperiodic; its row and column
+ * must then be zero off the diagonal.  Every pair vector is wrapped sequentially from the last axis to the first: for
+ * c = C-1 .. 0 with L_c = cell[c][c] periodic, n = rint(r_c * (1/L_c)), then r_d -= cell[c][d] * n (one fma) for every
+ * d <= c.  After the wrap |r_c| <= L_c / 2 on every periodic axis: the result lies in the centred box of the diagonal
+ * entries, a fundamental domain of the lattice, so it is the minimum image whenever the minimum image is shorter than
+ * min_c L_c / 2; pairs farther apart get that centred-box image, one image per neighbour.  A diagonal cell gives the
+ * outputs of egnn_layer_forward_periodic with its diagonal as the box, bit for bit.  The values are not validated here.
+ * Workspace and packed sizes are those of egnn_layer_forward. */
+int egnn_layer_forward_triclinic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                 const EgnnLayerIO* io, const void* cell, void* workspace, size_t workspace_bytes,
+                                 void* stream);
+
 /* Same call with HOST buffers for io.* (pinned or pageable): allocates device staging,
  * copies in, runs, copies feats_out / coors_out back and synchronises.  Parameters (`w`,
  * `packed`) stay device-resident.  This is the end-to-end entry `bench.py` times as `e2e`. */
@@ -237,6 +251,10 @@ int egnn_layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, co
 int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
                                  const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
                                  const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
+/* Backward of egnn_layer_forward_triclinic: pass the SAME `cell` as the forward.  No gradient with respect to the cell. */
+int egnn_layer_backward_triclinic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                  const EgnnLayerIO* io, const void* cell, const void* fwd_workspace,
+                                  const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
 
 /* Neighbour selection alone == ranking + topk of egnn_pytorch.py:237-260: for every node the k
  * lowest-ranked nodes (rank = squared distance; 1e5 if either end is masked out; -1 self and 0
@@ -273,6 +291,12 @@ int egnn_radius_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t 
 int egnn_radius_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors, const uint8_t* mask,
                        const void* box, double r2, int32_t* out_idx, int32_t* out_count, void* workspace,
                        size_t workspace_bytes, void* stream);
+/* egnn_radius_select under a triclinic cell [B, C, C] (as egnn_layer_forward_triclinic takes it; C in {2, 3}, else
+ * EGNN_ERR_SHAPE): the ok = 1 slots of the all-pairs select with the rank of the wrapped pair vector.  Periodic axes
+ * are binned in fractional coordinates.  Same workspace. */
+int egnn_radius_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                                 const uint8_t* mask, const void* cell, double r2, int32_t* out_idx, int32_t* out_count,
+                                 void* workspace, size_t workspace_bytes, void* stream);
 
 /* N-th degree adjacency of EGNN_Network (egnn_pytorch.py:414-428) without the dense A@A:
  * adj_in [N,N] or [B,N,N] 0/1; writes the expanded adjacency adj_out [B,N,N] 0/1, the degree

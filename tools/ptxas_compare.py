@@ -5,20 +5,21 @@
 Each log holds the output of compiling every csrc/*.cu with the library's flags plus `-Xptxas -v`
 (`nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -std=c++17 -Xcompiler -fPIC -Xptxas -v -c ...`).  Every kernel
 entry becomes one line `demangled name | registers, barriers, stack, static shared memory | stack frame, spills`,
-sorted.  In the second log the trailing `PBC = false` template argument of the kernels that have one (the
-periodic-boundary switch, which the parent lacks) is dropped, so a kernel that existing calls run keeps its parent's
-name.  Prints a unified diff of the two listings: a line present in both is an instantiation whose registers, spills,
-stack and shared memory are unchanged."""
+sorted.  The trailing periodic-boundary template argument PBC of the kernels that have one is written as an int in
+both logs (it was a bool, false / true, before triclinic cells made it none / box / cell = 0 / 1 / 2), so a kernel
+that existing calls run keeps its name across that change.  Prints a unified diff of the two listings: a line present
+in both is an instantiation whose registers, spills, stack and shared memory are unchanged."""
 import difflib
 import re
 import subprocess
 import sys
 
 PBC_KERNELS = ("pair_kernel<", "pair_dense_tiled_kernel<", "pair_bwd1_kernel<", "pair_bwd3_kernel<",
-               "knn_warp_select_kernel<", "knn_block_sort_kernel<", "tc_knn_kernel<", "tc_pair_kernel<")
+               "knn_warp_select_kernel<", "knn_block_sort_kernel<", "tc_knn_kernel<", "tc_pair_kernel<",
+               "radius_count_kernel<", "radius_scatter_kernel<", "radius_query_kernel<")
 
 
-def entries(path, strip_pbc):
+def entries(path):
     out, cur, owner = [], None, None
     for line in open(path):
         m = re.search(r"Compiling entry function '(_Z\w+)'", line)
@@ -36,14 +37,14 @@ def entries(path, strip_pbc):
                            check=True).stdout.splitlines()
     lines = []
     for (_, regs, frame), name in zip(out, names):
-        if strip_pbc and any(k in name for k in PBC_KERNELS):
-            name = name.replace(", (bool)0>(", ">(", 1)
+        if any(k in name for k in PBC_KERNELS):
+            name = re.sub(r", \(bool\)([01])>\(", r", (int)\1>(", name, count=1)
         lines.append(f"{name} | {regs} | {frame}\n")
     return sorted(lines)
 
 
 def main():
-    a, b = entries(sys.argv[1], False), entries(sys.argv[2], True)
+    a, b = entries(sys.argv[1]), entries(sys.argv[2])
     sys.stdout.writelines(difflib.unified_diff(a, b, sys.argv[1], sys.argv[2], n=0))
     print(f"# {len(a)} kernel entries before ({len(set(a))} distinct), {len(b)} after ({len(set(b))} distinct); "
           f"{sum(1 for x in a if x not in set(b))} of the entries before are missing or changed after")
