@@ -127,6 +127,12 @@ SYMBOLS = {
                                                C.c_void_p, _P(LayerGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
     "egnn_layer_backward_triclinic": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
                                                 C.c_void_p, _P(LayerGrads), C.c_void_p, C.c_size_t, C.c_void_p]),
+    "egnn_layer_backward_periodic_lattice": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
+                                                       C.c_void_p, _P(LayerGrads), C.c_void_p, C.c_void_p, C.c_size_t,
+                                                       C.c_void_p]),
+    "egnn_layer_backward_triclinic_lattice": (C.c_int, [_P(LayerDesc), _P(LayerWeights), C.c_void_p, _P(LayerIO), C.c_void_p,
+                                                        C.c_void_p, _P(LayerGrads), C.c_void_p, C.c_void_p, C.c_size_t,
+                                                        C.c_void_p]),
     "egnn_knn_select": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_int32, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p]),
     "egnn_adj_neighbors": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p]),

@@ -209,6 +209,12 @@ __device__ __forceinline__ void box_axis(const T* box, int b, int C, int c, T& L
 template <typename T> __device__ __forceinline__ T min_image(T r, T L, T inv);
 template <> __device__ __forceinline__ float min_image<float>(float r, float L, float inv) { return fmaf(-L, rintf(r * inv), r); }
 template <> __device__ __forceinline__ double min_image<double>(double r, double L, double inv) { return fma(-L, rint(r * inv), r); }
+// min_image with the same operations, also returning the image count n = rint(rel / L) it subtracts (0 on an aperiodic
+// axis, where inv = 0), which the box gradient needs: rel = (x_i - x_j) - n L.
+template <typename T> __device__ __forceinline__ T min_image_n(T r, T L, T inv, T& n) {
+  n = rint(r * inv);
+  return fma_t<T>(-L, n, r);
+}
 
 // ------------------------------------------------------------------ periodic boundaries (triclinic cells)
 // The PBC template parameter of every kernel that forms x_i - x_j: no wrap, an orthorhombic box ([B,C] lengths), or a
@@ -231,15 +237,22 @@ __device__ __forceinline__ T cell_staged(const T* cell, int b, int C, int t) {
 }
 // The sequential wrap under a staged cell pc, from the last axis to the first: n = rint(r_c / L_c), then
 // r_d -= cell[c][d] n for every d <= c.  Afterwards |r_c| <= L_c / 2 on every periodic axis.  With a diagonal cell
-// the off-diagonal steps subtract exact zeros, so the result is min_image's bit for bit.
+// the off-diagonal steps subtract exact zeros, so the result is min_image's bit for bit.  cell_wrap_n also returns the
+// image counts n[c] (0 on an aperiodic axis): the wrapped vector is (x_i - x_j) - sum_c n[c] a_c, which the cell
+// gradient needs.
+template <typename T>
+__device__ __forceinline__ void cell_wrap_n(T& r0, T& r1, T& r2, T (&n)[3], const T* pc) {
+  n[2] = rint(r2 * pc[5]);
+  r0 = fma_t<T>(-pc[7], n[2], r0); r1 = fma_t<T>(-pc[8], n[2], r1); r2 = fma_t<T>(-pc[2], n[2], r2);
+  n[1] = rint(r1 * pc[4]);
+  r0 = fma_t<T>(-pc[6], n[1], r0); r1 = fma_t<T>(-pc[1], n[1], r1);
+  n[0] = rint(r0 * pc[3]);
+  r0 = fma_t<T>(-pc[0], n[0], r0);
+}
 template <typename T>
 __device__ __forceinline__ void cell_wrap(T& r0, T& r1, T& r2, const T* pc) {
-  const T n2 = rint(r2 * pc[5]);
-  r0 = fma_t<T>(-pc[7], n2, r0); r1 = fma_t<T>(-pc[8], n2, r1); r2 = fma_t<T>(-pc[2], n2, r2);
-  const T n1 = rint(r1 * pc[4]);
-  r0 = fma_t<T>(-pc[6], n1, r0); r1 = fma_t<T>(-pc[1], n1, r1);
-  const T n0 = rint(r0 * pc[3]);
-  r0 = fma_t<T>(-pc[0], n0, r0);
+  T n[3];
+  cell_wrap_n<T>(r0, r1, r2, n, pc);
 }
 
 // 4 consecutive elements, 4-element aligned.

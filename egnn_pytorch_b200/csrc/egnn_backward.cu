@@ -4,9 +4,9 @@
 namespace egnn {
 
 template int simt_backward<float>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, int, const void*,
-                                  const EgnnLayerGrads&, void*, size_t, cudaStream_t);
+                                  const EgnnLayerGrads&, double*, void*, size_t, cudaStream_t);
 extern template int simt_backward<double>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, int, const void*,
-                                          const EgnnLayerGrads&, void*, size_t, cudaStream_t);   // egnn_backward_f64.cu
+                                          const EgnnLayerGrads&, double*, void*, size_t, cudaStream_t);   // egnn_backward_f64.cu
 
 static int check_grad_ptrs(const EgnnLayerDesc& d, const EgnnLayerGrads* g) {
   if (!g || !g->g_feats_out || !g->g_coors_out || !g->g_feats || !g->g_coors) return EGNN_ERR_NULL;
@@ -34,10 +34,11 @@ extern "C" int egnn_layer_backward_workspace_bytes(const EgnnLayerDesc* desc, si
   return EGNN_OK;
 }
 
-// box: [B,C] lengths (pbc = PBC_BOX), a [B,C,C] lower-triangular cell (PBC_CELL), or null
+// box: [B,C] lengths (pbc = PBC_BOX), a [B,C,C] lower-triangular cell (PBC_CELL), or null.  g_lat: null, or the fp64
+// gradient with respect to the box / cell (same shape), overwritten.
 static int layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed, const EgnnLayerIO* io,
-                          const void* box, int pbc, const void* fwd_workspace, const EgnnLayerGrads* grads, void* workspace,
-                          size_t workspace_bytes, void* stream) {
+                          const void* box, int pbc, const void* fwd_workspace, const EgnnLayerGrads* grads, double* g_lat,
+                          void* workspace, size_t workspace_bytes, void* stream) {
   EGNN_TRY(validate_desc(desc));
   if (pbc == PBC_CELL && (desc->C < 2 || desc->C > 3)) return EGNN_ERR_SHAPE;
   EGNN_TRY(backward_supported(*desc));
@@ -51,14 +52,22 @@ static int layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, 
   if (((uintptr_t)workspace | (uintptr_t)fwd_workspace) & 0xFF) return EGNN_ERR_ALIGN;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   if (desc->dtype == EGNN_DTYPE_F64)
-    return simt_backward<double>(*desc, *w, packed, *io, box, pbc, fwd_workspace, *grads, workspace, workspace_bytes, st);
-  return simt_backward<float>(*desc, *w, packed, *io, box, pbc, fwd_workspace, *grads, workspace, workspace_bytes, st);
+    return simt_backward<double>(*desc, *w, packed, *io, box, pbc, fwd_workspace, *grads, g_lat, workspace, workspace_bytes, st);
+  return simt_backward<float>(*desc, *w, packed, *io, box, pbc, fwd_workspace, *grads, g_lat, workspace, workspace_bytes, st);
 }
 
 extern "C" int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
                                             const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
                                             const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream) {
-  return layer_backward(desc, w, packed, io, box, PBC_BOX, fwd_workspace, grads, workspace, workspace_bytes, stream);
+  return layer_backward(desc, w, packed, io, box, PBC_BOX, fwd_workspace, grads, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_layer_backward_periodic_lattice(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                                    const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
+                                                    const EgnnLayerGrads* grads, double* g_box, void* workspace,
+                                                    size_t workspace_bytes, void* stream) {
+  if (!box || !g_box) return EGNN_ERR_NULL;
+  return layer_backward(desc, w, packed, io, box, PBC_BOX, fwd_workspace, grads, g_box, workspace, workspace_bytes, stream);
 }
 
 extern "C" int egnn_layer_backward_triclinic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
@@ -66,7 +75,15 @@ extern "C" int egnn_layer_backward_triclinic(const EgnnLayerDesc* desc, const Eg
                                              const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes,
                                              void* stream) {
   if (!cell) return EGNN_ERR_NULL;
-  return layer_backward(desc, w, packed, io, cell, PBC_CELL, fwd_workspace, grads, workspace, workspace_bytes, stream);
+  return layer_backward(desc, w, packed, io, cell, PBC_CELL, fwd_workspace, grads, nullptr, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_layer_backward_triclinic_lattice(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                                     const EgnnLayerIO* io, const void* cell, const void* fwd_workspace,
+                                                     const EgnnLayerGrads* grads, double* g_cell, void* workspace,
+                                                     size_t workspace_bytes, void* stream) {
+  if (!cell || !g_cell) return EGNN_ERR_NULL;
+  return layer_backward(desc, w, packed, io, cell, PBC_CELL, fwd_workspace, grads, g_cell, workspace, workspace_bytes, stream);
 }
 
 extern "C" int egnn_layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,

@@ -3,5 +3,5 @@
 
 namespace egnn {
 template int simt_backward<double>(const EgnnLayerDesc&, const EgnnLayerWeights&, const void*, const EgnnLayerIO&, const void*, int, const void*,
-                                   const EgnnLayerGrads&, void*, size_t, cudaStream_t);
+                                   const EgnnLayerGrads&, double*, void*, size_t, cudaStream_t);
 }  // namespace egnn

@@ -143,7 +143,12 @@ static int launch_pair_bwd(const BwdArgs<T>& a, cudaStream_t st) {
     else bwd2 = drop ? pair_bwd2_dense_kernel<T, MP, 0, true, BLK> : pair_bwd2_dense_kernel<T, MP, 0, false, BLK>;
   }
   EGNN_TRY(launch_simt(bwd2, g2, BW2_TH, smem2, st, a));
-  pair_bwd3_kernel<T, KNN, BLK, PBC><<<g1, PAIR_THREADS, 0, st>>>(a);
+  bool lat = false;
+  if constexpr (PBC != PBC_NONE) {     // the lattice gradient: its own bwd3 instantiation, launched only when asked for
+    lat = a.g_lat != nullptr;
+    if (lat) pair_bwd3_kernel<T, KNN, BLK, PBC, true><<<g1, PAIR_THREADS, 0, st>>>(a);
+  }
+  if (!lat) pair_bwd3_kernel<T, KNN, BLK, PBC><<<g1, PAIR_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
   return EGNN_OK;
 }
@@ -161,10 +166,11 @@ static int launch_edge_bwd(const BwdArgs<T>& a, T* pre2, bool saved, bool part, 
   return MP == 16 ? launch_pair_bwd<T, 16, false, false, PBC>(a, st) : launch_pair_bwd<T, 32, false, false, PBC>(a, st);
 }
 
+// g_lat: null, or the fp64 lattice gradient ([B,C] for a box, [B,C,C] for a cell), overwritten.
 template <typename T>
 int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* packed, const EgnnLayerIO& io,
-                  const void* box, int pbc, const void* fwd_ws, const EgnnLayerGrads& gr, void* ws, size_t ws_bytes,
-                  cudaStream_t st) {
+                  const void* box, int pbc, const void* fwd_ws, const EgnnLayerGrads& gr, double* g_lat, void* ws,
+                  size_t ws_bytes, cudaStream_t st) {
   const Dims s = make_dims(d);
   const SimtPackLayout L = simt_pack_layout(s);
   const SimtWs fl = simt_ws_layout(s, sizeof(T), d.flags);
@@ -228,6 +234,7 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
   EGNN_TRY(zero(gr.w.coors_w2, (size_t)4 * m * es));
   EGNN_TRY(zero(gr.w.coors_b2, es));
   EGNN_TRY(zero(gr.w.label_emb, (size_t)s.num_labels * s.label_dim * es));
+  if (box) EGNN_TRY(zero(g_lat, (size_t)s.B * s.C * (pbc == PBC_CELL ? s.C : 1) * sizeof(double)));
   // neighbour lists: bwd3 adds dL/d edges into [B,N,N,e] with atomics, or stores them per slot ([B,N,k,e]) -- empty slots
   // are skipped, so they keep these zeros
   const size_t edge_rows = (d.flags & EGNN_FLAG_EDGES_PER_SLOT) ? (size_t)s.k : (size_t)s.N;
@@ -319,6 +326,7 @@ int simt_backward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void*
     a.TS = 32; a.TI2 = 32;
   }
   a.box = static_cast<const T*>(box);
+  a.g_lat = box ? g_lat : nullptr;
   if (box && pbc == PBC_CELL) EGNN_TRY((launch_edge_bwd<T, PBC_CELL>(a, pre2, saved, part, st)));
   else if (box) EGNN_TRY((launch_edge_bwd<T, PBC_BOX>(a, pre2, saved, part, st)));
   else EGNN_TRY((launch_edge_bwd<T, PBC_NONE>(a, pre2, saved, part, st)));

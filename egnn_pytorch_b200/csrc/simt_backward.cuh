@@ -69,6 +69,8 @@ struct BwdArgs {
   T* g_edges;                     // [B,N,N,edge_dim], [B,N,k,edge_dim] under EGNN_FLAG_EDGES_PER_SLOT, | null
   DropCfg drop;                   // the forward's dropout configuration (masks are regenerated, never stored)
   const T* box;                   // [B,C] the forward's periodic box lengths (PBC instantiations only)
+  double* g_lat;                  // dL/dbox [B,C] or dL/dcell [B,C,C] in fp64, zeroed by the caller (bwd3's LAT
+                                  // instantiations only; null otherwise)
 };
 
 template <typename T> __device__ __forceinline__ T dsilu_from(T x, T sg) { return sg * (T(1) + x * (T(1) - sg)); }
@@ -844,10 +846,20 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
 // =====================================================================================
 // bwd3: dL/d(dist) -> coordinates and edges.  Same thread <-> pair mapping as bwd1.  PBC: the minimum image has the
 // derivative of x_i - x_j (rint is piecewise constant), so only rel changes.
+// LAT (PBC instantiations only): also the lattice gradient.  rel = (x_i - x_j) - sum_c n_c a_c with integer image
+// counts n, so with gr = dL/d rel:  dL/dcell[c][d] = -sum_pairs n_c gr_d (d <= c),  dL/dbox[c] = -sum_pairs n_c gr_c.
+// Each thread sums its pairs in fp64 (either T); the sums are reduced over the warp, then over the CTA's warps in
+// shared memory, and the CTA (one graph, blockIdx.y) adds them to g_lat[b] with one atomicAdd per entry.
 // =====================================================================================
-template <typename T, bool KNN, bool BLK, int PBC = PBC_NONE>
+// Lattice entries a bwd3 thread accumulates: the lower triangle of a cell (00, 10, 11, 20, 21, 22) or every box axis.
+template <int PBC> __host__ __device__ constexpr int lat_entries() { return PBC == PBC_CELL ? 6 : PAIR_CMAX; }
+__host__ __device__ constexpr int lat_row(int e) { return e == 0 ? 0 : e < 3 ? 1 : 2; }
+__host__ __device__ constexpr int lat_col(int e) { return e == 0 ? 0 : e < 3 ? e - 1 : e - 3; }
+
+template <typename T, bool KNN, bool BLK, int PBC = PBC_NONE, bool LAT = false>
 __global__ void __launch_bounds__(PAIR_THREADS)
 pair_bwd3_kernel(const BwdArgs<T> a) {
+  static_assert(!LAT || PBC != PBC_NONE, "the lattice gradient needs a box or a cell");
   const Dims& s = a.s;
   const int tid = threadIdx.x;
   const int TS = a.TS, TI = PAIR_THREADS / TS;
@@ -873,14 +885,21 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
     gxi[c] = T(0);
   }
   const bool per_slot = KNN && (a.flags & EGNN_FLAG_EDGES_PER_SLOT);
+  constexpr int NL = LAT ? lat_entries<PBC>() : 1;
+  double lat[NL];
+#pragma unroll
+  for (int e = 0; e < NL; ++e) lat[e] = 0.0;
   for (int s0 = 0; s0 < J; s0 += TS) {
     const int sidx = s0 + sl;
     const PairSlot ps = pair_slot<KNN>(a.nbr_idx, nullptr, s.k, node_i, sidx, row_valid && sidx < J);
     if (!ps.valid) continue;
     const int j = ps.j;
     const T* r = a.rec + rec_index<KNN, BLK>(s, b, s.N, J, i, sidx) * a.rl.R;
-    T rel[PAIR_CMAX];
-    const T d = pair_geometry<T, PBC>(xi, a.coors + ((size_t)b * s.N + j) * s.C, s.C, rel, pb);
+    T rel[PAIR_CMAX], nimg[PAIR_CMAX];
+    const T* xj = a.coors + ((size_t)b * s.N + j) * s.C;
+    T d;
+    if constexpr (LAT) d = pair_geometry<T, PBC>(xi, xj, s.C, rel, nimg, pb);
+    else d = pair_geometry<T, PBC>(xi, xj, s.C, rel, pb);
     T gd = r[a.rl.gf + qd] + r[a.rl.gdn];
     for (int q = 0; q < s.F; ++q) {                        // fourier_encode_dist :34-41 reversed
       const T sc = T(1 << q);
@@ -896,12 +915,22 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
     if (j == i) continue;        // x_i - x_i: the two contributions cancel exactly (and would be 1/eps-sized under CoorsNorm)
     const T coef = r[a.rl.coef];
     T* gxj = a.g_coors + ((size_t)b * s.N + j) * s.C;
+    T grv[PAIR_CMAX];
 #pragma unroll
     for (int c = 0; c < PAIR_CMAX; ++c) {
+      if constexpr (LAT) grv[c] = T(0);
       if (c < s.C) {
         const T gr = fma_t(coef, gxo[c], T(2) * gd * rel[c]);
         gxi[c] += gr;
         atomic_add_t<T>(gxj + c, -gr);
+        if constexpr (LAT) grv[c] = gr;
+      }
+    }
+    if constexpr (LAT) {        // n is 0 on aperiodic axes and beyond C, and gr is 0 beyond C
+#pragma unroll
+      for (int e = 0; e < NL; ++e) {
+        const int rr = PBC == PBC_CELL ? lat_row(e) : e, cc = PBC == PBC_CELL ? lat_col(e) : e;
+        lat[e] = fma(-(double)nimg[rr], (double)grv[cc], lat[e]);
       }
     }
   }
@@ -913,6 +942,28 @@ pair_bwd3_kernel(const BwdArgs<T> a) {
 #pragma unroll
     for (int c = 0; c < PAIR_CMAX; ++c)
       if (c < s.C) atomic_add_t<T>(a.g_coors + node_i * s.C + c, gxi[c]);
+  }
+  if constexpr (LAT) {
+    __shared__ double lat_s[PAIR_THREADS / 32][NL];
+    const int lane = tid % 32, warp = tid / 32;
+#pragma unroll
+    for (int e = 0; e < NL; ++e) {
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) lat[e] += shfl_xor_t<double>(lat[e], off);
+      if (lane == 0) lat_s[warp][e] = lat[e];
+    }
+    __syncthreads();
+    if (tid < NL) {
+      double t = 0.0;
+#pragma unroll
+      for (int w = 0; w < PAIR_THREADS / 32; ++w) t += lat_s[w][tid];
+      if (PBC == PBC_CELL) {
+        const int rr = lat_row(tid), cc = lat_col(tid);
+        if (rr < s.C) atomicAdd(a.g_lat + ((size_t)b * s.C + rr) * s.C + cc, t);
+      } else if (tid < s.C) {
+        atomicAdd(a.g_lat + (size_t)b * s.C + tid, t);
+      }
+    }
   }
 }
 

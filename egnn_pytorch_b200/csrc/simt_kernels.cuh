@@ -328,7 +328,39 @@ __device__ __forceinline__ PairSlot pair_slot(const int32_t* nbr_idx, const uint
 }
 
 // rel = x_i - x_j (zero beyond C) and the squared distance d (egnn_pytorch.py:232-233).  PBC: rel is the minimum image
-// under the box `pb` staged by stage_box (PBC_BOX), or wrapped by the cell it staged (PBC_CELL, C <= 3).
+// under the box `pb` staged by stage_box (PBC_BOX), or wrapped by the cell it staged (PBC_CELL, C <= 3).  `n` receives
+// the image count of every axis, rel = (x_i - x_j) - sum_c n[c] a_c (0 without PBC, on aperiodic axes and beyond C).
+template <typename T, int PBC = PBC_NONE>
+__device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&rel)[PAIR_CMAX], T (&n)[PAIR_CMAX],
+                                           const T* pb) {
+  T d = T(0);
+#pragma unroll
+  for (int c = 0; c < PAIR_CMAX; ++c) n[c] = T(0);
+  if constexpr (PBC == PBC_CELL) {
+#pragma unroll
+    for (int c = 0; c < PAIR_CMAX; ++c) rel[c] = c < C ? xi[c] - xj[c] : T(0);
+    T n3[3];
+    cell_wrap_n<T>(rel[0], rel[1], rel[2], n3, pb);
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      n[c] = n3[c];
+      if (c < C) d = sq_acc<T>(rel[c], d);
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < PAIR_CMAX; ++c) {
+      rel[c] = T(0);
+      if (c < C) {
+        rel[c] = xi[c] - xj[c];
+        if constexpr (PBC) rel[c] = min_image_n<T>(rel[c], pb[c], pb[PAIR_CMAX + c], n[c]);
+        d = sq_acc<T>(rel[c], d);
+      }
+    }
+  }
+  return d;
+}
+// The same without the image counts.  Its own copy of the operations above: routed through them, the backward's kNN
+// box kernel in fp64 is register-allocated differently (profiles/ptxas_lattice_grad.diff).
 template <typename T, int PBC = PBC_NONE>
 __device__ __forceinline__ T pair_geometry(const T* xi, const T* xj, int C, T (&rel)[PAIR_CMAX], const T* pb = nullptr) {
   T d = T(0);

@@ -129,13 +129,16 @@ def _mlp(d_in, d_hidden, d_out, dropout, final_act=False):
 
 class _EGNNLayerFunction(torch.autograd.Function):
     """forward = egnn_layer_forward on a private workspace that is kept for backward;
-    backward = egnn_layer_backward (what autograd derives from reference egnn_pytorch.py:224-341)."""
+    backward = egnn_layer_backward (what autograd derives from reference egnn_pytorch.py:224-341).  `lattice`: the
+    caller's box or cell when its gradient was asked for (`lattice_grad=True`), else None; the backward then runs the
+    `_lattice` entry point when autograd needs that gradient."""
 
     @staticmethod
-    def forward(ctx, run, feats, coors, edges, label_emb, *params):
+    def forward(ctx, run, feats, coors, edges, label_emb, lattice, *params):
         f_out, x_out, saved = run()
         ctx.saved = saved
-        tensors = (feats, coors, edges, label_emb) + params
+        ctx.lattice_dim = None if lattice is None else lattice.dim()
+        tensors = (feats, coors, edges, label_emb, lattice) + params
         ctx.meta = [(t.dtype, t.device) if t is not None else None for t in tensors]
         # the saved state aliases the inputs and (same device / dtype) the live parameters: remember their versions so
         # that an in-place edit between forward and backward is reported instead of silently differentiated
@@ -168,7 +171,18 @@ class _EGNNLayerFunction(torch.autograd.Function):
             nat.check("egnn_layer_backward_workspace_bytes",
                       lib.egnn_layer_backward_workspace_bytes(C.byref(sv["desc"]), C.byref(nb)))
             ws = _workspace(dev, nb.value)
-            if sv["cell"] is not None:
+            g_lat = None
+            if ctx.needs_input_grad[5]:
+                # dL/dbox [B, C] or dL/dcell [B, C, C], accumulated by the library in float64
+                lat = sv["cell"] if sv["cell"] is not None else sv["box"]
+                fn = "egnn_layer_backward_triclinic_lattice" if sv["cell"] is not None else "egnn_layer_backward_periodic_lattice"
+                g_lat = torch.empty(lat.shape, dtype=torch.float64, device=dev)
+                nat.check(fn, getattr(lib, fn)(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]), C.byref(sv["io"]),
+                                               _ptr(lat), _ptr(sv["ws"]), C.byref(grads), _ptr(g_lat), _ptr(ws), ws.numel(),
+                                               stream))
+                if ctx.lattice_dim == lat.dim() - 1:
+                    g_lat = g_lat.sum(0)              # one lattice shared by the batch
+            elif sv["cell"] is not None:
                 nat.check("egnn_layer_backward_triclinic",
                           lib.egnn_layer_backward_triclinic(C.byref(sv["desc"]), C.byref(sv["w"]), _ptr(sv["packed"]),
                                                             C.byref(sv["io"]), _ptr(sv["cell"]), _ptr(sv["ws"]),
@@ -192,8 +206,8 @@ class _EGNNLayerFunction(torch.autograd.Function):
         ctx.saved = None
         back = lambda g, m: None if (g is None or m is None) else g.to(device=m[1], dtype=m[0])
         out = [None, back(g_feats, ctx.meta[0]), back(g_coors, ctx.meta[1]), back(g_edges, ctx.meta[2]),
-               back(gw.get("label_emb"), ctx.meta[3])]
-        for f, m in zip(sv["param_fields"], ctx.meta[4:]):
+               back(gw.get("label_emb"), ctx.meta[3]), back(g_lat, ctx.meta[4])]
+        for f, m in zip(sv["param_fields"], ctx.meta[5:]):
             out.append(back(gw.get(f), m))
         return tuple(g if need else None for g, need in zip(out, ctx.needs_input_grad))
 
@@ -307,7 +321,7 @@ class EGNN(nn.Module):
 
     # -------------------------------------------------------------- forward
     def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, neighbor_edges=None, box=None,
-                cell=None, _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
+                cell=None, lattice_grad=False, _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
         """Reference signature `forward(feats, coors, edges=None, mask=None, adj_mat=None)` (egnn_pytorch.py:224).
 
         `neighbors` (additive, keyword-only): int tensor [B, N, k] of neighbour indices, -1 = empty slot.  When
@@ -323,7 +337,7 @@ class EGNN(nn.Module):
         [B, C], on any device; every pair geometry x_i - x_j becomes its minimum image rel - L rint(rel / L) on the axes
         with a finite L > 0 (L = 0 or inf: not periodic).  Distances, neighbour ranking, CoorsNorm and the coordinate
         update follow; the output coordinates are not wrapped back into the box.  Orthorhombic boxes, one image per
-        neighbour, no gradient with respect to the box (a box that requires grad is rejected).
+        neighbour.  A box that requires grad is rejected unless `lattice_grad=True`.
 
         `cell` (additive, keyword-only, instead of `box`): periodic boundaries in a triclinic cell.  Float tensor [C, C]
         (shared by the batch) or [B, C, C], C in {2, 3}, row k = lattice vector a_k, lower-triangular (the LAMMPS
@@ -333,21 +347,24 @@ class EGNN(nn.Module):
         |r_c| <= L_c / 2 on every periodic axis: the result lies in the centred box of the diagonal entries, a
         fundamental domain of the lattice, so it is the minimum image whenever the minimum image is shorter than
         min_c L_c / 2; pairs farther apart get that centred-box image, one image per neighbour.  A diagonal cell gives
-        exactly the outputs of `box=` with the same lengths.  No gradient with respect to the cell."""
+        exactly the outputs of `box=` with the same lengths.  A cell that requires grad is rejected unless
+        `lattice_grad=True`.
+
+        `lattice_grad` (additive, keyword-only, needs `box` or `cell`): accept a box / cell that requires grad and give
+        it its gradient through autograd, for stress and virial (README).  The wrap is rel = (x_i - x_j) - sum_c n_c a_c
+        with integer image counts n, so dL/dcell[c, d] = -sum_pairs n_c dL/drel_d for d <= c (0 above the diagonal),
+        dL/dbox[c] = -sum_pairs n_c dL/drel_c, and 0 on aperiodic axes; neighbour selection contributes nothing.  A [C] /
+        [C, C] lattice gets the sum over the batch.  No effect under torch.no_grad()."""
         if neighbor_edges is not None:
             edges = self._check_neighbor_edges(feats, edges, neighbors, neighbor_edges, _label_emb)
-        if box is not None:
-            if cell is not None:
-                raise ValueError("pass either box= or cell=, not both")
-            _check_box(box, feats.shape[0], coors.shape[-1], self.__dict__)
-        if cell is not None:
-            _check_cell(cell, feats.shape[0], coors.shape[-1], self.__dict__)
+        lattice = _check_lattice(box, cell, feats.shape[0], coors.shape[-1], self.__dict__, lattice_grad)
         if torch.is_grad_enabled():             # (the parameter scan is skipped entirely under torch.no_grad())
             fields = self._state_fields()
             if (feats.requires_grad or coors.requires_grad or (edges is not None and edges.requires_grad) or
-                    (_label_emb is not None and _label_emb.requires_grad) or any(p.requires_grad for _, _, _, p in fields)):
+                    (_label_emb is not None and _label_emb.requires_grad) or any(p.requires_grad for _, _, _, p in fields) or
+                    (lattice is not None and lattice.requires_grad)):
                 return self._forward_train(fields, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb,
-                                           _k_hint, _rows, neighbor_edges is not None, box, cell)
+                                           _k_hint, _rows, neighbor_edges is not None, box, cell, lattice)
             with torch.no_grad():
                 return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint,
                                           _rows, slot_edges=neighbor_edges is not None, box=box, cell=cell)
@@ -370,7 +387,7 @@ class EGNN(nn.Module):
         return neighbor_edges
 
     def _forward_train(self, fields, feats, coors, edges, mask, adj_mat, neighbors, labels, label_emb, k_hint, rows,
-                       slot_edges=False, box=None, cell=None):
+                       slot_edges=False, box=None, cell=None, lattice=None):
         """With a row range (`_rows=(r0, r1)`) the layer is differentiated as the function it returns: rows r0:r1 are the
         layer's output, every other row is its input unchanged.  The library's backward then yields this block's share
         of every gradient (EGNN_FLAG_ROW_PARTIAL_GRADS): the blocks of a partition of the rows sum to the full gradient."""
@@ -381,7 +398,7 @@ class EGNN(nn.Module):
                                       train=True, param_fields=[f for _, _, f, _ in fields], slot_edges=slot_edges, box=box,
                                       cell=cell)
 
-        return _EGNNLayerFunction.apply(run, feats, coors, edges, label_emb, *params)
+        return _EGNNLayerFunction.apply(run, feats, coors, edges, label_emb, lattice, *params)
 
     def _forward_impl(self, feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
                       train=False, param_fields=None, slot_edges=False, box=None, cell=None):
@@ -582,7 +599,22 @@ class EGNN(nn.Module):
         return outs + (saved,)
 
 
-def _check_box(box, b, c, cache):
+def _check_lattice(box, cell, b, c, cache, lattice_grad):
+    """The checks of `box=` / `cell=` and `lattice_grad=` -> the box or cell whose gradient is asked for, else None."""
+    if box is not None:
+        if cell is not None:
+            raise ValueError("pass either box= or cell=, not both")
+        _check_box(box, b, c, cache, lattice_grad)
+    if cell is not None:
+        _check_cell(cell, b, c, cache, lattice_grad)
+    if not lattice_grad:
+        return None
+    if box is None and cell is None:
+        raise ValueError("lattice_grad=True needs box= or cell=: it asks for the gradient with respect to the lattice")
+    return box if box is not None else cell
+
+
+def _check_box(box, b, c, cache, lattice_grad=False):
     """Misuse of `box=` raises ValueError here, before anything launches.  The value check (no negative or NaN length)
     reads the box on the host.  It is skipped for the very tensor object this module checked last, unchanged since (the
     same object alive and the same version counter: an in-place write bumps it, a write through `.data` does not), and
@@ -592,9 +624,9 @@ def _check_box(box, b, c, cache):
                          f"{'' if not torch.is_tensor(box) else ' ' + str(box.dtype)}")
     if tuple(box.shape) not in ((c,), (b, c)):
         raise ValueError(f"box must have shape (C,) = ({c},) or (B, C) = ({b}, {c}), got {tuple(box.shape)}")
-    if box.requires_grad:
-        raise ValueError("box.requires_grad is set, but the layer has no gradient with respect to the box "
-                         "(stress / virial are not computed): pass box.detach()")
+    if box.requires_grad and not lattice_grad:
+        raise ValueError("box.requires_grad is set: pass lattice_grad=True for the gradient with respect to the box "
+                         "(stress / virial), or box.detach()")
     last = cache.get("_box_checked")
     if last is not None and last[0]() is box and last[1] == box._version:
         return
@@ -605,7 +637,7 @@ def _check_box(box, b, c, cache):
     cache["_box_checked"] = (weakref.ref(box), box._version)
 
 
-def _check_cell(cell, b, c, cache):
+def _check_cell(cell, b, c, cache, lattice_grad=False):
     """Misuse of `cell=` raises ValueError here, before anything launches, with the caching and capture rules of
     _check_box: the value checks read the cell on the host, except for the very tensor object this module checked last,
     unchanged since, and while a CUDA graph is being captured."""
@@ -616,9 +648,9 @@ def _check_cell(cell, b, c, cache):
         raise ValueError(f"cell= needs C = 2 or 3 coordinates, got C={c}")
     if tuple(cell.shape) not in ((c, c), (b, c, c)):
         raise ValueError(f"cell must have shape (C, C) = ({c}, {c}) or (B, C, C) = ({b}, {c}, {c}), got {tuple(cell.shape)}")
-    if cell.requires_grad:
-        raise ValueError("cell.requires_grad is set, but the layer has no gradient with respect to the cell "
-                         "(stress / virial are not computed): pass cell.detach()")
+    if cell.requires_grad and not lattice_grad:
+        raise ValueError("cell.requires_grad is set: pass lattice_grad=True for the gradient with respect to the cell "
+                         "(stress / virial), or cell.detach()")
     last = cache.get("_cell_checked")
     if last is not None and last[0]() is cell and last[1] == cell._version:
         return
@@ -907,16 +939,12 @@ class EGNN_Network(nn.Module):
             ]))
 
     def forward(self, feats, coors, adj_mat=None, edges=None, mask=None, return_coor_changes=False, *, box=None,
-                cell=None):
+                cell=None, lattice_grad=False):
         """`box` (additive, keyword-only): periodic box lengths [C] or [B, C], passed to every layer (EGNN.forward).
         `cell` (additive, keyword-only, instead of `box`): a lower-triangular triclinic cell [C, C] or [B, C, C], passed
-        to every layer (EGNN.forward)."""
-        if box is not None:
-            if cell is not None:
-                raise ValueError("pass either box= or cell=, not both")
-            _check_box(box, feats.shape[0], coors.shape[-1], self.__dict__)
-        if cell is not None:
-            _check_cell(cell, feats.shape[0], coors.shape[-1], self.__dict__)
+        to every layer (EGNN.forward).  `lattice_grad` (additive, keyword-only): passed to every layer, so a box / cell
+        that requires grad gets the sum of the layers' lattice gradients, through the chained coordinates too."""
+        _check_lattice(box, cell, feats.shape[0], coors.shape[-1], self.__dict__, lattice_grad)
         lib = nat.load()
         out_dev = coors.device
         dev = _compute_device(coors)
@@ -999,7 +1027,8 @@ class EGNN_Network(nn.Module):
             if exists(global_attn):
                 feats, global_tokens = global_attn(feats, global_tokens, mask=mask)
             feats, coors = egnn(feats, coors, edges, mask, adj_mat, _edge_labels=labels, _label_emb=label_emb,
-                                _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None, box=box, cell=cell)
+                                _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None, box=box, cell=cell,
+                                lattice_grad=lattice_grad)
             coor_changes.append(coors)
 
         if out_dev != dev:

@@ -247,14 +247,33 @@ int egnn_layer_backward(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, co
                         const EgnnLayerIO* io, const void* fwd_workspace, const EgnnLayerGrads* grads,
                         void* workspace, size_t workspace_bytes, void* stream);
 /* Backward of egnn_layer_forward_periodic: pass the SAME `box` as the forward (NULL = egnn_layer_backward).  The wrap's
- * derivative with respect to the coordinates is the identity; there is no gradient with respect to the box. */
+ * derivative with respect to the coordinates is the identity; egnn_layer_backward_periodic_lattice adds the gradient
+ * with respect to the box. */
 int egnn_layer_backward_periodic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
                                  const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
                                  const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
-/* Backward of egnn_layer_forward_triclinic: pass the SAME `cell` as the forward.  No gradient with respect to the cell. */
+/* Backward of egnn_layer_forward_triclinic: pass the SAME `cell` as the forward.  egnn_layer_backward_triclinic_lattice
+ * adds the gradient with respect to the cell. */
 int egnn_layer_backward_triclinic(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
                                   const EgnnLayerIO* io, const void* cell, const void* fwd_workspace,
                                   const EgnnLayerGrads* grads, void* workspace, size_t workspace_bytes, void* stream);
+/* Lattice gradients (stress / virial): egnn_layer_backward_periodic / _triclinic, returning every gradient they return,
+ * plus the gradient of the loss with respect to the box or the cell.  The wrap is rel = (x_i - x_j) - sum_c n_c a_c with
+ * integer image counts n (piecewise constant), so with gr = dL/d rel of a pair
+ *   g_box  [B, C]    (float64): g_box[b][c]     = - sum_pairs n_c gr_c;
+ *   g_cell [B, C, C] (float64): g_cell[b][c][d] = - sum_pairs n_c gr_d for d <= c, 0 above the diagonal;
+ * 0 on aperiodic axes and rows.  Neighbour selection contributes nothing.  The buffer is overwritten (zeroed on the
+ * stream) and accumulated in float64 whatever the layer's type, with atomics: reproducible to fp64 rounding.  A row
+ * block (EGNN_FLAG_ROW_PARTIAL_GRADS) returns its share, so the shares of a partition of the rows sum to the whole.
+ * A NULL box / cell or gradient: EGNN_ERR_NULL; C outside {2, 3} for a cell: EGNN_ERR_SHAPE.  Same workspace. */
+int egnn_layer_backward_periodic_lattice(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                         const EgnnLayerIO* io, const void* box, const void* fwd_workspace,
+                                         const EgnnLayerGrads* grads, double* g_box, void* workspace,
+                                         size_t workspace_bytes, void* stream);
+int egnn_layer_backward_triclinic_lattice(const EgnnLayerDesc* desc, const EgnnLayerWeights* w, const void* packed,
+                                          const EgnnLayerIO* io, const void* cell, const void* fwd_workspace,
+                                          const EgnnLayerGrads* grads, double* g_cell, void* workspace,
+                                          size_t workspace_bytes, void* stream);
 
 /* Neighbour selection alone == ranking + topk of egnn_pytorch.py:237-260: for every node the k
  * lowest-ranked nodes (rank = squared distance; 1e5 if either end is masked out; -1 self and 0
