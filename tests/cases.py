@@ -143,7 +143,7 @@ def gen_inputs(spec, rs):
     else:
         cfg = spec["_cfg"]
         ins["feats"] = rs.standard_normal((B, N, cfg["dim"]))
-        if cfg["edge_dim"] > 0:
+        if cfg["edge_dim"] > 0 and spec.get("dense_edges", True):     # (False: the caller supplies per-slot edges)
             ins["edges"] = rs.standard_normal((B, N, N, cfg["edge_dim"]))
     ins["coors"] = rs.standard_normal((B, N, C)) * spec.get("coor_scale", 1.0)
     mk = spec.get("mask", "none")

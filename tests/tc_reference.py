@@ -14,11 +14,18 @@ where the bf16 path rounds:
   LN(h) | m_i, h1           bf16 on the GEMM node path (dim > 64); the small-node kernels (dim <= 64) keep LN(h) and
                             the hidden layer in fp32 -- `node_fp32`
   output (after residual)   bf16
+  periodic pair vector      fp32, op for op (`box=` / `cell=`, below)
 
 s_q are the per-pair scalar channels in the kernels' order: the squared distance, sin / cos of the fourier features,
 the continuous edge channels, and the one-hot degree labels (whose weights are the label embedding folded through the
 label columns of W1, computed in fp32).  The reference uses exact tanh and fp64 arithmetic elsewhere; what remains
 between it and a correct kernel is tanh.approx in the SiLUs, fp32 arithmetic, and bf16 rounding-boundary flips.
+
+Under a periodic box or triclinic cell the pair vector is formed and wrapped with the kernels' fp32 operations
+(common.cuh: box_axis / min_image, cell_staged / cell_wrap_n), so the image of every pair is the kernels' bit for bit:
+r = fp32(x_i - x_j); per periodic axis inv = fp32(1 / L), n = rint(fp32(r * inv)) (half to even) and r = fma(-L, n, r),
+a cell from its last axis to its first.  The fma is fp32(float64(-L) * n + float64(r)): L n has at most about 28
+significant bits and r 24, so the float64 sum is exact and only the final rounding to fp32 remains.
 
 With `rounding=False` nothing is rounded, and the functions equal oracle.egnn_layer_forward /
 egnn_layer_forward_edge_list / egnn_network_forward to fp64 accuracy (test_gpu_tc_boundaries pins that)."""
@@ -45,6 +52,56 @@ def fp32(x, on=True):
     return x.float().double() if on else x
 
 
+def _rint(x):
+    """Round half to even, as rintf / rint."""
+    return torch.round(x)
+
+
+def _staged_axes(diag, rounding):
+    """(L, 1/L) of each axis as the kernels stage them: both 0 on an axis that is not periodic (0 or inf)."""
+    per = (diag > 0) & torch.isfinite(diag)
+    L = torch.where(per, diag, torch.zeros_like(diag))
+    one = torch.where(per, diag, torch.ones_like(diag))
+    inv = (1.0 / one.float()).double() if rounding else 1.0 / one      # fp32 division, correctly rounded
+    return L, torch.where(per, inv, torch.zeros_like(inv))
+
+
+def _fma(a, b, c, rounding):
+    """fmaf(a, b, c) for fp32 values a * b (<= 2^29) and c: the float64 sum is exact, one rounding to fp32."""
+    return fp32(a * b + c, rounding)
+
+
+def wrap_box(r, box, rounding=True):
+    """min_image of r [..., C] under box lengths [C] (0 or inf: the axis is not periodic)."""
+    L, inv = _staged_axes(fp32(_t(box), rounding), rounding)
+    return _fma(-L, _rint(fp32(r * inv, rounding)), r, rounding)
+
+
+def wrap_cell(r, cell, rounding=True, first_to_last=False):
+    """cell_wrap of r [..., C] under a lower-triangular cell [C, C] (rows: lattice vectors; a diagonal entry of 0 or inf
+    leaves that axis aperiodic): from the last axis to the first, n = rint(r_c / L_c), r_d -= cell[c, d] n for d <= c.
+    `first_to_last` runs the axes the wrong way round (a mistake the tests must see)."""
+    A = fp32(_t(cell), rounding)
+    C = A.shape[-1]
+    L, inv = _staged_axes(torch.diagonal(A), rounding)
+    r = list(r.unbind(-1))
+    for c in (range(C) if first_to_last else reversed(range(C))):
+        n = _rint(fp32(r[c] * inv[c], rounding))
+        for d in range(c + 1):
+            r[d] = _fma(-(L[c] if d == c else A[c, d]), n, r[d], rounding)
+    return torch.stack(r, -1)
+
+
+def lattice_bc(box, cell, b, c):
+    """The per-graph lattice: ('box', [B, C]) / ('cell', [B, C, C]) from [C] / [B, C] and [C, C] / [B, C, C], or None."""
+    assert box is None or cell is None, "a box or a cell, not both"
+    if box is not None:
+        return "box", _t(box).expand(b, c)
+    if cell is not None:
+        return "cell", _t(cell).expand(b, c, c)
+    return None
+
+
 def _silu(x):
     return x * torch.sigmoid(x)
 
@@ -56,7 +113,8 @@ def _layer_norm(x, g, b, eps=1e-5):
 
 
 def tc_layer_forward(params, cfg, feats, coors, edges=None, mask=None, neighbors=None, nbr_ok=None, slot_edges=False,
-                     labels=None, label_emb=None, rows=None, rounding=True, node_fp32=None, messages=True):
+                     labels=None, label_emb=None, rows=None, rounding=True, node_fp32=None, messages=True, box=None,
+                     cell=None):
     """One layer as the bf16 path computes it.
 
     feats [B,N,dim], coors [B,N,C]; edges: continuous edge channels [B,N,N,e], or [B,N,k,e] per neighbour slot with
@@ -66,7 +124,8 @@ def tc_layer_forward(params, cfg, feats, coors, edges=None, mask=None, neighbors
     layer's cfg edge_dim counts the continuous channels plus label_dim).  `rows=(r0, r1)` evaluates rows r0:r1 only
     and returns those rows.  `node_fp32` (default: dim <= 64, the small-node kernels) keeps LN(h) and the node MLP's
     hidden layer in fp32.  `messages=False` feeds m_i = 0 to the node MLP (how much of the output the edge step
-    decides)."""
+    decides).  `box` ([C] or [B, C]) or `cell` ([C, C] or [B, C, C]) wraps x_i - x_j before the distance, the fourier
+    features and the coordinate update use it (fp32 op for op with `rounding`, float64 without)."""
     rd = rounding
     P = {k: _t(v) for k, v in params.items()}
     h = _t(feats)
@@ -96,6 +155,7 @@ def tc_layer_forward(params, cfg, feats, coors, edges=None, mask=None, neighbors
     ok = None if nbr_ok is None else torch.as_tensor(np.asarray(nbr_ok).astype(bool))
     nlab = 0 if label_emb is None else np.shape(label_emb)[0]
     r0, r1 = (0, n) if rows is None else rows
+    lat = lattice_bc(box, cell, b_, x.shape[-1])
     R = r1 - r0
     J = n if nb is None else nb.shape[-1]
     feats_out = h[:, r0:r1].clone()
@@ -114,6 +174,9 @@ def tc_layer_forward(params, cfg, feats, coors, edges=None, mask=None, neighbors
                 sv = jj >= 0
                 jj = torch.where(sv, jj, ii[:, None])                           # an empty slot reads the node itself
             rel = x[b, s:e, None, :] - x[b][jj]                                   # [R,J,C]  x_i - x_j
+            if lat is not None:
+                rel = fp32(rel, rd)
+                rel = (wrap_box if lat[0] == "box" else wrap_cell)(rel, lat[1][b], rd)
             d = fp32((rel ** 2).sum(-1), rd)
             sc = [d]
             if F > 0:
@@ -169,10 +232,12 @@ def tc_layer_forward(params, cfg, feats, coors, edges=None, mask=None, neighbors
     return feats_out.numpy(), coors_out.numpy()
 
 
-def tc_network_forward(params, ncfg, feats, coors, adj_mat=None, edges=None, mask=None, rounding=True):
+def tc_network_forward(params, ncfg, feats, coors, adj_mat=None, edges=None, mask=None, rounding=True, box=None,
+                       cell=None):
     """EGNN_Network as the bf16 path computes it: token (+ position) embedding rounded to bf16, edge tokens embedded,
     degree labels from the expanded adjacency handed to every layer as labels with the adjacency embedding as their
-    table, layers chained on bf16 features and fp32 coordinates.  Global attention blocks are not modelled."""
+    table, layers chained on bf16 features and fp32 coordinates, `box` / `cell` passed to every layer.  Global
+    attention blocks are not modelled, nor a neighbour selection under a lattice."""
     assert not ncfg.get("global_layers"), "global attention blocks are not part of this reference"
     P = {k: np.asarray(v, np.float64) for k, v in params.items()}
     b = np.shape(feats)[0]
@@ -197,7 +262,8 @@ def tc_network_forward(params, ncfg, feats, coors, adj_mat=None, edges=None, mas
         lp = {k[len(pre):]: v for k, v in P.items() if k.startswith(pre)}
         nbr = ok = None
         if cfg["num_nearest_neighbors"] > 0 or cfg["only_sparse_neighbors"]:
+            assert box is None and cell is None, "the oracle's neighbour selection has no lattice"
             nbr, ok, _ = O.neighbour_selection(cfg, x, None if mask is None else np.asarray(mask).astype(bool), adj)
         h, x = tc_layer_forward(lp, cfg, h, x, edges=edges, mask=mask, neighbors=nbr, nbr_ok=ok, labels=labels,
-                                label_emb=label_emb, rounding=rounding)
+                                label_emb=label_emb, rounding=rounding, box=box, cell=cell)
     return h, x

@@ -17,6 +17,16 @@ mirrored in `geometry` and held there by test_table_covers_every_boundary:
   tc_knn    k = 1 / 8 / 31 / 32; the lean, edges and generic instantiations at 8 and 16 rows per CTA, each with a
             partial last CTA; caller lists with -1 slots (mean without a mask too); per-slot edges; row ranges
   node path small-node kernels (dim <= 64, B*N <= 4096), tc_gemm tables at dim <= 64 with B*N > 4096, dim > 64
+  lattices  the PBC_BOX and PBC_CELL instantiations of both kernels (cases "pb_" / "pc_" / "kb_" / "kc_"): the tc_pair
+            and tc_knn boundaries above under a box and under a cell (k = 1 under a cell); ring slots refilled with
+            a row group of another graph whose lattice differs (j-split 1 and 2, odd laps), the only route through
+            the per-slot lattice staging; generic C = 5 / 8 boxes with aperiodic axes; 2-D, hexagonal-slab and 0.9-tilt cells;
+            the c2 shape with a box and a cell, and c4 (B=8, N=4096, k=32, per-slot edges) with a box per graph
+The lattice cases place nodes so that most compared pairs wrap (>= 20 %) and every wrap decision lies >= 1e-3 from
+1/2, so the reference's fp32 wrap and the fp64 restatement pick the kernels' images; the CPU tests pin that fp32 wrap
+to an exact rational evaluation and, unrounded, to torch_reference / test_triclinic's float64 restatements, and check
+that each lattice case fails a gate when the reference is given a wrong lattice (none, the next graph's, a cell's
+diagonal, the axes wrapped first to last, floor for rint).  A diagonal cell gives the box's outputs bit for bit.
 Every case uses xavier weights, so that the coordinate update is O(1) and the messages move the features
 (test_every_case_sees_the_edge_kernel checks that on the reference).
 
@@ -25,9 +35,11 @@ each tolerance is 2.6x - 4x that, `TOL`):
   feats   max and mean |error| in bf16 ulps of the reference value (ulps below 1 % of the tensor's scale are
           counted at that floor)
   coors   per row: max |error| over the row / that row's update; over all rows: RMS error / RMS update
-plus the gate of test_gpu_fast.py against the fp64 oracle.  Large cases compare row windows (`check`) that include
-the first and last rows of every graph and of the range."""
+plus the gate of test_gpu_fast.py against the fp64 oracle (under a lattice: the float64 periodic restatement).  Large
+cases compare row windows (`check`) that include the first and last rows of every graph and of the range."""
+import contextlib
 import functools
+from fractions import Fraction
 
 import numpy as np
 import pytest
@@ -35,6 +47,9 @@ import torch
 
 import cases
 import tc_reference as T
+import test_periodic as PER
+import test_triclinic as TRI
+import torch_reference as R
 import util
 from oracle import egnn_oracle as O
 
@@ -126,6 +141,101 @@ CASES = {
                             check=[(0, 16), (2500, 2516), (4990, 5000)]),
 }
 
+# ---------------- periodic boxes (`box`, key "pb_" / "kb_") and triclinic cells (`cell`, key "pc_" / "kc_")
+# box: [C] lengths (0 / inf: aperiodic) or "per_graph" (one box per graph); cell: a kind of `lattice_inputs`.  Every
+# lattice is smaller than the coordinate spread (nodes are moved by whole lattice vectors), so most pairs wrap.
+BOX3, INF = [3.0, 3.25, 3.5], float("inf")
+LATTICE_SHAPES = [
+    # (name, spec, box, cell)
+    # ring reuse with odd laps, where a CTA's consecutive items lie in graphs with different lattices: j-split 1
+    # (875 items) and j-split 2 (800 items)
+    ("js1_ring", dict(kind=L, cfg=dict(dim=16), B=5, N=700, seed=601, mask="padded",
+                      check=[(0, 8), (172, 180), (344, 352), (690, 700)]), "per_graph", "per_graph"),
+    ("js2_ring", dict(kind=L, cfg=dict(dim=24, fourier_features=1, soft_edges=True), B=2, N=800, seed=602,
+                      mask="random",
+                      check=[(0, 8), (396, 404), (792, 800)]), "per_graph", "per_graph"),
+    # j-split 4 over a whole graph (generic: fourier + edges), on a row range ending with 3 valid rows; j-split 8 on a
+    # row range ending with 1 valid row (lean)
+    ("js4_full", dict(kind=L, cfg=dict(dim=16, fourier_features=2, edge_dim=4), B=1, N=1100, seed=603,
+                      check=[(0, 8), (548, 556), (1092, 1100)]), BOX3, "tilt"),
+    ("js4_range", dict(kind=L, cfg=dict(dim=24, fourier_features=2, edge_dim=4, norm_coors=True), B=2, N=1024,
+                       seed=604, rows=(0, 63), mask="padded"), "per_graph", "per_graph"),
+    ("js8_range", dict(kind=L, cfg=dict(dim=16, coor_weights_clamp_value=2.0), B=1, N=2048, seed=605, rows=(5, 34)),
+     BOX3, "tilt"),
+    # one active warpgroup, one fully masked graph
+    ("n100_empty", dict(kind=L, cfg=dict(dim=64, m_pool_method="mean"), B=3, N=100, seed=606, mask="one_empty"),
+     "per_graph", "per_graph"),
+    # partial / full / one-more warp and warpgroup tiles
+    ("n63", dict(kind=L, cfg=dict(dim=32, coor_weights_clamp_value=0.5), B=2, N=63, seed=607, mask="random"),
+     "per_graph", "per_graph"),
+    ("n64", dict(kind=L, cfg=dict(dim=32, m_pool_method="mean"), B=2, N=64, seed=608, mask="padded"), BOX3, "tilt"),
+    ("n65", dict(kind=L, cfg=dict(dim=24, soft_edges=True), B=2, N=65, seed=609), "per_graph", "per_graph"),
+    ("n127", dict(kind=L, cfg=dict(dim=32, norm_coors=True), B=2, N=127, seed=610), BOX3, "tilt"),
+    ("n128", dict(kind=L, cfg=dict(dim=32, soft_edges=True), B=2, N=128, seed=611, mask="random"), "per_graph",
+     "per_graph"),
+    ("n129", dict(kind=L, cfg=dict(dim=24, coor_weights_clamp_value=1.0), B=2, N=129, seed=612), BOX3, "tilt"),
+    ("n255", dict(kind=L, cfg=dict(dim=40, m_pool_method="mean"), B=2, N=255, seed=613), "per_graph", "per_graph"),
+    ("n256", dict(kind=L, cfg=dict(dim=16, soft_edges=True, coor_weights_clamp_value=2.0), B=2, N=256, seed=614,
+                  mask="padded"), BOX3, "tilt"),
+    ("n257", dict(kind=L, cfg=dict(dim=16, norm_coors=True), B=2, N=257, seed=615, mask="random"), "per_graph",
+     "per_graph"),
+    # the widest lean layer (Hp = 2736)
+    ("d680", dict(kind=L, cfg=dict(dim=680), B=1, N=70, seed=616, mask="padded"), BOX3, "tilt"),
+    # generic: fourier features, edges and degree labels (Q = 12) through EGNN_Network
+    ("net_q12", dict(kind=NW, cfg=dict(depth=1, dim=16, fourier_features=2, edge_dim=3, num_adj_degrees=3, adj_dim=2,
+                                       soft_edges=True), B=2, N=150, seed=617, adj="chain", edges=True, mask="padded"),
+     "per_graph", "per_graph"),
+    # neighbour lists: k = 1 / 8 / 31 / 32, lean / edges / generic at 8 and 16 rows per CTA, partial last CTAs
+    ("k8_edges8_slot", dict(kind=L, cfg=dict(dim=64, edge_dim=4), B=2, N=150, k=8, seed=622, holes=True,
+                            slot_edges=True, mask="padded"), "per_graph", "per_graph"),
+    ("k31_gen8_mean", dict(kind=L, cfg=dict(dim=32, fourier_features=2, m_pool_method="mean"), B=2, N=100, k=31,
+                           seed=623, holes=True), BOX3, "tilt"),
+    ("k32_lean16", dict(kind=L, cfg=dict(dim=344, coor_weights_clamp_value=3.0), B=1, N=150, k=32, seed=624,
+                        holes=True), BOX3, "tilt"),
+    ("k32_edges16", dict(kind=L, cfg=dict(dim=280, edge_dim=4), B=2, N=100, k=32, seed=625, holes=True,
+                         mask="random"), "per_graph", "per_graph"),
+    ("k31_gen16_rows", dict(kind=L, cfg=dict(dim=264, fourier_features=2, edge_dim=1, m_pool_method="mean"), B=2,
+                            N=150, k=31, seed=628, holes=True, slot_edges=True, mask="padded", rows=(19, 140)),
+     "per_graph", "per_graph"),
+    # the BASELINE shapes as the lattice benches time them: c2 (dense dim 512, B=4, N=1024) with a box and with a
+    # tilted cell
+    ("c2", dict(kind=L, cfg=dict(dim=512), B=4, N=1024, seed=631, check=[(0, 8), (508, 516), (1016, 1024)]),
+     [4.0, 4.0, 4.0], "tilt"),
+]
+LATTICE_CASES = {}
+for _n, _s, _box, _cell in LATTICE_SHAPES:
+    _k = "k" if _s.get("k") else "p"
+    LATTICE_CASES[f"{_k}b_{_n}"] = dict(_s, box=_box)
+    LATTICE_CASES[f"{_k}c_{_n}"] = dict(_s, cell=_cell, seed=_s["seed"] + 100)
+LATTICE_CASES.update({
+    # the lean 8-row list kernel: k = 1 under a cell, k = 8 under a box (at k = 1 the per-row coordinate gate compares
+    # the error of one coordinate weight with its value; DESIGN section 5 gives what that measured under a box)
+    "kc_k1_lean8":     dict(kind=L, cfg=dict(dim=32), B=2, N=203, k=1, seed=734, cell="per_graph"),
+    "kb_k8_lean8":     dict(kind=L, cfg=dict(dim=32), B=2, N=203, k=8, seed=635, holes=True, box="per_graph"),
+    # box only: the generic instantiation at C = 5 and C = 8 with aperiodic (0, inf) and periodic axes
+    "pb_c5_mixed":     dict(kind=L, cfg=dict(dim=16, edge_dim=2, soft_edges=True), B=2, N=90, C=5, seed=641,
+                            mask="random", box=[3.0, INF, 2.5, 0.0, 3.5]),
+    "pb_c8_mixed":     dict(kind=L, cfg=dict(dim=32, fourier_features=1, m_pool_method="mean"), B=2, N=100, C=8,
+                            seed=642, box=[3.0, 0.0, 2.75, INF, 3.25, 3.0, 0.0, 3.5]),
+    "pb_net_q12_c8":   dict(kind=NW, cfg=dict(depth=1, dim=16, fourier_features=2, edge_dim=3, num_adj_degrees=3,
+                                              adj_dim=2), B=2, N=120, C=8, seed=643, adj="chain", edges=True,
+                            box=[2.5, INF, 3.0, 0.0, 3.5, 2.75, INF, 3.25]),
+    # j-split 8 on a row range, generic (for the diagonal-cell identity)
+    "pb_js8_range_gen": dict(kind=L, cfg=dict(dim=16, fourier_features=1), B=1, N=2048, seed=644, rows=(5, 34),
+                             box=BOX3),
+    # cell only: a 2-D cell (generic), a hexagonal slab, a tilt of 0.9
+    "pc_c2_gen":       dict(kind=L, cfg=dict(dim=16, m_pool_method="mean"), B=2, N=300, C=2, seed=651, mask="padded",
+                            cell="c2"),
+    "pc_hex_slab":     dict(kind=L, cfg=dict(dim=32, soft_edges=True), B=2, N=60, seed=652, cell="hex_slab"),
+    "pc_tilt09":       dict(kind=L, cfg=dict(dim=32, norm_coors=True), B=2, N=300, seed=653, mask="random",
+                            cell="tilt09"),
+    "kc_c2_gen8":      dict(kind=L, cfg=dict(dim=32), B=2, N=90, C=2, k=8, seed=654, holes=True, cell="c2"),
+    # c4 (dim 256, edge_dim 4, B=8, N=4096) on caller lists of 32 with per-slot edges and a box per graph
+    "kb_c4":           dict(kind=L, cfg=dict(dim=256, edge_dim=4), B=8, N=4096, k=32, seed=661, slot_edges=True,
+                            box="per_graph", check=[(0, 16), (2040, 2056), (4080, 4096)]),
+})
+CASES.update(LATTICE_CASES)
+
 # ------------------------------------------------------------------ launch geometry (mirrors the launch code)
 
 H100_SMS = 132
@@ -183,7 +293,9 @@ def geometry(spec, sms=H100_SMS):
     g = dict(dim=dim, B=B, N=N, C=C, k=k, R=R, Hp=Hp, Q=QT, F=F, edge_dim=ed, labels=nlab,
              nsl_last=(Hp - (nchunks - 1) * TP_KC) // 16, rows_range=spec.get("rows") is not None,
              tables="small" if dim <= SN_DIM_MAX and M <= SN_TABLES_M_MAX else "tc_gemm",
-             node="small" if dim <= SN_DIM_MAX else "tc_gemm")
+             node="small" if dim <= SN_DIM_MAX else "tc_gemm", lattice=lattice_kind(spec),
+             per_graph_lattice=isinstance(spec.get("box", spec.get("cell")), str)
+             and spec.get("box", spec.get("cell")) == "per_graph" and B > 1)
     if k == 0:
         gen = not (C == 3 and QT == 1)
         items = B * _ceil(R, TP_TI)
@@ -193,7 +305,13 @@ def geometry(spec, sms=H100_SMS):
             js *= 2
         n_items = items * js
         grid = min(n_items, sms)
+        # a ring slot refilled with a row group of another graph (tc_pair.cuh: the last warpgroup stages item
+        # x + 2 grid into the slot of item x)
+        rg = _ceil(R, TP_TI)
+        graph = lambda item: item // js // rg
+        refill_other_graph = any(graph(x) != graph(x + 2 * grid) for x in range(n_items - 2 * grid))
         g.update(kernel="tc_pair<generic>" if gen else "tc_pair<lean>", jsplit=js, items=n_items, grid=grid,
+                 refill_other_graph=refill_other_graph,
                  laps=_ceil(n_items, grid), active_wgs=min(2, _ceil(N, 128)),
                  last_rows_valid=R - TP_TI * (_ceil(R, TP_TI) - 1),
                  supported=QT <= TP_QMAX and C <= TP_CMAX and _pair_smem(Hp, QT, 1 + 2 * F, gen) <= SMEM_MAX)
@@ -257,6 +375,56 @@ def test_table_covers_every_boundary():
     assert any(c.get("m_pool_method") == "mean" and s.get("k") and not s.get("mask") for s in CASES.values()
                for c in [s["cfg"]]), "mean over lists without a mask"
     assert any(s.get("holes") for s in CASES.values()) and any(s.get("slot_edges") for s in CASES.values())
+    # ... and again under a box and under a cell
+    for lat in ("box", "cell"):
+        lp = {n: g for n, g in pair.items() if g["lattice"] == lat}
+        lk = {n: g for n, g in knn.items() if g["lattice"] == lat}
+        ls = [CASES[n] for n in list(lp) + list(lk)]
+        want = {
+            "jsplit 1 / 2 / 4 / 8": {g["jsplit"] for g in lp.values()} >= {1, 2, 4, 8},
+            "jsplit 4 and 8 on row ranges ending with 3 / 1 valid rows": {
+                (g["jsplit"], g["last_rows_valid"]) for g in lp.values() if g["rows_range"]} >= {(4, 3), (8, 1)},
+            "ring refilled with another graph's row group, per-graph lattices, odd laps, at jsplit 1 and >= 2": {
+                min(g["jsplit"], 2) for g in lp.values()
+                if g["refill_other_graph"] and g["per_graph_lattice"] and g["laps"] % 2 == 1} == {1, 2},
+            "one active warpgroup": any(g["active_wgs"] == 1 for g in lp.values()),
+            "N 63..65 / 127..129 / 255..257": {g["N"] for g in lp.values()} >= {63, 64, 65, 127, 128, 129, 255, 256,
+                                                                                257},
+            "dense lean at Hp 2736": any(g["kernel"] == "tc_pair<lean>" and g["Hp"] == 2736 for g in lp.values()),
+            "dense lean and generic": {g["kernel"] for g in lp.values()} == {"tc_pair<lean>", "tc_pair<generic>"},
+            "network, Q 12 with labels, fourier and edges": any(
+                CASES[n]["kind"] == NW and g["Q"] == TP_QMAX and g["labels"] > 0 and g["F"] > 0 and g["edge_dim"] > 0
+                for n, g in lp.items()),
+            "knn k 1 (cell) / 8 / 31 / 32": {g["k"] for g in lk.values()} >= ({1} if lat == "cell" else set()) | {
+                8, 31, 32},
+            "knn every instantiation at 8 and 16 rows": {g["kernel"] for g in lk.values()} >= {
+                f"tc_knn<{m},{r}>" for m in ("LEAN", "EDGES", "GEN") for r in (8, 16)},
+            "knn partial last CTA at 8 and 16 rows": {
+                g["ROWS"] for g in lk.values() if g["last_rows_valid"] < g["ROWS"]} == {8, 16},
+            "knn row ranges": any(g["rows_range"] for g in lk.values()),
+            "knn per-graph lattices": any(g["per_graph_lattice"] for g in lk.values()),
+            "knn -1 slots and per-slot edges": any(s.get("holes") for s in ls if s.get("k"))
+            and any(s.get("slot_edges") for s in ls if s.get("k")),
+            "c2 (dense dim 512, B 4, N 1024)": any(g["dim"] == 512 and g["B"] == 4 and g["N"] == 1024 and g["k"] == 0
+                                                   for g in lp.values()),
+        }
+        missing = [k for k, v in want.items() if not v]
+        assert not missing, (lat, missing)
+        assert {s.get("mask") for s in ls} >= {"padded", "random", "one_empty"}, lat
+        for key in ("soft_edges", "norm_coors", "coor_weights_clamp_value"):
+            assert any(key in s["cfg"] for s in ls), (lat, key)
+        assert any(s["cfg"].get("m_pool_method") == "mean" for s in ls), lat
+    # box only: the generic kernel at C = 5 and C = 8 with aperiodic (0, inf) and periodic axes
+    mixed = lambda b: not isinstance(b, str) and {0.0, INF} <= set(b) and any(0 < v < INF for v in b)
+    assert {g["C"] for n, g in pair.items() if g["kernel"] == "tc_pair<generic>" and mixed(CASES[n].get("box", "x"))
+            } >= {5, 8}
+    # cell only: a 2-D cell on the generic kernel, a hexagonal slab, a tilt of 0.9
+    assert any(g["C"] == 2 and g["kernel"] == "tc_pair<generic>" and g["lattice"] == "cell" for g in pair.values())
+    assert {CASES[n].get("cell") for n in pair} >= {"hex_slab", "tilt09"}
+    # c4 (dim 256, edge_dim 4, k 32, B 8, N 4096) on caller lists with per-slot edges and a box per graph
+    assert any(g["dim"] == 256 and g["edge_dim"] == 4 and g["k"] == 32 and g["B"] == 8 and g["N"] == 4096
+               and g["lattice"] == "box" and g["per_graph_lattice"] and CASES[n].get("slot_edges")
+               for n, g in knn.items())
 
 
 # ------------------------------------------------------------------ inputs and the reference
@@ -266,12 +434,73 @@ def _bf16(a):
     return torch.from_numpy(np.asarray(a, np.float64)).float().bfloat16().double().numpy()
 
 
+def _f32(a):
+    return np.asarray(a, np.float64).astype(np.float32).astype(np.float64)
+
+
+def lattice_kind(spec):
+    return "box" if "box" in spec else ("cell" if "cell" in spec else None)
+
+
+# Cells: fractional coordinates on an odd 1/21 grid (plus a jitter below 1e-5) and tilts that are whole multiples of
+# L_c / 21, so that every wrap decision r_c / L_c lies within 1e-4 of a multiple of 1/441, and 1/441 (odd) keeps
+# those 1.13e-3 away from 1/2: fp32 and fp64 pick the same image at any N.  The hexagonal slab's a / 2 tilt is no
+# such multiple; its nodes are redrawn until they clear the margin (test_triclinic.cell_coors), at small N.
+CELL_GRID = 21
+
+
+def _grid_cell(rs, Ls, tilt):
+    A = np.diag(np.asarray(Ls, np.float64))
+    m = int(tilt * CELL_GRID)
+    for r in range(1, len(Ls)):
+        for c in range(r):
+            A[r, c] = rs.choice([-1, 1]) * rs.randint(3, m + 1) * Ls[c] / CELL_GRID
+    return A
+
+
+def lattice_inputs(spec, rs):
+    """(lattice, coordinates [B, N, C]) of a case, both fp32 values as float64.  Box: coordinates on an odd lattice of
+    the box (test_periodic.lattice_coors); cell: on the CELL_GRID; both moved by whole lattice vectors in [-2, 2]."""
+    B, N, C = spec["B"], spec["N"], spec.get("C", 3)
+    if "box" in spec:
+        box = spec["box"]
+        if isinstance(box, str):                                  # "per_graph"
+            box = np.round(rs.uniform(2.5, 4.0, (B, C)) * 64) / 64
+        box = np.asarray(box, np.float64)
+        scale = np.where(np.isfinite(box) & (box > 0), box, 3.0)
+        x = np.concatenate([PER.lattice_coors(rs, 1, N, C, sc) for sc in np.broadcast_to(scale, (B, C))])
+        return box, _f32(x)
+    kind = spec["cell"]
+    if kind == "hex_slab":
+        cell = _f32(TRI.make_cell(kind, B, rs))
+        return cell, TRI.cell_coors(rs, B, N, cell, dtype=torch.float32)
+    Ls = [3.0, 3.25, 3.5][:C] if kind != "c2" else [3.0, 2.75]
+    if kind == "tilt":
+        cell = _grid_cell(rs, Ls, 0.5)
+    elif kind == "tilt09":
+        cell = _grid_cell(rs, Ls, 0.3)
+        cell[2, 0] = 19 * Ls[0] / CELL_GRID                       # 0.905 L_0
+    elif kind == "c2":
+        cell = _grid_cell(rs, Ls, 0.5)
+    else:                                                         # "per_graph"
+        cell = np.stack([_grid_cell(rs, np.round(rs.uniform(2.8, 3.6, C) * 64) / 64, 0.5) for _ in range(B)])
+    cell = _f32(cell)
+    A = np.broadcast_to(cell, (B, C, C))
+    s = (rs.randint(0, CELL_GRID, (B, N, C)) / CELL_GRID + rs.uniform(-1e-5, 1e-5, (B, N, C))
+         + rs.randint(-2, 3, (B, N, C)))
+    return cell, _f32(np.einsum("bnk,bkd->bnd", s, A))
+
+
 @functools.lru_cache(maxsize=None)
 def build(name):
     """The case with bf16 parameters / features / edges and fp32 coordinates, plus its neighbour lists."""
     spec = CASES[name]
-    case = cases.build_case(dict({k: v for k, v in spec.items() if k not in ("check", "rows")}, init="xavier"))
+    lat = lattice_kind(spec)
+    case = cases.build_case(dict({k: v for k, v in spec.items() if k not in ("check", "rows", "box", "cell")},
+                                 init="xavier", dense_edges=not (lat and spec.get("slot_edges"))))
     ins = case["inputs"]
+    if lat:
+        case[lat], ins["coors"] = lattice_inputs(spec, np.random.RandomState(spec["seed"] + 11))
     case["params"] = {k: _bf16(v) for k, v in case["params"].items()}
     if np.issubdtype(np.asarray(ins["feats"]).dtype, np.floating):
         ins["feats"] = _bf16(ins["feats"])
@@ -282,8 +511,8 @@ def build(name):
     if k:
         B, N = spec["B"], spec["N"]
         rs = np.random.RandomState(spec["seed"] + 7)
-        if spec.get("slot_edges"):      # distinct neighbours per row: the oracle takes per-slot edges as [B, N, N, e]
-            nbr = rs.uniform(size=(B, N, N)).argsort(-1)[..., :k]
+        if spec.get("slot_edges") and not lat:   # distinct neighbours per row: the oracle takes per-slot edges as
+            nbr = rs.uniform(size=(B, N, N)).argsort(-1)[..., :k]     # [B, N, N, e] (the restatement takes them per slot)
         else:
             nbr = rs.randint(0, N, (B, N, k))
         if spec.get("holes"):
@@ -301,14 +530,22 @@ def windows(name):
     return spec.get("check") or [spec.get("rows") or (0, spec["N"])]
 
 
-def reference(name, rounding=True, messages=True):
-    """[(window, feats, coors)] of the reference over the case's check windows."""
+def lattice_kw(name):
+    """{'box': [C] | [B, C]} or {'cell': [C, C] | [B, C, C]} (fp32 values as float64) of a case, or {}."""
+    case = build(name)
+    return {k: case[k] for k in ("box", "cell") if k in case}
+
+
+def reference(name, rounding=True, messages=True, lattice=None):
+    """[(window, feats, coors)] of the reference over the case's check windows.  `lattice`: a {'box' | 'cell': ...}
+    to use instead of the case's own ({} for none)."""
     case = build(name)
     ins = case["inputs"]
+    lat = lattice_kw(name) if lattice is None else lattice
     if case["kind"] == NW:
         assert messages
         f, x = T.tc_network_forward(case["params"], case["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
-                                    ins.get("edges"), ins.get("mask"), rounding=rounding)
+                                    ins.get("edges"), ins.get("mask"), rounding=rounding, **lat)
         return [((0, CASES[name]["N"]), f, x)]
     spec = CASES[name]
     out = []
@@ -316,7 +553,7 @@ def reference(name, rounding=True, messages=True):
         f, x = T.tc_layer_forward(case["params"], case["cfg"], ins["feats"], ins["coors"], edges=ins.get("edges"),
                                   mask=ins.get("mask"), neighbors=ins.get("neighbors"),
                                   slot_edges=bool(spec.get("slot_edges")), rows=w, rounding=rounding,
-                                  messages=messages)
+                                  messages=messages, **lat)
         out.append((w, f, x))
     return out
 
@@ -327,9 +564,12 @@ def reference_cached(name):
 
 
 def oracle(name):
-    """[(window, feats, coors)] of the fp64 oracle over the same windows."""
+    """[(window, feats, coors)] of the fp64 oracle over the same windows (under a lattice: the float64 periodic
+    restatement, torch_reference.layer / .network, with test_triclinic's cell wrap for a cell)."""
     case = build(name)
     ins = case["inputs"]
+    if lattice_kind(CASES[name]):
+        return restatement(name)
     if case["kind"] == NW:
         f, x = cases.run_oracle(case)
         return [((0, CASES[name]["N"]), f, x)]
@@ -347,6 +587,27 @@ def oracle(name):
     return [(w,) + tuple(O.egnn_layer_forward(case["params"], case["cfg"], ins["feats"], ins["coors"],
                                               edges=ins.get("edges"), mask=ins.get("mask"), rows=w))
             for w in windows(name)]
+
+
+def restatement(name):
+    case = build(name)
+    ins = case["inputs"]
+    lat = lattice_kw(name)
+    geometry_ctx = TRI._cell_geometry() if "cell" in lat else contextlib.nullcontext()
+    with geometry_ctx:
+        lattice = next(iter(lat.values()))
+        if case["kind"] == NW:
+            f, x, _ = R.network(case["params"], case["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
+                                ins.get("edges"), ins.get("mask"), box=lattice)
+            return [((0, CASES[name]["N"]), f.numpy(), x.numpy())]
+        slot = CASES[name].get("slot_edges")
+        out = []
+        for w in windows(name):
+            f, x = R.layer(case["params"], case["cfg"], ins["feats"], ins["coors"], None if slot else ins.get("edges"),
+                           ins.get("mask"), None, lattice, ins.get("neighbors"), ins.get("edges") if slot else None,
+                           rows=w)
+            out.append((w, f.numpy(), x.numpy()))
+    return out
 
 
 def test_every_case_sees_the_edge_kernel():
@@ -450,11 +711,200 @@ def test_rounded_reference_stays_within_the_oracle_gate_on_pinned_cases():
         assert np.abs(got[1] - want[1]).max() <= 1e-2 * max(np.abs(want[1] - ins["coors"]).max(), 1.0), name
 
 
+# ------------------------------------------------------------------ periodic cases: inputs, the wrap, sensitivity (CPU)
+
+
+def graph_lattice(name, b):
+    kind = lattice_kind(CASES[name])
+    lat = np.asarray(lattice_kw(name)[kind])
+    return lat[b] if lat.ndim == (2 if kind == "box" else 3) else lat
+
+
+def compared_pairs(name):
+    """[(graph, rel [P, C])]: fp32(x_i - x_j) of every unmasked pair the gates compare (check windows, listed slots)."""
+    ins = build(name)["inputs"]
+    x, mk, nb = ins["coors"], ins.get("mask"), ins.get("neighbors")
+    out = []
+    for b in range(x.shape[0]):
+        for w in windows(name):
+            ii = np.arange(*w)
+            if nb is None:
+                jj = np.broadcast_to(np.arange(x.shape[1]), (len(ii), x.shape[1]))
+                ok = np.ones(jj.shape, bool)
+            else:
+                jj = nb[b, w[0]:w[1]]
+                ok = jj >= 0
+                jj = np.where(ok, jj, ii[:, None])
+            if mk is not None:
+                ok = ok & mk[b, ii][:, None] & mk[b, jj]
+            out.append((b, _f32(x[b, ii][:, None] - x[b, jj])[ok]))
+    return out
+
+
+def wrap_decisions(rel, kind, lat):
+    """Float64 wrap of rel [P, C] under one graph's box [C] or cell [C, C] -> (smallest distance of r_c / L_c from 1/2
+    (mod 1) over each pair's decisions, whether any image count of the pair is nonzero)."""
+    A = np.diag(lat) if kind == "box" else np.asarray(lat)
+    r = rel.copy()
+    margin, moved = np.ones(len(r)), np.zeros(len(r), bool)
+    for c in reversed(range(r.shape[-1])):
+        Lc = A[c, c]
+        if not (np.isfinite(Lc) and Lc > 0):
+            continue
+        t = r[:, c] / Lc
+        margin = np.minimum(margin, np.abs(np.abs(t - np.rint(t)) - 0.5))
+        n = np.rint(t)
+        moved |= n != 0
+        r[:, :c + 1] -= n[:, None] * A[c, :c + 1]
+    return margin, moved
+
+
+@pytest.mark.parametrize("name", list(LATTICE_CASES))
+def test_lattice_inputs_wrap_often_and_stay_off_one_half(name):
+    """Every wrap decision of a compared pair lies >= 1e-3 from 1/2, so fp32 and fp64 pick the same image (and the
+    fp64 restatement's gate holds), and >= 20 % of the compared, unmasked pairs are moved by a lattice vector."""
+    kind = lattice_kind(CASES[name])
+    margin, moved, total = 1.0, 0, 0
+    for b, rel in compared_pairs(name):
+        m, mv = wrap_decisions(rel, kind, graph_lattice(name, b))
+        margin = min(margin, float(m.min(initial=1.0)))
+        moved += int(mv.sum())
+        total += len(mv)
+    assert margin >= 1e-3, (name, margin)
+    assert moved >= 0.2 * total, (name, moved / total)
+
+
+def _fp32_exact(q):
+    """The Fraction q rounded to the nearest fp32 (ties to even; normal range)."""
+    if q == 0:
+        return Fraction(0)
+    a = abs(q)
+    e = a.numerator.bit_length() - a.denominator.bit_length() - 23
+    while a / Fraction(2) ** e >= 2 ** 24:
+        e += 1
+    while a / Fraction(2) ** e < 2 ** 23:
+        e -= 1
+    return (1 if q > 0 else -1) * round(a / Fraction(2) ** e) * Fraction(2) ** e
+
+
+def _exact_step(r, L, inv, coef=None):
+    """n = rint(fp32(r * inv)) and fp32(-coef * n + r) (coef: L), exactly."""
+    n = round(_fp32_exact(r * inv))
+    return n, _fp32_exact(-(L if coef is None else coef) * n + r)
+
+
+def _near_half(rs, L, size):
+    """fp32 values within 3 ulps of (n + 1/2) L, n in [-4, 4]."""
+    v = ((rs.randint(-4, 5, size) + 0.5) * L).astype(np.float32)
+    for _ in range(3):
+        step = rs.randint(-1, 2, size)
+        v = np.where(step > 0, np.nextafter(v, np.float32(np.inf)),
+                     np.where(step < 0, np.nextafter(v, np.float32(-np.inf)), v))
+    return v
+
+
+def test_rounded_wrap_is_the_kernels_fp32_sequence_exactly():
+    """tc_reference's fp32 wrap (box: min_image, cell: cell_wrap_n) equals an exact rational evaluation of the same
+    operation sequence, with one rounding to fp32 per operation, on 10^4 draws of each -- half of them within 3 ulps
+    of (n + 1/2) L, where the image flips."""
+    rs = np.random.RandomState(17)
+    M = 10000
+    L = rs.uniform(0.3, 12.0, M).astype(np.float32)
+    r = np.where(rs.uniform(size=M) < 0.5, _near_half(rs, L, M), (rs.uniform(-6, 6, M) * L).astype(np.float32))
+    got = T.wrap_box(torch.as_tensor(r, dtype=torch.float64)[None], torch.as_tensor(L, dtype=torch.float64))[0].numpy()
+    for rv, Lv, g in zip(r, L, got):
+        Lq = Fraction(float(Lv))
+        inv = _fp32_exact(1 / Lq)
+        assert Fraction(float(g)) == _exact_step(Fraction(float(rv)), Lq, inv)[1]
+    for _ in range(200):
+        A = np.tril(rs.uniform(-1.5, 1.5, (3, 3))) + np.diag(rs.uniform(0.5, 6.0, 3))
+        if rs.uniform() < 0.2:
+            A[rs.randint(3)] = 0.0                                # an aperiodic axis (its whole row: a slab)
+        A = A.astype(np.float32)
+        rv = (rs.uniform(-8, 8, (50, 3)) * np.abs(np.diag(A)).max()).astype(np.float32)
+        if A[2, 2] > 0:
+            rv[:25, 2] = _near_half(rs, np.full(25, A[2, 2], np.float32), 25)
+        got = T.wrap_cell(torch.as_tensor(rv, dtype=torch.float64), torch.as_tensor(A, dtype=torch.float64)).numpy()
+        Aq = [[Fraction(float(v)) for v in row] for row in A]
+        invq = [_fp32_exact(1 / Aq[c][c]) if Aq[c][c] > 0 else Fraction(0) for c in range(3)]
+        for v, g in zip(rv, got):
+            x = [Fraction(float(t)) for t in v]
+            for c in (2, 1, 0):
+                Lc = Aq[c][c] if Aq[c][c] > 0 else Fraction(0)
+                n = round(_fp32_exact(x[c] * invq[c]))
+                for d in range(c + 1):
+                    x[d] = _fp32_exact(-(Lc if d == c else Aq[c][d]) * n + x[d])
+            assert [Fraction(float(t)) for t in g] == x
+
+
+def _pin(case, **lat):
+    """tc_layer_forward(rounding=False) under `lat` against torch_reference.layer (the float64 restatement), dense, or
+    on the lists of the restatement's own selection."""
+    ins, cfg = case["inputs"], case["cfg"]
+    lattice = next(iter(lat.values()))
+    want = R.layer(case["params"], cfg, ins["feats"], ins["coors"], ins.get("edges"), ins.get("mask"),
+                   ins.get("adj_mat"), lattice)
+    nbr = ok = None
+    if cfg["num_nearest_neighbors"] > 0 or cfg["only_sparse_neighbors"]:
+        x = R._t(ins["coors"])
+        b, n, c = x.shape
+        d = (R.wrap(x[:, :, None] - x[:, None], R.box_bc(lattice, b, c)[:, None, None, :]) ** 2).sum(-1)
+        nbr, ok = R.select(cfg, d, ins.get("mask"), ins.get("adj_mat"))
+    got = T.tc_layer_forward(case["params"], cfg, ins["feats"], ins["coors"], edges=ins.get("edges"),
+                             mask=ins.get("mask"), neighbors=None if nbr is None else nbr.numpy(),
+                             nbr_ok=None if ok is None else ok.numpy(), rounding=False, **lat)
+    for g, w in zip(got, want):
+        w = w.numpy()
+        assert np.abs(g - w).max() <= 1e-12 * max(1.0, np.abs(w).max())
+
+
+@pytest.mark.parametrize("name", sorted(PER.PCASES))
+def test_unrounded_reference_equals_the_periodic_restatement(name):
+    case, box = PER.build(name)
+    _pin(case, box=box)
+
+
+@pytest.mark.parametrize("name", sorted(TRI.TCASES))
+def test_unrounded_reference_equals_the_triclinic_restatement(name):
+    case, cell = TRI.build(name)
+    with TRI._cell_geometry():
+        _pin(case, cell=cell)
+
+
+def wrong_lattices(name):
+    """[(what, lattice, (tc_reference attribute, replacement) | None)]: mistakes a lattice case must see."""
+    kind = lattice_kind(CASES[name])
+    lat = np.asarray(lattice_kw(name)[kind])
+    out = [("no lattice", {}, None)]
+    if lat.ndim == (2 if kind == "box" else 3):
+        out.append(("each graph given the next graph's lattice", {kind: np.roll(lat, -1, 0)}, None))
+    if kind == "cell":
+        eye = np.eye(lat.shape[-1], dtype=bool)
+        out.append(("the cell's diagonal", {kind: np.where(eye, lat, 0.0)}, None))
+        out.append(("axes wrapped first to last", {kind: lat},
+                    ("wrap_cell", functools.partial(T.wrap_cell, first_to_last=True))))
+    out.append(("floor for rint", {kind: lat}, ("_rint", torch.floor)))
+    return out
+
+
+@pytest.mark.parametrize("name", list(LATTICE_CASES))
+def test_a_wrong_lattice_fails_a_gate(name, monkeypatch):
+    """The rounded reference under a wrong lattice fails at least one TOL gate against the right one, for each
+    mistake of `wrong_lattices`: a case that passes one could not see that mistake in a kernel."""
+    for what, lat, patch in wrong_lattices(name):
+        with monkeypatch.context() as m:
+            if patch:
+                m.setattr(T, *patch)
+            g = gates(name, [(f, x) for _, f, x in reference(name, lattice=lat)])
+        assert any(g[k] > TOL[k] for k in TOL), (name, what, g)
+
+
 # ------------------------------------------------------------------ the GPU runs
 
 
-def run_gpu(name, rows="spec"):
-    """Forward of the case on the bf16 path; -> (feats [B,N,dim] float64, coors [B,N,C] float64) as numpy."""
+def run_gpu(name, rows="spec", lattice=None):
+    """Forward of the case on the bf16 path -> (feats [B,N,dim] bf16, coors [B,N,C] fp32) on the device.  `lattice`:
+    a {'box' | 'cell': ...} to pass instead of the case's own."""
     case = build(name)
     spec = CASES[name]
     ins = case["inputs"]
@@ -464,14 +914,16 @@ def run_gpu(name, rows="spec"):
     coors = torch.from_numpy(ins["coors"]).float().to(dev)
     mask = None if ins.get("mask") is None else torch.from_numpy(ins["mask"]).to(dev)
     tb = lambda a: None if a is None else torch.from_numpy(np.asarray(a, np.float64)).to(dev, torch.bfloat16)
+    lat = {k: torch.as_tensor(np.asarray(v), dtype=torch.float32, device=dev)
+           for k, v in (lattice_kw(name) if lattice is None else lattice).items()}
     with torch.no_grad():
         if case["kind"] == NW:
             f, x = mod(torch.from_numpy(ins["feats"]).to(dev) if not np.issubdtype(ins["feats"].dtype, np.floating)
                        else tb(ins["feats"]), coors, adj_mat=torch.from_numpy(ins["adj_mat"]).to(dev),
-                       edges=tb(ins.get("edges")), mask=mask)
+                       edges=tb(ins.get("edges")), mask=mask, **lat)
             layers = [l[1] for l in mod.layers]
         else:
-            kw = dict(mask=mask, _rows=rows)
+            kw = dict(mask=mask, _rows=rows, **lat)
             edges = tb(ins.get("edges"))
             if "neighbors" in ins:
                 kw["neighbors"] = torch.from_numpy(ins["neighbors"]).to(dev)
@@ -486,11 +938,15 @@ def run_gpu(name, rows="spec"):
 
 def metrics(name, f, x):
     """The four gate values of one GPU output against the rounding-matched reference."""
+    return gates(name, [(f[:, w[0]:w[1]].double().cpu().numpy(), x[:, w[0]:w[1]].double().cpu().numpy())
+                        for w in windows(name)])
+
+
+def gates(name, outs):
+    """The four gate values of outputs [(feats, coors)] over the case's windows against the rounding-matched reference."""
     x_in = build(name)["inputs"]["coors"]
     fu, fe, cr, ce, cu = [], [], [], [], []
-    for w, rf, rx in reference_cached(name):
-        gf = f[:, w[0]:w[1]].double().cpu().numpy()
-        gx = x[:, w[0]:w[1]].double().cpu().numpy()
+    for (w, rf, rx), (gf, gx) in zip(reference_cached(name), outs):
         floor = 1e-2 * np.abs(rf).max()
         ulp = 2.0 ** (np.floor(np.log2(np.maximum(np.abs(rf), floor))) - 7)
         fu.append((np.abs(gf - rf) / ulp).ravel())
@@ -527,7 +983,27 @@ def test_matches_rounding_matched_reference(name):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name,full_js", [("p_js8_range", 2), ("p_js4_range", 2)])
+@pytest.mark.parametrize("name", ["pb_js1_ring", "pb_js2_ring", "pb_js8_range", "pb_js8_range_gen"])
+def test_a_diagonal_cell_is_the_box_bit_for_bit(name):
+    """DESIGN's claim that the off-diagonal steps of a diagonal cell subtract exact zeros, at the ring-reuse (per-graph
+    boxes) and j-split 8 row-range shapes, lean and generic."""
+    box = np.asarray(lattice_kw(name)["box"])
+    cell = np.stack([np.diag(b) for b in box]) if box.ndim == 2 else np.diag(box)
+    f_box, x_box = run_gpu(name)
+    f_cell, x_cell = run_gpu(name, lattice=dict(cell=cell))
+    assert torch.equal(f_box, f_cell) and torch.equal(x_box, x_cell)
+
+
+def test_the_diagonal_cell_cases_cover_ring_reuse_and_jsplit_8_ranges_lean_and_generic():
+    geo = [geometry(CASES[n]) for n in ["pb_js1_ring", "pb_js2_ring", "pb_js8_range", "pb_js8_range_gen"]]
+    assert {(g["refill_other_graph"], g["kernel"]) for g in geo if g["per_graph_lattice"]} == {
+        (True, "tc_pair<lean>"), (True, "tc_pair<generic>")}
+    assert {g["kernel"] for g in geo if g["jsplit"] == 8 and g["rows_range"]} == {"tc_pair<lean>", "tc_pair<generic>"}
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("name,full_js", [("p_js8_range", 2), ("p_js4_range", 2), ("pb_js8_range", 2),
+                                          ("pc_js8_range", 2)])
 def test_jsplit_row_range_is_bit_identical_to_the_full_forward(name, full_js):
     """DESIGN's claim for the row-sharded dense kernel: the fp64 sums across tiles make the rows independent of how
     the j-blocks were dealt, so a row range run at j-split 4 / 8 equals the full forward (j-split 1 / 2) bit for bit.
@@ -544,7 +1020,7 @@ def test_jsplit_row_range_is_bit_identical_to_the_full_forward(name, full_js):
 
 
 @pytest.mark.gpu
-@pytest.mark.parametrize("name", ["k32_lean16", "k31_gen16_rows"])
+@pytest.mark.parametrize("name", ["k32_lean16", "k31_gen16_rows", "kb_k32_lean16", "kc_k31_gen16_rows"])
 def test_knn_16_rows_row_range_is_bit_identical(name):
     """The 16-row neighbour-list kernel on a row range that starts off the CTA grid equals its full forward."""
     sms = torch.cuda.get_device_properties(0).multi_processor_count
