@@ -79,8 +79,7 @@ int fast_supported(const EgnnLayerDesc& d) {
     if (f.QT > TP_QMAX) return EGNN_ERR_UNSUPPORTED;
     const size_t smem = pair_is_lean(f) ? tc_pair_smem_bytes<false>(f.Hp, 1) : tc_pair_smem_bytes<true>(f.Hp, f.QT, 1 + 2 * f.s.F);
     if (smem > 227 * 1024) return EGNN_ERR_UNSUPPORTED;
-  } else {                                                         // neighbour lists: tc_knn_kernel<lean | edges | generic>
-    if (d.k > 32) return EGNN_ERR_UNSUPPORTED;
+  } else {                                                         // neighbour lists (any k): tc_knn_kernel<lean | edges | generic>
     const int mode = knn_mode(f);
     if (mode == TK_GEN && f.QT > TP_QMAX) return EGNN_ERR_UNSUPPORTED;
     if (tc_knn_smem_bytes(f.Hp, mode, f.QT) > 227 * 1024) return EGNN_ERR_UNSUPPORTED;
@@ -424,18 +423,24 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
     const size_t smem = tc_knn_smem_bytes(f.Hp, mode, f.QT, rows);
     dim3 grid(ceil_div(R, rows), s.B);
     if (R > 0) {
-#define EGNN_TC_KNN_LAUNCH(MODE_, ROWS_)                                                  \
-  do {                                                                              \
-    if (pbc == PBC_CELL) {                                                          \
-      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_CELL>, smem))); \
-      tc_knn_kernel<MODE_, ROWS_, PBC_CELL><<<grid, ROWS_ * 32, smem, st>>>(a);     \
-    } else if (pbc == PBC_BOX) {                                                    \
-      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_BOX>, smem)));  \
-      tc_knn_kernel<MODE_, ROWS_, PBC_BOX><<<grid, ROWS_ * 32, smem, st>>>(a);      \
-    } else {                                                                        \
-      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_>, smem)));           \
-      tc_knn_kernel<MODE_, ROWS_><<<grid, ROWS_ * 32, smem, st>>>(a);               \
-    }                                                                               \
+#define EGNN_TC_KNN_LAUNCH_PBC(MODE_, ROWS_, WIDE_)                                              \
+  do {                                                                                           \
+    if (pbc == PBC_CELL) {                                                                       \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_CELL, WIDE_>, smem)));       \
+      tc_knn_kernel<MODE_, ROWS_, PBC_CELL, WIDE_><<<grid, ROWS_ * 32, smem, st>>>(a);           \
+    } else if (pbc == PBC_BOX) {                                                                 \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_BOX, WIDE_>, smem)));        \
+      tc_knn_kernel<MODE_, ROWS_, PBC_BOX, WIDE_><<<grid, ROWS_ * 32, smem, st>>>(a);            \
+    } else {                                                                                     \
+      EGNN_TRY((ensure_dynamic_smem(tc_knn_kernel<MODE_, ROWS_, PBC_NONE, WIDE_>, smem)));       \
+      tc_knn_kernel<MODE_, ROWS_, PBC_NONE, WIDE_><<<grid, ROWS_ * 32, smem, st>>>(a);           \
+    }                                                                                            \
+  } while (0)
+// k <= 32: one slot group per row (WIDE = false, straight-line code); k > 32: the slot-group loop
+#define EGNN_TC_KNN_LAUNCH(MODE_, ROWS_)                                                         \
+  do {                                                                                           \
+    if (s.k > 32) EGNN_TC_KNN_LAUNCH_PBC(MODE_, ROWS_, true);                                    \
+    else EGNN_TC_KNN_LAUNCH_PBC(MODE_, ROWS_, false);                                            \
   } while (0)
       if (mode == TK_LEAN) {
         if (rows == 8) EGNN_TC_KNN_LAUNCH(TK_LEAN, 8); else EGNN_TC_KNN_LAUNCH(TK_LEAN, 16);
@@ -445,6 +450,7 @@ int fast_forward(const EgnnLayerDesc& d, const EgnnLayerWeights& w, const void* 
         if (rows == 8) EGNN_TC_KNN_LAUNCH(TK_GEN, 8); else EGNN_TC_KNN_LAUNCH(TK_GEN, 16);
       }
 #undef EGNN_TC_KNN_LAUNCH
+#undef EGNN_TC_KNN_LAUNCH_PBC
       EGNN_LAUNCH_CHECK();
       count_launch();
     }

@@ -452,6 +452,8 @@ class EGNN(nn.Module):
                                    f"which holds at most N={SELECT_SORT_MAX_N}, got N={n}: use k <= 32, or pass "
                                    f"neighbors= (e.g. from radius_neighbors)")
 
+        # support does not depend on the list length (any k > 0 runs the tensor cores), so one cached "unsupported"
+        # entry for all k > 32 stays correct
         cfg_key = (c, k > 0, min(k, 33), cont_edge_dim, label_dim, _rows is None)
         if kdt == torch.bfloat16 and cfg_key in self._tc_unsupported:
             kdt = torch.float32

@@ -8,7 +8,8 @@ entry becomes one line `demangled name | registers, barriers, stack, static shar
 sorted.  The trailing periodic-boundary template argument PBC of the kernels that have one is written as an int in
 both logs (it was a bool, false / true, before triclinic cells made it none / box / cell = 0 / 1 / 2), so a kernel
 that existing calls run keeps its name across that change.  pair_bwd3_kernel's trailing lattice-gradient argument
-LAT is dropped from the name when it is false, for the same reason.  Prints a unified diff of the two listings: a line present
+LAT and tc_knn_kernel's trailing slot-group argument WIDE are dropped from the name when they are false, for the same
+reason.  Prints a unified diff of the two listings: a line present
 in both is an instantiation whose registers, spills, stack and shared memory are unchanged."""
 import difflib
 import re
@@ -38,7 +39,7 @@ def entries(path):
                            check=True).stdout.splitlines()
     lines = []
     for (_, regs, frame), name in zip(out, names):
-        if "pair_bwd3_kernel<" in name:      # its trailing LAT argument: dropped when false (the kernels that existed
+        if "pair_bwd3_kernel<" in name or "tc_knn_kernel<" in name:     # the trailing LAT / WIDE argument: dropped when false
             name = re.sub(r"(\(int\)\d), \(bool\)([01])>\(",    # before it), written as `true` otherwise
                           lambda m: m.group(1) + (">(" if m.group(2) == "0" else ", (bool)true>("), name, count=1)
         if any(k in name for k in PBC_KERNELS):
