@@ -146,25 +146,33 @@ __device__ __forceinline__ E* edge_row(E* edges, bool per_slot, size_t node_i, i
 // kernel (forward, recompute, backward) regenerates the keep/drop decision of an element from a counter hash of
 // (seed, stream, element index) -- stream 0: edge hidden (pair, channel), 1: coors hidden (pair, unit), 2: node hidden
 // (node, channel).  Statistically equivalent to the reference's Philox masks, not bit-equal (nothing could be).
+// A kept unit is scaled by 1/(1-p) in the kernel's type, as nn.Dropout scales in the layer's dtype: the fp64 kernels
+// use the double (float(1/(1-p)) differs from it by up to 5e-8 relative, e.g. at p = 0.1).
 struct DropCfg {
   unsigned int thr;            // drop when hash < thr;  0 = dropout off
-  float inv_keep;              // 1 / (1 - p)
+  float inv_keep;              // 1 / (1 - p) rounded to float: the fp32 kernels' scale
   unsigned long long seed;
+  double inv_keep_d;           // 1 / (1 - p): the fp64 kernels' scale
 };
 __host__ __device__ inline DropCfg make_drop(double p, unsigned long long seed) {
   DropCfg d;
   d.thr = p > 0.0 ? (unsigned int)(p * 4294967296.0 > 4294967295.0 ? 4294967295.0 : p * 4294967296.0) : 0u;
-  d.inv_keep = p > 0.0 && p < 1.0 ? (float)(1.0 / (1.0 - p)) : 1.f;
+  d.inv_keep_d = p > 0.0 && p < 1.0 ? 1.0 / (1.0 - p) : 1.0;
+  d.inv_keep = (float)d.inv_keep_d;
   d.seed = seed;
   return d;
 }
-// multiplier of the pre-activation: 0 (dropped) or 1/(1-p) (kept)
-__device__ __forceinline__ float drop_mul(const DropCfg& d, unsigned int stream, unsigned long long idx) {
+template <typename T> __device__ __forceinline__ T drop_scale(const DropCfg& d);
+template <> __device__ __forceinline__ float drop_scale<float>(const DropCfg& d) { return d.inv_keep; }
+template <> __device__ __forceinline__ double drop_scale<double>(const DropCfg& d) { return d.inv_keep_d; }
+// multiplier of the pre-activation in type T: 0 (dropped) or 1/(1-p) (kept)
+template <typename T>
+__device__ __forceinline__ T drop_mul(const DropCfg& d, unsigned int stream, unsigned long long idx) {
   unsigned long long z = idx * 0x9E3779B97F4A7C15ull + d.seed + (unsigned long long)stream * 0xD1B54A32D192ED03ull;
   z ^= z >> 30; z *= 0xBF58476D1CE4E5B9ull;
   z ^= z >> 27; z *= 0x94D049BB133111EBull;
   z ^= z >> 31;
-  return (unsigned int)(z >> 32) < d.thr ? 0.f : d.inv_keep;
+  return (unsigned int)(z >> 32) < d.thr ? T(0) : drop_scale<T>(d);
 }
 
 // ------------------------------------------------------------------ scalar math

@@ -262,7 +262,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
           for (int z = 0; z < 4; ++z) t = fma_t(wv.v[z], mm[o + z], t);
         }
         if (a.drop.thr) {                                // coors_mlp Dropout: a dropped unit is stored as NaN (silu(0) = 0
-          const T f = (T)drop_mul(a.drop, 1u, (unsigned long long)pair * U + u);   // adds nothing)
+          const T f = drop_mul<T>(a.drop, 1u, (unsigned long long)pair * U + u);   // adds nothing)
           t = f == T(0) ? T(NAN) : t * f;
         }
         tt[tid * UP + u] = t;
@@ -302,7 +302,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
         const T t = tt[tid * UP + u];
         if (t != t) continue;                            // dropped unit: no gradient
         const T sg = sigmoid_acc<T>(t);
-        const T gt = gw0 * w4s[u] * dsilu_from<T>(t, sg) * (a.drop.thr ? (T)a.drop.inv_keep : T(1));
+        const T gt = gw0 * w4s[u] * dsilu_from<T>(t, sg) * (a.drop.thr ? drop_scale<T>(a.drop) : T(1));
         const T* w3 = w3s + u * MP;
 #pragma unroll
         for (int o = 0; o < MP; o += 4) {
@@ -364,7 +364,7 @@ pair_bwd1_kernel(const BwdArgs<T> a) {
         const T t = tt[p * UP + role_u];
         if (t != t) continue;                            // dropped unit
         const T sg = sigmoid_acc<T>(t);
-        const T gt = g0 * w4u * dsilu_from<T>(t, sg) * (a.drop.thr ? (T)a.drop.inv_keep : T(1));
+        const T gt = g0 * w4u * dsilu_from<T>(t, sg) * (a.drop.thr ? drop_scale<T>(a.drop) : T(1));
         accb3 += gt;
         accw4 = fma_t(g0, t * sg, accw4);
         const T* mrow = mms + p * MP;
@@ -550,7 +550,7 @@ pair_bwd2_knn_kernel(const BwdArgs<T> a) {
         T fdrop = T(1);
         if (DROP) {                                      // edge_mlp Dropout: same mask as the forward (own instantiation: the
                                                          // key arithmetic costs 50 registers when unrolled over the rows)
-          fdrop = (T)drop_mul(a.drop, 0u, (((unsigned long long)b * N + i0 + row) * N + j) * s.Hp + hh);
+          fdrop = drop_mul<T>(a.drop, 0u, (((unsigned long long)b * N + i0 + row) * N + j) * s.Hp + hh);
           pre *= fdrop;
         }
         const T sg = sigmoid_bw(pre);
@@ -755,7 +755,7 @@ pair_bwd2_dense_kernel(const BwdArgs<T> a) {
       }
       T fdrop = T(1);
       if (DROP) {                                        // edge_mlp Dropout: same mask as the forward
-        fdrop = (T)drop_mul(a.drop, 0u, (((unsigned long long)b * N + i0 + p) * N + j) * s.Hp + hh);
+        fdrop = drop_mul<T>(a.drop, 0u, (((unsigned long long)b * N + i0 + p) * N + j) * s.Hp + hh);
         pre *= fdrop;
       }
       const T sg = sigmoid_bw(pre);
@@ -1068,7 +1068,7 @@ __global__ void dsilu_mul_kernel(T* __restrict__ g, const T* __restrict__ pre, s
   for (size_t x = (size_t)blockIdx.x * blockDim.x + threadIdx.x; x < n; x += (size_t)gridDim.x * blockDim.x) {
     const size_t e = MAP ? map((int)(x / cols)) * cols + x % cols : x;
     T p = pre[e], f = T(1);
-    if (drop.thr) { f = (T)drop_mul(drop, 2u, (unsigned long long)e); p *= f; }
+    if (drop.thr) { f = drop_mul<T>(drop, 2u, (unsigned long long)e); p *= f; }
     g[e] *= dsilu_from<T>(p, sigmoid_acc<T>(p)) * f;
   }
 }

@@ -117,7 +117,7 @@ static int launch_pair_dense(const PairArgs<T>& a, cudaStream_t st) {
 
 template <typename T, int ACT, bool RES>
 static int launch_gemm(const T* A, int lda, const T* W, int ldw, const T* bias, const T* R, int ldr, T* C,
-                       int ldo, int Mr, int Nv, int Nout, int K, RowMap map, cudaStream_t st, DropCfg drop = DropCfg{0u, 1.f, 0ull}) {
+                       int ldo, int Mr, int Nv, int Nout, int K, RowMap map, cudaStream_t st, DropCfg drop = make_drop(0.0, 0ull)) {
   constexpr int V = 16 / (int)sizeof(T);
   const size_t skinny_smem = (size_t)16 * ((K + V - 1) / V * V) * sizeof(T);
   if (Mr <= 16 && skinny_smem <= 96 * 1024) {

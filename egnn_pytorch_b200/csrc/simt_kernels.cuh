@@ -132,7 +132,7 @@ gemm_nt_kernel(const T* __restrict__ A, int lda, const T* __restrict__ W, int ld
       T v = T(0);
       if (col < Nv) {
         v = acc[i][j] + (bias ? bias[col] : T(0));
-        if (ACT == 1 && drop.thr) v *= (T)drop_mul(drop, 2u, (unsigned long long)row * Nout + col);     // node_mlp Dropout, :198
+        if (ACT == 1 && drop.thr) v *= drop_mul<T>(drop, 2u, (unsigned long long)row * Nout + col);     // node_mlp Dropout, :198
         if (ACT == 1) v = silu_acc<T>(v);
         if (ACT == 2) v = gelu_acc<T>(v);
         if (RES) v += R[row * ldr + col];
@@ -231,7 +231,7 @@ gemm_skinny_kernel(const T* __restrict__ A, int lda, const T* __restrict__ W, in
       const size_t row = map(m);
       if (col < Nv) {
         v += bias ? bias[col] : T(0);
-        if (ACT == 1 && drop.thr) v *= (T)drop_mul(drop, 2u, (unsigned long long)row * Nout + col);
+        if (ACT == 1 && drop.thr) v *= drop_mul<T>(drop, 2u, (unsigned long long)row * Nout + col);
         if (ACT == 1) v = silu_acc<T>(v);
         if (ACT == 2) v = gelu_acc<T>(v);
         if (RES) v += R[row * ldr + col];
@@ -443,7 +443,7 @@ __device__ __forceinline__ T pair_coord_weight(const PairArgs<T>& a, const T (&m
 #pragma unroll
       for (int z = 0; z < 4; ++z) t = fma_t(wv.v[z], mm[o + z], t);
     }
-    if (a.drop.thr) t *= (T)drop_mul(a.drop, 1u, (unsigned long long)pair * U + u);    // coors_mlp Dropout, :205
+    if (a.drop.thr) t *= drop_mul<T>(a.drop, 1u, (unsigned long long)pair * U + u);    // coors_mlp Dropout, :205
     w = fma_t(w4s[u], silu_acc<T>(t), w);
   }
   if (!pm) w = T(0);                                   // :309 (and padding lanes of the tile)
@@ -582,7 +582,7 @@ pair_kernel(const PairArgs<T> a) {
         if (a.drop.thr) {                                // egnn_pytorch.py:180
           const unsigned long long pkey = (unsigned long long)pair * s.Hp + c0 + cc;
 #pragma unroll
-          for (int u = 0; u < 4; ++u) pre[u] *= (T)drop_mul(a.drop, 0u, pkey + u);
+          for (int u = 0; u < 4; ++u) pre[u] *= drop_mul<T>(a.drop, 0u, pkey + u);
         }
 #pragma unroll
         for (int u = 0; u < 4; ++u) {
@@ -811,7 +811,7 @@ pair_dense_tiled_kernel(const PairArgs<T> a) {
           for (int p = 0; p < PP; ++p) {
             const unsigned long long pkey = (((unsigned long long)b * s.N + irow[p]) * s.N + j) * s.Hp + c0 + cc;
 #pragma unroll
-            for (int u = 0; u < 4; ++u) pre[p][u] *= (T)drop_mul(a.drop, 0u, pkey + u);
+            for (int u = 0; u < 4; ++u) pre[p][u] *= drop_mul<T>(a.drop, 0u, pkey + u);
           }
         }
 #pragma unroll

@@ -99,11 +99,12 @@ def _edge_rows(edges, ref, r0, r1, idx=None):
 
 
 def layer(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neighbors=None, slot_edges=None, ok=None,
-          rows=None):
+          rows=None, drop=None):
     """One EGNN layer (periodic geometry with `box`) in the type and on the device of `feats` (float64 for numpy).
     `neighbors` [B,N,k]: edge-list mode (-1 = empty slot), or with `ok` [B,N,k] a select's lists and their
     valid_radius flags; `slot_edges` [B,N,k,e] are per-slot edge features.  `rows` (r0, r1): the outputs of those rows
-    only -> ([B, r1-r0, dim], [B, r1-r0, C])."""
+    only -> ([B, r1-r0, dim], [B, r1-r0, C]).  `drop`: training-mode dropout with the kernels' masks (a
+    tests/dropout_reference.Drop), multiplying the outputs of edge_mlp.0, coors_mlp.0 and node_mlp.0, bias included."""
     feats = _t(feats)
     coors = _like(coors, feats)
     P = {k: _like(v, feats) for k, v in P.items()}
@@ -143,6 +144,9 @@ def layer(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neigh
         feats_j = feats[:, None].expand(b, R, n, d)
         edges = _edge_rows(edges, feats, r0, r1)
     j = feats_j.shape[2]
+    if drop is not None:                    # the neighbour of every (row, slot): the masks are keyed by it
+        nbr_j = idx.cpu().numpy() if use_nearest else np.arange(n)
+        rows_i = np.arange(r0, r1)
     F = cfg["fourier_features"]
     dfeat = dist[..., None]
     if F > 0:
@@ -150,7 +154,11 @@ def layer(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neigh
         dfeat = torch.cat([torch.sin(sc), torch.cos(sc), dist[..., None]], -1)
     edge_in = torch.cat([fi[:, :, None].expand(b, R, j, d), feats_j, dfeat] + ([edges] if edges is not None else []), -1)
     lin = lambda x, key: x @ P[key + ".weight"].T + P[key + ".bias"]
-    m = TF.silu(lin(TF.silu(lin(edge_in, "edge_mlp.0")), "edge_mlp.3"))
+    h1 = lin(edge_in, "edge_mlp.0")
+    if drop is not None:
+        h1 = h1 * drop.edge(b, n, rows_i, nbr_j, h1.shape[-1], feats.dtype, dev)
+    m = TF.silu(lin(TF.silu(h1), "edge_mlp.3"))
+    del h1
     del edge_in
     if cfg["soft_edges"]:
         m = m * torch.sigmoid(lin(m, "edge_gate.0"))
@@ -162,7 +170,10 @@ def layer(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neigh
             live = live & nbhd
     coors_out = xi
     if cfg["update_coors"]:
-        w = lin(TF.silu(lin(m, "coors_mlp.0")), "coors_mlp.3")[..., 0]
+        t = lin(m, "coors_mlp.0")
+        if drop is not None:
+            t = t * drop.coors(b, n, rows_i, nbr_j, t.shape[-1], feats.dtype, dev)
+        w = lin(TF.silu(t), "coors_mlp.3")[..., 0]
         if live is not None:
             w = torch.where(live, w, torch.zeros_like(w))
         cv = cfg["coor_weights_clamp_value"]
@@ -185,7 +196,10 @@ def layer(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neigh
             else:
                 m_i = m_i / j
         normed = TF.layer_norm(fi, (d,), P["node_norm.weight"], P["node_norm.bias"], 1e-5) if cfg["norm_feats"] else fi
-        feats_out = lin(TF.silu(lin(torch.cat([normed, m_i], -1), "node_mlp.0")), "node_mlp.3") + fi
+        t = lin(torch.cat([normed, m_i], -1), "node_mlp.0")
+        if drop is not None:
+            t = t * drop.node(b, n, rows_i, t.shape[-1], feats.dtype, dev)
+        feats_out = lin(TF.silu(t), "node_mlp.3") + fi
     return feats_out, coors_out
 
 
@@ -214,18 +228,20 @@ def _width(cfg, n, neighbors, adj):
     return min(n, cfg["num_nearest_neighbors"]) if cfg["num_nearest_neighbors"] > 0 else n
 
 
-def layer_forward(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neighbors=None, ok=None, chunk=None):
+def layer_forward(P, cfg, feats, coors, edges=None, mask=None, adj=None, box=None, neighbors=None, ok=None, chunk=None,
+                  drop=None):
     """Whole-graph outputs of `layer`, computed block by block without a graph."""
     feats = _t(feats)
     b, n, _ = feats.shape
     chunk = chunk or chunk_rows(cfg, b, n, _width(cfg, n, neighbors, adj), feats.element_size())
     with torch.no_grad():
-        outs = [layer(P, cfg, feats, coors, edges, mask, adj, box, neighbors, None, ok, rows=r) for r in _blocks(n, chunk)]
+        outs = [layer(P, cfg, feats, coors, edges, mask, adj, box, neighbors, None, ok, rows=r, drop=drop)
+                for r in _blocks(n, chunk)]
     return torch.cat([o[0] for o in outs], 1), torch.cat([o[1] for o in outs], 1)
 
 
 def layer_grads_chunked(P, cfg, feats, coors, gf, gx, edges=None, mask=None, adj=None, box=None, neighbors=None,
-                        ok=None, slot_edges=None, chunk=None, leaves=None):
+                        ok=None, slot_edges=None, chunk=None, leaves=None, drop=None):
     """Gradients of sum(fo * gf) + sum(xo * gx) through `layer`, forward + backward one row block at a time, in the type
     and on the device of `feats` -> {'in.feats', 'in.coors', ['in.edges'], 'p.<key>'}.  `leaves`: existing leaf
     tensors (feats, coors, params) to accumulate into instead of fresh ones."""
@@ -244,7 +260,7 @@ def layer_grads_chunked(P, cfg, feats, coors, gf, gx, edges=None, mask=None, adj
     with torch.enable_grad():
         for r0, r1 in _blocks(n, chunk):
             fo, xo = layer(LP, cfg, lf, lx, None if slot_edges is not None else e, mask, adj, box, neighbors,
-                           e if slot_edges is not None else None, ok, rows=(r0, r1))
+                           e if slot_edges is not None else None, ok, rows=(r0, r1), drop=drop)
             ((fo * gf[:, r0:r1]).sum() + (xo * gx[:, r0:r1]).sum()).backward()
     out = {"in.feats": lf.grad, "in.coors": lx.grad}
     if le is not None:
@@ -324,8 +340,9 @@ def _leaves(P, feats, edges, coors, ref):
 
 
 def network(P, ncfg, feats, coors, adj_mat=None, edges=None, mask=None, box=None, chunk=None, dtype=torch.float64,
-            device="cpu"):
-    """`EGNN_Network.forward` (no global attention) -> (feats, coors, [(h, x) input of every layer]), without a graph."""
+            device="cpu", drop=None):
+    """`EGNN_Network.forward` (no global attention) -> (feats, coors, [(h, x) input of every layer]), without a graph.
+    `drop`: one `layer` dropout per layer (a list), or None."""
     ref = torch.zeros((), dtype=dtype, device=device)
     LP, f, e, x = _leaves(P, feats, edges, coors, ref)
     with torch.no_grad():
@@ -333,13 +350,14 @@ def network(P, ncfg, feats, coors, adj_mat=None, edges=None, mask=None, box=None
         E, adj = _edge_input(LP, ncfg, e, adj_mat, h.shape[0], ref.device)
         states = [(h, x)]
         for l in range(ncfg["depth"]):
-            h, x = layer_forward(_layer_params(LP, l), ncfg["layer"], h, x, E, mask, adj, box, chunk=chunk)
+            h, x = layer_forward(_layer_params(LP, l), ncfg["layer"], h, x, E, mask, adj, box, chunk=chunk,
+                                 drop=None if drop is None else drop[l])
             states.append((h, x))
     return h, x, states[:-1]
 
 
 def network_grads(P, ncfg, feats, coors, gf, gx, adj_mat=None, edges=None, mask=None, box=None, chunk=None,
-                  dtype=torch.float64, device="cpu"):
+                  dtype=torch.float64, device="cpu", drop=None):
     """Gradients of sum(fo * gf) + sum(xo * gx) through `network`: the layers' inputs by a forward without a graph,
     then each layer in reverse, block by block, then the embeddings -> {'in.coors', ['in.feats'], ['in.edges'],
     'p.<state-dict key>'}."""
@@ -351,7 +369,8 @@ def network_grads(P, ncfg, feats, coors, gf, gx, adj_mat=None, edges=None, mask=
     E, adj = _edge_input(LP, ncfg, e, adj_mat, h.shape[0], ref.device)
     states = [(h, x.detach())]
     for l in range(ncfg["depth"] - 1):
-        states.append(layer_forward(_layer_params(LP, l), cfg, *states[-1], E, mask, adj, box, chunk=chunk))
+        states.append(layer_forward(_layer_params(LP, l), cfg, *states[-1], E, mask, adj, box, chunk=chunk,
+                                    drop=None if drop is None else drop[l]))
     gh, gxx = _like(gf, ref), _like(gx, ref)
     b, n = gh.shape[:2]
     with torch.enable_grad():
@@ -361,7 +380,7 @@ def network_grads(P, ncfg, feats, coors, gf, gx, adj_mat=None, edges=None, mask=
             lp = _layer_params(LP, l)
             c = chunk or chunk_rows(cfg, b, n, _width(cfg, n, None, adj), ref.element_size())
             for r0, r1 in _blocks(n, c):
-                fo, xo = layer(lp, cfg, hin, xin, E, mask, adj, box, rows=(r0, r1))
+                fo, xo = layer(lp, cfg, hin, xin, E, mask, adj, box, rows=(r0, r1), drop=None if drop is None else drop[l])
                 ((fo * gh[:, r0:r1]).sum() + (xo * gxx[:, r0:r1]).sum()).backward()
             gh, gxx = hin.grad, xin.grad
         h0 = _embed(LP, ncfg, f, ref.device)
