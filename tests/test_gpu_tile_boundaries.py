@@ -78,8 +78,20 @@ def _gemm_acc_splits(Mr, Nc, K, sms=H100_SMS):
     return math.ceil(K / kper), kper
 
 
-def geometry(spec, k=0, C=3):
-    """The tile counts a case runs with.  k > 0: neighbour lists of width k."""
+SIMT_SMEM_MAX = 220 * 1024     # simt_host.cuh: the dense edge step falls back to one row per thread above it
+
+
+def pair_tiled_smem_bytes(g, PP, itemsize):
+    """Dynamic shared memory of pair_dense_tiled_kernel at PP rows per thread (simt_kernels.cuh)."""
+    MP, Q, m = g["MP"], g["Q"], g["m"]
+    n = 64 * MP + Q * 64 + 64 * 33 + (PP * Q * 128 if Q > 1 else 0) + 4 * m * MP + 8 * m + 2 * MP + 4
+    if PP > 1:
+        n += 4 * PP * (MP + 8 + 4)
+    return _round_up(n * itemsize, 16) + 16
+
+
+def geometry(spec, k=0, C=3, rows=None):
+    """The tile counts a case runs with.  k > 0: neighbour lists of width k.  rows: a row block (r0, r1)."""
     if spec["kind"] == NW:
         ncfg = cases.O.network_cfg(**spec["cfg"])
         cfg = ncfg["layer"]
@@ -108,6 +120,15 @@ def geometry(spec, k=0, C=3):
         g.update(TS=TS, slot_passes=math.ceil(k / TS), partial_slots=k % TS != 0,
                  bwd2_steps=math.ceil(k / 32), partial_step=k % 32 != 0, partial_list_rows=N % 16 != 0,
                  QR=1 if (Q == 1 and not labels) else (8 if Q <= 8 else 0))
+    # launch decisions: rows per thread of the dense forward per element size (launch_pair_dense), the split hidden
+    # axis (simt_hsplit), and bwd3's grid over the rows of the call (TS lanes per row, 128 threads per CTA)
+    r0, r1 = rows or (0, N)
+    g["PP"] = {es: 1 if (MP == 32 and es == 8) or pair_tiled_smem_bytes(g, 2, es) > SIMT_SMEM_MAX else 2
+               for es in (8, 4)}
+    g["hsplit"] = min(32, math.ceil(Hp / 64)) if (k == 0 and B * N * N <= 4096 and Hp >= 512 and rows is None) else 1
+    per_cta = 128 // (g["TS"] if k else 32)
+    g.update(rows=r1 - r0, bwd3_rows_per_cta=per_cta, bwd3_ctas=math.ceil((r1 - r0) / per_cta),
+             bwd3_partial=(r1 - r0) % per_cta != 0)
     return g
 
 
@@ -222,12 +243,13 @@ class _LibWithoutForward:
         return getattr(self._lib, name)
 
 
-def _assert_training_forward_rejected(case, dtype, monkeypatch):
+def _assert_training_forward_rejected(case, dtype, monkeypatch, run=None):
+    """`run`: the training step to try (default: util.module_grads of the case)."""
     from egnn_pytorch_b200 import _native as nat
     real = nat.load()
     monkeypatch.setattr(nat, "load", lambda: _LibWithoutForward(real))
     with pytest.raises(RuntimeError, match="egnn_layer_backward_workspace_bytes"):
-        util.module_grads(case, dtype)
+        (run or (lambda: util.module_grads(case, dtype)))()
 
 
 @pytest.mark.gpu
