@@ -2,7 +2,7 @@
 tests/torch_reference.py run on the device in float64.
 
 The small-graph gradient tests never reach the schedule branches that only large graphs take (mirrored in `geometry`
-and held by test_table_covers_every_size_boundary, with H100_SMS = 132):
+through tests/launch_geometry.py and held by test_table_covers_every_size_boundary, with H100_SMS = 132):
   gemm_acc   one CTA over all of K (tiles >= 2 SMs: g_h += gA W1_i at c2) and large splits with a partial last one
              (dWn2 at c2: K = 4096 in 3 splits of 1376)
   dsilu_mul  its grid-stride loop (the grid stops at 2048 CTAs: more than 524,288 elements)
@@ -24,7 +24,6 @@ Gates (in.feats / in.coors compare grad - cotangent: the identity path is copied
   exact  dense edge gradients are 0 outside the selected slots and on masked pairs; every gradient is finite and has
          its parameter's type
 Measured on an H100 80GB HBM3 (700 W power limit): see DESIGN.md section 8."""
-import math
 import time
 
 import numpy as np
@@ -32,6 +31,7 @@ import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 import torch_reference as TR
 import util
 from test_gpu_knn_select import ref_select
@@ -64,49 +64,23 @@ SIZE_CASES = {
 C4_BOX = 16.0                # 4096 nodes in [0, 16)^3: about one per unit volume, 32 neighbours within ~2
 
 
-# ------------------------------------------------------------------ launch geometry (mirrors egnn_backward_impl.cuh)
-
-H100_SMS = 132
-BW2_TH, BW2_ROWS, DSILU_CTAS = 128, 32, 2048
-
-
-def _gemm_acc(Mr, Nc, K, sms=H100_SMS):
-    """(splits, K per split, K of the last split) of launch_gemm_acc."""
-    tiles = math.ceil(Mr / 64) * math.ceil(Nc / 64)
-    splits = max(1, min(math.ceil(2 * sms / tiles), math.ceil(K / 64)))
-    kper = -(-math.ceil(K / splits) // 16) * 16
-    splits = math.ceil(K / kper)
-    return splits, kper, K - (splits - 1) * kper
+# ------------------------------------------------------------------ launch geometry (tests/launch_geometry.py)
 
 
 def geometry(name, dt="fp64"):
     spec = SIZE_CASES[name]
-    if spec["kind"] == NW:
-        ncfg = cases.O.network_cfg(**spec["cfg"])
-        cfg, labels = ncfg["layer"], (ncfg["num_adj_degrees"] + 1 if ncfg["num_adj_degrees"] else 0)
-    else:
-        cfg, labels = cases.O.layer_cfg(**spec["cfg"]), 0
-    B, N, dim, m = spec["B"], spec["N"], cfg["dim"], cfg["m_dim"]
-    E = cases.O.edge_input_dim(cfg)
-    H = 2 * E
-    Hp = -(-H // 8) * 8
-    Q = E - 2 * dim - (ncfg["adj_dim"] if labels else 0)
-    M = B * N
-    k = 9 if cfg["only_sparse_neighbors"] else cfg["num_nearest_neighbors"]     # chain, 3 degrees: |i - j| <= 4
-    J = k if k else N
-    es = 8 if dt == "fp64" else 4
-    g = dict(Hp=Hp, Q=Q, labels=labels, k=k, M=M,
-             gemm={"g_h_gA": _gemm_acc(M, dim, H), "g_h_gB": _gemm_acc(M, dim, H), "dW1_i": _gemm_acc(H, dim, M),
-                   "dWn2": _gemm_acc(dim, 2 * dim, M), "ga": _gemm_acc(M, 2 * dim, dim),
-                   "dWn1": _gemm_acc(2 * dim, dim + m, M), "g_node_in": _gemm_acc(M, dim + m, 2 * dim)},
-             dsilu_strides=math.ceil(M * 2 * dim / (min(DSILU_CTAS, math.ceil(M * 2 * dim / 256)) * 256)),
-             bwd2_ch_ctas=math.ceil(Hp / BW2_TH), bwd2_last_ch=Hp - (math.ceil(Hp / BW2_TH) - 1) * BW2_TH,
-             pre2_saved=B * N * J * (16 if m <= 16 else 32) * es <= 1024 * 2 ** 20)
-    if k:
-        g.update(TS=min(32, 1 << (k - 1).bit_length()), bwd2_row_ctas=math.ceil(N / 16))
-    else:
-        g.update(bwd2_row_ctas=math.ceil(N / BW2_ROWS), bwd2_last_rows=N - (math.ceil(N / BW2_ROWS) - 1) * BW2_ROWS,
-                 generic_bwd2=Q > 1)
+    layer = LG.layer_dims(spec["kind"], spec["cfg"])[0]
+    B, N, dim, m = spec["B"], spec["N"], layer["dim"], layer["m_dim"]
+    k = 9 if layer["only_sparse_neighbors"] else layer["num_nearest_neighbors"]     # chain, 3 degrees: |i - j| <= 4
+    g = LG.simt_layer(spec["kind"], spec["cfg"], B, N, k=k)
+    M, H, acc = B * N, 2 * g["E"], LG.launch_gemm_acc
+    g.update(M=M, gemm={"g_h_gA": acc(M, dim, H), "g_h_gB": acc(M, dim, H), "dW1_i": acc(H, dim, M),
+                        "dWn2": acc(dim, 2 * dim, M), "ga": acc(M, 2 * dim, dim), "dWn1": acc(2 * dim, dim + m, M),
+                        "g_node_in": acc(M, dim + m, 2 * dim)},
+             dsilu_strides=LG.dsilu_strides(M * 2 * dim), bwd2_last_ch=g["Hp"] - (g["bwd2_ch_ctas"] - 1) * LG.BW2_TH,
+             pre2_saved=LG.pre2_saved(B, N, k or N, m, 8 if dt == "fp64" else 4))
+    if not k:
+        g.update(bwd2_last_rows=N - (g["bwd2_row_ctas"] - 1) * LG.BW2_ROWS, generic_bwd2=g["Q"] > 1)
     return g
 
 
@@ -119,7 +93,7 @@ def test_table_covers_every_size_boundary():
     assert (c2["bwd2_ch_ctas"], c2["bwd2_last_ch"], c2["bwd2_row_ctas"]) == (17, 8, 32) and not c2["generic_bwd2"]
     assert c2["pre2_saved"] and geometry("c2", "fp32")["pre2_saved"]               # c2_recompute sets the budget to 0
     gen = geometry("dense_generic")
-    assert gen["generic_bwd2"] and 0 < gen["bwd2_last_rows"] < BW2_ROWS and gen["bwd2_ch_ctas"] > 1
+    assert gen["generic_bwd2"] and 0 < gen["bwd2_last_rows"] < LG.BW2_ROWS and gen["bwd2_ch_ctas"] > 1
     c4 = geometry("c4")
     assert c4["TS"] == 32 and c4["bwd2_ch_ctas"] == 9 and c4["dsilu_strides"] > 1
     c5 = geometry("c5")
@@ -133,17 +107,8 @@ def test_table_covers_every_size_boundary():
 @pytest.fixture(autouse=True)
 def _no_tf32():
     """The fp32 restatement measures fp32 arithmetic: no TF32 in its matmuls."""
-    prev = torch.backends.cuda.matmul.allow_tf32, torch.get_float32_matmul_precision()
-    torch.backends.cuda.matmul.allow_tf32 = False
-    torch.set_float32_matmul_precision("highest")
-    yield
-    torch.backends.cuda.matmul.allow_tf32 = prev[0]
-    torch.set_float32_matmul_precision(prev[1])
-
-
-def _rounded(a, dtype):
-    return a if dtype == torch.float64 or not np.issubdtype(np.asarray(a).dtype, np.floating) else \
-        np.asarray(a, np.float32).astype(np.float64)
+    with util.no_tf32():
+        yield
 
 
 def build(name, dt, depth=None):
@@ -159,10 +124,10 @@ def build(name, dt, depth=None):
     if name == "c4_box":
         case["inputs"]["coors"] = rs.uniform(0.0, C4_BOX, case["inputs"]["coors"].shape)
         box = np.full(3, C4_BOX)
-    case["params"] = {k: _rounded(v, dtype) for k, v in case["params"].items()}
-    case["inputs"] = {k: _rounded(v, dtype) for k, v in case["inputs"].items()}
+    case["params"] = {k: util.rounded(v, dtype) for k, v in case["params"].items()}
+    case["inputs"] = {k: util.rounded(v, dtype) for k, v in case["inputs"].items()}
     gf, gx = cases.upstream_grads(case)
-    case["grads"] = (_rounded(gf, dtype), _rounded(gx, dtype))
+    case["grads"] = (util.rounded(gf, dtype), util.rounded(gx, dtype))
     case["box"] = box
     cfg = case["cfg"] if spec["kind"] == L else None
     if cfg is not None and cfg["num_nearest_neighbors"] > 0:

@@ -42,6 +42,7 @@ import torch
 
 import cases
 import dropout_reference as DR
+import launch_geometry as LG
 import test_gpu_backward_at_size as BAS
 import test_triclinic as TRI
 import torch_reference as TR
@@ -51,7 +52,6 @@ L, NW = "layer", "network"
 DT = {"fp64": torch.float64, "fp32": torch.float32}
 TAU64 = 1e-12
 SEED = 2024                  # torch.manual_seed before every training call: the module draws its dropout seeds from it
-H100_SMS = 132
 
 # spec: a cases.py spec (cfg carries dropout) plus
 #   lists  "knn" (the layer's own select), "edge" (caller lists, neighbors=), "slot" (caller lists, neighbor_edges=)
@@ -109,13 +109,11 @@ CASES = {
 FP32_RATIO_WIDE = {"skinny4_dim1056": 16.0}
 
 
-# ------------------------------------------------------------------ launch geometry (mirrors simt_host.cuh / egnn_api.cu)
+# ------------------------------------------------------------------ launch geometry (tests/launch_geometry.py)
 
 
 def _layer_cfg(spec):
-    if spec["kind"] == NW:
-        return cases.O.network_cfg(**spec["cfg"])["layer"]
-    return cases.O.layer_cfg(**spec["cfg"])
+    return LG.layer_dims(spec["kind"], spec["cfg"])[0]
 
 
 def list_width(spec):
@@ -128,40 +126,21 @@ def list_width(spec):
     return cfg["num_nearest_neighbors"]
 
 
-def node_gemm(Mr, K, Nout, es, sms):
-    """The node_mlp.0 launch of launch_gemm: ('skinny', columns per warp) or ('tiled', partial 64 x 64 tiles)."""
-    V = 16 // es
-    if Mr <= 16 and 16 * ((K + V - 1) // V * V) * es <= 96 * 1024:
-        return "skinny", 4 if Nout >= sms * 16 else (2 if Nout >= sms * 8 else 1)
-    return "tiled", Mr % 64 != 0 or Nout % 64 != 0
-
-
-def geometry(name, dt, sms=H100_SMS):
+def geometry(name, dt, sms=LG.H100_SMS):
+    """The case's SIMT launch (launch_geometry.simt_layer) at its element size, and node_mlp.0's GEMM (launch_gemm)."""
     spec = CASES[name]
     cfg = _layer_cfg(spec)
     dim, m = cfg["dim"], cfg["m_dim"]
-    E = cases.O.edge_input_dim(cfg)
-    H = 2 * E
-    Hp = DR.round_up(H, 8)
-    MP = 16 if m <= 16 else 32
     B, N = spec["B"], spec["N"]
     r0, r1 = spec.get("rows", (0, N))
-    R = r1 - r0
     es = 8 if dt == "fp64" else 4
     k = list_width(spec)
-    g = dict(B=B, N=N, R=R, H=H, Hp=Hp, MP=MP, k=k, p=cfg["dropout"], rows=r0 > 0 or r1 < N,
-             node=node_gemm(B * R, dim + m, 2 * dim, es, sms))
+    g = LG.simt_layer(spec["kind"], spec["cfg"], B, N, k=k, rows=spec.get("rows"))
+    R, PP = g["rows"], g["PP"][es]
+    g.update(B=B, R=R, H=2 * g["E"], p=cfg["dropout"], rows=r0 > 0 or r1 < N,
+             node=LG.launch_gemm(B * R, dim + m, 2 * dim, es, sms), PP=PP)
     if k == 0:
-        PP = 1 if (MP == 32 and dt == "fp64") else 2
-        whole = R == N
-        g.update(PP=PP, row_ctas=math.ceil(R / (4 * PP)), partial_row_cta=R % (4 * PP) != 0,
-                 chunks=math.ceil(Hp / 64), partial_chunk=Hp % 64 != 0,
-                 hsplit=min(32, math.ceil(Hp / 64)) if (B * N * N <= 4096 and Hp >= 512 and whole) else 1,
-                 bwd2_ch_ctas=math.ceil(Hp / 128), partial_ch_cta=Hp % 128 != 0,
-                 bwd2_row_ctas=math.ceil(R / 32), partial_bwd2_rows=R % 32 != 0)
-    else:
-        TS = min(32, 1 << (k - 1).bit_length())
-        g.update(TS=TS, slot_passes=math.ceil(k / TS), bwd2_steps=math.ceil(k / 32))
+        g.update(row_ctas=LG.ceil_div(R, 4 * PP), partial_row_cta=R % (4 * PP) != 0, partial_bwd2_rows=g["partial_rows"])
     return g
 
 
@@ -248,16 +227,16 @@ def build(name, dt):
             cell = np.diag(np.diag(cell))
         case["inputs"]["coors"] = TRI.cell_coors(rs, B, N, cell, dtype=torch.float32)
         out["box" if spec["lattice"] == "box" else "cell"] = np.diag(cell).copy() if spec["lattice"] == "box" else cell
-    case["params"] = {k: BAS._rounded(v, dtype) for k, v in case["params"].items()}
-    case["inputs"] = {k: BAS._rounded(v, dtype) for k, v in case["inputs"].items()}
+    case["params"] = {k: util.rounded(v, dtype) for k, v in case["params"].items()}
+    case["inputs"] = {k: util.rounded(v, dtype) for k, v in case["inputs"].items()}
     if out["slot_edges"] is not None:
-        out["slot_edges"] = BAS._rounded(out["slot_edges"], dtype)
+        out["slot_edges"] = util.rounded(out["slot_edges"], dtype)
     gf, gx = cases.upstream_grads(case)
     if spec.get("rows"):
         r0, r1 = spec["rows"]
         keep = ((np.arange(N) >= r0) & (np.arange(N) < r1))[None, :, None]
         gf, gx = gf * keep, gx * keep
-    out["grads"] = (BAS._rounded(gf, dtype), BAS._rounded(gx, dtype))
+    out["grads"] = (util.rounded(gf, dtype), util.rounded(gx, dtype))
     if spec.get("lists") == "knn":
         out["sel"] = _select(case, out)
     return out
@@ -305,16 +284,6 @@ def drops(name, wrong=None, order=None):
     return [DR.Drop(spec["cfg"]["dropout"], s, wrong) for s in seeds]
 
 
-@contextlib.contextmanager
-def _no_tf32():
-    prev = torch.backends.cuda.matmul.allow_tf32
-    torch.backends.cuda.matmul.allow_tf32 = False
-    try:
-        yield
-    finally:
-        torch.backends.cuda.matmul.allow_tf32 = prev
-
-
 def reference(name, dt, dtype=torch.float64, device="cpu", drop=None):
     """Outputs and gradients of the restatement with the kernels' masks -> {name: float64 tensor}: 'out.feats' /
     'out.coors' (the outputs of the case's rows), 'in.*' and 'p.<state-dict key>'."""
@@ -323,7 +292,7 @@ def reference(name, dt, dtype=torch.float64, device="cpu", drop=None):
     ins, cfg = case["inputs"], case.get("cfg")
     drop = drops(name) if drop is None else drop
     gf, gx = (torch.as_tensor(g).to(device, dtype) for g in b["grads"])
-    with torch.enable_grad(), _no_tf32():
+    with torch.enable_grad(), util.no_tf32():
         if spec["kind"] == NW:
             g = TR.network_grads(case["params"], case["ncfg"], ins["feats"], ins["coors"], gf, gx, ins.get("adj_mat"),
                                  None, ins.get("mask"), dtype=dtype, device=device, drop=drop)

@@ -50,9 +50,10 @@ import torch
 
 import cases
 import util
+from launch_geometry import H100_SMS
 from oracle import egnn_oracle as O
+from util import nat  # noqa: F401  (module-scoped fixture)
 
-H100_SMS = 132
 SKINNY_WARPS, SKINNY_SMEM = 4, 96 * 1024
 T_MAX = 32                     # ga_attn2_kernel's sc[32]; the module runs more tokens through PyTorch
 TOL_F32 = 2.5e-6
@@ -290,14 +291,6 @@ def test_shape_errors_raise_value_error_before_any_launch(x_shape, q_shape, m_sh
     mod = GlobalLinearAttention(dim=16, heads=2, dim_head=8)
     with pytest.raises(ValueError, match=match):
         mod(torch.randn(x_shape), torch.randn(q_shape), torch.ones(m_shape, dtype=torch.bool))
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from egnn_pytorch_b200 import build, _native
-    build.build()                     # nvcc cross-compiles sm_90a without a GPU
-    _native.load()
-    return _native
 
 
 def test_c_abi_return_codes_without_a_launch(nat):

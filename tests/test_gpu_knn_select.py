@@ -6,7 +6,7 @@ coordinates' type (fp32 for fp32 and bf16 layers, fp64 for fp64): per axis r = f
 stable argsort (NaN last, ties to the lower index) keeps k, and ok = rank <= T(valid_radius).  Lists and ok are compared
 exactly.  (The oracle's (rel**2).sum(-1) sums 8 axes pairwise, so its fp32 ranks can differ from the kernel's by an ulp.)
 
-The case table crosses the boundaries of launch_select, mirrored in `geometry` and held there by
+The case table crosses the boundaries of launch_select, mirrored in launch_geometry.py and held there by
 test_table_covers_every_boundary:
   warp select (k <= 32)  8 and 16 warps per CTA on both sides of the switch (B ceil(N/16) >= 2 SMs); 1, 2 and 3 staging
                          passes of SEL_JC = 1024 candidates; partial 64-candidate groups and partial last CTAs; the CDIM = 3
@@ -27,6 +27,7 @@ import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 
 DEV = "cuda"
 F32, F64 = "f32", "f64"
@@ -78,26 +79,6 @@ def ref_select(x, k, valid_radius, rows=None, mask=None, adj=None, box=None, chu
         idx.append(o)
         ok.append(v <= T(valid_radius))
     return np.concatenate(idx, 1), np.concatenate(ok, 1)
-
-
-# ------------------------------------------------------------------ launch geometry (mirrors launch_select)
-
-H100_SMS = 132
-SEL_JC, SEL_WARPS_MAX, SORT_SMEM_MAX = 1024, 16, 200 * 1024
-
-
-def geometry(B, N, C, k, dt, sms=H100_SMS):
-    esz = 8 if dt == F64 else 4
-    if k <= 32:
-        warps = 16 if B * -(-N // 16) >= 2 * sms else 8
-        passes = -(-N // SEL_JC)
-        tail = N - (passes - 1) * SEL_JC                      # candidates in the last staging pass
-        return dict(kernel="warp", warps=warps, passes=passes, cdim=3 if C == 3 else 0, tail64=tail % 64,
-                    last_cta_rows=N - (-(-N // warps) - 1) * warps,
-                    smem=C * SEL_JC * esz + SEL_JC + warps * 64 * (esz + 4) + 64)
-    npad = 1 << max(0, (N - 1).bit_length())
-    smem = npad * (esz + 4)
-    return dict(kernel="sort", npad=npad, smem=smem, supported=smem <= SORT_SMEM_MAX)
 
 
 # ------------------------------------------------------------------ the case table
@@ -298,7 +279,7 @@ def test_reference_orders_non_finite_like_a_stable_torch_sort():
 
 
 def test_table_covers_every_boundary():
-    geo = {name: geometry(s["B"], s["N"], s["C"], s["k"], s["dt"]) for name, s in CASES.items()}
+    geo = {name: LG.launch_select(s["B"], s["N"], s["C"], s["k"], 8 if s["dt"] == F64 else 4) for name, s in CASES.items()}
     warp = {n: g for n, g in geo.items() if g["kernel"] == "warp"}
     sort = {n: g for n, g in geo.items() if g["kernel"] == "sort"}
     assert {g["warps"] for g in warp.values()} == {8, 16}
@@ -327,7 +308,7 @@ def test_table_covers_every_boundary():
     assert {g["npad"] for g in sort.values()} >= {64, 128, 256, 512, 1024, 8192, 16384}
     assert all(g["supported"] for g in sort.values())
     assert {CASES[n]["dt"] for n in sort if CASES[n]["N"] == 16384} == {F32, F64}
-    assert not geometry(1, 16385, 3, 33, F32)["supported"] and not geometry(1, 16385, 3, 33, F64)["supported"]
+    assert not LG.launch_select(1, 16385, 3, 33, 4)["supported"] and not LG.launch_select(1, 16385, 3, 33, 8)["supported"]
     # inputs
     coords = {s["coords"] for s in CASES.values()}
     assert coords >= {"rand", "dyadic", "line", "zero", "lattice"}

@@ -8,7 +8,7 @@ inf in another, C = 5 on the generic path; cells: tilt, tilt09, per_graph with B
 plus rows the non-periodic tables do not need: the split hidden axis (dim 512, N 16 and dim 128, B N^2 = 4096), the
 largest fp64 configurations that still train (m_dim 30, and 23 with soft edges), row blocks that end inside a dense
 and a list CTA, and networks with 4 and 16 degree-label rows.  test_table_covers_every_lattice_boundary recomputes
-from the specs, through test_gpu_tile_boundaries.geometry, that each boundary is reached under a box and under a cell.
+from the specs, through launch_geometry.simt_layer, that each boundary is reached under a box and under a cell.
 
 Inputs: coordinates from test_triclinic.cell_coors (a box is a diagonal cell), rounded to the compute type, so every
 wrap decision is at least 1e-3 from 1/2; each case wraps at least 20 % of the pairs it compares.
@@ -29,7 +29,7 @@ CPU: the coverage tables, the input margins, the Fraction pin of the select refe
 its fp64 gate under a wrong lattice (no lattice, the next graph's, a cell's diagonal, the axes wrapped first to last,
 floor for rint).
 GPU: the comparisons above, fp64 training rejected over the shared-memory budget under a lattice, row blocks, and the
-launched kernels' template arguments and grids against `geometry` under torch.profiler.
+launched kernels' template arguments and grids against launch_geometry.simt_layer under torch.profiler.
 
 Worst measured value per gate, on an NVIDIA H100 80GB HBM3 at its 700 W power limit (error over max(1, scale)):
   forward            fp64 1.8e-15 (net_labels4_tilt09); fp32 7.3e-7 (net_labels4_cubic)
@@ -53,13 +53,14 @@ import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 import tc_reference as T
 import test_triclinic as TRI
 import torch_reference as R
 import util
 import test_edge_list
 from test_edge_list import EDGE_CASES
-from test_gpu_tile_boundaries import FP64_BACKWARD_REJECTED, TILE_CASES, _assert_training_forward_rejected, geometry
+from test_gpu_tile_boundaries import FP64_BACKWARD_REJECTED, TILE_CASES, _assert_training_forward_rejected
 from test_lattice_grad import check32, check64
 
 L, NW = "layer", "network"
@@ -197,7 +198,7 @@ def build_spec(full, dtype=torch.float64):
     B, N, Cd = spec["B"], spec["N"], spec.get("C", 3)
     rs = np.random.RandomState(spec["seed"] + 17)
     lat, cell = make_lattice(full["lat"], B, Cd, rs)
-    lat, cell = TRI.rounded(lat, cdt(dtype)), TRI.rounded(cell, cdt(dtype))
+    lat, cell = util.rounded(lat, cdt(dtype)), util.rounded(cell, cdt(dtype))
     case["inputs"]["coors"] = TRI.cell_coors(rs, B, N, cell, dtype=cdt(dtype))
     for _ in range(20):           # a network's later layers wrap the coordinates the earlier ones moved
         if case["kind"] != NW or _layer_margin(case, lat, cell, lattice_kind(full)) > 1e-4:
@@ -301,7 +302,8 @@ def _images(x, cell):
 
 def case_geometry(name, rows=None):
     s = CASES[name]
-    return dict(geometry(s, k=s.get("k", 0), C=s.get("C", 3), rows=rows), kind=kind_of(name), lat=s["lat"])
+    return dict(LG.simt_layer(s["kind"], s["cfg"], s["B"], s["N"], k=s.get("k", 0), C=s.get("C", 3), rows=rows),
+                kind=kind_of(name), lat=s["lat"])
 
 
 def test_table_covers_every_lattice_boundary():
@@ -378,7 +380,8 @@ def test_table_covers_every_lattice_boundary():
     # every lattice kind is in the table, and the boxes include the generic C = 5 path
     assert {s["lat"] for s in CASES.values()} == set(BOXES) | set(CELLS)
     assert any(g["C"] == 5 and g["k"] > 0 for g in every.values())
-    assert FP64_REJECTED and all(geometry(TILE_CASES[r])["m"] for r in FP64_BACKWARD_REJECTED)
+    assert FP64_REJECTED and all(LG.simt_layer(s["kind"], s["cfg"], s["B"], s["N"])["m"]
+                             for s in (TILE_CASES[r] for r in FP64_BACKWARD_REJECTED))
     # the q77 shape infers in fp64 at one row per thread
     assert every["q77_tilt"]["PP"][8] == 1 and every["q77_tilt"]["PP"][4] == 2
     # a row range turns the split hidden axis off, so no row-block case uses a split shape
@@ -670,8 +673,8 @@ PROFILED = ["mdim30_tilt", "mdim20_soft_cubic", "q77_tilt", "hsplit512_tilt", "h
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", PROFILED)
 def test_cases_launch_what_the_table_claims(name):
-    """The demangled names of the launched kernels agree with `geometry`: PBC, MP, PP, BLK and LAT, the phase-1 grid of
-    the split hidden axis, and bwd3's grid."""
+    """The demangled names of the launched kernels agree with launch_geometry.simt_layer: PBC, MP, PP, BLK and LAT, the
+    phase-1 grid of the split hidden axis, and bwd3's grid."""
     g = case_geometry(name)
     pbc = "1" if g["kind"] == "box" else "2"
     for dt in ("fp64", "fp32"):
@@ -837,7 +840,6 @@ def test_cell_ranks_are_pinned_to_exact_arithmetic(name, dt):
 @pytest.mark.parametrize("name", list(SELECT))
 def test_select_cases_wrap_and_reach_their_boundaries(name):
     """At least a fifth of each graph's selected pairs wrap; the launch geometry is the one the row names."""
-    import test_gpu_knn_select as KS
     B, N, Cd, k, kind, masked = SELECT[name]
     for dt in SELECT_DTYPES[name]:
         x, cell, _, mask, vr = select_inputs(name, dt)
@@ -845,7 +847,7 @@ def test_select_cases_wrap_and_reach_their_boundaries(name):
         moved = _images(x.astype(np.float64), cell.astype(np.float64))
         sel = np.take_along_axis(moved, idx, -1)
         assert sel.mean() >= 0.2, (name, dt, sel.mean())
-        g = KS.geometry(B, N, Cd, k, KS.F64 if dt == "fp64" else KS.F32)
+        g = LG.launch_select(B, N, Cd, k, 8 if dt == "fp64" else 4)
         if k <= 32:
             assert g["kernel"] == "warp" and (g["cdim"] == 3) == (Cd == 3)
         else:
@@ -854,12 +856,11 @@ def test_select_cases_wrap_and_reach_their_boundaries(name):
 
 def test_select_table_covers_the_schedule_boundaries():
     """Each schedule boundary of launch_select under a cell in fp32 and fp64, and under a box in fp64."""
-    import test_gpu_knn_select as KS
     got = set()
     for name, (B, N, Cd, k, kind, masked) in SELECT.items():
         lk = "box" if kind in BOXES else "cell"
         for dt in SELECT_DTYPES[name]:
-            g = KS.geometry(B, N, Cd, k, KS.F64 if dt == "fp64" else KS.F32)
+            g = LG.launch_select(B, N, Cd, k, 8 if dt == "fp64" else 4)
             m = " masked" if masked else ""
             if g["kernel"] == "warp":
                 tags = [f"warp{g['warps']} passes{g['passes']} {'cdim3' if g['cdim'] == 3 else 'generic'}{m}"]

@@ -8,7 +8,7 @@ workspace and share their offset with the region after them, so a stale read or 
 without faulting: the poisoned-scratch test fills every workspace with 0xFF bytes (NaN in every float type) first.
 
 Case tables (test_table_covers_every_boundary recomputes each boundary from the specs, through the launch mirrors
-`geometry` of test_gpu_tile_boundaries.py, test_gpu_tc_boundaries.py and test_gpu_tc_wide_lists.py):
+simt_layer and tc_layer of tests/launch_geometry.py):
   SIMT dense   PP = 2 and PP = 1 with a partial last 32-neighbour pass (N 33 / 70 / 97), the split hidden axis at 9 and
                32 CTAs, MP = 16 with a tail (m_dim 12) and MP = 32 (m_dim 20 / 24); soft edges, mean pooling over a
                mask, norm_feats (feats-only), CoorsNorm and clamp (coors-only)
@@ -43,6 +43,7 @@ import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 import test_gpu_dropout_reference as DRT
 import test_gpu_lattice_tile_boundaries as LTB
 import test_gpu_radius_select as RS
@@ -52,7 +53,7 @@ import test_triclinic as TRI
 import torch_reference as R
 import util
 from test_edge_list import EDGE_CASES
-from test_gpu_tile_boundaries import TILE_CASES, geometry
+from test_gpu_tile_boundaries import TILE_CASES
 from test_lattice_grad import check32, check64
 
 L, NW = "layer", "network"
@@ -264,7 +265,8 @@ def assert_identity(name, cfg, out, inp, rows=None):
 
 def case_geometry(name, rows=None):
     s = CASES[name]
-    return dict(geometry(s, k=s.get("k") or s["cfg"].get("num_nearest_neighbors", 0), C=s.get("C", 3), rows=rows),
+    k = s.get("k") or s["cfg"].get("num_nearest_neighbors", 0)
+    return dict(LG.simt_layer(s["kind"], s["cfg"], s["B"], s["N"], k=k, C=s.get("C", 3), rows=rows),
                 flag=flag_of(name), lat=kind_of(name), net=s["kind"] == NW, slot=bool(s.get("slot")),
                 select=bool(s["cfg"].get("num_nearest_neighbors")), radius="valid_radius" in s["cfg"],
                 masked=s.get("mask") not in (None, "none"), cfg=s["cfg"])
@@ -555,8 +557,8 @@ def _tc_flag(spec):
 
 def tc_missing():
     """The bf16 boundaries, for each flag (the node path: feats-only; the new C: each flag setting)."""
-    geo = {n: dict(TCB.geometry(s), flag=_tc_flag(s), holes=bool(s.get("holes"))) for n, s in TC_CASES.items()}
-    geo.update({n: dict(TCW.geometry(s), flag=_tc_flag(s), holes=bool(s.get("holes"))) for n, s in WIDE_CASES.items()})
+    geo = {n: dict(LG.tc_layer(s["kind"], s["cfg"], s["B"], s["N"], C=s.get("C", 3), k=s.get("k", 0), rows=s.get("rows")),
+                   flag=_tc_flag(s), holes=bool(s.get("holes"))) for n, s in {**TC_CASES, **WIDE_CASES}.items()}
     missing = [n for n, g in geo.items() if not g["supported"]]
     pair = lambda g: g["k"] == 0
     want = {

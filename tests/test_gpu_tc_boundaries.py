@@ -46,6 +46,7 @@ import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 import tc_reference as T
 import test_periodic as PER
 import test_triclinic as TRI
@@ -236,100 +237,21 @@ LATTICE_CASES.update({
 })
 CASES.update(LATTICE_CASES)
 
-# ------------------------------------------------------------------ launch geometry (mirrors the launch code)
-
-H100_SMS = 132
-TP_TI, TP_JB, TP_KC, TP_JSPLIT_MAX, TP_QMAX, TP_CMAX = 4, 256, 64, 8, 12, 8
-TP_EPI_FLOATS = 64 * 16 + 64 + 64 + 16 + 16 + 4
-TK_QE, TK_LEAN, TK_EDGES, TK_GEN = 4, 0, 1, 2
-SN_DIM_MAX, SN_TABLES_M_MAX = 64, 4096
-SMEM_MAX = 227 * 1024
+# ------------------------------------------------------------------ launch geometry (launch_geometry.tc_layer)
 
 
-def _ceil(a, b):
-    return -(-a // b)
-
-
-def _knn_smem(Hp, mode, Q, rows):
-    """tc_knn_smem_bytes (tc_knn.cuh)."""
-    wq_rows = 1 if mode == TK_LEAN else (1 + TK_QE if mode == TK_EDGES else Q)
-    n = Hp * 32 + rows * Hp * 4 + wq_rows * Hp * 4 + TP_EPI_FLOATS * 4
-    n += rows * Q * 32 * 4 if mode == TK_GEN else 0
-    return n + rows * 32 * 18 * 4 + 64 + 8 + 128
-
-
-def _pair_smem(Hp, Q, Qf, gen):
-    """tc_pair_smem_bytes (tc_pair.cuh)."""
-    PW, XC = (28, 8) if gen else (20, 4)
-    n = Hp * 32 + Q * Hp * 4 + 2 * TP_TI * Hp * 4 + TP_EPI_FLOATS * 4 + 2 * 8 * TP_TI * PW * 8 + 8 * 32 * 18 * 4
-    n += 2 * TP_TI * XC * 4 + 2 * TP_TI * 4 + 64 + (0 if gen else TP_TI * TP_JB * 4)
-    n += TP_TI * TP_JB * (Qf * 4 + (Q - Qf) * 2) if gen else 0
-    return n + 64 + 256
-
-
-def layer_shape(spec):
-    """(layer cfg, continuous edge channels, degree labels) of a case."""
-    if spec["kind"] == NW:
-        ncfg = O.network_cfg(**spec["cfg"])
-        cfg = ncfg["layer"]
-        nlab = ncfg["num_adj_degrees"] + 1 if ncfg["num_adj_degrees"] is not None and ncfg["adj_dim"] > 0 else 0
-        return cfg, cfg["edge_dim"] - (ncfg["adj_dim"] if nlab else 0), nlab, (ncfg["adj_dim"] if nlab else 0)
-    cfg = O.layer_cfg(**spec["cfg"])
-    return cfg, cfg["edge_dim"], 0, 0
-
-
-def geometry(spec, sms=H100_SMS):
-    """What the launch code (fast_path.cu) runs a case with."""
-    cfg, ed, nlab, label_dim = layer_shape(spec)
-    dim, F = cfg["dim"], cfg["fourier_features"]
-    B, N, C, k = spec["B"], spec["N"], spec.get("C", 3), spec.get("k", 0)
-    r0, r1 = spec.get("rows") or (0, N)
-    R = r1 - r0
-    E = 2 * dim + 1 + 2 * F + ed + label_dim
-    Hp = _ceil(2 * E, 16) * 16
-    QT = 1 + 2 * F + ed + nlab
-    nchunks = _ceil(Hp, TP_KC)
-    M = B * N
-    g = dict(dim=dim, B=B, N=N, C=C, k=k, R=R, Hp=Hp, Q=QT, F=F, edge_dim=ed, labels=nlab,
-             nsl_last=(Hp - (nchunks - 1) * TP_KC) // 16, rows_range=spec.get("rows") is not None,
-             tables="small" if dim <= SN_DIM_MAX and M <= SN_TABLES_M_MAX else "tc_gemm",
-             node="small" if dim <= SN_DIM_MAX else "tc_gemm", lattice=lattice_kind(spec),
-             per_graph_lattice=isinstance(spec.get("box", spec.get("cell")), str)
-             and spec.get("box", spec.get("cell")) == "per_graph" and B > 1)
-    if k == 0:
-        gen = not (C == 3 and QT == 1)
-        items = B * _ceil(R, TP_TI)
-        njb = _ceil(N, TP_JB)
-        js = 1
-        while js < TP_JSPLIT_MAX and items * js < 6 * sms and js * 2 <= njb:
-            js *= 2
-        n_items = items * js
-        grid = min(n_items, sms)
-        # a ring slot refilled with a row group of another graph (tc_pair.cuh: the last warpgroup stages item
-        # x + 2 grid into the slot of item x)
-        rg = _ceil(R, TP_TI)
-        graph = lambda item: item // js // rg
-        refill_other_graph = any(graph(x) != graph(x + 2 * grid) for x in range(n_items - 2 * grid))
-        g.update(kernel="tc_pair<generic>" if gen else "tc_pair<lean>", jsplit=js, items=n_items, grid=grid,
-                 refill_other_graph=refill_other_graph,
-                 laps=_ceil(n_items, grid), active_wgs=min(2, _ceil(N, 128)),
-                 last_rows_valid=R - TP_TI * (_ceil(R, TP_TI) - 1),
-                 supported=QT <= TP_QMAX and C <= TP_CMAX and _pair_smem(Hp, QT, 1 + 2 * F, gen) <= SMEM_MAX)
-    else:
-        mode = TK_LEAN if ed == 0 else (TK_EDGES if ed <= TK_QE else TK_GEN)
-        if not (C == 3 and F == 0 and nlab == 0):
-            mode = TK_GEN
-        rows = 8 if 2 * (_knn_smem(Hp, mode, QT, 8) + 1024) <= SMEM_MAX else 16
-        g.update(kernel=f"tc_knn<{['LEAN', 'EDGES', 'GEN'][mode]},{rows}>", mode=mode, ROWS=rows,
-                 last_rows_valid=R - rows * (_ceil(R, rows) - 1),
-                 supported=k <= 32 and (mode != TK_GEN or QT <= TP_QMAX) and _knn_smem(Hp, mode, QT, 16) <= SMEM_MAX)
-    return g
+def geometry(spec, sms=LG.H100_SMS):
+    """What the launch code (fast_path.cu) runs a case with, and the case's lattice."""
+    lat = spec.get("box", spec.get("cell"))
+    g = LG.tc_layer(spec["kind"], spec["cfg"], spec["B"], spec["N"], C=spec.get("C", 3), k=spec.get("k", 0),
+                    rows=spec.get("rows"), sms=sms)
+    return dict(g, lattice=lattice_kind(spec), per_graph_lattice=lat == "per_graph" and spec["B"] > 1)
 
 
 def test_table_covers_every_boundary():
     """Each boundary the table is meant to reach, recomputed from the specs: an edit to a shape that drops one fails
     here.  The SM count is the H100's 132, or the device's when one is present."""
-    sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else H100_SMS
+    sms = torch.cuda.get_device_properties(0).multi_processor_count if torch.cuda.is_available() else LG.H100_SMS
     geo = {n: geometry(s, sms) for n, s in CASES.items()}
     assert all(g["supported"] for g in geo.values()), [n for n, g in geo.items() if not g["supported"]]
     pair = {n: g for n, g in geo.items() if g["k"] == 0}
@@ -350,7 +272,7 @@ def test_table_covers_every_boundary():
         "dense last chunk 1 / 2 / 3 / 4 slabs": {g["nsl_last"] for g in pair.values()} >= {1, 2, 3, 4},
         "dense batches": any(g["B"] >= 2 and g["N"] % 128 != 0 for g in pair.values()),
         "dense lean and generic": {g["kernel"] for g in pair.values()} == {"tc_pair<lean>", "tc_pair<generic>"},
-        "dense Q 12, C 8, labels": any(g["Q"] == TP_QMAX and g["C"] == TP_CMAX and g["labels"] > 0
+        "dense Q 12, C 8, labels": any(g["Q"] == LG.TP_QMAX and g["C"] == LG.TP_CMAX and g["labels"] > 0
                                        for g in pair.values()),
         "dense fourier and edges": any(g["F"] > 0 and g["edge_dim"] > 0 for g in pair.values()),
         "knn k 1 / 8 / 31 / 32": {g["k"] for g in knn.values()} >= {1, 8, 31, 32},
@@ -393,7 +315,7 @@ def test_table_covers_every_boundary():
             "dense lean at Hp 2736": any(g["kernel"] == "tc_pair<lean>" and g["Hp"] == 2736 for g in lp.values()),
             "dense lean and generic": {g["kernel"] for g in lp.values()} == {"tc_pair<lean>", "tc_pair<generic>"},
             "network, Q 12 with labels, fourier and edges": any(
-                CASES[n]["kind"] == NW and g["Q"] == TP_QMAX and g["labels"] > 0 and g["F"] > 0 and g["edge_dim"] > 0
+                CASES[n]["kind"] == NW and g["Q"] == LG.TP_QMAX and g["labels"] > 0 and g["F"] > 0 and g["edge_dim"] > 0
                 for n, g in lp.items()),
             "knn k 1 (cell) / 8 / 31 / 32": {g["k"] for g in lk.values()} >= ({1} if lat == "cell" else set()) | {
                 8, 31, 32},
@@ -430,14 +352,6 @@ def test_table_covers_every_boundary():
 # ------------------------------------------------------------------ inputs and the reference
 
 
-def _bf16(a):
-    return torch.from_numpy(np.asarray(a, np.float64)).float().bfloat16().double().numpy()
-
-
-def _f32(a):
-    return np.asarray(a, np.float64).astype(np.float32).astype(np.float64)
-
-
 def lattice_kind(spec):
     return "box" if "box" in spec else ("cell" if "cell" in spec else None)
 
@@ -469,10 +383,10 @@ def lattice_inputs(spec, rs):
         box = np.asarray(box, np.float64)
         scale = np.where(np.isfinite(box) & (box > 0), box, 3.0)
         x = np.concatenate([PER.lattice_coors(rs, 1, N, C, sc) for sc in np.broadcast_to(scale, (B, C))])
-        return box, _f32(x)
+        return box, util.rounded(x, torch.float32)
     kind = spec["cell"]
     if kind == "hex_slab":
-        cell = _f32(TRI.make_cell(kind, B, rs))
+        cell = util.rounded(TRI.make_cell(kind, B, rs), torch.float32)
         return cell, TRI.cell_coors(rs, B, N, cell, dtype=torch.float32)
     Ls = [3.0, 3.25, 3.5][:C] if kind != "c2" else [3.0, 2.75]
     if kind == "tilt":
@@ -484,11 +398,11 @@ def lattice_inputs(spec, rs):
         cell = _grid_cell(rs, Ls, 0.5)
     else:                                                         # "per_graph"
         cell = np.stack([_grid_cell(rs, np.round(rs.uniform(2.8, 3.6, C) * 64) / 64, 0.5) for _ in range(B)])
-    cell = _f32(cell)
+    cell = util.rounded(cell, torch.float32)
     A = np.broadcast_to(cell, (B, C, C))
     s = (rs.randint(0, CELL_GRID, (B, N, C)) / CELL_GRID + rs.uniform(-1e-5, 1e-5, (B, N, C))
          + rs.randint(-2, 3, (B, N, C)))
-    return cell, _f32(np.einsum("bnk,bkd->bnd", s, A))
+    return cell, util.rounded(np.einsum("bnk,bkd->bnd", s, A), torch.float32)
 
 
 @functools.lru_cache(maxsize=None)
@@ -501,12 +415,12 @@ def build(name):
     ins = case["inputs"]
     if lat:
         case[lat], ins["coors"] = lattice_inputs(spec, np.random.RandomState(spec["seed"] + 11))
-    case["params"] = {k: _bf16(v) for k, v in case["params"].items()}
+    case["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in case["params"].items()}
     if np.issubdtype(np.asarray(ins["feats"]).dtype, np.floating):
-        ins["feats"] = _bf16(ins["feats"])
+        ins["feats"] = util.rounded(ins["feats"], torch.bfloat16)
     ins["coors"] = np.asarray(ins["coors"], np.float32).astype(np.float64)
     if ins.get("edges") is not None and np.issubdtype(np.asarray(ins["edges"]).dtype, np.floating):
-        ins["edges"] = _bf16(ins["edges"])
+        ins["edges"] = util.rounded(ins["edges"], torch.bfloat16)
     k = spec.get("k", 0)
     if k:
         B, N = spec["B"], spec["N"]
@@ -521,7 +435,7 @@ def build(name):
             nbr[holes] = -1
         ins["neighbors"] = nbr
         if spec.get("slot_edges"):
-            ins["edges"] = _bf16(rs.standard_normal((B, N, k, case["cfg"]["edge_dim"])))
+            ins["edges"] = util.rounded(rs.standard_normal((B, N, k, case["cfg"]["edge_dim"])), torch.bfloat16)
     return case
 
 
@@ -692,11 +606,11 @@ def test_unrounded_reference_equals_the_edge_list_oracle(masked, mean):
 def test_rounded_reference_stays_within_the_oracle_gate_on_pinned_cases():
     for name in ["dense_everything", "knn_edges_mask", "net_adj_dense"]:
         c = cases.build_case(cases.SPECS[name])
-        c["params"] = {k: _bf16(v) for k, v in c["params"].items()}
+        c["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in c["params"].items()}
         ins = c["inputs"]
         for key in ("feats", "coors", "edges"):
             if ins.get(key) is not None and np.issubdtype(np.asarray(ins[key]).dtype, np.floating):
-                ins[key] = _bf16(ins[key])
+                ins[key] = util.rounded(ins[key], torch.bfloat16)
         want = cases.run_oracle(c)
         if c["kind"] == NW:
             got = T.tc_network_forward(c["params"], c["ncfg"], ins["feats"], ins["coors"], ins.get("adj_mat"),
@@ -737,7 +651,7 @@ def compared_pairs(name):
                 jj = np.where(ok, jj, ii[:, None])
             if mk is not None:
                 ok = ok & mk[b, ii][:, None] & mk[b, jj]
-            out.append((b, _f32(x[b, ii][:, None] - x[b, jj])[ok]))
+            out.append((b, util.rounded(x[b, ii][:, None] - x[b, jj], torch.float32)[ok]))
     return out
 
 

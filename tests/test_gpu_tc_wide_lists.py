@@ -20,6 +20,7 @@ import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 import tc_reference as T
 import test_gpu_tc_boundaries as TB
 import torch_reference as R
@@ -64,14 +65,11 @@ CASES["wc_c2_gen8"] = dict(kind=L, cfg=dict(dim=32, m_pool_method="mean"), B=2, 
                            holes=True, cell="c2", mask="padded")
 
 
-def geometry(spec, sms=TB.H100_SMS):
+def geometry(spec, sms=LG.H100_SMS):
     """What the launch code runs a case with: tc_knn_kernel<MODE, ROWS, PBC, WIDE = k > 32>, ceil(k / 32) groups."""
-    g = TB.geometry(spec, sms)
-    k = g["k"]
-    mode, Q, Hp = g["mode"], g["Q"], g["Hp"]
-    g.update(groups=-(-k // 32), last_group=k - 32 * (-(-k // 32) - 1), wide=k > 32,
-             supported=(mode != TB.TK_GEN or Q <= TB.TP_QMAX) and TB._knn_smem(Hp, mode, Q, 16) <= TB.SMEM_MAX)
-    return g
+    g = LG.tc_layer(spec["kind"], spec["cfg"], spec["B"], spec["N"], C=spec.get("C", 3), k=spec["k"],
+                    rows=spec.get("rows"), sms=sms)
+    return dict(g, lattice=TB.lattice_kind(spec))
 
 
 def test_table_covers_every_boundary():
@@ -86,8 +84,8 @@ def test_table_covers_every_boundary():
             f"tc_knn<{m},{r}>" for m in ("LEAN", "EDGES", "GEN") for r in (8, 16)}, lat
         assert {g["ROWS"] for g in sub.values() if g["last_rows_valid"] < g["ROWS"]} == {8, 16}, lat
         assert any(g["rows_range"] for g in sub.values()), lat
-        assert any(CASES[n].get("slot_edges") and g["mode"] == m for n, g in sub.items() for m in (TB.TK_EDGES,
-                                                                                                    TB.TK_GEN)), lat
+        assert any(CASES[n].get("slot_edges") and g["mode"] == m for n, g in sub.items() for m in (LG.TK_EDGES,
+                                                                                                    LG.TK_GEN)), lat
     assert {g["C"] for g in geo.values()} >= {2, 3, 5}
     specs = list(CASES.values())
     assert {s.get("mask") for s in specs} >= {None, "padded", "random"}
@@ -139,11 +137,11 @@ def build(name):
     ins = case["inputs"]
     if lat:
         case[lat], ins["coors"] = TB.lattice_inputs(spec, np.random.RandomState(spec["seed"] + 11))
-    case["params"] = {k: TB._bf16(v) for k, v in case["params"].items()}
-    ins["feats"] = TB._bf16(ins["feats"])
+    case["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in case["params"].items()}
+    ins["feats"] = util.rounded(ins["feats"], torch.bfloat16)
     ins["coors"] = np.asarray(ins["coors"], np.float32).astype(np.float64)
     if ins.get("edges") is not None:
-        ins["edges"] = TB._bf16(ins["edges"])
+        ins["edges"] = util.rounded(ins["edges"], torch.bfloat16)
     B, N, k = spec["B"], spec["N"], spec["k"]
     rs = np.random.RandomState(spec["seed"] + 7)
     if slot:     # distinct neighbours per row: the oracle takes per-slot edges as a dense [B, N, N, e] tensor
@@ -152,7 +150,7 @@ def build(name):
         nbr = rs.randint(0, N, (B, N, k))
     ins["neighbors"] = _holes(nbr, rs, slot) if spec.get("holes") else nbr
     if slot:
-        ins["edges"] = TB._bf16(rs.standard_normal((B, N, k, case["cfg"]["edge_dim"])))
+        ins["edges"] = util.rounded(rs.standard_normal((B, N, k, case["cfg"]["edge_dim"])), torch.bfloat16)
     _BUILT[name] = case
     return case
 
@@ -381,10 +379,10 @@ def test_own_select_at_k_64_with_valid_radius_and_a_mask(kind):
     # uniform in the lattice's cell (no ties between distances), moved by whole lattice vectors so that pairs wrap
     A = {"plain": np.diag(SEL_L), "box": np.diag(SEL_L), "cell": TB._grid_cell(rs, SEL_L, 0.5)}[kind]
     frac = rs.uniform(0, 1, (2, SEL_N, 3)) + (rs.randint(-1, 2, (2, SEL_N, 3)) if kind != "plain" else 0)
-    ins["coors"] = TB._f32(frac @ A)
-    lat = {"plain": {}, "box": {"box": np.asarray(SEL_L)}, "cell": {"cell": TB._f32(A)}}[kind]
-    case["params"] = {k: TB._bf16(v) for k, v in case["params"].items()}
-    ins["feats"] = TB._bf16(ins["feats"])
+    ins["coors"] = util.rounded(frac @ A, torch.float32)
+    lat = {"plain": {}, "box": {"box": np.asarray(SEL_L)}, "cell": {"cell": util.rounded(A, torch.float32)}}[kind]
+    case["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in case["params"].items()}
+    ins["feats"] = util.rounded(ins["feats"], torch.bfloat16)
     nbr, ok = select_lists(ins["coors"], ins["mask"], SEL_K, SEL_R, lat)
     assert ok.mean() > 0.2 and (~ok).mean() > 0.2, ok.mean()            # the radius cuts inside the lists
     mod = util.make_module(case, torch.bfloat16)
@@ -411,8 +409,8 @@ def test_only_sparse_network_with_expanded_adjacency_above_32():
                 init="xavier")
     case = cases.build_case(spec)
     ins = case["inputs"]
-    case["params"] = {k: TB._bf16(v) for k, v in case["params"].items()}
-    ins["coors"] = TB._f32(ins["coors"])
+    case["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in case["params"].items()}
+    ins["coors"] = util.rounded(ins["coors"], torch.float32)
     adj, _ = O.adjacency_degrees(ins["adj_mat"], 2, 2)
     k = int(np.asarray(adj).sum(-1).max())
     assert 32 < k < 120, k
@@ -420,10 +418,10 @@ def test_only_sparse_network_with_expanded_adjacency_above_32():
     dev = "cuda"
     with torch.no_grad(), warnings.catch_warnings():
         warnings.simplefilter("error")
-        f, x = mod(torch.from_numpy(TB._bf16(ins["feats"])).to(dev, torch.bfloat16),
+        f, x = mod(torch.from_numpy(util.rounded(ins["feats"], torch.bfloat16)).to(dev, torch.bfloat16),
                    torch.from_numpy(ins["coors"]).float().to(dev), adj_mat=torch.from_numpy(ins["adj_mat"]).to(dev), mask=torch.from_numpy(ins["mask"]).to(dev))
     assert all(l[1].last_path == "bf16-tc" for l in mod.layers)
-    rf, rx = T.tc_network_forward(case["params"], case["ncfg"], TB._bf16(ins["feats"]), ins["coors"], ins["adj_mat"],
+    rf, rx = T.tc_network_forward(case["params"], case["ncfg"], util.rounded(ins["feats"], torch.bfloat16), ins["coors"], ins["adj_mat"],
                                   mask=ins["mask"])
     m = gates([((0, 120), rf, rx)], ins["coors"], [(f.double().cpu().numpy(), x.double().cpu().numpy())])
     print("TCW net_sparse_k%d " % k + " ".join(f"{n}={v:.3e}" for n, v in m.items()))

@@ -12,12 +12,12 @@ Each case: forward in fp64 and fp32 at util.TOL; gradients in fp64 and fp32 at u
 by the forward and recomputed by the backward.  Configurations whose backward needs more shared memory than the SIMT
 budget must fail at the training forward, before it runs."""
 import functools
-import math
 
 import pytest
 import torch
 
 import cases
+import launch_geometry as LG
 import util
 from tests import test_edge_list
 
@@ -61,85 +61,17 @@ TILE_CASES = {
 }
 FP64_BACKWARD_REJECTED = {"dense_mdim24_soft", "dense_mdim32", "dense_q77"}
 
-# ------------------------------------------------------------------ tile geometry (mirrors the launch code)
-
-H100_SMS = 132          # H100 SXM; only the split-K count of the per-node backward GEMMs depends on it
-
-
-def _round_up(x, m):
-    return (x + m - 1) // m * m
-
-
-def _gemm_acc_splits(Mr, Nc, K, sms=H100_SMS):
-    """(splits, rows per split) of launch_gemm_acc (egnn_backward_impl.cuh)."""
-    tiles = math.ceil(Mr / 64) * math.ceil(Nc / 64)
-    splits = max(1, min(math.ceil(2 * sms / tiles), math.ceil(K / 64)))
-    kper = _round_up(math.ceil(K / splits), 16)
-    return math.ceil(K / kper), kper
-
-
-SIMT_SMEM_MAX = 220 * 1024     # simt_host.cuh: the dense edge step falls back to one row per thread above it
-
-
-def pair_tiled_smem_bytes(g, PP, itemsize):
-    """Dynamic shared memory of pair_dense_tiled_kernel at PP rows per thread (simt_kernels.cuh)."""
-    MP, Q, m = g["MP"], g["Q"], g["m"]
-    n = 64 * MP + Q * 64 + 64 * 33 + (PP * Q * 128 if Q > 1 else 0) + 4 * m * MP + 8 * m + 2 * MP + 4
-    if PP > 1:
-        n += 4 * PP * (MP + 8 + 4)
-    return _round_up(n * itemsize, 16) + 16
-
-
-def geometry(spec, k=0, C=3, rows=None):
-    """The tile counts a case runs with.  k > 0: neighbour lists of width k.  rows: a row block (r0, r1)."""
-    if spec["kind"] == NW:
-        ncfg = cases.O.network_cfg(**spec["cfg"])
-        cfg = ncfg["layer"]
-        label_dim = ncfg["adj_dim"] if ncfg["num_adj_degrees"] is not None else 0
-        labels = ncfg["num_adj_degrees"] + 1 if label_dim else 0
-    else:
-        cfg = cases.O.layer_cfg(**spec["cfg"])
-        label_dim, labels = 0, 0
-    dim, m, F = cfg["dim"], cfg["m_dim"], cfg["fourier_features"]
-    E = cases.O.edge_input_dim(cfg)                  # 2 dim + Q + label_dim
-    Q = E - 2 * dim - label_dim
-    Hp = _round_up(2 * E, 8)
-    MP = 16 if m <= 16 else 32
-    B, N = spec["B"], spec["N"]
-    g = dict(E=E, Q=Q, Hp=Hp, MP=MP, m=m, dim=dim, N=N, C=C, labels=labels, k=k, F=F,
-             chunks=math.ceil(Hp / 64), partial_chunk=Hp % 64 != 0,
-             bwd2_ch_ctas=math.ceil(Hp / 128), partial_ch_cta=Hp % 128 != 0,
-             generic_node_gemm=dim > 64)
-    splits, kper = _gemm_acc_splits(dim, 2 * dim, B * N)          # dWn2 = go^T h1, K = B*N
-    g.update(splitk=splits, partial_split=splits > 1 and (B * N) % kper != 0)
-    if k == 0:
-        g.update(j_passes=math.ceil(N / 32), partial_j=N % 32 != 0,
-                 bwd2_row_ctas=math.ceil(N / 32), partial_rows=N % 32 != 0)
-    else:
-        TS = min(32, 1 << (k - 1).bit_length())
-        g.update(TS=TS, slot_passes=math.ceil(k / TS), partial_slots=k % TS != 0,
-                 bwd2_steps=math.ceil(k / 32), partial_step=k % 32 != 0, partial_list_rows=N % 16 != 0,
-                 QR=1 if (Q == 1 and not labels) else (8 if Q <= 8 else 0))
-    # launch decisions: rows per thread of the dense forward per element size (launch_pair_dense), the split hidden
-    # axis (simt_hsplit), and bwd3's grid over the rows of the call (TS lanes per row, 128 threads per CTA)
-    r0, r1 = rows or (0, N)
-    g["PP"] = {es: 1 if (MP == 32 and es == 8) or pair_tiled_smem_bytes(g, 2, es) > SIMT_SMEM_MAX else 2
-               for es in (8, 4)}
-    g["hsplit"] = min(32, math.ceil(Hp / 64)) if (k == 0 and B * N * N <= 4096 and Hp >= 512 and rows is None) else 1
-    per_cta = 128 // (g["TS"] if k else 32)
-    g.update(rows=r1 - r0, bwd3_rows_per_cta=per_cta, bwd3_ctas=math.ceil((r1 - r0) / per_cta),
-             bwd3_partial=(r1 - r0) % per_cta != 0)
-    return g
+# ------------------------------------------------------------------ tile geometry (launch_geometry.simt_layer)
 
 
 def list_geometry(name):
     cfg, B, N, k, C, _, _ = test_edge_list.EDGE_CASES[name]
-    return geometry(dict(kind=L, cfg=cfg, B=B, N=N), k=k, C=C)
+    return LG.simt_layer(L, cfg, B, N, k=k, C=C)
 
 
 def test_table_covers_every_tile_boundary():
     """Each boundary the table is meant to reach, recomputed from the specs: an edit to a shape that drops one fails here."""
-    dense = {n: geometry(s) for n, s in TILE_CASES.items()}
+    dense = {n: LG.simt_layer(s["kind"], s["cfg"], s["B"], s["N"]) for n, s in TILE_CASES.items()}
     trained64 = {n: g for n, g in dense.items() if n not in FP64_BACKWARD_REJECTED}
     lists = {n: list_geometry(n) for n in test_edge_list.BACKWARD_CASES}
     want = {
@@ -173,7 +105,7 @@ def test_table_covers_every_tile_boundary():
                                                 for g in lists.values()),
         "list TS < 32": any(g["TS"] < 32 for g in lists.values()),
         "list bwd2 two 32-slot steps": any(g["bwd2_steps"] == 2 and g["partial_step"] for g in lists.values()),
-        "list bwd2 16-row CTAs, partial last": any(g["partial_list_rows"] and g["N"] > 32 for g in lists.values()),
+        "list bwd2 16-row CTAs, partial last": any(g["partial_rows"] and g["N"] > 32 for g in lists.values()),
         "list QR 1 / 8 / 0": {g["QR"] for g in lists.values() if g["N"] > 32} == {0, 1, 8},
         "list Q 1, 5, 10": {g["Q"] for g in lists.values()} >= {1, 5, 10},
         "list C 2 and 5": {g["C"] for g in lists.values()} >= {2, 5},

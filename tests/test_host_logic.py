@@ -12,17 +12,10 @@ import pytest
 import torch
 
 import cases
+from util import nat  # noqa: F401  (module-scoped fixture)
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 HEADER = os.path.join(REPO, "include", "egnn_b200.h")
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from egnn_pytorch_b200 import build, _native
-    build.build()                     # nvcc cross-compiles sm_90a without a GPU
-    _native.load()
-    return _native
 
 
 def declared_functions():

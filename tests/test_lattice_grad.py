@@ -22,8 +22,8 @@ import cases
 import torch_reference as R
 import util
 from oracle import egnn_oracle_grad as G
-from test_triclinic import (SUPER, TCASES, _cell_geometry, build, cell_bc, cell_coors, knn_gap, make_cell, rounded,
-                            supercell, wrap_margin, wrapped_d2)
+from test_triclinic import (SUPER, TCASES, _cell_geometry, build, cell_bc, cell_coors, knn_gap, make_cell, supercell,
+                            wrap_margin, wrapped_d2)
 
 DT = {"fp64": torch.float64, "fp32": torch.float32}
 TAU64 = 1e-12            # fp64: error over the largest magnitude of the lattice gradient
@@ -206,7 +206,7 @@ def build_box(name, dtype=torch.float64):
     case = cases.build_case(dict(kind="layer", cfg=cfg, B=B, N=N, C=Cd, seed=910, init="xavier", mask=mask or "none"))
     for seed in range(20):
         rs = np.random.RandomState(810 + seed)
-        L = rounded(np.diagonal(make_cell(kind, B, rs), axis1=-2, axis2=-1).copy(), cdt)
+        L = util.rounded(np.diagonal(make_cell(kind, B, rs), axis1=-2, axis2=-1).copy(), cdt)
         diag = np.eye(Cd) * L[..., None, :]
         diag[~np.isfinite(diag)] = 0.0
         diag[..., np.arange(Cd), np.arange(Cd)] = L
@@ -300,7 +300,7 @@ def test_thousands_of_ctas_reduce_into_each_graph(dt):
                                  mask="padded"))
     rs = np.random.RandomState(17)
     cell = make_cell("per_graph", B, rs)
-    cell = rounded(cell, _cdt(dtype))
+    cell = util.rounded(cell, _cdt(dtype))
     x = rs.uniform(-6, 6, (B, N, 3))
     x = x.astype(np.float32).astype(np.float64) if dtype == torch.float32 else x
     case["inputs"]["coors"] = x

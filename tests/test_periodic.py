@@ -59,10 +59,6 @@ def half_box_margin(coors, box):
     return float(np.where(per[:, None, None], m, 1.0).min())
 
 
-def rounded(x, dtype):
-    return None if x is None else torch.as_tensor(np.asarray(x, np.float64)).to(dtype).double().numpy()
-
-
 # name: (layer cfg, B, N, C, box [C] or None for [B, C], mask, adj).  inf / 0 entries: aperiodic axes.
 PCASES = {
     "dense":          (dict(dim=16), 2, 40, 3, [3.0, 2.5, 4.0], None, None),
@@ -96,12 +92,12 @@ def build(name, seed=0, dtype=torch.float64):
     scale = np.where(np.isfinite(box) & (box > 0), box, 3.0)
     case["inputs"]["coors"] = np.concatenate([lattice_coors(rs, 1, N, Cd, sc) for sc in np.broadcast_to(scale, (B, Cd))])
     if dtype != torch.float64:                       # the restatement sees the coordinates / features the kernels see
-        case["inputs"]["coors"] = rounded(case["inputs"]["coors"], torch.float32)
+        case["inputs"]["coors"] = util.rounded(case["inputs"]["coors"], torch.float32)
     if dtype == torch.bfloat16:
-        case["params"] = {k: rounded(v, torch.bfloat16) for k, v in case["params"].items()}
+        case["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in case["params"].items()}
         for k in ("feats", "edges"):
             if k in case["inputs"]:
-                case["inputs"][k] = rounded(case["inputs"][k], torch.bfloat16)
+                case["inputs"][k] = util.rounded(case["inputs"][k], torch.bfloat16)
     return case, box
 
 
@@ -382,7 +378,7 @@ def test_edge_list_mode_matches_the_restatement(name, dt):
     case, box = build(name, dtype=dtype)
     nb, se = _lists(case, 12)
     if se is not None and dtype == torch.bfloat16:
-        se = rounded(se, torch.bfloat16)
+        se = util.rounded(se, torch.bfloat16)
     ins = case["inputs"]
     want = [t.numpy() for t in layer(case["params"], case["cfg"], ins["feats"], ins["coors"], None, ins.get("mask"),
                                      None, box, nb, se)]

@@ -8,14 +8,7 @@ import torch
 
 import cases
 from oracle import egnn_oracle as O
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from egnn_pytorch_b200 import build, _native
-    build.build()
-    _native.load()
-    return _native
+from util import nat  # noqa: F401  (module-scoped fixture)
 
 
 def _r256(n):

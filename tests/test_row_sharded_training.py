@@ -18,6 +18,7 @@ import cases
 import util
 from oracle import egnn_oracle as O
 from oracle import egnn_oracle_grad as G
+from util import nat  # noqa: F401  (module-scoped fixture)
 
 # dense N = 97 with Hp = 152: blocks cross the 32-row tiles and the 128-channel tiles of the dense bwd2
 N97 = dict(kind="layer", cfg=dict(dim=36, edge_dim=2, norm_feats=True), B=1, N=97, seed=70, init="xavier", mask="padded")
@@ -46,14 +47,6 @@ def zero_outside(g, rows):
 
 
 # ----------------------------------------------------------------------------- C ABI (CPU)
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from egnn_pytorch_b200 import build, _native
-    build.build()
-    _native.load()
-    return _native
 
 
 def _desc(nat, **kw):

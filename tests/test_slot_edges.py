@@ -24,6 +24,7 @@ import cases
 import util
 from oracle import egnn_oracle as O
 from oracle import egnn_oracle_grad as G
+from util import nat  # noqa: F401  (module-scoped fixture)
 
 CASES = {
     # name: (layer cfg, B, N, k, C, mask?).  Comments: the bf16 list kernel mode and the bwd2 channel instantiation
@@ -236,14 +237,6 @@ def test_edge_index_to_neighbors_places_edge_attr_in_its_slot():
     assert torch.equal(g[4], torch.zeros(2, dtype=torch.float64))          # edge 3 -> 0 was truncated
     assert torch.equal(g[0], torch.tensor([1.0, 2.0], dtype=torch.float64))  # edge 1 -> 0: node 0 slot 0
     assert torch.equal(g[5], torch.tensor([15.0, 16.0], dtype=torch.float64))  # edge 1 -> 3: node 3 slot 1
-
-
-@pytest.fixture(scope="module")
-def nat():
-    from egnn_pytorch_b200 import build, _native
-    build.build()
-    _native.load()
-    return _native
 
 
 def test_descriptor_validation_of_the_per_slot_flag(nat):

@@ -102,10 +102,6 @@ def wrapped_d2(x, cell):
     return (cell_wrap(x[:, :, None] - x[:, None], torch.as_tensor(cell_bc(cell, B, Cd).copy())[:, None, None]) ** 2).sum(-1)
 
 
-def rounded(x, dtype):
-    return None if x is None else torch.as_tensor(np.asarray(x, np.float64)).to(dtype).double().numpy()
-
-
 def make_cell(kind, B, rs):
     """Lower-triangular cells: `tilt` (tilts up to 0.5 of the diagonal), `tilt09` (one tilt of 0.9), `per_graph` (a
     different tilted cell per graph), `hex_slab` (hexagonal, z aperiodic), `c2` (a 2-D oblique cell)."""
@@ -143,10 +139,10 @@ def cell_coors(rs, B, N, cell, shift=2, margin=1e-3, dtype=torch.float64):
 
     def place(u):
         s = u + rs.randint(-shift, shift + 1, u.shape) * per[:, None, :]
-        return rounded(np.einsum("bnk,bkd->bnd", s, Af), dtype)
+        return util.rounded(np.einsum("bnk,bkd->bnd", s, Af), dtype)
     x = place(u)
     for _ in range(200):
-        m = wrap_margin(x, rounded(cell, dtype))
+        m = wrap_margin(x, util.rounded(cell, dtype))
         bad = (m < margin).any(-1)
         if not bad.any():
             return x
@@ -179,13 +175,13 @@ def build(name, seed=0, dtype=torch.float64):
     rs = np.random.RandomState(710 + seed)
     cell = make_cell(kind, B, rs)
     cdt = torch.float64 if dtype == torch.float64 else torch.float32
-    cell = rounded(cell, cdt)
+    cell = util.rounded(cell, cdt)
     case["inputs"]["coors"] = cell_coors(rs, B, N, cell, dtype=cdt)
     if dtype == torch.bfloat16:
-        case["params"] = {k: rounded(v, torch.bfloat16) for k, v in case["params"].items()}
+        case["params"] = {k: util.rounded(v, torch.bfloat16) for k, v in case["params"].items()}
         for k in ("feats", "edges"):
             if k in case["inputs"]:
-                case["inputs"][k] = rounded(case["inputs"][k], torch.bfloat16)
+                case["inputs"][k] = util.rounded(case["inputs"][k], torch.bfloat16)
     return case, cell
 
 

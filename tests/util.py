@@ -1,8 +1,12 @@
 """Helpers shared by the GPU parity tests, smoke() and bench.py: build the product modules from
-a tests/cases.py case, move numpy inputs to torch, and run / compare forward and backward."""
+a tests/cases.py case, move numpy inputs to torch, and run / compare forward and backward; plus the small helpers the
+test files share (rounding, the native-library fixture, TF32 off)."""
 from __future__ import annotations
 
+import contextlib
+
 import numpy as np
+import pytest
 import torch
 
 import cases
@@ -107,3 +111,34 @@ def assert_close(got, want, atol, rtol, what=""):
     tol = atol + rtol * np.abs(want)
     worst = float((err - tol).max())
     assert worst <= 0, f"{what}: max|err|={err.max():.3e} exceeds atol={atol} rtol={rtol} (|want|max={np.abs(want).max():.3e})"
+
+
+def rounded(x, dtype):
+    """`x` rounded to the torch float type `dtype` (a bfloat16 through float32, as torch converts) and returned as
+    float64 numpy: the values a kernel of that type sees.  None and arrays that are not floating point are returned
+    as they are (masks, token ids, adjacency)."""
+    if x is None or not np.issubdtype(np.asarray(x).dtype, np.floating):
+        return x
+    return torch.as_tensor(np.asarray(x, np.float64)).to(dtype).double().numpy()
+
+
+@pytest.fixture(scope="module")
+def nat():
+    """egnn_pytorch_b200._native with the library built for sm_90a (nvcc cross-compiles without a GPU) and loaded."""
+    from egnn_pytorch_b200 import build, _native
+    build.build()
+    _native.load()
+    return _native
+
+
+@contextlib.contextmanager
+def no_tf32():
+    """fp32 matmuls in full fp32 (no TF32), so that an fp32 restatement measures fp32 arithmetic."""
+    prev = torch.backends.cuda.matmul.allow_tf32, torch.get_float32_matmul_precision()
+    torch.backends.cuda.matmul.allow_tf32 = False
+    torch.set_float32_matmul_precision("highest")
+    try:
+        yield
+    finally:
+        torch.backends.cuda.matmul.allow_tf32 = prev[0]
+        torch.set_float32_matmul_precision(prev[1])
