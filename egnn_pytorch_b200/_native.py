@@ -24,6 +24,7 @@ FLAG_ONLY_SPARSE = 1 << 7
 FLAG_ADJ_BATCHED = 1 << 8
 FLAG_EDGES_PER_SLOT = 1 << 9
 FLAG_ROW_PARTIAL_GRADS = 1 << 10
+FLAG_CELL_SELECT_WIDE = 1 << 11
 
 ERR_UNSUPPORTED = -3
 
@@ -142,6 +143,13 @@ SYMBOLS = {
     "egnn_radius_select_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                                C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                                C.c_size_t, C.c_void_p]),
+    "egnn_radius_select_wide_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P(C.c_size_t)]),
+    "egnn_radius_select_wide": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                          C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t,
+                                          C.c_void_p]),
+    "egnn_radius_select_wide_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                    C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p,
+                                                    C.c_void_p, C.c_size_t, C.c_void_p]),
     "egnn_adj_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_size_t)]),
     "egnn_adj_expand": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
@@ -201,6 +209,7 @@ def strerror(code: int) -> str:
 
 class EgnnNativeError(RuntimeError):
     def __init__(self, fn, code):
+        self.fn = fn
         self.code = code
         super().__init__(f"{fn} failed: {strerror(code)} (code {code})")
 

@@ -80,8 +80,8 @@ inline int sm_count(int* out) {
 int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nbr_idx, uint8_t** nbr_ok, cudaStream_t st,
                      const void* box = nullptr, void* cell_ws = nullptr, int pbc = 0);
 
-// The cell-grid radius select (radius_select.cu).  A layer is eligible from its descriptor alone (1 <= k <= 32, C <= 3,
-// 0 < (T)valid_radius < 1e5, no only_sparse / batched adjacency / per-slot edges); its forward workspace then carries
+// The cell-grid radius select (radius_select.cu).  A layer is eligible from its descriptor alone (1 <= k <= 32, or <= 256
+// under EGNN_FLAG_CELL_SELECT_WIDE, C <= 3, 0 < (T)valid_radius < 1e5, no only_sparse / batched adjacency / per-slot edges); its forward workspace then carries
 // cell_select_layer_ws_bytes(d) bytes of scratch (0 for a layer that is not eligible), whatever the size threshold.
 // cell_select_runs adds what the call decides: a mask, no adjacency, no caller lists and N >= the threshold.
 bool cell_select_eligible(const EgnnLayerDesc& d);

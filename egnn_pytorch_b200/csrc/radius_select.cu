@@ -20,7 +20,7 @@
 //   scatter coordinates (SoA) and node indices into cell order; afterwards end[t] is the end of bucket t
 //   query   one warp per node, nodes taken in cell order: the deduplicated buckets of the 3^C cells around the node
 //           are read as one flattened candidate stream, filtered by rank <= r2 and against the current k-th entry,
-//           queued and merged 32 at a time.
+//           queued and merged 32 at a time; for k > 32 (radius_query_wide_kernel) the list lives in shared memory.
 #include "common.cuh"
 #include "profile.h"
 #include "warp_select.cuh"
@@ -31,6 +31,8 @@ namespace egnn {
 constexpr int RS_THREADS = 256;          // count / scatter
 constexpr int RS_SCAN_THREADS = 1024;    // scan: one CTA per graph, 4 buckets per thread per tile
 constexpr int RS_WARPS = 8;              // query rows per CTA
+constexpr int RS_WIDE_MAX_K = 256;       // the longest list the query keeps (radius_query_wide_kernel above 32)
+constexpr size_t RS_WIDE_SMEM = 32768;   // wide query: dynamic shared memory per CTA, within the 48 KiB default
 constexpr double RS_CLAMP = 1073741824.0;     // 2^30: aperiodic cell coordinates and periodic cell counts
 
 // Buckets per graph: next_pow2(2N).
@@ -57,7 +59,8 @@ static CellWs cell_ws_layout(int B, int N, int C, size_t coord_bytes) {
 size_t cell_select_ws_bytes(int B, int N, int C, size_t coord_bytes) { return cell_ws_layout(B, N, C, coord_bytes).total; }
 
 bool cell_select_eligible(const EgnnLayerDesc& d) {
-  if (d.k < 1 || d.k > 32 || d.C < 1 || d.C > 3) return false;
+  const int max_k = (d.flags & EGNN_FLAG_CELL_SELECT_WIDE) ? RS_WIDE_MAX_K : 32;
+  if (d.k < 1 || d.k > max_k || d.C < 1 || d.C > 3) return false;
   if (d.flags & (EGNN_FLAG_ONLY_SPARSE | EGNN_FLAG_ADJ_BATCHED | EGNN_FLAG_EDGES_PER_SLOT)) return false;
   // the radius in the coordinates' type, as the select compares it; at or above 1e5 padded pairs (rank 1e5) could
   // take slots in the reference
@@ -255,34 +258,13 @@ __global__ void __launch_bounds__(RS_THREADS) radius_scatter_kernel(const RadArg
   a.idx[g0 + pos] = i;
 }
 
+// The candidate stream of node i of graph b, which its warp reads t = lane, lane + 32, ...: the deduplicated buckets of
+// the 3^C cells around xi, flattened.  Returns its length; wexcl / wdelta (the warp's 32 ints each) receive per kept
+// bucket its first stream position and its cell-order position minus that.
 template <typename T, int CD, int PBC>
-__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadArgs<T> a) {
+__device__ __forceinline__ int row_stream(const RadArgs<T>& a, int b, int lane, const T (&xi)[CD], const int* cnt,
+                                          const int* end, int* wexcl, int* wdelta) {
   constexpr int NB = CD == 1 ? 3 : (CD == 2 ? 9 : 27);           // neighbouring cells
-  __shared__ T qkey[RS_WARPS][64];
-  __shared__ int qidx[RS_WARPS][64];
-  __shared__ int sexcl[RS_WARPS][32];                            // per kept bucket: first position in the stream
-  __shared__ int sdelta[RS_WARPS][32];                           // per kept bucket: cell-order position - stream position
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const size_t gw = (size_t)blockIdx.x * RS_WARPS + warp;
-  if (gw >= (size_t)a.B * a.N) return;
-  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
-  const int* cnt = a.cnt + (size_t)b * a.Tb;
-  const int* end = a.end + (size_t)b * a.Tb;
-  if (p >= end[a.Tb - 1]) return;                                // beyond the nodes graph b put into its grid
-  const size_t g0 = (size_t)b * a.N, BN = (size_t)a.B * a.N;
-  const int i = a.idx[g0 + p];
-  T xi[CD];
-#pragma unroll
-  for (int c = 0; c < CD; ++c) xi[c] = a.xs[c * BN + g0 + p];
-  T bl[CD], binv[CD], pc[PBC == PBC_CELL ? CELL_STAGED : 1];
-  if constexpr (PBC == PBC_CELL) {
-#pragma unroll
-    for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, CD, t);
-  } else if constexpr (PBC) {
-#pragma unroll
-    for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);
-  }
-
   // lane l < NB: the bucket of neighbouring cell l; a bucket reached twice (a periodic axis of 1 or 2 cells, or two cells
   // hashing alike) is kept by its lowest lane only, so that no node enters the stream twice
   int bkt = -1 - lane;
@@ -319,9 +301,74 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
   const int total = __shfl_sync(0xffffffffu, incl, 31);
-  sexcl[warp][lane] = incl - len;
-  sdelta[warp][lane] = beg - (incl - len);
+  wexcl[lane] = incl - len;
+  wdelta[lane] = beg - (incl - len);
   __syncwarp();
+  return total;
+}
+
+// Candidate t of the stream: its node index j and its rank, as the all-pairs select computes it (bl / binv: the box of
+// graph b under PBC_BOX, pc: its staged cell under PBC_CELL).
+template <typename T, int CD, int PBC>
+__device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t BN, int t, const int* wexcl,
+                                         const int* wdelta, const T (&xi)[CD], const T (&bl)[CD], const T (&binv)[CD],
+                                         const T* pc, int& j) {
+  int s = 0;                                                     // the last kept bucket that starts at or before t
+#pragma unroll
+  for (int step = 16; step > 0; step >>= 1)
+    if (wexcl[s + step] <= t) s += step;
+  const size_t pos = g0 + wdelta[s] + t;
+  j = a.idx[pos];
+  T d = T(0);
+  if constexpr (PBC == PBC_CELL) {
+    T r[3];
+#pragma unroll
+    for (int c = 0; c < 3; ++c) r[c] = c < CD ? xi[c < CD ? c : 0] - a.xs[(c < CD ? c : 0) * BN + pos] : T(0);
+    cell_wrap<T>(r[0], r[1], r[2], pc);
+#pragma unroll
+    for (int c = 0; c < CD; ++c) d = sq_acc<T>(r[c], d);
+  } else {
+#pragma unroll
+    for (int c = 0; c < CD; ++c) {
+      T r = xi[c] - a.xs[c * BN + pos];
+      if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
+      d = sq_acc<T>(r, d);
+    }
+  }
+  return d;
+}
+
+// The prologue of both query kernels: the node at cell-order position p of graph b (false: beyond the nodes the graph
+// put into its grid), its coordinates xi and its graph's box (bl, binv) or cell (pc).
+#define RS_QUERY_ROW()                                                                                                  \
+  const int* cnt = a.cnt + (size_t)b * a.Tb;                                                                            \
+  const int* end = a.end + (size_t)b * a.Tb;                                                                            \
+  if (p >= end[a.Tb - 1]) return;                                                                                       \
+  const size_t g0 = (size_t)b * a.N, BN = (size_t)a.B * a.N;                                                            \
+  const int i = a.idx[g0 + p];                                                                                          \
+  T xi[CD];                                                                                                             \
+  _Pragma("unroll") for (int c = 0; c < CD; ++c) xi[c] = a.xs[c * BN + g0 + p];                                         \
+  T bl[CD], binv[CD], pc[PBC == PBC_CELL ? CELL_STAGED : 1];                                                            \
+  if constexpr (PBC == PBC_CELL) {                                                                                      \
+    _Pragma("unroll") for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, CD, t);                    \
+  } else if constexpr (PBC) {                                                                                           \
+    _Pragma("unroll") for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);                        \
+  }
+
+// k <= 32: lane l keeps the l-th smallest (rank, j) so far; candidates in radius that beat the k-th are queued and merged
+// 32 at a time (warp_merge).
+template <typename T, int CD, int PBC>
+__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadArgs<T> a) {
+  __shared__ T qkey[RS_WARPS][64];
+  __shared__ int qidx[RS_WARPS][64];
+  __shared__ int sexcl[RS_WARPS][32];
+  __shared__ int sdelta[RS_WARPS][32];
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const size_t gw = (size_t)blockIdx.x * RS_WARPS + warp;
+  if (gw >= (size_t)a.B * a.N) return;
+  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  RS_QUERY_ROW()
+  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
 
   const T INF = T(INFINITY);
   const int IMAX = 0x7fffffff;
@@ -337,28 +384,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
     int j = IMAX;
     bool pass = false;
     if (t < total) {
-      int s = 0;                                        // the last kept bucket that starts at or before t
-#pragma unroll
-      for (int step = 16; step > 0; step >>= 1)
-        if (sexcl[warp][s + step] <= t) s += step;
-      const size_t pos = g0 + sdelta[warp][s] + t;
-      j = a.idx[pos];
-      T d = T(0);
-      if constexpr (PBC == PBC_CELL) {
-        T r[3];
-#pragma unroll
-        for (int c = 0; c < 3; ++c) r[c] = c < CD ? xi[c < CD ? c : 0] - a.xs[(c < CD ? c : 0) * BN + pos] : T(0);
-        cell_wrap<T>(r[0], r[1], r[2], pc);
-#pragma unroll
-        for (int c = 0; c < CD; ++c) d = sq_acc<T>(r[c], d);
-      } else {
-#pragma unroll
-        for (int c = 0; c < CD; ++c) {
-          T r = xi[c] - a.xs[c * BN + pos];
-          if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-          d = sq_acc<T>(r, d);
-        }
-      }
+      const T d = stream_rank<T, CD, PBC>(a, g0, BN, t, sexcl[warp], sdelta[warp], xi, bl, binv, pc, j);
       const bool in = d <= a.r2;
       nin += in ? 1 : 0;
       key = d;
@@ -407,6 +433,114 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
   }
 }
 
+// Sorts n = 2^m (rank, j) pairs in shared memory ascending (lexicographic), one warp: the bitonic network of
+// knn_block_sort_kernel.
+template <typename T>
+__device__ __forceinline__ void warp_smem_sort(T* key, int* idx, int n, int lane) {
+  for (int size = 2; size <= n; size <<= 1) {
+    for (int stride = size >> 1; stride > 0; stride >>= 1) {
+      for (int t = lane; t < n / 2; t += 32) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        const bool asc = (lo & size) == 0;
+        if (lex_less<T>(key[hi], idx[hi], key[lo], idx[lo]) == asc) {
+          const T tk = key[lo]; key[lo] = key[hi]; key[hi] = tk;
+          const int ti = idx[lo]; idx[lo] = idx[hi]; idx[hi] = ti;
+        }
+      }
+      __syncwarp();
+    }
+  }
+}
+
+// 32 < k <= RS_WIDE_MAX_K: the candidate stream of radius_query_kernel, with the top k kept in shared memory instead of
+// lanes.  Per warp, KP = next_pow2(k) (>= 64) pairs `list`, sorted ascending (the KP smallest (rank, j) so far, padded
+// with (inf, IMAX)), and KP more `queue`.  A candidate in radius that beats the current k-th list entry is queued.  Once
+// the queue could not take another 32, it is padded, sorted and merged into the list: list[s] = min(list[s],
+// queue[KP-1-s]) leaves the KP smallest of both as a bitonic sequence, which log2(KP) merge steps sort.  The list is a
+// function of the set of pairs queued, and every pair the filter drops is beaten by k listed ones, so the k kept pairs
+// are the k smallest of the stream whatever order the scatter put the candidates in.
+template <typename T, int CD, int PBC>
+__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const RadArgs<T> a, int KP) {
+  extern __shared__ __align__(16) unsigned char rsw_sm[];         // [warps][2 KP] ranks, then [warps][2 KP] indices
+  __shared__ int sexcl[RS_WARPS][32];
+  __shared__ int sdelta[RS_WARPS][32];
+  const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const size_t gw = (size_t)blockIdx.x * warps + warp;
+  if (gw >= (size_t)a.B * a.N) return;
+  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  RS_QUERY_ROW()
+  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
+
+  const T INF = T(INFINITY);
+  const int IMAX = 0x7fffffff;
+  T* lk = reinterpret_cast<T*>(rsw_sm) + (size_t)warp * 2 * KP;
+  int* li = reinterpret_cast<int*>(reinterpret_cast<T*>(rsw_sm) + (size_t)warps * 2 * KP) + (size_t)warp * 2 * KP;
+  T* qk = lk + KP;
+  int* qi = li + KP;
+  for (int s = lane; s < KP; s += 32) { lk[s] = INF; li[s] = IMAX; }
+  T thr_key = INF; int thr_idx = IMAX; // the k-th smallest so far
+  int count = 0;                       // queued candidates (warp-uniform)
+  int nin = 0;                         // this lane's in-radius candidates
+  auto flush = [&]() {
+    for (int s = count + lane; s < KP; s += 32) { qk[s] = INF; qi[s] = IMAX; }
+    __syncwarp();
+    warp_smem_sort<T>(qk, qi, KP, lane);
+    for (int s = lane; s < KP; s += 32) {
+      const T ck = qk[KP - 1 - s];
+      const int ci = qi[KP - 1 - s];
+      if (lex_less<T>(ck, ci, lk[s], li[s])) { lk[s] = ck; li[s] = ci; }
+    }
+    __syncwarp();
+    for (int stride = KP >> 1; stride > 0; stride >>= 1) {
+      for (int t = lane; t < KP / 2; t += 32) {
+        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
+        if (lex_less<T>(lk[hi], li[hi], lk[lo], li[lo])) {
+          const T tk = lk[lo]; lk[lo] = lk[hi]; lk[hi] = tk;
+          const int ti = li[lo]; li[lo] = li[hi]; li[hi] = ti;
+        }
+      }
+      __syncwarp();
+    }
+    count = 0;
+    thr_key = lk[a.k - 1];
+    thr_idx = li[a.k - 1];
+  };
+  for (int t0 = 0; t0 < total; t0 += 32) {
+    const int t = t0 + lane;
+    T key = INF;
+    int j = IMAX;
+    bool pass = false;
+    if (t < total) {
+      key = stream_rank<T, CD, PBC>(a, g0, BN, t, sexcl[warp], sdelta[warp], xi, bl, binv, pc, j);
+      const bool in = key <= a.r2;
+      nin += in ? 1 : 0;
+      pass = in && lex_less<T>(key, j, thr_key, thr_idx);
+    }
+    const unsigned bal = __ballot_sync(0xffffffffu, pass);
+    if (bal == 0) continue;
+    if (pass) {
+      const int q = count + __popc(bal & ((1u << lane) - 1));
+      qk[q] = key;
+      qi[q] = j;
+    }
+    count += __popc(bal);
+    if (count > KP - 32) flush();
+  }
+  if (count > 0) flush();
+  const size_t row = g0 + i;
+  for (int s = lane; s < a.k; s += 32) {
+    const size_t o = row * a.k + s;
+    const bool kept = li[s] != IMAX;
+    a.out_idx[o] = kept ? li[s] : (a.out_ok ? i : -1);
+    if (a.out_ok) a.out_ok[o] = kept ? 1 : 0;
+  }
+  if (a.out_count) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) nin += __shfl_xor_sync(0xffffffffu, nin, o);
+    if (lane == 0) a.out_count[row] = nin;
+  }
+}
+
 template <typename T, int CD, int PBC>
 static int launch_cell(const RadArgs<T>& a, cudaStream_t st) {
   const size_t nodes = (size_t)a.B * a.N;
@@ -418,7 +552,16 @@ static int launch_cell(const RadArgs<T>& a, cudaStream_t st) {
   EGNN_LAUNCH_CHECK();
   radius_scatter_kernel<T, CD, PBC><<<gn, RS_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
-  radius_query_kernel<T, CD, PBC><<<(unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), RS_WARPS * 32, 0, st>>>(a);
+  if (a.k <= 32) {
+    radius_query_kernel<T, CD, PBC><<<(unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), RS_WARPS * 32, 0, st>>>(a);
+  } else {
+    int KP = 64;
+    while (KP < a.k) KP <<= 1;
+    const size_t per_warp = (size_t)2 * KP * (sizeof(T) + sizeof(int));
+    const int warps = per_warp * RS_WARPS <= RS_WIDE_SMEM ? RS_WARPS : RS_WARPS / 2;      // fp64 at k > 128: 4 warps
+    radius_query_wide_kernel<T, CD, PBC><<<(unsigned)((nodes + warps - 1) / warps), warps * 32, warps * per_warp, st>>>(
+        a, KP);
+  }
   EGNN_LAUNCH_CHECK();
   count_launch(4);
   return EGNN_OK;
@@ -455,19 +598,20 @@ static int cell_select(int B, int N, int C, int k, const void* coors, const uint
   }
 }
 
-static int radius_check(int B, int N, int C, int k) {
+static int radius_check(int B, int N, int C, int k, int max_k) {
   if (B <= 0 || N <= 0 || C <= 0 || k <= 0 || k > N) return EGNN_ERR_SHAPE;
-  if (k > 32 || C > 3) return EGNN_ERR_UNSUPPORTED;
+  if (k > max_k || C > 3) return EGNN_ERR_UNSUPPORTED;
   if ((long long)B * rs_buckets(N) > 0x7fffffffLL) return EGNN_ERR_SHAPE;    // int bucket and node offsets
   return EGNN_OK;
 }
 
-// r2 is the radius as the caller passes it; the kernels compare against (T)r2.
+// r2 is the radius as the caller passes it; the kernels compare against (T)r2.  k up to RS_WIDE_MAX_K: the callers bound
+// it (egnn_radius_select at 32, cell_select_eligible by the descriptor's flags).
 int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
                          const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
                          cudaStream_t st, int pbc) {
   if (!coors || !out_idx || !ws) return EGNN_ERR_NULL;
-  EGNN_TRY(radius_check(B, N, C, k));
+  EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
   if (dtype == EGNN_DTYPE_F64) {
     if (!(r2 > 0.0)) return EGNN_ERR_SHAPE;
     return cell_select<double>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
@@ -477,34 +621,62 @@ int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* 
   return cell_select<float>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
 }
 
+// The public entries: egnn_radius_select* with k <= 32, egnn_radius_select_wide* with k <= RS_WIDE_MAX_K.
+static int radius_ws_entry(int max_k, int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
+  if (!out_bytes) return EGNN_ERR_NULL;
+  EGNN_TRY(radius_check(B, N, C, k, max_k));
+  *out_bytes = cell_select_ws_bytes(B, N, C, 8);               // sized for float64 coordinates: covers both types
+  return EGNN_OK;
+}
+
+// lattice: a [B,C] box (pbc = PBC_BOX, may be null) or a [B,C,C] cell (PBC_CELL)
+static int radius_entry(int max_k, int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                        const uint8_t* mask, const void* lattice, double r2, int32_t* out_idx, int32_t* out_count,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  if (!workspace || (pbc == PBC_CELL && !lattice)) return EGNN_ERR_NULL;
+  if (pbc == PBC_CELL && (C < 2 || C > 3)) return EGNN_ERR_SHAPE;    // a cell is 2-D or 3-D (before radius_check's C > 3)
+  EGNN_TRY(radius_check(B, N, C, k, max_k));
+  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
+  if (workspace_bytes < cell_select_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
+  return cell_select_dispatch(dtype, B, N, C, k, coors, mask, lattice, r2, out_idx, nullptr, out_count, workspace,
+                              static_cast<cudaStream_t>(stream), pbc);
+}
+
 }  // namespace egnn
 
 extern "C" int egnn_radius_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
-  if (!out_bytes) return EGNN_ERR_NULL;
-  EGNN_TRY(egnn::radius_check(B, N, C, k));
-  *out_bytes = egnn::cell_select_ws_bytes(B, N, C, 8);      // sized for float64 coordinates: covers both types
-  return EGNN_OK;
+  return egnn::radius_ws_entry(32, B, N, C, k, out_bytes);
 }
 
 extern "C" int egnn_radius_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
                                   const uint8_t* mask, const void* box, double r2, int32_t* out_idx, int32_t* out_count,
                                   void* workspace, size_t workspace_bytes, void* stream) {
-  if (!workspace) return EGNN_ERR_NULL;
-  EGNN_TRY(egnn::radius_check(B, N, C, k));
-  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
-  if (workspace_bytes < egnn::cell_select_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
-  return egnn::cell_select_dispatch(dtype, B, N, C, k, coors, mask, box, r2, out_idx, nullptr, out_count, workspace,
-                                    static_cast<cudaStream_t>(stream), egnn::PBC_BOX);
+  return egnn::radius_entry(32, egnn::PBC_BOX, dtype, B, N, C, k, coors, mask, box, r2, out_idx, out_count, workspace,
+                            workspace_bytes, stream);
 }
 
 extern "C" int egnn_radius_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
                                             const uint8_t* mask, const void* cell, double r2, int32_t* out_idx,
                                             int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream) {
-  if (!workspace || !cell) return EGNN_ERR_NULL;
-  if (C < 2 || C > 3) return EGNN_ERR_SHAPE;               // a cell is 2-D or 3-D (before radius_check's C > 3)
-  EGNN_TRY(egnn::radius_check(B, N, C, k));
-  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
-  if (workspace_bytes < egnn::cell_select_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
-  return egnn::cell_select_dispatch(dtype, B, N, C, k, coors, mask, cell, r2, out_idx, nullptr, out_count, workspace,
-                                    static_cast<cudaStream_t>(stream), egnn::PBC_CELL);
+  return egnn::radius_entry(32, egnn::PBC_CELL, dtype, B, N, C, k, coors, mask, cell, r2, out_idx, out_count, workspace,
+                            workspace_bytes, stream);
+}
+
+extern "C" int egnn_radius_select_wide_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
+  return egnn::radius_ws_entry(egnn::RS_WIDE_MAX_K, B, N, C, k, out_bytes);
+}
+
+extern "C" int egnn_radius_select_wide(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                                       const uint8_t* mask, const void* box, double r2, int32_t* out_idx,
+                                       int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream) {
+  return egnn::radius_entry(egnn::RS_WIDE_MAX_K, egnn::PBC_BOX, dtype, B, N, C, k, coors, mask, box, r2, out_idx,
+                            out_count, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_radius_select_wide_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k,
+                                                 const void* coors, const uint8_t* mask, const void* cell, double r2,
+                                                 int32_t* out_idx, int32_t* out_count, void* workspace,
+                                                 size_t workspace_bytes, void* stream) {
+  return egnn::radius_entry(egnn::RS_WIDE_MAX_K, egnn::PBC_CELL, dtype, B, N, C, k, coors, mask, cell, r2, out_idx,
+                            out_count, workspace, workspace_bytes, stream);
 }

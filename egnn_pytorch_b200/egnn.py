@@ -38,7 +38,8 @@ import torch.nn.functional as F
 
 from . import _native as nat
 
-__all__ = ["EGNN", "EGNN_Network", "CoorsNorm", "GlobalLinearAttention", "edge_index_to_neighbors", "radius_neighbors"]
+__all__ = ["EGNN", "EGNN_Network", "CoorsNorm", "GlobalLinearAttention", "edge_index_to_neighbors", "radius_neighbors",
+           "radius_neighbors_wide"]
 
 
 def exists(v):
@@ -73,6 +74,17 @@ _KERNEL_DTYPE = {torch.float32: nat.DTYPE_F32, torch.float64: nat.DTYPE_F64, tor
 _PATH_NAME = {torch.float64: "fp64-simt", torch.float32: "fp32-simt", torch.bfloat16: "bf16-tc"}
 # k > 32: knn_block_sort_kernel sorts a row's next_pow2(N) (rank, index) pairs in at most 200 KiB of shared memory
 SELECT_SORT_MAX_N = 16384
+
+
+def _raise_if_sort_limit(err, sort_limited, k, n):
+    """A layer with k > 32 that the cell grid does not serve (no mask, no finite valid_radius, N below the grid's
+    threshold, ...) ranks each row with a shared-memory sort of all N nodes; the forward rejects such a layer beyond
+    SELECT_SORT_MAX_N as unsupported.  That error, and only that one, is reported as the sort's limit."""
+    if sort_limited and err.code == nat.ERR_UNSUPPORTED and err.fn.startswith("egnn_layer_forward"):
+        raise RuntimeError(f"num_nearest_neighbors={k} > 32 ranks each node with a shared-memory sort of all N nodes, "
+                           f"which holds at most N={SELECT_SORT_MAX_N}, got N={n}: use k <= 32, give the layer a mask "
+                           f"and a finite valid_radius (the cell grid then selects up to 256 neighbours), or pass "
+                           f"neighbors= (e.g. from radius_neighbors_wide)") from None
 
 
 def _ptr(t):
@@ -421,6 +433,7 @@ class EGNN(nn.Module):
 
         use_nearest = self.num_nearest_neighbors > 0 or self.only_sparse_neighbors          # reference :230
         adj_u8 = None
+        sort_limited = False
         k = 0
         flags = self._flags()
         if slot_edges:
@@ -447,10 +460,10 @@ class EGNN(nn.Module):
             if not (0 < k <= n):
                 raise RuntimeError(f"number of neighbours k={k} must satisfy 0 < k <= N={n} (torch.topk would raise)")
             row_scan = self.only_sparse_neighbors and exists(mask) and adj_u8 is not None     # no ranking (select_neighbors)
-            if k > 32 and n > SELECT_SORT_MAX_N and not row_scan:
-                raise RuntimeError(f"num_nearest_neighbors={k} > 32 ranks each node with a shared-memory sort of all N nodes, "
-                                   f"which holds at most N={SELECT_SORT_MAX_N}, got N={n}: use k <= 32, or pass "
-                                   f"neighbors= (e.g. from radius_neighbors)")
+            if k > 32:
+                flags |= nat.FLAG_CELL_SELECT_WIDE       # a radius graph with a mask may select on the cell grid
+                # otherwise the all-pairs sort ranks each row, which the library rejects beyond SELECT_SORT_MAX_N
+                sort_limited = n > SELECT_SORT_MAX_N and not row_scan
 
         # support does not depend on the list length (any k > 0 runs the tensor cores), so one cached "unsupported"
         # entry for all k > 32 stays correct
@@ -461,6 +474,7 @@ class EGNN(nn.Module):
             return self._run(lib, dev, kdt, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
                              b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, train, param_fields, drop_p, box, cell)
         except nat.EgnnNativeError as e:
+            _raise_if_sort_limit(e, sort_limited, k, n)
             if e.code != nat.ERR_UNSUPPORTED or kdt != torch.bfloat16:
                 raise
         # the tensor-core kernels do not cover this option set: fp32 SIMT kernels (still on the GPU); remembered
@@ -469,8 +483,12 @@ class EGNN(nn.Module):
                       f"edge_dim={cont_edge_dim}, label_dim={label_dim}, m_dim={self.m_dim}, fourier={self.fourier_features}); "
                       f"running the fp32 SIMT kernels instead (about 5x slower, same results to fp32 accuracy)", UserWarning,
                       stacklevel=3)
-        return self._run(lib, dev, torch.float32, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
-                         b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, box=box, cell=cell)
+        try:
+            return self._run(lib, dev, torch.float32, feats, coors, edges, mask, adj_u8, _edge_labels, _label_emb,
+                             b, n, c, k, flags, cont_edge_dim, label_dim, _rows, nbr, box=box, cell=cell)
+        except nat.EgnnNativeError as e:
+            _raise_if_sort_limit(e, sort_limited, k, n)
+            raise
 
     def _run(self, lib, dev, kdt, feats, coors, edges, mask, adj_u8, labels, label_emb, b, n, c, k, flags,
              cont_edge_dim, label_dim, rows, nbr=None, train=False, param_fields=None, drop_p=0.0, box=None, cell=None):
@@ -716,7 +734,7 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return
     `coors` float32 or float64 [B, N, C] with C <= 3, on any device (CPU tensors are staged to the current CUDA
     device; the results come back on `coors`'s device).  `cutoff` is a distance: the squared distance computed in the
     coordinates' type is compared with `float(cutoff) ** 2` cast to that type.  (The layer's `valid_radius`, as in the
-    reference, is a *squared* distance.)  `k` in [1, min(32, N)].  `mask` [B, N] bool / 0-1: a padded node is never a
+    reference, is a *squared* distance.)  `k` in [1, min(32, N)] (`radius_neighbors_wide` takes up to 256).  `mask` [B, N] bool / 0-1: a padded node is never a
     neighbour and its own list is empty.  `box` [C] or [B, C]: periodic box lengths as `EGNN.forward(box=)` takes them
     (minimum-image distances; 0 or inf: the axis is not periodic).  `cell` [C, C] or [B, C, C] (C in {2, 3}), instead
     of `box`: a lower-triangular triclinic cell as `EGNN.forward(cell=)` takes it (distances of the wrapped pair
@@ -726,6 +744,19 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return
     With `return_counts=True` it returns `(neighbors, counts)`: counts int32 [B, N] is the number of nodes within the
     cutoff before the truncation at k (the node itself included), so `counts > k` shows where k cut the list short.
     Nothing synchronises with the host: the call can be captured in a CUDA graph."""
+    return _radius_graph("radius_neighbors", 32, coors, cutoff, k, mask, box, cell, return_counts)
+
+
+def radius_neighbors_wide(coors, cutoff, k, *, mask=None, box=None, cell=None, return_counts=False):
+    """`radius_neighbors` for lists of up to 256 neighbours: `k` in [1, min(256, N)], everything else the same -- the
+    lists equal the all-pairs select's kept slots exactly, nearest first, ties to the lower index, -1 in the empty
+    slots; `return_counts=True` also returns the in-radius counts before truncation.  For k <= 32 the result is
+    `radius_neighbors`'s.  Longer lists (40-100 neighbours within a cutoff are common in condensed-phase atomistic
+    systems) are kept in shared memory instead of one warp's lanes (`egnn_radius_select_wide`)."""
+    return _radius_graph("radius_neighbors_wide", 256, coors, cutoff, k, mask, box, cell, return_counts)
+
+
+def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts):
     if not torch.is_tensor(coors) or coors.dim() != 3:
         raise ValueError(f"coors must be a [B, N, C] tensor, got {type(coors).__name__}"
                          f"{' of shape ' + str(tuple(coors.shape)) if torch.is_tensor(coors) else ''}")
@@ -735,9 +766,9 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return
     if b < 1 or n < 1:
         raise ValueError(f"coors must hold at least one node in at least one graph, got shape {tuple(coors.shape)}")
     if not 1 <= c <= 3:
-        raise ValueError(f"radius_neighbors supports C <= 3 coordinates, got C={c}")
-    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(32, n):
-        raise ValueError(f"k must be an int in [1, min(32, N)] = [1, {min(32, n)}], got {k!r}")
+        raise ValueError(f"{name} supports C <= 3 coordinates, got C={c}")
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(max_k, n):
+        raise ValueError(f"k must be an int in [1, min({max_k}, N)] = [1, {min(max_k, n)}], got {k!r}")
     cutoff = float(cutoff)
     if not (cutoff > 0.0 and math.isfinite(cutoff)):
         raise ValueError(f"cutoff must be a finite distance > 0, got {cutoff}")
@@ -764,15 +795,16 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return
         out = torch.empty((b, n, k), dtype=torch.int32, device=dev)
         counts = torch.empty((b, n), dtype=torch.int32, device=dev) if return_counts else None
         nb = C.c_size_t()
-        nat.check("egnn_radius_select_workspace_bytes", lib.egnn_radius_select_workspace_bytes(b, n, c, k, C.byref(nb)))
+        entry = "egnn_radius_select" if max_k == 32 else "egnn_radius_select_wide"
+        nat.check(f"{entry}_workspace_bytes", getattr(lib, f"{entry}_workspace_bytes")(b, n, c, k, C.byref(nb)))
         stream_handle = torch.cuda.current_stream(dev).cuda_stream
         ws = _workspace(dev, nb.value, stream_handle)
         if cl is not None:
-            nat.check("egnn_radius_select_triclinic", lib.egnn_radius_select_triclinic(
+            nat.check(f"{entry}_triclinic", getattr(lib, f"{entry}_triclinic")(
                 _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(cl), r2, _ptr(out), _ptr(counts),
                 _ptr(ws), ws.numel(), C.c_void_p(stream_handle)))
         else:
-            nat.check("egnn_radius_select", lib.egnn_radius_select(
+            nat.check(entry, getattr(lib, entry)(
                 _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(bx), r2, _ptr(out), _ptr(counts),
                 _ptr(ws), ws.numel(), C.c_void_p(stream_handle)))
     if out.device != coors.device:

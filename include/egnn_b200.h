@@ -72,6 +72,11 @@ extern "C" {
                                                backward's per-pair buffers are sized by the block, [B, R, J, *] with
                                                R = row_end - row_begin; egnn_layer_backward returns the gradient of
                                                sum_{b, i in block} <g_out[b,i], out[b,i]>.  See EgnnLayerGrads */
+#define EGNN_FLAG_CELL_SELECT_WIDE (1u << 11) /* lets a layer with 32 < k <= 256 select its lists on the cell grid
+                                               (egnn_radius_select_wide) when it is otherwise eligible (C <= 3, a finite
+                                               valid_radius, no adjacency or per-slot edges; DESIGN.md section 5).  Such a
+                                               descriptor's workspace ends in the cell grid's scratch.  Without the flag a
+                                               layer with k > 32 ranks all pairs, and its workspace is unchanged */
 
 /*
  * Static description of one layer call.  E = 2*dim + 2*fourier + 1 + edge_dim + label_dim
@@ -297,8 +302,9 @@ int egnn_adj_neighbors(int32_t B, int32_t N, int32_t k, const uint8_t* adj, int3
  * with rank <= r2, ascending, ties to the lowest index -- exactly the ok = 1 slots of egnn_knn_select with the same
  * coordinates, mask and valid_radius = r2 (rank = squared distance computed in the coordinates' type; minimum image
  * under `box`).  A padded node (mask 0) or one with a non-finite coordinate is never a neighbour, and its own row is
- * empty.  egnn_layer_forward runs the same search for an eligible layer (k <= 32, C <= 3, a mask, a finite
- * valid_radius, no adjacency; DESIGN.md section 5) once N reaches a size threshold (EGNN_B200_CELL_SELECT_MIN_N).
+ * empty.  egnn_layer_forward runs the same search for an eligible layer (k <= 32, or k <= 256 under
+ * EGNN_FLAG_CELL_SELECT_WIDE; C <= 3, a mask, a finite valid_radius, no adjacency; DESIGN.md section 5) once N
+ * reaches a size threshold (EGNN_B200_CELL_SELECT_MIN_N).
  * coors [B,N,C] (float32, or float64 when dtype == EGNN_DTYPE_F64); mask [B,N] 0/1 or NULL (all valid); box [B,C] in
  * the coordinates' type or NULL, as egnn_layer_forward_periodic takes it; r2 > 0 (EGNN_ERR_SHAPE otherwise), a squared
  * distance, compared as (float)r2 for float32 coordinates.  out_idx int32 [B,N,k]: the kept neighbours, then -1 in every
@@ -316,6 +322,17 @@ int egnn_radius_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k
 int egnn_radius_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
                                  const uint8_t* mask, const void* cell, double r2, int32_t* out_idx, int32_t* out_count,
                                  void* workspace, size_t workspace_bytes, void* stream);
+/* egnn_radius_select / egnn_radius_select_triclinic / their workspace size for lists of 1 <= k <= min(256, N)
+ * (k > 256: EGNN_ERR_UNSUPPORTED); the same arguments, checks, error codes and workspace.  For k <= 32 the output is
+ * exactly that of the k <= 32 entries; longer lists are kept in shared memory instead of a warp's lanes, with the same
+ * result: the ok = 1 slots of egnn_knn_select, independent of the order the grid was filled in. */
+int egnn_radius_select_wide_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes);
+int egnn_radius_select_wide(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                            const uint8_t* mask, const void* box, double r2, int32_t* out_idx, int32_t* out_count,
+                            void* workspace, size_t workspace_bytes, void* stream);
+int egnn_radius_select_wide_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                                      const uint8_t* mask, const void* cell, double r2, int32_t* out_idx,
+                                      int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream);
 
 /* N-th degree adjacency of EGNN_Network (egnn_pytorch.py:414-428) without the dense A@A:
  * adj_in [N,N] or [B,N,N] 0/1; writes the expanded adjacency adj_out [B,N,N] 0/1, the degree
