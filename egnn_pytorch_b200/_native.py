@@ -25,6 +25,7 @@ FLAG_ADJ_BATCHED = 1 << 8
 FLAG_EDGES_PER_SLOT = 1 << 9
 FLAG_ROW_PARTIAL_GRADS = 1 << 10
 FLAG_CELL_SELECT_WIDE = 1 << 11
+FLAG_KNN_GRID = 1 << 12
 
 ERR_UNSUPPORTED = -3
 
@@ -150,6 +151,12 @@ SYMBOLS = {
     "egnn_radius_select_wide_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                                     C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p,
                                                     C.c_void_p, C.c_size_t, C.c_void_p]),
+    "egnn_knn_grid_select_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P(C.c_size_t)]),
+    "egnn_knn_grid_select": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "egnn_knn_grid_select_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                 C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                 C.c_size_t, C.c_void_p]),
     "egnn_adj_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_size_t)]),
     "egnn_adj_expand": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -82,7 +82,8 @@ int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nb
 
 // The cell-grid radius select (radius_select.cu).  A layer is eligible from its descriptor alone (1 <= k <= 32, or <= 256
 // under EGNN_FLAG_CELL_SELECT_WIDE, C <= 3, 0 < (T)valid_radius < 1e5, no only_sparse / batched adjacency / per-slot edges); its forward workspace then carries
-// cell_select_layer_ws_bytes(d) bytes of scratch (0 for a layer that is not eligible), whatever the size threshold.
+// cell_select_layer_ws_bytes(d) bytes of scratch (0 for a layer that neither grid may serve; the kNN grid's, which
+// contains the radius grid's, under EGNN_FLAG_KNN_GRID), whatever the size thresholds.
 // cell_select_runs adds what the call decides: a mask, no adjacency, no caller lists and N >= the threshold.
 bool cell_select_eligible(const EgnnLayerDesc& d);
 size_t cell_select_layer_ws_bytes(const EgnnLayerDesc& d);
@@ -90,6 +91,13 @@ bool cell_select_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io);
 int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
                          const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
                          cudaStream_t st, int pbc);
+// The kNN grid (radius_select.cu): under EGNN_FLAG_KNN_GRID a layer is eligible from its descriptor alone (1 <= k <= 32,
+// or <= 256 under EGNN_FLAG_CELL_SELECT_WIDE, C <= 3, no only_sparse / batched adjacency / per-slot edges), and its
+// workspace then ends in the kNN grid's scratch (cell_select_layer_ws_bytes).  knn_grid_runs adds what the call decides:
+// the radius grid does not run, no adjacency, no caller lists and N >= the threshold.
+bool knn_grid_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io);
+int knn_grid_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box,
+                      double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st, int pbc);
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {

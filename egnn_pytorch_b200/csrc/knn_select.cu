@@ -431,6 +431,9 @@ int select_neighbors(const EgnnLayerDesc& d, const EgnnLayerIO& io, int32_t** nb
   if (cell_ws && cell_select_runs(d, io))            // a radius graph with a mask: the same kept slots from a cell grid
     return cell_select_dispatch(cdt, d.B, d.N, d.C, d.k, io.coors, io.mask, box, d.valid_radius, *nbr_idx, *nbr_ok,
                                 nullptr, cell_ws, st, pbc);
+  if (cell_ws && knn_grid_runs(d, io))               // the same lists from the kNN grid
+    return knn_grid_dispatch(cdt, d.B, d.N, d.C, d.k, io.coors, io.mask, box, d.valid_radius, *nbr_idx, *nbr_ok, cell_ws,
+                             st, pbc);
   count_launch();
   const int adj_batched = (d.flags & EGNN_FLAG_ADJ_BATCHED) ? 1 : 0;
   if ((d.flags & EGNN_FLAG_ONLY_SPARSE) && io.mask && io.adj)      // every slot top-k could add is masked out: row scan

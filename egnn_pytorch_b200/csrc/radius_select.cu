@@ -21,9 +21,17 @@
 //   query   one warp per node, nodes taken in cell order: the deduplicated buckets of the 3^C cells around the node
 //           are read as one flattened candidate stream, filtered by rank <= r2 and against the current k-th entry,
 //           queued and merged 32 at a time; for k > 32 (radius_query_wide_kernel) the list lives in shared memory.
+//
+// The kNN grid (egnn_knn_grid_select, the second half of this file) answers the plain k-nearest query with no cutoff on
+// the same count / scan / scatter, with a dense grid whose cell edge each graph sizes on the device from its extent
+// (knn_grid_setup_kernel), and a query that visits Chebyshev rings of cells until no unvisited node can rank before
+// the k-th (knn_ring_kernel).  Rows the grid cannot decide are ranked against every node of their graph
+// (knn_scan_kernel); padded rows are written directly.  Its lists equal egnn_knn_select's bit for bit (DESIGN.md
+// section 5).
 #include "common.cuh"
 #include "profile.h"
 #include "warp_select.cuh"
+#include <cub/block/block_reduce.cuh>
 #include <cub/block/block_scan.cuh>
 
 namespace egnn {
@@ -34,6 +42,7 @@ constexpr int RS_WARPS = 8;              // query rows per CTA
 constexpr int RS_WIDE_MAX_K = 256;       // the longest list the query keeps (radius_query_wide_kernel above 32)
 constexpr size_t RS_WIDE_SMEM = 32768;   // wide query: dynamic shared memory per CTA, within the 48 KiB default
 constexpr double RS_CLAMP = 1073741824.0;     // 2^30: aperiodic cell coordinates and periodic cell counts
+constexpr int GRID_RADIUS = 0, GRID_KNN = 1;  // which grid the count / scatter kernels bin into
 
 // Buckets per graph: next_pow2(2N).
 static inline int rs_buckets(int N) {
@@ -68,8 +77,15 @@ bool cell_select_eligible(const EgnnLayerDesc& d) {
   return r2 > 0.0 && r2 < 1e5;
 }
 
+size_t knn_grid_ws_bytes(int B, int N, int C, size_t coord_bytes);
+bool knn_grid_eligible(const EgnnLayerDesc& d);
+
+// The radius grid's scratch for a layer it may serve; under EGNN_FLAG_KNN_GRID the kNN grid's, which is larger, for a
+// layer the kNN grid may serve (either can run, depending on the call's mask).
 size_t cell_select_layer_ws_bytes(const EgnnLayerDesc& d) {
-  return cell_select_eligible(d) ? cell_select_ws_bytes(d.B, d.N, d.C, d.dtype == EGNN_DTYPE_F64 ? 8 : 4) : 0;
+  const size_t cb = d.dtype == EGNN_DTYPE_F64 ? 8 : 4;
+  if (knn_grid_eligible(d)) return knn_grid_ws_bytes(d.B, d.N, d.C, cb);
+  return cell_select_eligible(d) ? cell_select_ws_bytes(d.B, d.N, d.C, cb) : 0;
 }
 
 // Smallest N per graph at which an eligible layer runs the cell grid (DESIGN.md section 6).  EGNN_B200_CELL_SELECT_MIN_N
@@ -83,6 +99,21 @@ static long cell_select_min_n() {
 bool cell_select_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io) {
   return io.mask && !io.adj && !io.nbr_idx && cell_select_eligible(d) && d.N >= cell_select_min_n();
 }
+
+// The kNN grid of one graph, set by knn_grid_setup_kernel and read by every later launch (no host round trip).
+// Cell coordinate c of a node: on an aperiodic axis floor((x_c - lo[c]) / cs), in [0, n[c]); on a periodic axis the
+// position (x_c, or the fractional coordinate under a cell) wrapped into [0, L[c]) and cut into n[c] cells.
+struct KGrid {
+  double cs;          // cell edge of the aperiodic axes
+  double lo[3];       // aperiodic axis: the smallest coordinate of the graph's insertable nodes
+  double L[3];        // periodic axis: the binned period (the box length, or 1 for a fractional coordinate); 0 aperiodic
+  double w[3];        // a node one cell further along axis c is at least this much further away (cs, L / n, w_c / n)
+  double G[3][3];     // PBC_CELL: the inverse cell (cell_inverse)
+  double err;         // absolute rounding allowance of the stopping test
+  int n[3];           // cells per axis (1 beyond C); their product is at most Tb
+  int ok;             // 0: no usable grid (fewer than k insertable nodes, a non-finite extent): every row is scanned
+};
+static_assert(sizeof(KGrid) == 176, "KGrid layout");
 
 template <typename T>
 struct RadArgs {
@@ -99,6 +130,11 @@ struct RadArgs {
   int32_t* out_idx;                // [B,N,k]
   uint8_t* out_ok;                 // [B,N,k] or null (then empty slots hold -1)
   int32_t* out_count;              // [B,N] in-radius nodes per row, or null
+  // the kNN grid only
+  KGrid* kg;                       // [B]
+  int* fb_rows;                    // [B*N] rows (b*N + i) left to knn_scan_kernel
+  int* fb_count;                   // their number
+  T vr;                            // ok = rank <= vr
 };
 
 // Axis c of graph b's grid: n[c] > 0 cells of width w[c] on a periodic axis of length L[c]; n[c] = 0 on an aperiodic one.
@@ -153,11 +189,11 @@ __device__ __forceinline__ bool load_node(const RadArgs<T>& a, size_t t, T (&x)[
 // A with 1 in place of every aperiodic diagonal, wrapped into [0, 1) and cut into n_k = max(1, floor(w_k / cs)) cells,
 // w_k = 1 / |column k of G| being the cell's perpendicular width along a_k.  An aperiodic axis (its row and column of
 // A are zero but for the diagonal, so s_k = x_k) is binned as without a cell.  Double precision throughout.
+// G = A^-1 of graph b's lower-triangular cell A (m: [CD][CD]) with 1 in place of every aperiodic diagonal (per[r]:
+// axis r is periodic); column k of G by forward substitution down the rows, in double.
 template <typename T, int CD>
-__device__ __forceinline__ void frac_cells(const RadArgs<T>& a, int b, const T (&x)[CD], int (&cc)[CD], int (&n)[CD]) {
-  const T* m = a.box + (size_t)b * CD * CD;
-  double A[CD][CD], G[CD][CD];
-  bool per[CD];
+__device__ __forceinline__ void cell_inverse(const T* m, double (&G)[CD][CD], bool (&per)[CD]) {
+  double A[CD][CD];
 #pragma unroll
   for (int r = 0; r < CD; ++r) {
 #pragma unroll
@@ -166,7 +202,7 @@ __device__ __forceinline__ void frac_cells(const RadArgs<T>& a, int b, const T (
     if (!per[r]) A[r][r] = 1.0;
   }
 #pragma unroll
-  for (int k = 0; k < CD; ++k) {                       // column k of G: forward substitution down the rows
+  for (int k = 0; k < CD; ++k) {
     G[k][k] = 1.0 / A[k][k];
 #pragma unroll
     for (int r = k + 1; r < CD; ++r) {
@@ -176,6 +212,18 @@ __device__ __forceinline__ void frac_cells(const RadArgs<T>& a, int b, const T (
       G[r][k] = -acc / A[r][r];
     }
   }
+}
+
+// PBC_CELL: the cell coordinates cc of x in graph b's grid, and the cell count n of every axis (0: aperiodic).  A
+// periodic axis k is binned in the fractional coordinate s_k = sum_d x_d G[d][k] (cell_inverse), wrapped into [0, 1)
+// and cut into n_k = max(1, floor(w_k / cs)) cells, w_k = 1 / |column k of G| being the cell's perpendicular width
+// along a_k.  An aperiodic axis (its row and column of A are zero but for the diagonal, so s_k = x_k) is binned as
+// without a cell.  Double precision throughout.
+template <typename T, int CD>
+__device__ __forceinline__ void frac_cells(const RadArgs<T>& a, int b, const T (&x)[CD], int (&cc)[CD], int (&n)[CD]) {
+  double G[CD][CD];
+  bool per[CD];
+  cell_inverse<T, CD>(a.box + (size_t)b * CD * CD, G, per);
 #pragma unroll
   for (int k = 0; k < CD; ++k) {
     double s = 0.0, g2 = 0.0;
@@ -200,21 +248,77 @@ __device__ __forceinline__ int node_bucket(const RadArgs<T>& a, int b, const T (
   return cell_bucket<CD>(cc, a.Tb);
 }
 
+// Cell coordinates of x in the kNN grid g, each in [0, g.n[c]).
 template <typename T, int CD, int PBC>
-__global__ void __launch_bounds__(RS_THREADS) radius_count_kernel(const RadArgs<T> a) {
-  const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
-  if (t >= (size_t)a.B * a.N) return;
-  const int b = (int)(t / a.N), i = (int)(t % a.N);
-  T x[CD];
-  if (!load_node<T, CD>(a, t, x)) {                   // not in the grid: its row is empty
+__device__ __forceinline__ void knn_cell(const KGrid& g, const T (&x)[CD], int (&cc)[CD]) {
+#pragma unroll
+  for (int c = 0; c < CD; ++c) {
+    double s = (double)x[c];
+    if constexpr (PBC == PBC_CELL) {
+      s = 0.0;
+#pragma unroll
+      for (int d = c; d < CD; ++d) s = fma((double)x[d], g.G[d][c], s);
+    }
+    const int n = g.n[c];
+    if (g.L[c] > 0.0) cc[c] = cell_coord(s, g.cs, g.L[c], g.L[c] / n, n);
+    else cc[c] = (int)fmin(fmax(floor((s - g.lo[c]) / g.cs), 0.0), (double)(n - 1));
+  }
+}
+
+template <int CD>
+__device__ __forceinline__ int knn_index(const KGrid& g, const int (&cc)[CD]) {
+  int t = cc[CD - 1];
+#pragma unroll
+  for (int c = CD - 2; c >= 0; --c) t = t * g.n[c] + cc[c];
+  return t;
+}
+
+// The bucket node x of graph b goes to: a hashed radius cell, or a dense kNN cell.
+template <typename T, int CD, int PBC, int GRID>
+__device__ __forceinline__ int grid_bucket(const RadArgs<T>& a, int b, const T (&x)[CD]) {
+  if constexpr (GRID == GRID_KNN) {
+    int cc[CD];
+    knn_cell<T, CD, PBC>(a.kg[b], x, cc);
+    return knn_index<CD>(a.kg[b], cc);
+  } else {
+    return node_bucket<T, CD, PBC>(a, b, x);
+  }
+}
+
+// Row t = b*N + i of a node the grid does not hold.  The radius grid leaves it empty.  The kNN grid writes a padded
+// row (every rank 1e5 in egnn_knn_select: slots 0 .. k-1 with ok = (1e5 <= vr)) and leaves a non-finite node's row to
+// the full scan.
+template <typename T, int GRID>
+__device__ __forceinline__ void outside_row(const RadArgs<T>& a, size_t t, int i) {
+  if constexpr (GRID == GRID_KNN) {
+    if (a.mask && !a.mask[t]) {
+      for (int s = 0; s < a.k; ++s) {
+        a.out_idx[t * a.k + s] = s;
+        if (a.out_ok) a.out_ok[t * a.k + s] = T(1e5) <= a.vr ? 1 : 0;
+      }
+    } else {
+      a.fb_rows[atomicAdd(a.fb_count, 1)] = (int)t;
+    }
+  } else {
     for (int s = 0; s < a.k; ++s) {
       a.out_idx[t * a.k + s] = a.out_ok ? i : -1;
       if (a.out_ok) a.out_ok[t * a.k + s] = 0;
     }
     if (a.out_count) a.out_count[t] = 0;
+  }
+}
+
+template <typename T, int CD, int PBC, int GRID = GRID_RADIUS>
+__global__ void __launch_bounds__(RS_THREADS) radius_count_kernel(const RadArgs<T> a) {
+  const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
+  if (t >= (size_t)a.B * a.N) return;
+  const int b = (int)(t / a.N), i = (int)(t % a.N);
+  T x[CD];
+  if (!load_node<T, CD>(a, t, x)) {                   // not in the grid
+    outside_row<T, GRID>(a, t, i);
     return;
   }
-  atomicAdd(a.cnt + (size_t)b * a.Tb + node_bucket<T, CD, PBC>(a, b, x), 1);
+  atomicAdd(a.cnt + (size_t)b * a.Tb + grid_bucket<T, CD, PBC, GRID>(a, b, x), 1);
 }
 
 __global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_kernel(const int* __restrict__ cnt, int* __restrict__ start, int Tb) {
@@ -244,7 +348,7 @@ __global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_kernel(const int*
   }
 }
 
-template <typename T, int CD, int PBC>
+template <typename T, int CD, int PBC, int GRID = GRID_RADIUS>
 __global__ void __launch_bounds__(RS_THREADS) radius_scatter_kernel(const RadArgs<T> a) {
   const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
   if (t >= (size_t)a.B * a.N) return;
@@ -252,10 +356,26 @@ __global__ void __launch_bounds__(RS_THREADS) radius_scatter_kernel(const RadArg
   T x[CD];
   if (!load_node<T, CD>(a, t, x)) return;
   const size_t g0 = (size_t)b * a.N, BN = (size_t)a.B * a.N;
-  const int pos = atomicAdd(a.end + (size_t)b * a.Tb + node_bucket<T, CD, PBC>(a, b, x), 1);
+  const int pos = atomicAdd(a.end + (size_t)b * a.Tb + grid_bucket<T, CD, PBC, GRID>(a, b, x), 1);
 #pragma unroll
   for (int c = 0; c < CD; ++c) a.xs[c * BN + g0 + pos] = x[c];
   a.idx[g0 + pos] = i;
+}
+
+// The stream of the buckets the warp's lanes hold (bkt, where keep is set), flattened in lane order: returns its
+// length; wexcl / wdelta receive per lane its bucket's first stream position and its cell-order position minus that.
+__device__ __forceinline__ int bucket_stream(int lane, bool keep, int bkt, const int* cnt, const int* end, int* wexcl,
+                                             int* wdelta) {
+  int len = 0, beg = 0;
+  if (keep) { len = cnt[bkt]; beg = end[bkt] - len; }
+  int incl = len;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
+  const int total = __shfl_sync(0xffffffffu, incl, 31);
+  wexcl[lane] = incl - len;
+  wdelta[lane] = beg - (incl - len);
+  __syncwarp();
+  return total;
 }
 
 // The candidate stream of node i of graph b, which its warp reads t = lane, lane + 32, ...: the deduplicated buckets of
@@ -294,17 +414,30 @@ __device__ __forceinline__ int row_stream(const RadArgs<T>& a, int b, int lane, 
     bkt = cell_bucket<CD>(cc, a.Tb);
   }
   const unsigned same = __match_any_sync(0xffffffffu, bkt);
-  const bool keep = lane < NB && __ffs(same) - 1 == lane;
-  int len = 0, beg = 0;
-  if (keep) { len = cnt[bkt]; beg = end[bkt] - len; }
-  int incl = len;
+  return bucket_stream(lane, lane < NB && __ffs(same) - 1 == lane, bkt, cnt, end, wexcl, wdelta);
+}
+
+// The rank of the pair (xi, xj), as the all-pairs select computes it (xj(c) reads coordinate c of the other node;
+// bl / binv: the box of the graph under PBC_BOX, pc: its staged cell under PBC_CELL).
+template <typename T, int CD, int PBC, class XJ>
+__device__ __forceinline__ T pair_rank(const T (&xi)[CD], XJ xj, const T (&bl)[CD], const T (&binv)[CD], const T* pc) {
+  T d = T(0);
+  if constexpr (PBC == PBC_CELL) {
+    T r[3];
 #pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const int v = __shfl_up_sync(0xffffffffu, incl, o); if (lane >= o) incl += v; }
-  const int total = __shfl_sync(0xffffffffu, incl, 31);
-  wexcl[lane] = incl - len;
-  wdelta[lane] = beg - (incl - len);
-  __syncwarp();
-  return total;
+    for (int c = 0; c < 3; ++c) r[c] = c < CD ? xi[c < CD ? c : 0] - xj(c < CD ? c : 0) : T(0);
+    cell_wrap<T>(r[0], r[1], r[2], pc);
+#pragma unroll
+    for (int c = 0; c < CD; ++c) d = sq_acc<T>(r[c], d);
+  } else {
+#pragma unroll
+    for (int c = 0; c < CD; ++c) {
+      T r = xi[c] - xj(c);
+      if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
+      d = sq_acc<T>(r, d);
+    }
+  }
+  return d;
 }
 
 // Candidate t of the stream: its node index j and its rank, as the all-pairs select computes it (bl / binv: the box of
@@ -319,23 +452,7 @@ __device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t 
     if (wexcl[s + step] <= t) s += step;
   const size_t pos = g0 + wdelta[s] + t;
   j = a.idx[pos];
-  T d = T(0);
-  if constexpr (PBC == PBC_CELL) {
-    T r[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) r[c] = c < CD ? xi[c < CD ? c : 0] - a.xs[(c < CD ? c : 0) * BN + pos] : T(0);
-    cell_wrap<T>(r[0], r[1], r[2], pc);
-#pragma unroll
-    for (int c = 0; c < CD; ++c) d = sq_acc<T>(r[c], d);
-  } else {
-#pragma unroll
-    for (int c = 0; c < CD; ++c) {
-      T r = xi[c] - a.xs[c * BN + pos];
-      if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-      d = sq_acc<T>(r, d);
-    }
-  }
-  return d;
+  return pair_rank<T, CD, PBC>(xi, [&](int c) { return a.xs[c * BN + pos]; }, bl, binv, pc);
 }
 
 // The prologue of both query kernels: the node at cell-order position p of graph b (false: beyond the nodes the graph
@@ -355,83 +472,57 @@ __device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t 
     _Pragma("unroll") for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);                        \
   }
 
-// k <= 32: lane l keeps the l-th smallest (rank, j) so far; candidates in radius that beat the k-th are queued and merged
-// 32 at a time (warp_merge).
-template <typename T, int CD, int PBC>
-__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadArgs<T> a) {
-  __shared__ T qkey[RS_WARPS][64];
-  __shared__ int qidx[RS_WARPS][64];
-  __shared__ int sexcl[RS_WARPS][32];
-  __shared__ int sdelta[RS_WARPS][32];
-  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const size_t gw = (size_t)blockIdx.x * RS_WARPS + warp;
-  if (gw >= (size_t)a.B * a.N) return;
-  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
-  RS_QUERY_ROW()
-  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
-
-  const T INF = T(INFINITY);
-  const int IMAX = 0x7fffffff;
-  T* myqk = qkey[warp];
-  int* myqi = qidx[warp];
-  T bkey = INF; int bidx = IMAX;       // lane l: l-th smallest so far
-  T thr_key = INF; int thr_idx = IMAX; // the k-th smallest so far
-  int count = 0;                       // queued candidates (warp-uniform)
-  int nin = 0;                         // this lane's in-radius candidates
-  for (int t0 = 0; t0 < total; t0 += 32) {
-    const int t = t0 + lane;
-    T key = INF;
-    int j = IMAX;
-    bool pass = false;
-    if (t < total) {
-      const T d = stream_rank<T, CD, PBC>(a, g0, BN, t, sexcl[warp], sdelta[warp], xi, bl, binv, pc, j);
-      const bool in = d <= a.r2;
-      nin += in ? 1 : 0;
-      key = d;
-      pass = in && lex_less<T>(d, j, thr_key, thr_idx);
-    }
+// k <= 32: lane l keeps the l-th smallest (rank, j) so far (bkey, bidx); pairs that beat the k-th are queued in the
+// warp's 64 queue slots and merged 32 at a time (warp_merge).
+template <typename T>
+struct LaneList {
+  T* qk;
+  int* qi;
+  int k;
+  T bkey = T(INFINITY), thr_key = T(INFINITY);   // lane l: l-th smallest so far; the k-th smallest so far
+  int bidx = 0x7fffffff, thr_idx = 0x7fffffff;
+  int count = 0;                                 // queued pairs (warp-uniform)
+  __device__ __forceinline__ LaneList(T* qk_, int* qi_, int k_) : qk(qk_), qi(qi_), k(k_) {}
+  __device__ __forceinline__ bool beats(T key, int j) const { return lex_less<T>(key, j, thr_key, thr_idx); }
+  // queues the pairs of the lanes whose `pass` is set; called by the whole warp
+  __device__ __forceinline__ void push(bool pass, T key, int j, int lane) {
     const unsigned bal = __ballot_sync(0xffffffffu, pass);
-    if (bal == 0) continue;
+    if (bal == 0) return;
     if (pass) {
       const int q = count + __popc(bal & ((1u << lane) - 1));
-      myqk[q] = key;
-      myqi[q] = j;
+      qk[q] = key;
+      qi[q] = j;
     }
     count += __popc(bal);
     __syncwarp();
     if (count >= 32) {
-      T ckey = myqk[lane];
-      int cidx = myqi[lane];
+      T ckey = qk[lane];
+      int cidx = qi[lane];
       __syncwarp();
       if (lane + 32 < count) {         // shift the tail of the queue down
-        T tk = myqk[lane + 32]; int ti = myqi[lane + 32];
-        myqk[lane] = tk; myqi[lane] = ti;
+        T tk = qk[lane + 32]; int ti = qi[lane + 32];
+        qk[lane] = tk; qi[lane] = ti;
       }
       count -= 32;
       __syncwarp();
       warp_merge<T>(bkey, bidx, ckey, cidx, lane);
-      thr_key = shfl_idx_t<T>(bkey, a.k - 1);
-      thr_idx = __shfl_sync(0xffffffffu, bidx, a.k - 1);
+      refresh();
     }
   }
-  if (count > 0) {
-    T ckey = lane < count ? myqk[lane] : INF;
-    int cidx = lane < count ? myqi[lane] : IMAX;
-    warp_merge<T>(bkey, bidx, ckey, cidx, lane);
+  // merges what is still queued: lane l then holds the l-th smallest of every pair pushed
+  __device__ __forceinline__ void finish(int lane) {
+    if (count > 0) {
+      T ckey = lane < count ? qk[lane] : T(INFINITY);
+      int cidx = lane < count ? qi[lane] : 0x7fffffff;
+      warp_merge<T>(bkey, bidx, ckey, cidx, lane);
+      count = 0;
+    }
   }
-  const size_t row = g0 + i;
-  if (lane < a.k) {
-    const size_t o = row * a.k + lane;
-    const bool kept = bidx != IMAX;
-    a.out_idx[o] = kept ? bidx : (a.out_ok ? i : -1);
-    if (a.out_ok) a.out_ok[o] = kept ? 1 : 0;
+  __device__ __forceinline__ void refresh() {
+    thr_key = shfl_idx_t<T>(bkey, k - 1);
+    thr_idx = __shfl_sync(0xffffffffu, bidx, k - 1);
   }
-  if (a.out_count) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) nin += __shfl_xor_sync(0xffffffffu, nin, o);
-    if (lane == 0) a.out_count[row] = nin;
-  }
-}
+};
 
 // Sorts n = 2^m (rank, j) pairs in shared memory ascending (lexicographic), one warp: the bitonic network of
 // knn_block_sort_kernel.
@@ -452,37 +543,30 @@ __device__ __forceinline__ void warp_smem_sort(T* key, int* idx, int n, int lane
   }
 }
 
-// 32 < k <= RS_WIDE_MAX_K: the candidate stream of radius_query_kernel, with the top k kept in shared memory instead of
-// lanes.  Per warp, KP = next_pow2(k) (>= 64) pairs `list`, sorted ascending (the KP smallest (rank, j) so far, padded
-// with (inf, IMAX)), and KP more `queue`.  A candidate in radius that beats the current k-th list entry is queued.  Once
-// the queue could not take another 32, it is padded, sorted and merged into the list: list[s] = min(list[s],
-// queue[KP-1-s]) leaves the KP smallest of both as a bitonic sequence, which log2(KP) merge steps sort.  The list is a
-// function of the set of pairs queued, and every pair the filter drops is beaten by k listed ones, so the k kept pairs
-// are the k smallest of the stream whatever order the scatter put the candidates in.
-template <typename T, int CD, int PBC>
-__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const RadArgs<T> a, int KP) {
-  extern __shared__ __align__(16) unsigned char rsw_sm[];         // [warps][2 KP] ranks, then [warps][2 KP] indices
-  __shared__ int sexcl[RS_WARPS][32];
-  __shared__ int sdelta[RS_WARPS][32];
-  const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
-  const size_t gw = (size_t)blockIdx.x * warps + warp;
-  if (gw >= (size_t)a.B * a.N) return;
-  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
-  RS_QUERY_ROW()
-  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
-
-  const T INF = T(INFINITY);
-  const int IMAX = 0x7fffffff;
-  T* lk = reinterpret_cast<T*>(rsw_sm) + (size_t)warp * 2 * KP;
-  int* li = reinterpret_cast<int*>(reinterpret_cast<T*>(rsw_sm) + (size_t)warps * 2 * KP) + (size_t)warp * 2 * KP;
-  T* qk = lk + KP;
-  int* qi = li + KP;
-  for (int s = lane; s < KP; s += 32) { lk[s] = INF; li[s] = IMAX; }
-  T thr_key = INF; int thr_idx = IMAX; // the k-th smallest so far
-  int count = 0;                       // queued candidates (warp-uniform)
-  int nin = 0;                         // this lane's in-radius candidates
-  auto flush = [&]() {
-    for (int s = count + lane; s < KP; s += 32) { qk[s] = INF; qi[s] = IMAX; }
+// 32 < k <= RS_WIDE_MAX_K: the top k kept in shared memory instead of lanes.  Per warp, KP = next_pow2(k) (>= 64) pairs
+// `list` (lk, li), sorted ascending (the KP smallest (rank, j) so far, padded with (inf, IMAX)), and KP more `queue`.  A
+// pair that beats the current k-th list entry is queued.  Once the queue could not take another 32, it is padded,
+// sorted and merged into the list: list[s] = min(list[s], queue[KP-1-s]) leaves the KP smallest of both as a bitonic
+// sequence, which log2(KP) merge steps sort.  The list is a function of the set of pairs queued, and every pair the
+// filter drops is beaten by k listed ones, so the k kept pairs are the k smallest of all pairs offered, whatever order
+// they arrive in.
+template <typename T>
+struct SmemList {
+  T* lk;
+  int* li;
+  T* qk;
+  int* qi;
+  int KP, k;
+  T thr_key = T(INFINITY);             // the k-th smallest so far
+  int thr_idx = 0x7fffffff;
+  int count = 0;                       // queued pairs (warp-uniform)
+  __device__ __forceinline__ SmemList(T* lk_, int* li_, int KP_, int k_, int lane)
+      : lk(lk_), li(li_), qk(lk_ + KP_), qi(li_ + KP_), KP(KP_), k(k_) {
+    for (int s = lane; s < KP; s += 32) { lk[s] = T(INFINITY); li[s] = 0x7fffffff; }
+  }
+  __device__ __forceinline__ bool beats(T key, int j) const { return lex_less<T>(key, j, thr_key, thr_idx); }
+  __device__ __forceinline__ void flush(int lane) {
+    for (int s = count + lane; s < KP; s += 32) { qk[s] = T(INFINITY); qi[s] = 0x7fffffff; }
     __syncwarp();
     warp_smem_sort<T>(qk, qi, KP, lane);
     for (int s = lane; s < KP; s += 32) {
@@ -502,35 +586,126 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const 
       __syncwarp();
     }
     count = 0;
-    thr_key = lk[a.k - 1];
-    thr_idx = li[a.k - 1];
-  };
-  for (int t0 = 0; t0 < total; t0 += 32) {
-    const int t = t0 + lane;
-    T key = INF;
-    int j = IMAX;
-    bool pass = false;
-    if (t < total) {
-      key = stream_rank<T, CD, PBC>(a, g0, BN, t, sexcl[warp], sdelta[warp], xi, bl, binv, pc, j);
-      const bool in = key <= a.r2;
-      nin += in ? 1 : 0;
-      pass = in && lex_less<T>(key, j, thr_key, thr_idx);
-    }
+    thr_key = lk[k - 1];
+    thr_idx = li[k - 1];
+  }
+  // queues the pairs of the lanes whose `pass` is set; called by the whole warp
+  __device__ __forceinline__ void push(bool pass, T key, int j, int lane) {
     const unsigned bal = __ballot_sync(0xffffffffu, pass);
-    if (bal == 0) continue;
+    if (bal == 0) return;
     if (pass) {
       const int q = count + __popc(bal & ((1u << lane) - 1));
       qk[q] = key;
       qi[q] = j;
     }
     count += __popc(bal);
-    if (count > KP - 32) flush();
+    if (count > KP - 32) flush(lane);
   }
-  if (count > 0) flush();
+  __device__ __forceinline__ void finish(int lane) {
+    if (count > 0) flush(lane);
+  }
+  __device__ __forceinline__ void refresh() {
+    __syncwarp();
+    thr_key = lk[k - 1];
+    thr_idx = li[k - 1];
+  }
+};
+
+// Dynamic shared memory of a SmemList warp, and the warps per CTA that keep a CTA within RS_WIDE_SMEM (8, or 4 for
+// fp64 at k > 128).
+static inline size_t smem_list_bytes(int KP, size_t tbytes) { return (size_t)2 * KP * (tbytes + sizeof(int)); }
+static inline int smem_list_warps(int KP, size_t tbytes) {
+  return smem_list_bytes(KP, tbytes) * RS_WARPS <= RS_WIDE_SMEM ? RS_WARPS : RS_WARPS / 2;
+}
+static inline int list_kp(int k) {
+  int KP = 64;
+  while (KP < k) KP <<= 1;
+  return KP;
+}
+
+// The lists of the warp in dynamic shared memory laid out [warps][2 KP] ranks, then [warps][2 KP] indices.
+#define RS_SMEM_LIST(sm)                                                                                                \
+  T* lk = reinterpret_cast<T*>(sm) + (size_t)warp * 2 * KP;                                                             \
+  int* li = reinterpret_cast<int*>(reinterpret_cast<T*>(sm) + (size_t)warps * 2 * KP) + (size_t)warp * 2 * KP;
+
+// k <= 32: the candidate stream, filtered by rank <= r2 and against the current k-th, in a LaneList.
+template <typename T, int CD, int PBC>
+__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadArgs<T> a) {
+  __shared__ T qkey[RS_WARPS][64];
+  __shared__ int qidx[RS_WARPS][64];
+  __shared__ int sexcl[RS_WARPS][32];
+  __shared__ int sdelta[RS_WARPS][32];
+  const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const size_t gw = (size_t)blockIdx.x * RS_WARPS + warp;
+  if (gw >= (size_t)a.B * a.N) return;
+  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  RS_QUERY_ROW()
+  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
+
+  LaneList<T> L(qkey[warp], qidx[warp], a.k);
+  int nin = 0;                         // this lane's in-radius candidates
+  for (int t0 = 0; t0 < total; t0 += 32) {
+    const int t = t0 + lane;
+    T key = T(INFINITY);
+    int j = 0x7fffffff;
+    bool pass = false;
+    if (t < total) {
+      key = stream_rank<T, CD, PBC>(a, g0, BN, t, sexcl[warp], sdelta[warp], xi, bl, binv, pc, j);
+      const bool in = key <= a.r2;
+      nin += in ? 1 : 0;
+      pass = in && L.beats(key, j);
+    }
+    L.push(pass, key, j, lane);
+  }
+  L.finish(lane);
+  const size_t row = g0 + i;
+  if (lane < a.k) {
+    const size_t o = row * a.k + lane;
+    const bool kept = L.bidx != 0x7fffffff;
+    a.out_idx[o] = kept ? L.bidx : (a.out_ok ? i : -1);
+    if (a.out_ok) a.out_ok[o] = kept ? 1 : 0;
+  }
+  if (a.out_count) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) nin += __shfl_xor_sync(0xffffffffu, nin, o);
+    if (lane == 0) a.out_count[row] = nin;
+  }
+}
+
+// 32 < k <= RS_WIDE_MAX_K: the candidate stream of radius_query_kernel with the same filter, in a SmemList.
+template <typename T, int CD, int PBC>
+__global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const RadArgs<T> a, int KP) {
+  extern __shared__ __align__(16) unsigned char rsw_sm[];
+  __shared__ int sexcl[RS_WARPS][32];
+  __shared__ int sdelta[RS_WARPS][32];
+  const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const size_t gw = (size_t)blockIdx.x * warps + warp;
+  if (gw >= (size_t)a.B * a.N) return;
+  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  RS_QUERY_ROW()
+  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
+
+  RS_SMEM_LIST(rsw_sm)
+  SmemList<T> L(lk, li, KP, a.k, lane);
+  int nin = 0;                         // this lane's in-radius candidates
+  for (int t0 = 0; t0 < total; t0 += 32) {
+    const int t = t0 + lane;
+    T key = T(INFINITY);
+    int j = 0x7fffffff;
+    bool pass = false;
+    if (t < total) {
+      key = stream_rank<T, CD, PBC>(a, g0, BN, t, sexcl[warp], sdelta[warp], xi, bl, binv, pc, j);
+      const bool in = key <= a.r2;
+      nin += in ? 1 : 0;
+      pass = in && L.beats(key, j);
+    }
+    L.push(pass, key, j, lane);
+  }
+  L.finish(lane);
   const size_t row = g0 + i;
   for (int s = lane; s < a.k; s += 32) {
     const size_t o = row * a.k + s;
-    const bool kept = li[s] != IMAX;
+    const bool kept = li[s] != 0x7fffffff;
     a.out_idx[o] = kept ? li[s] : (a.out_ok ? i : -1);
     if (a.out_ok) a.out_ok[o] = kept ? 1 : 0;
   }
@@ -555,12 +730,9 @@ static int launch_cell(const RadArgs<T>& a, cudaStream_t st) {
   if (a.k <= 32) {
     radius_query_kernel<T, CD, PBC><<<(unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), RS_WARPS * 32, 0, st>>>(a);
   } else {
-    int KP = 64;
-    while (KP < a.k) KP <<= 1;
-    const size_t per_warp = (size_t)2 * KP * (sizeof(T) + sizeof(int));
-    const int warps = per_warp * RS_WARPS <= RS_WIDE_SMEM ? RS_WARPS : RS_WARPS / 2;      // fp64 at k > 128: 4 warps
-    radius_query_wide_kernel<T, CD, PBC><<<(unsigned)((nodes + warps - 1) / warps), warps * 32, warps * per_warp, st>>>(
-        a, KP);
+    const int KP = list_kp(a.k), warps = smem_list_warps(KP, sizeof(T));
+    radius_query_wide_kernel<T, CD, PBC><<<(unsigned)((nodes + warps - 1) / warps), warps * 32,
+                                           warps * smem_list_bytes(KP, sizeof(T)), st>>>(a, KP);
   }
   EGNN_LAUNCH_CHECK();
   count_launch(4);
@@ -642,6 +814,439 @@ static int radius_entry(int max_k, int pbc, int32_t dtype, int32_t B, int32_t N,
                               static_cast<cudaStream_t>(stream), pbc);
 }
 
+// ====================================================================== the kNN grid: k nearest, no cutoff
+//
+// egnn_knn_select's lists (the same rank, (rank, j) order, 1e5 rank of padded pairs, NaN-last rule and ok bytes) in
+// O(N) per graph for C <= 3 and k <= 256.  Seven launches, none synchronising with the host:
+//   memsets  bucket counts and the full-scan row count
+//   setup    one CTA per graph: extent and count of its insertable nodes -> its KGrid (cell edge, cells per axis)
+//   count / scan / scatter   as the radius grid, into the dense cells of the KGrid; padded rows are written here and
+//            rows of non-finite nodes listed for the full scan
+//   ring     one warp per node in cell order: Chebyshev rings of cells around it until no unvisited node can rank
+//            before the k-th; rows the grid cannot decide are listed for the full scan
+//   scan     the listed rows against all N nodes of their graph (a SmemList for every k)
+constexpr int KG_SETUP_THREADS = 256;
+constexpr double KG_FILL = 8.0;            // nodes aimed at per 3^C block of cells, in units of k (DESIGN.md section 6)
+constexpr int KG_MAX_RING_CELLS = 4096;    // the largest (2R+1)^C cube of cells a row visits before the full scan
+constexpr double KG_MARGIN = 1.0 - 0x1p-10;   // relative rounding margin of the stopping test
+
+struct KnnWs { CellWs cell; size_t kg, fb, nfb, total; };
+static KnnWs knn_ws_layout(int B, int N, int C, size_t coord_bytes) {
+  KnnWs w;
+  w.cell = cell_ws_layout(B, N, C, coord_bytes);
+  size_t o = w.cell.total;
+  auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
+  w.kg = take((size_t)B * sizeof(KGrid));
+  w.fb = take((size_t)B * N * sizeof(int));
+  w.nfb = take(sizeof(int));
+  w.total = o;
+  return w;
+}
+
+struct DMin { __device__ __forceinline__ double operator()(double x, double y) const { return fmin(x, y); } };
+struct DMax { __device__ __forceinline__ double operator()(double x, double y) const { return fmax(x, y); } };
+
+// Graph blockIdx.x: the extent lo..hi of its insertable nodes per axis, their count and largest |x|, then its KGrid.
+// The cell edge aims at KG_FILL * k nodes per 3^D block of cells, D the number of axes longer than one cell (an axis of
+// zero or small extent -- coincident points, a line in 3-D -- gets one cell and leaves the volume), and grows until the
+// dense grid fits the Tb buckets.  Periodic axes have their length L (or the cell's perpendicular width) instead of the
+// extent and n = max(1, floor(L / cs)) cells of width L / n >= cs, as in the radius grid.
+template <typename T, int CD, int PBC>
+__global__ void __launch_bounds__(KG_SETUP_THREADS) knn_grid_setup_kernel(const RadArgs<T> a) {
+  using Red = cub::BlockReduce<double, KG_SETUP_THREADS>;
+  __shared__ typename Red::TempStorage tmp;
+  __shared__ double res[2 * CD + 2];
+  const int b = blockIdx.x;
+  double mn[CD], mx[CD], amax = 0.0, count = 0.0;
+#pragma unroll
+  for (int c = 0; c < CD; ++c) { mn[c] = INFINITY; mx[c] = -INFINITY; }
+  for (int i = threadIdx.x; i < a.N; i += KG_SETUP_THREADS) {
+    T x[CD];
+    if (!load_node<T, CD>(a, (size_t)b * a.N + i, x)) continue;
+    count += 1.0;
+#pragma unroll
+    for (int c = 0; c < CD; ++c) {
+      const double v = (double)x[c];
+      mn[c] = fmin(mn[c], v); mx[c] = fmax(mx[c], v); amax = fmax(amax, fabs(v));
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < CD; ++c) {
+    const double lo = Red(tmp).Reduce(mn[c], DMin());
+    __syncthreads();
+    const double hi = Red(tmp).Reduce(mx[c], DMax());
+    __syncthreads();
+    if (threadIdx.x == 0) { res[c] = lo; res[CD + c] = hi; }
+  }
+  const double am = Red(tmp).Reduce(amax, DMax());
+  __syncthreads();
+  const double cnt = Red(tmp).Sum(count);
+  if (threadIdx.x != 0) return;
+  res[2 * CD] = am; res[2 * CD + 1] = cnt;
+
+  KGrid g;
+  g.cs = 1.0; g.err = 0.0; g.ok = 0;
+  for (int c = 0; c < 3; ++c) {
+    g.lo[c] = 0.0; g.L[c] = 0.0; g.w[c] = 1.0; g.n[c] = 1;
+    for (int d = 0; d < 3; ++d) g.G[c][d] = 0.0;
+  }
+  const double ins = res[2 * CD + 1];
+  double len[CD];
+  bool per[CD];
+  if constexpr (PBC == PBC_CELL) {
+    double G[CD][CD];
+    cell_inverse<T, CD>(a.box + (size_t)b * CD * CD, G, per);
+#pragma unroll
+    for (int c = 0; c < CD; ++c) {
+      double g2 = 0.0;
+#pragma unroll
+      for (int d = c; d < CD; ++d) g2 = fma(G[d][c], G[d][c], g2);
+      len[c] = per[c] ? 1.0 / sqrt(g2) : res[CD + c] - res[c];
+#pragma unroll
+      for (int d = 0; d < CD; ++d) g.G[c][d] = G[c][d];
+    }
+  } else {
+#pragma unroll
+    for (int c = 0; c < CD; ++c) {
+      const T l = PBC == PBC_BOX ? a.box[(size_t)b * CD + c] : T(0);
+      per[c] = l > T(0) && l < T(INFINITY);
+      len[c] = per[c] ? (double)l : res[CD + c] - res[c];
+    }
+  }
+  bool usable = ins >= (double)a.k;
+#pragma unroll
+  for (int c = 0; c < CD; ++c) usable = usable && len[c] >= 0.0 && len[c] < INFINITY;
+  if (usable) {
+    // the cell edge over the axes longer than it, recomputed as short axes drop out
+    bool act[CD];
+#pragma unroll
+    for (int c = 0; c < CD; ++c) act[c] = len[c] > 0.0;
+    double cs = 1.0;
+    for (int it = 0; it < CD; ++it) {
+      int D = 0;
+      double V = 1.0, blk = 1.0;
+      for (int c = 0; c < CD; ++c) if (act[c]) { ++D; V *= len[c]; blk *= 3.0; }
+      if (D == 0) break;
+      cs = pow(KG_FILL * a.k * V / (blk * ins), 1.0 / D);
+      bool dropped = false;
+      for (int c = 0; c < CD; ++c) if (act[c] && len[c] < cs) { act[c] = false; dropped = true; }
+      if (!dropped) break;
+    }
+    usable = cs > 0.0 && cs < INFINITY;
+    for (int grow = 0; usable; ++grow) {             // the dense grid must fit the Tb buckets
+      double cells = 1.0;
+      for (int c = 0; c < CD; ++c) {
+        const double q = floor(len[c] / cs);
+        cells *= per[c] ? fmax(q, 1.0) : q + 1.0;
+      }
+      if (cells <= (double)a.Tb) break;
+      cs *= 2.0;
+      usable = grow < 2100;
+    }
+    if (usable) {
+      g.cs = cs;
+      g.ok = 1;
+      for (int c = 0; c < CD; ++c) {
+        const double q = floor(len[c] / cs);
+        g.n[c] = per[c] ? (int)fmax(q, 1.0) : (int)q + 1;
+        g.lo[c] = per[c] ? 0.0 : res[c];
+        g.L[c] = per[c] ? (PBC == PBC_CELL ? 1.0 : len[c]) : 0.0;
+        g.w[c] = per[c] ? len[c] / g.n[c] : cs;
+      }
+      // Rounding allowance (DESIGN.md section 5): binning in double moves a cell face by at most a few ulp of the
+      // coordinates, and under a box or cell the wrapped pair vector carries the rounding of the unwrapped difference,
+      // u |x_i - x_j| per step, with |x_i - x_j| <= 2 max |x|.
+      const double u = sizeof(T) == 4 ? 0x1p-24 : 0x1p-53;
+      const double am2 = 2.0 * CD * res[2 * CD];
+      g.err = 0x1p-40 * am2 + (PBC != PBC_NONE ? 16.0 * u * am2 : 0.0);
+    }
+  }
+  if (!usable) {                                       // every node into cell 0; the ring kernel lists every row
+    g.ok = 0;
+    for (int c = 0; c < 3; ++c) { g.n[c] = 1; g.L[c] = 0.0; g.lo[c] = 0.0; }
+    g.cs = 1.0;
+  }
+  a.kg[b] = g;
+}
+
+// Row of node i (b, cell-order position p): the rings of cells around its cell, R = 0, 1, ..., each read as streams
+// of up to 32 cells (bucket_stream) whose nodes are offered to the list L.  Offsets along a periodic axis of n cells
+// are taken in [-(n-1)/2, n-1-(n-1)/2], so every cell is visited once; along an aperiodic axis they are clipped to the
+// graph's cells.  After ring R an unvisited node is at least R w_c away along some axis c whose cells are not all
+// visited, so once the k-th (rank, j) ranks below that distance squared, with the rounding margin, no unvisited pair
+// can rank before or tie with it.  Returns false when the row is left to the full scan: no usable grid, the ring
+// budget exhausted, or a k-th rank that is not finite or (under a mask) reaches the padded pairs' 1e5.
+template <typename T, int CD, int PBC, class List>
+__device__ __forceinline__ bool knn_ring_row(const RadArgs<T>& a, List& L, int b, int lane, const T (&xi)[CD],
+                                             const T (&bl)[CD], const T (&binv)[CD], const T* pc, const int* cnt,
+                                             const int* end, size_t g0, size_t BN, int* wexcl, int* wdelta) {
+  const KGrid& g = a.kg[b];
+  if (!g.ok) return false;
+  int cc[CD], dlo[CD], dhi[CD], n[CD];
+  knn_cell<T, CD, PBC>(g, xi, cc);
+#pragma unroll
+  for (int c = 0; c < CD; ++c) {
+    n[c] = g.n[c];
+    dlo[c] = g.L[c] > 0.0 ? -((n[c] - 1) / 2) : -cc[c];
+    dhi[c] = g.L[c] > 0.0 ? n[c] - 1 - (n[c] - 1) / 2 : n[c] - 1 - cc[c];
+  }
+  for (int R = 0;; ++R) {
+    const int side = 2 * R + 1;
+    int ncube = 1;
+#pragma unroll
+    for (int c = 0; c < CD; ++c) ncube *= side;
+    for (int u0 = 0; u0 < ncube; u0 += 32) {
+      const int u = u0 + lane;
+      int cell = -1;
+      if (u < ncube) {
+        int r = u, t = 0, mul = 1;
+        bool in = true, ring = false;
+#pragma unroll
+        for (int c = 0; c < CD; ++c) {
+          const int d = r % side - R;
+          r /= side;
+          in = in && d >= dlo[c] && d <= dhi[c];
+          ring = ring || d == R || d == -R;
+          int v = cc[c] + d;
+          v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
+          t += v * mul;
+          mul *= n[c];
+        }
+        if (in && ring) cell = t;
+      }
+      __syncwarp();                                    // the previous stream has been read
+      const int total = bucket_stream(lane, cell >= 0, cell, cnt, end, wexcl, wdelta);
+      for (int t0 = 0; t0 < total; t0 += 32) {
+        const int t = t0 + lane;
+        T key = T(INFINITY);
+        int j = 0x7fffffff;
+        bool pass = false;
+        if (t < total) {
+          key = stream_rank<T, CD, PBC>(a, g0, BN, t, wexcl, wdelta, xi, bl, binv, pc, j);
+          pass = L.beats(key, j);
+        }
+        L.push(pass, key, j, lane);
+      }
+    }
+    L.finish(lane);
+    L.refresh();                                       // thr_key / thr_idx: the k-th of every pair offered so far
+    bool covered = true;
+    double w = INFINITY;
+#pragma unroll
+    for (int c = 0; c < CD; ++c)
+      if (dlo[c] < -R || dhi[c] > R) { covered = false; w = fmin(w, g.w[c]); }
+    if (covered) break;
+    const T thr = L.thr_key;
+    if (L.thr_idx != 0x7fffffff) {
+      const double bd = R * w * KG_MARGIN - g.err;
+      if (bd > 0.0 && bd * bd >= 0x1p-96 && (double)thr < bd * bd * KG_MARGIN) break;
+    }
+    int next = 1;
+#pragma unroll
+    for (int c = 0; c < CD; ++c) next *= side + 2;
+    if (next > KG_MAX_RING_CELLS) return false;
+  }
+  const T thr = L.thr_key;
+  return thr < T(INFINITY) && !(a.mask && thr >= T(1e5));
+}
+
+// The ring query: one warp per node in cell order; k <= 32 in a LaneList, larger k in a SmemList (KP > 0).
+template <typename T, int CD, int PBC, bool WIDE>
+__global__ void __launch_bounds__(RS_WARPS * 32) knn_ring_kernel(const RadArgs<T> a, int KP) {
+  extern __shared__ __align__(16) unsigned char kgr_sm[];
+  __shared__ T qkey[WIDE ? 1 : RS_WARPS][64];
+  __shared__ int qidx[WIDE ? 1 : RS_WARPS][64];
+  __shared__ int sexcl[RS_WARPS][32];
+  __shared__ int sdelta[RS_WARPS][32];
+  const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  const size_t gw = (size_t)blockIdx.x * warps + warp;
+  if (gw >= (size_t)a.B * a.N) return;
+  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  RS_QUERY_ROW()
+  const size_t row = g0 + i;
+  if constexpr (WIDE) {
+    RS_SMEM_LIST(kgr_sm)
+    SmemList<T> L(lk, li, KP, a.k, lane);
+    if (!knn_ring_row<T, CD, PBC>(a, L, b, lane, xi, bl, binv, pc, cnt, end, g0, BN, sexcl[warp], sdelta[warp])) {
+      if (lane == 0) a.fb_rows[atomicAdd(a.fb_count, 1)] = (int)row;
+      return;
+    }
+    for (int s = lane; s < a.k; s += 32) {
+      a.out_idx[row * a.k + s] = li[s];
+      if (a.out_ok) a.out_ok[row * a.k + s] = lk[s] <= a.vr ? 1 : 0;
+    }
+  } else {
+    LaneList<T> L(qkey[warp], qidx[warp], a.k);
+    if (!knn_ring_row<T, CD, PBC>(a, L, b, lane, xi, bl, binv, pc, cnt, end, g0, BN, sexcl[warp], sdelta[warp])) {
+      if (lane == 0) a.fb_rows[atomicAdd(a.fb_count, 1)] = (int)row;
+      return;
+    }
+    if (lane < a.k) {
+      a.out_idx[row * a.k + lane] = L.bidx;
+      if (a.out_ok) a.out_ok[row * a.k + lane] = L.bkey <= a.vr ? 1 : 0;
+    }
+  }
+}
+
+// The listed rows, each against all N nodes of its graph with egnn_knn_select's rank: 1e5 to a padded node, and a NaN
+// rank ordered as (+inf, j + N), after every +inf and by index, written as j with ok = 0 (knn_block_sort_kernel's
+// rule).  Grid-stride over the list, whose length only the device knows.
+template <typename T, int CD, int PBC>
+__global__ void __launch_bounds__(RS_WARPS * 32) knn_scan_kernel(const RadArgs<T> a, int KP) {
+  extern __shared__ __align__(16) unsigned char kgs_sm[];
+  const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
+  RS_SMEM_LIST(kgs_sm)
+  const int rows = *a.fb_count;
+  for (int r = blockIdx.x * warps + warp; r < rows; r += gridDim.x * warps) {
+    const size_t row = (size_t)a.fb_rows[r];
+    const int b = (int)(row / a.N);
+    const size_t g0 = (size_t)b * a.N;
+    T xi[CD];
+#pragma unroll
+    for (int c = 0; c < CD; ++c) xi[c] = a.coors[row * CD + c];
+    T bl[CD], binv[CD], pc[PBC == PBC_CELL ? CELL_STAGED : 1];
+    if constexpr (PBC == PBC_CELL) {
+#pragma unroll
+      for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, CD, t);
+    } else if constexpr (PBC) {
+#pragma unroll
+      for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);
+    }
+    SmemList<T> L(lk, li, KP, a.k, lane);
+    for (int j0 = 0; j0 < a.N; j0 += 32) {
+      const int j = j0 + lane;
+      T key = T(INFINITY);
+      int jk = 0x7fffffff;
+      bool pass = false;
+      if (j < a.N) {
+        const T* xj = a.coors + (g0 + j) * CD;
+        key = pair_rank<T, CD, PBC>(xi, [&](int c) { return xj[c]; }, bl, binv, pc);
+        if (a.mask && !a.mask[g0 + j]) key = T(1e5);
+        jk = j;
+        if (key != key) { key = T(INFINITY); jk = j + a.N; }
+        pass = L.beats(key, jk);
+      }
+      L.push(pass, key, jk, lane);
+    }
+    L.finish(lane);
+    for (int s = lane; s < a.k; s += 32) {
+      const bool nan_rank = li[s] >= a.N;
+      a.out_idx[row * a.k + s] = nan_rank ? li[s] - a.N : li[s];
+      if (a.out_ok) a.out_ok[row * a.k + s] = !nan_rank && lk[s] <= a.vr ? 1 : 0;
+    }
+    __syncwarp();
+  }
+}
+
+template <typename T, int CD, int PBC>
+static int launch_knn(const RadArgs<T>& a, cudaStream_t st) {
+  const size_t nodes = (size_t)a.B * a.N;
+  const unsigned gn = (unsigned)((nodes + RS_THREADS - 1) / RS_THREADS);
+  EGNN_CUDA_TRY(cudaMemsetAsync(a.cnt, 0, (size_t)a.B * a.Tb * sizeof(int), st));
+  EGNN_CUDA_TRY(cudaMemsetAsync(a.fb_count, 0, sizeof(int), st));
+  knn_grid_setup_kernel<T, CD, PBC><<<a.B, KG_SETUP_THREADS, 0, st>>>(a);
+  EGNN_LAUNCH_CHECK();
+  radius_count_kernel<T, CD, PBC, GRID_KNN><<<gn, RS_THREADS, 0, st>>>(a);
+  EGNN_LAUNCH_CHECK();
+  radius_scan_kernel<<<a.B, RS_SCAN_THREADS, 0, st>>>(a.cnt, a.end, a.Tb);
+  EGNN_LAUNCH_CHECK();
+  radius_scatter_kernel<T, CD, PBC, GRID_KNN><<<gn, RS_THREADS, 0, st>>>(a);
+  EGNN_LAUNCH_CHECK();
+  const int KP = list_kp(a.k), warps = smem_list_warps(KP, sizeof(T));
+  const size_t smem = warps * smem_list_bytes(KP, sizeof(T));
+  if (a.k <= 32) {
+    knn_ring_kernel<T, CD, PBC, false><<<(unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), RS_WARPS * 32, 0, st>>>(a, 0);
+  } else {
+    knn_ring_kernel<T, CD, PBC, true><<<(unsigned)((nodes + warps - 1) / warps), warps * 32, smem, st>>>(a, KP);
+  }
+  EGNN_LAUNCH_CHECK();
+  int sms = 0;
+  EGNN_TRY(sm_count(&sms));
+  const size_t need = (nodes + warps - 1) / warps;
+  knn_scan_kernel<T, CD, PBC><<<(unsigned)(need < (size_t)4 * sms ? need : (size_t)4 * sms), warps * 32, smem, st>>>(
+      a, KP);
+  EGNN_LAUNCH_CHECK();
+  count_launch(6);
+  return EGNN_OK;
+}
+
+template <typename T>
+static int knn_grid(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box, double vr,
+                    int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st, int pbc) {
+  const KnnWs L = knn_ws_layout(B, N, C, sizeof(T));
+  char* base = static_cast<char*>(ws);
+  RadArgs<T> a;
+  a.B = B; a.N = N; a.k = k; a.Tb = rs_buckets(N);
+  a.r2 = T(0); a.cs = 0.0;
+  a.vr = (T)vr;
+  a.coors = static_cast<const T*>(coors); a.mask = mask; a.box = static_cast<const T*>(box);
+  a.cnt = reinterpret_cast<int*>(base + L.cell.cnt);
+  a.end = reinterpret_cast<int*>(base + L.cell.end);
+  a.xs = reinterpret_cast<T*>(base + L.cell.xs);
+  a.idx = reinterpret_cast<int*>(base + L.cell.idx);
+  a.kg = reinterpret_cast<KGrid*>(base + L.kg);
+  a.fb_rows = reinterpret_cast<int*>(base + L.fb);
+  a.fb_count = reinterpret_cast<int*>(base + L.nfb);
+  a.out_idx = out_idx; a.out_ok = out_ok; a.out_count = nullptr;
+  if (box && pbc == PBC_CELL) {
+    if (C == 2) return launch_knn<T, 2, PBC_CELL>(a, st);
+    if (C == 3) return launch_knn<T, 3, PBC_CELL>(a, st);
+    return EGNN_ERR_SHAPE;
+  }
+  switch (C * 2 + (box ? 1 : 0)) {
+    case 2: return launch_knn<T, 1, PBC_NONE>(a, st);
+    case 3: return launch_knn<T, 1, PBC_BOX>(a, st);
+    case 4: return launch_knn<T, 2, PBC_NONE>(a, st);
+    case 5: return launch_knn<T, 2, PBC_BOX>(a, st);
+    case 6: return launch_knn<T, 3, PBC_NONE>(a, st);
+    case 7: return launch_knn<T, 3, PBC_BOX>(a, st);
+    default: return EGNN_ERR_UNSUPPORTED;
+  }
+}
+
+size_t knn_grid_ws_bytes(int B, int N, int C, size_t coord_bytes) { return knn_ws_layout(B, N, C, coord_bytes).total; }
+
+bool knn_grid_eligible(const EgnnLayerDesc& d) {
+  if (!(d.flags & EGNN_FLAG_KNN_GRID)) return false;
+  const int max_k = (d.flags & EGNN_FLAG_CELL_SELECT_WIDE) ? RS_WIDE_MAX_K : 32;
+  if (d.k < 1 || d.k > max_k || d.C < 1 || d.C > 3) return false;
+  return !(d.flags & (EGNN_FLAG_ONLY_SPARSE | EGNN_FLAG_ADJ_BATCHED | EGNN_FLAG_EDGES_PER_SLOT));
+}
+
+// Smallest N per graph at which a flagged layer selects on the kNN grid (DESIGN.md section 6).
+// EGNN_B200_KNN_GRID_MIN_N overrides it at every call (0 = always, a huge value = never).
+constexpr long KNN_GRID_MIN_N = 8192;
+static long knn_grid_min_n() {
+  const char* e = getenv("EGNN_B200_KNN_GRID_MIN_N");
+  return e ? strtol(e, nullptr, 10) : KNN_GRID_MIN_N;
+}
+
+bool knn_grid_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io) {
+  return !io.adj && !io.nbr_idx && knn_grid_eligible(d) && !cell_select_runs(d, io) && d.N >= knn_grid_min_n();
+}
+
+int knn_grid_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box,
+                      double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st, int pbc) {
+  if (!coors || !out_idx || !ws) return EGNN_ERR_NULL;
+  EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
+  if (dtype == EGNN_DTYPE_F64)
+    return knn_grid<double>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, ws, st, pbc);
+  if (dtype != EGNN_DTYPE_F32) return EGNN_ERR_UNSUPPORTED;
+  return knn_grid<float>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, ws, st, pbc);
+}
+
+static int knn_entry(int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                     const uint8_t* mask, const void* lattice, double valid_radius, int32_t* out_idx, uint8_t* out_ok,
+                     void* workspace, size_t workspace_bytes, void* stream) {
+  if (!workspace || (pbc == PBC_CELL && !lattice)) return EGNN_ERR_NULL;
+  if (pbc == PBC_CELL && (C < 2 || C > 3)) return EGNN_ERR_SHAPE;
+  EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
+  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
+  if (workspace_bytes < knn_grid_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
+  return knn_grid_dispatch(dtype, B, N, C, k, coors, mask, lattice, valid_radius, out_idx, out_ok, workspace,
+                           static_cast<cudaStream_t>(stream), pbc);
+}
+
 }  // namespace egnn
 
 extern "C" int egnn_radius_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
@@ -679,4 +1284,26 @@ extern "C" int egnn_radius_select_wide_triclinic(int32_t dtype, int32_t B, int32
                                                  size_t workspace_bytes, void* stream) {
   return egnn::radius_entry(egnn::RS_WIDE_MAX_K, egnn::PBC_CELL, dtype, B, N, C, k, coors, mask, cell, r2, out_idx,
                             out_count, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_knn_grid_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
+  if (!out_bytes) return EGNN_ERR_NULL;
+  EGNN_TRY(egnn::radius_check(B, N, C, k, egnn::RS_WIDE_MAX_K));
+  *out_bytes = egnn::knn_grid_ws_bytes(B, N, C, 8);          // sized for float64 coordinates: covers both types
+  return EGNN_OK;
+}
+
+extern "C" int egnn_knn_grid_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                                    const uint8_t* mask, const void* box, double valid_radius, int32_t* out_idx,
+                                    uint8_t* out_ok, void* workspace, size_t workspace_bytes, void* stream) {
+  return egnn::knn_entry(egnn::PBC_BOX, dtype, B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, workspace,
+                         workspace_bytes, stream);
+}
+
+extern "C" int egnn_knn_grid_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k,
+                                              const void* coors, const uint8_t* mask, const void* cell,
+                                              double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                              size_t workspace_bytes, void* stream) {
+  return egnn::knn_entry(egnn::PBC_CELL, dtype, B, N, C, k, coors, mask, cell, valid_radius, out_idx, out_ok, workspace,
+                         workspace_bytes, stream);
 }

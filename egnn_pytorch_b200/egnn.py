@@ -39,7 +39,7 @@ import torch.nn.functional as F
 from . import _native as nat
 
 __all__ = ["EGNN", "EGNN_Network", "CoorsNorm", "GlobalLinearAttention", "edge_index_to_neighbors", "radius_neighbors",
-           "radius_neighbors_wide"]
+           "radius_neighbors_wide", "knn_neighbors"]
 
 
 def exists(v):
@@ -84,7 +84,25 @@ def _raise_if_sort_limit(err, sort_limited, k, n):
         raise RuntimeError(f"num_nearest_neighbors={k} > 32 ranks each node with a shared-memory sort of all N nodes, "
                            f"which holds at most N={SELECT_SORT_MAX_N}, got N={n}: use k <= 32, give the layer a mask "
                            f"and a finite valid_radius (the cell grid then selects up to 256 neighbours), or pass "
-                           f"neighbors= (e.g. from radius_neighbors_wide)") from None
+                           f"neighbors= (e.g. from radius_neighbors_wide); for plain k-nearest lists of any N, build "
+                           f"them with knn_neighbors(coors, k, mask=, box=, cell=) and pass neighbors=") from None
+
+
+def _select_flags(k, n, row_scan):
+    """-> (select flags, sort_limited) of a layer that ranks its own k-nearest lists over N nodes (`row_scan`: an
+    only_sparse layer with a mask and an adjacency, which ranks nothing).  EGNN_FLAG_CELL_SELECT_WIDE lets a radius
+    graph with k > 32 select on the cell grid; otherwise the all-pairs sort ranks each such row, which the library
+    rejects beyond SELECT_SORT_MAX_N (sort_limited).  EGNN_FLAG_KNN_GRID lets the library take the same lists from the
+    kNN grid where it applies (C <= 3, no adjacency, N at its threshold); a layer beyond the sort's limit keeps its
+    error, and knn_neighbors + neighbors= is the way through.  Mask and valid_radius do not enter: the library decides
+    from the descriptor and the call."""
+    fl, sort_limited = 0, False
+    if k > 32:
+        fl |= nat.FLAG_CELL_SELECT_WIDE
+        sort_limited = n > SELECT_SORT_MAX_N and not row_scan
+    if not sort_limited:
+        fl |= nat.FLAG_KNN_GRID
+    return fl, sort_limited
 
 
 def _ptr(t):
@@ -460,10 +478,8 @@ class EGNN(nn.Module):
             if not (0 < k <= n):
                 raise RuntimeError(f"number of neighbours k={k} must satisfy 0 < k <= N={n} (torch.topk would raise)")
             row_scan = self.only_sparse_neighbors and exists(mask) and adj_u8 is not None     # no ranking (select_neighbors)
-            if k > 32:
-                flags |= nat.FLAG_CELL_SELECT_WIDE       # a radius graph with a mask may select on the cell grid
-                # otherwise the all-pairs sort ranks each row, which the library rejects beyond SELECT_SORT_MAX_N
-                sort_limited = n > SELECT_SORT_MAX_N and not row_scan
+            sel_flags, sort_limited = _select_flags(k, n, row_scan)
+            flags |= sel_flags
 
         # support does not depend on the list length (any k > 0 runs the tensor cores), so one cached "unsupported"
         # entry for all k > 32 stays correct
@@ -756,7 +772,9 @@ def radius_neighbors_wide(coors, cutoff, k, *, mask=None, box=None, cell=None, r
     return _radius_graph("radius_neighbors_wide", 256, coors, cutoff, k, mask, box, cell, return_counts)
 
 
-def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts):
+def _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff=None):
+    """The argument checks of the neighbour-list builders (ValueError before anything launches) -> (B, N, C).
+    `cutoff` None: a builder without one (knn_neighbors)."""
     if not torch.is_tensor(coors) or coors.dim() != 3:
         raise ValueError(f"coors must be a [B, N, C] tensor, got {type(coors).__name__}"
                          f"{' of shape ' + str(tuple(coors.shape)) if torch.is_tensor(coors) else ''}")
@@ -769,12 +787,13 @@ def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts)
         raise ValueError(f"{name} supports C <= 3 coordinates, got C={c}")
     if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(max_k, n):
         raise ValueError(f"k must be an int in [1, min({max_k}, N)] = [1, {min(max_k, n)}], got {k!r}")
-    cutoff = float(cutoff)
-    if not (cutoff > 0.0 and math.isfinite(cutoff)):
-        raise ValueError(f"cutoff must be a finite distance > 0, got {cutoff}")
-    r2 = cutoff * cutoff
-    if not torch.tensor(r2, dtype=coors.dtype).item() > 0.0:
-        raise ValueError(f"cutoff {cutoff} squared is 0 in {coors.dtype}")
+    if cutoff is not None:
+        cutoff = float(cutoff)
+        if not (cutoff > 0.0 and math.isfinite(cutoff)):
+            raise ValueError(f"cutoff must be a finite distance > 0, got {cutoff}")
+        r2 = cutoff * cutoff
+        if not torch.tensor(r2, dtype=coors.dtype).item() > 0.0:
+            raise ValueError(f"cutoff {cutoff} squared is 0 in {coors.dtype}")
     if mask is not None and (not torch.is_tensor(mask) or tuple(mask.shape) != (b, n)):
         raise ValueError(f"mask must be a [B, N] = [{b}, {n}] tensor, got "
                          f"{tuple(mask.shape) if torch.is_tensor(mask) else type(mask).__name__}")
@@ -784,6 +803,53 @@ def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts)
         _check_box(box, b, c, _RADIUS_BOX_CHECKED)
     if cell is not None:
         _check_cell(cell, b, c, _RADIUS_BOX_CHECKED)
+    return b, n, c
+
+
+def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
+    """k-nearest-neighbour graph of a point cloud: for every node its `k` nearest nodes (itself included, distance 0),
+    as int32 neighbour lists [B, N, k] for `EGNN.forward(..., neighbors=...)`, nearest first, ties to the lower index.
+    The lists are those of the layer's own select (`num_nearest_neighbors=k`, no adjacency), computed on a cell grid
+    (`egnn_knn_grid_select`) in O(N) per graph, with -1 in every slot the layer would not use: slots that point at a
+    padded node or at a node with a non-finite coordinate, and every slot of a padded row.  Any N works, also where a
+    layer with k > 32 cannot select its own lists (N > 16384).
+
+    `coors` float32 or float64 [B, N, C] with C <= 3, on any device (CPU tensors are staged to the current CUDA
+    device; the result comes back on `coors`'s device).  `k` in [1, min(256, N)].  `mask` [B, N] bool / 0-1.  `box`
+    [C] or [B, C] periodic box lengths, or `cell` [C, C] or [B, C, C], as `EGNN.forward` takes them (distances of the
+    wrapped pair vector).  Nothing synchronises with the host: the call can be captured in a CUDA graph."""
+    b, n, c = _check_graph_args("knn_neighbors", 256, coors, k, mask, box, cell)
+    lib = nat.load()
+    dev = _compute_device(coors)
+    ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)
+    with ctx:
+        x = _as(coors, dev, coors.dtype)
+        m = _as_u8(mask, dev)
+        bx = None if box is None else _as(box, dev, coors.dtype).expand(b, c).contiguous()
+        cl = None if cell is None else _as(cell, dev, coors.dtype).expand(b, c, c).contiguous()
+        out = torch.empty((b, n, k), dtype=torch.int32, device=dev)
+        nb = C.c_size_t()
+        nat.check("egnn_knn_grid_select_workspace_bytes", lib.egnn_knn_grid_select_workspace_bytes(b, n, c, k, C.byref(nb)))
+        stream_handle = torch.cuda.current_stream(dev).cuda_stream
+        ws = _workspace(dev, nb.value, stream_handle)
+        lat, entry = (cl, "egnn_knn_grid_select_triclinic") if cl is not None else (bx, "egnn_knn_grid_select")
+        nat.check(entry, getattr(lib, entry)(_KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(lat),
+                                             float("inf"), _ptr(out), None, _ptr(ws), ws.numel(),
+                                             C.c_void_p(stream_handle)))
+        usable = torch.isfinite(x).all(dim=-1)                                   # [B, N]: nodes the layer uses
+        if m is not None:
+            usable = usable & m.bool()
+        row_ok = usable if m is None else m.bool()
+        keep = torch.gather(usable, 1, out.view(b, n * k).long()).view(b, n, k) & row_ok.unsqueeze(-1)
+        out = out.masked_fill(~keep, -1)
+    if out.device != coors.device:
+        out = out.to(coors.device)
+    return out
+
+
+def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts):
+    b, n, c = _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff)
+    r2 = float(cutoff) * float(cutoff)
     lib = nat.load()
     dev = _compute_device(coors)
     ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)

@@ -77,6 +77,13 @@ extern "C" {
                                                valid_radius, no adjacency or per-slot edges; DESIGN.md section 5).  Such a
                                                descriptor's workspace ends in the cell grid's scratch.  Without the flag a
                                                layer with k > 32 ranks all pairs, and its workspace is unchanged */
+#define EGNN_FLAG_KNN_GRID (1u << 12)         /* lets a layer select its k nearest neighbours on the kNN cell grid
+                                               (egnn_knn_grid_select) when the radius grid does not run and the layer
+                                               is eligible: C <= 3, 1 <= k <= 32 (<= 256 with EGNN_FLAG_CELL_SELECT_WIDE),
+                                               no adjacency, only_sparse, caller lists or per-slot edges, and N at least
+                                               a size threshold (EGNN_B200_KNN_GRID_MIN_N overrides it per call).  The
+                                               lists equal the all-pairs select's.  Such a descriptor's workspace ends in
+                                               the kNN grid's scratch; without the flag nothing changes */
 
 /*
  * Static description of one layer call.  E = 2*dim + 2*fourier + 1 + edge_dim + label_dim
@@ -333,6 +340,26 @@ int egnn_radius_select_wide(int32_t dtype, int32_t B, int32_t N, int32_t C, int3
 int egnn_radius_select_wide_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
                                       const uint8_t* mask, const void* cell, double r2, int32_t* out_idx,
                                       int32_t* out_count, void* workspace, size_t workspace_bytes, void* stream);
+
+/* k-nearest-neighbour lists from a cell grid, O(N) per graph instead of egnn_knn_select's O(N^2): out_idx and out_ok
+ * equal egnn_knn_select's with the same coordinates, mask and valid_radius (no adjacency) bit for bit -- the same rank
+ * (squared distance in the coordinates' type, minimum image under `box`), ascending, ties to the lowest index, 1e5 to
+ * and from padded nodes, NaN ranks last, ok = (rank <= valid_radius).  Each graph sizes its grid on the device from the
+ * extent of its nodes; rows the grid cannot decide (non-finite coordinates, fewer than k valid nodes, a k-th rank at
+ * the 1e5 of padded pairs, very uneven clouds) are ranked against every node of their graph (DESIGN.md section 5).
+ * coors [B,N,C] (float32, or float64 when dtype == EGNN_DTYPE_F64); mask [B,N] 0/1 or NULL; box [B,C] or NULL as
+ * egnn_radius_select takes it; out_idx int32 [B,N,k]; out_ok uint8 [B,N,k] or NULL.  1 <= k <= min(256, N) and C <= 3
+ * (k > 256 or C > 3: EGNN_ERR_UNSUPPORTED).  workspace: egnn_knn_grid_select_workspace_bytes(B, N, C, k) bytes (O(B N),
+ * enough for either coordinate type), 256-byte aligned.  Enqueued on `stream`, no host synchronisation. */
+int egnn_knn_grid_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes);
+int egnn_knn_grid_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                         const uint8_t* mask, const void* box, double valid_radius, int32_t* out_idx, uint8_t* out_ok,
+                         void* workspace, size_t workspace_bytes, void* stream);
+/* egnn_knn_grid_select under a triclinic cell [B, C, C] (C in {2, 3}, else EGNN_ERR_SHAPE), as egnn_radius_select_triclinic
+ * takes it: egnn_knn_select's lists with the rank of the wrapped pair vector.  Same workspace. */
+int egnn_knn_grid_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                                   const uint8_t* mask, const void* cell, double valid_radius, int32_t* out_idx,
+                                   uint8_t* out_ok, void* workspace, size_t workspace_bytes, void* stream);
 
 /* N-th degree adjacency of EGNN_Network (egnn_pytorch.py:414-428) without the dense A@A:
  * adj_in [N,N] or [B,N,N] 0/1; writes the expanded adjacency adj_out [B,N,N] 0/1, the degree
