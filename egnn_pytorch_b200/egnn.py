@@ -110,7 +110,7 @@ def _ptr(t):
 
 
 def _as_u8(t, dev):
-    """bool / uint8 / numeric 0-1 tensor -> contiguous uint8 on `dev`, zero-copy when it already is one."""
+    """bool / uint8 / numeric 0-1 tensor -> contiguous, 16-byte aligned uint8 on `dev`, zero-copy when it already is one."""
     if t is None:
         return None
     if t.device != dev:
@@ -119,15 +119,17 @@ def _as_u8(t, dev):
         t = t.view(torch.uint8)
     elif t.dtype != torch.uint8:
         t = t.ne(0).view(torch.uint8)
-    return t if t.is_contiguous() else t.contiguous()
+    return t if (t.is_contiguous() and t.data_ptr() % 16 == 0) else t.clone(memory_format=torch.contiguous_format)
 
 
 def _as(t, dev, dtype):
-    """Tensor on `dev` in `dtype`, contiguous; no work when it already is."""
+    """Tensor on `dev` in `dtype`, contiguous and 16-byte aligned (the library's pointer contract, include/egnn_b200.h);
+    no work when it already is.  A contiguous view that starts off a 16-byte boundary (a batch slice `x[1:3]`, `x[:, 1:]`
+    of a single graph) is copied."""
     if t is None:
         return None
     if t.device == dev and t.dtype == dtype and t.is_contiguous():
-        return t.detach()
+        return t.detach() if t.data_ptr() % 16 == 0 else t.detach().clone(memory_format=torch.contiguous_format)
     return t.detach().to(device=dev, dtype=dtype, non_blocking=True).contiguous()
 
 
@@ -1005,6 +1007,13 @@ class GlobalLinearAttention(nn.Module):
 # ----------------------------------------------------------------------------- the network
 
 
+def _adj_cache_key(adj_mat, b, num_adj_degrees):
+    """What EGNN_Network's expanded adjacency depends on: the storage and its version, and the view of it -- `A.t()` or a
+    dtype view shares A's pointer, version counter and shape but holds another matrix."""
+    return (adj_mat.data_ptr(), adj_mat._version, tuple(adj_mat.shape), adj_mat.stride(), adj_mat.dtype, b,
+            num_adj_degrees)
+
+
 class EGNN_Network(nn.Module):
     """Drop-in for `egnn_pytorch.EGNN_Network` (reference egnn_pytorch.py:343-454).
 
@@ -1084,9 +1093,9 @@ class EGNN_Network(nn.Module):
         labels = label_emb = k_hint = nbr_lists = None
         if exists(self.num_adj_degrees):
             assert exists(adj_mat), "adjacency matrix must be passed in (keyword argument adj_mat)"
-            # the expansion depends on the adjacency only: cached per (storage, version), which also keeps the
+            # the expansion depends on the adjacency only: cached per view of a storage version, which also keeps the
             # reference's host sync (:249) out of repeated calls and makes the forward CUDA-graph capturable
-            akey = (adj_mat.data_ptr(), adj_mat._version, tuple(adj_mat.shape), b, self.num_adj_degrees)
+            akey = _adj_cache_key(adj_mat, b, self.num_adj_degrees)
             cached = self.__dict__.get("_adj_cache")
             if cached is None or cached[0] != akey:
                 n = adj_mat.shape[-1]
