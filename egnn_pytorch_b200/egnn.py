@@ -62,6 +62,32 @@ def _workspace(device: torch.device, nbytes: int, stream_handle=None) -> torch.T
     return ws
 
 
+class _Built:
+    """Stream order of a cache entry: the stream whose work writes the entry's device tensors, and an event recorded on
+    it after that work.  A later call on another stream runs `use_on(stream)` first: that stream waits for the event,
+    so it never reads the entry before it is written, and the tensors are recorded as in use there (record_stream), so
+    the caching allocator does not hand their blocks to the building stream's next allocation while this stream may
+    still read them.  Once per entry and stream; a call on the building stream compares two handles and nothing else.
+    Nothing synchronises with the host.  An entry built while a CUDA graph is being captured gets no event, and no
+    wait is issued during a capture: the graph orders its own replay."""
+    __slots__ = ("stream", "event", "tensors", "seen")
+
+    def __init__(self, stream, tensors):
+        self.stream, self.tensors, self.seen, self.event = stream.cuda_stream, tensors, set(), None
+        if not torch.cuda.is_current_stream_capturing():
+            self.event = torch.cuda.Event()
+            self.event.record(stream)
+
+    def use_on(self, stream):
+        h = stream.cuda_stream
+        if self.event is None or h in self.seen or torch.cuda.is_current_stream_capturing():
+            return
+        stream.wait_event(self.event)
+        for t in self.tensors:
+            t.record_stream(stream)
+        self.seen.add(h)
+
+
 def _compute_device(t: torch.Tensor) -> torch.device:
     if t.is_cuda:
         return t.device
@@ -315,6 +341,8 @@ class EGNN(nn.Module):
         self.__dict__.pop("_fields_cache", None)
 
     def _staged(self, device, dtype):
+        """-> the staged entry for (device, dtype).  A new entry's "built" (its stream order, `_Built`) is set by _run
+        once its packed parameters are enqueued: one call, on one stream, writes its copies, label table and pack."""
         fields = self._state_fields()
         sig = [x for _, _, _, p in fields for x in (p.data_ptr(), p._version)]
         key = (device, dtype)
@@ -323,7 +351,7 @@ class EGNN(nn.Module):
         if st is None or st["sig"] != sig or always:
             with torch.no_grad():
                 tensors = {f: p.detach().to(device=device, dtype=dtype).contiguous() for _, _, f, p in fields}
-            st = dict(sig=sig, tensors=tensors, packed={}, wstruct={})
+            st = dict(sig=sig, tensors=tensors, packed={}, wstruct={}, built=None)
             self._stage[key] = st
         return st
 
@@ -511,7 +539,12 @@ class EGNN(nn.Module):
     def _run(self, lib, dev, kdt, feats, coors, edges, mask, adj_u8, labels, label_emb, b, n, c, k, flags,
              cont_edge_dim, label_dim, rows, nbr=None, train=False, param_fields=None, drop_p=0.0, box=None, cell=None):
         cdt = torch.float64 if kdt == torch.float64 else torch.float32
+        cs = torch.cuda.current_stream(dev)
+        stream_handle = cs.cuda_stream
         st = self._staged(dev, kdt)
+        built = st["built"]
+        if built is not None and built.stream != stream_handle:
+            built.use_on(cs)                     # an entry another stream built (None: this call builds it)
         T = dict(st["tensors"])
         lab_w = None
         if label_emb is not None:
@@ -557,7 +590,6 @@ class EGNN(nn.Module):
             st["wstruct"] = {wkey: w}
             st["lab_keepalive"] = lab_w
 
-        stream_handle = torch.cuda.current_stream(dev).cuda_stream
         stream = C.c_void_p(stream_handle)
         ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)
         with ctx:
@@ -571,6 +603,7 @@ class EGNN(nn.Module):
                 nat.check("egnn_layer_pack_weights",
                           lib.egnn_layer_pack_weights(C.byref(desc), C.byref(w), _ptr(packed), nb.value, stream))
                 st["packed"] = {pkey: packed}
+                st["built"] = _Built(cs, list(T.values()) + [packed])       # the staged copies, label table and pack
 
             f_in, x_in, e_in = _as(feats, dev, kdt), _as(coors, dev, cdt), _as(edges, dev, kdt)
             bx = None if box is None else _as(box, dev, cdt).expand(b, c).contiguous()     # [B, C], like coors
@@ -937,6 +970,7 @@ class GlobalLinearAttention(nn.Module):
         return self.ff(x) + x, queries
 
     def _staged(self, device, dtype):
+        """-> (sig, tensors, weights struct, built): the staged parameters for (device, dtype) and their stream order."""
         named = [(k, p) for k, p in self.named_parameters() if k in nat.GA_STATE_KEY_TO_FIELD]
         sig = tuple((p.data_ptr(), p._version) for _, p in named)
         st = self._stage.get((device, dtype))
@@ -944,7 +978,7 @@ class GlobalLinearAttention(nn.Module):
             with torch.no_grad():
                 tensors = {nat.GA_STATE_KEY_TO_FIELD[k]: p.detach().to(device=device, dtype=dtype).contiguous() for k, p in named}
             w = nat.GlobalAttnWeights(**{f: t.data_ptr() for f, t in tensors.items()})
-            st = (sig, tensors, w)
+            st = (sig, tensors, w, _Built(torch.cuda.current_stream(device), list(tensors.values())))
             self._stage[(device, dtype)] = st
         return st
 
@@ -984,7 +1018,10 @@ class GlobalLinearAttention(nn.Module):
         lib = nat.load()
         dev = _compute_device(x)
         kdt = torch.float64 if x.dtype == torch.float64 else torch.float32
-        _, _, w = self._staged(dev, kdt)
+        cs = torch.cuda.current_stream(dev)
+        _, _, w, built = self._staged(dev, kdt)
+        if built.stream != cs.cuda_stream:
+            built.use_on(cs)
         n, d, t = x.shape[1], x.shape[2], queries.shape[1]
         x, queries = x.expand(b, -1, -1), queries.expand(b, -1, -1)
         mask = None if mask is None else mask.expand(b, -1)
@@ -1000,7 +1037,7 @@ class GlobalLinearAttention(nn.Module):
             ws = _workspace(dev, nb.value)
             nat.check("egnn_global_attn_forward",
                       lib.egnn_global_attn_forward(C.byref(desc), C.byref(w), C.byref(io), _ptr(ws), ws.numel(),
-                                                   C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                                                   C.c_void_p(cs.cuda_stream)))
         return x_out.to(device=x.device, dtype=x.dtype), q_out.to(device=queries.device, dtype=queries.dtype)
 
 
@@ -1097,7 +1134,11 @@ class EGNN_Network(nn.Module):
             # reference's host sync (:249) out of repeated calls and makes the forward CUDA-graph capturable
             akey = _adj_cache_key(adj_mat, b, self.num_adj_degrees)
             cached = self.__dict__.get("_adj_cache")
-            if cached is None or cached[0] != akey:
+            cs = torch.cuda.current_stream(dev)
+            if cached is not None and cached[0] == akey:
+                if cached[6].stream != cs.cuda_stream:
+                    cached[6].use_on(cs)
+            else:
                 n = adj_mat.shape[-1]
                 adj_in = adj_mat.ne(0).to(torch.uint8).contiguous()
                 adj_out = torch.empty((b, n, n), dtype=torch.uint8, device=dev)
@@ -1109,7 +1150,7 @@ class EGNN_Network(nn.Module):
                     ws = _workspace(dev, nb.value)
                     nat.check("egnn_adj_expand", lib.egnn_adj_expand(
                         b, n, self.num_adj_degrees, _ptr(adj_in), 1 if adj_in.dim() == 3 else 0, _ptr(adj_out), _ptr(lab),
-                        _ptr(max_sum), _ptr(ws), ws.numel(), C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
+                        _ptr(max_sum), _ptr(ws), ws.numel(), C.c_void_p(cs.cuda_stream)))
                 kmax = int(max_sum.item()) if self.layers[0][1].only_sparse_neighbors else None   # the reference's sync at :249
                 # only_sparse_neighbors with a node mask: the surviving slots of every layer's top-k are the node and its
                 # adjacent nodes (valid_radius = 0, :250, :296) -- lists that depend on the adjacency only.  Built once
@@ -1119,10 +1160,11 @@ class EGNN_Network(nn.Module):
                     lists = torch.empty((b, n, kmax), dtype=torch.int32, device=dev)
                     with torch.cuda.device(dev):
                         nat.check("egnn_adj_neighbors", lib.egnn_adj_neighbors(
-                            b, n, kmax, _ptr(adj_out), 1, _ptr(lists), None, C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)))
-                cached = (akey, adj_out, lab, kmax, adj_mat, lists)     # adj_mat kept alive so the key cannot be recycled
+                            b, n, kmax, _ptr(adj_out), 1, _ptr(lists), None, C.c_void_p(cs.cuda_stream)))
+                built = _Built(cs, [adj_out, lab] + ([] if lists is None else [lists]))
+                cached = (akey, adj_out, lab, kmax, adj_mat, lists, built)   # adj_mat kept alive so the key cannot be recycled
                 self.__dict__["_adj_cache"] = cached
-            _, adj_out, lab, k_hint, _, nbr_lists = cached
+            _, adj_out, lab, k_hint, _, nbr_lists, _ = cached
             adj_mat = adj_out                                                        # layers see the expanded matrix (:428, :448)
             if exists(self.adj_emb):
                 labels, label_emb = lab, self.adj_emb.weight

@@ -21,6 +21,8 @@ nat.load = lambda: _Stub()
 E.nat.load = nat.load
 E._compute_device = lambda t: t.device
 torch.cuda.current_stream = lambda dev=None: types.SimpleNamespace(cuda_stream=0)
+torch.cuda.is_current_stream_capturing = lambda: False
+torch.cuda.Event = lambda **kw: types.SimpleNamespace(record=lambda stream=None: None)
 torch.cuda.current_device = lambda: None
 import contextlib
 torch.cuda.device = lambda dev=None: contextlib.nullcontext()
