@@ -90,37 +90,9 @@ knn_warp_select_kernel(const SelArgs<T> a) {
 #pragma unroll
   for (int c = 0; c < NC; ++c) xi[c] = (CDIM || c < a.C) ? a.coors[row * a.C + c] : T(0);
   const bool mask_i = a.mask ? a.mask[row] != 0 : true;
-  T bl[PBC == PBC_BOX ? NC : 1], binv[PBC == PBC_BOX ? NC : 1];   // the box of graph b, once per row (box_axis)
-  T pc[PBC == PBC_CELL ? CELL_STAGED : 1];         // or its cell (cell_staged)
-  if constexpr (PBC == PBC_CELL) {
-#pragma unroll
-    for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, a.C, t);
-  } else if constexpr (PBC) {
-#pragma unroll
-    for (int c = 0; c < NC; ++c) box_axis<T>(a.box, b, a.C, c, bl[c], binv[c]);
-  }
-  // the rank of x_i - x_j(c) (xj(c) reads candidate coordinate c): the squared length of the wrapped pair vector
-  auto dist = [&](auto xj) {
-    T d = T(0);
-    if constexpr (PBC == PBC_CELL) {
-      T r[3];
-#pragma unroll
-      for (int c = 0; c < 3; ++c) r[c] = (c < NC && (CDIM || c < a.C)) ? xi[c < NC ? c : 0] - xj(c) : T(0);
-      cell_wrap<T>(r[0], r[1], r[2], pc);
-#pragma unroll
-      for (int c = 0; c < 3; ++c)
-        if (c < NC && (CDIM || c < a.C)) d = sq_acc<T>(r[c], d);
-    } else {
-#pragma unroll
-      for (int c = 0; c < NC; ++c)
-        if (CDIM || c < a.C) {
-          T r = xi[c] - xj(c);
-          if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-          d = sq_acc<T>(r, d);
-        }
-    }
-    return d;
-  };
+  const int C = CDIM ? CDIM : a.C;
+  const RowLattice<T, NC, PBC> lat(a.box, b, a.C);
+  auto dist = [&](auto xj) { return pair_rank<T, NC, PBC>(xi, xj, C, lat.bl, lat.binv, lat.pc); };   // xj(c): coordinate c
   const uint8_t* adjrow = a.adj ? a.adj + ((size_t)(a.adj_batched ? b : 0) * a.N + i) * a.N : nullptr;
   const T INF = T(INFINITY);
   const int IMAX = 0x7fffffff;
@@ -154,13 +126,8 @@ knn_warp_select_kernel(const SelArgs<T> a) {
         const bool jvalid = jj < jn;
         key[u] = INF;
         if (jvalid) {
-          T d = dist([&](int c) { return xs[c * SEL_JC + jj]; });
-          if (a.mask && !(mask_i && ms[jj])) d = T(1e5);
-          if (adjrow) {
-            if (i == j) d = T(-1);
-            else if (adjrow[j]) d = T(0);
-          }
-          key[u] = d;
+          key[u] = select_rank<T>(dist([&](int c) { return xs[c * SEL_JC + jj]; }), a.mask && !(mask_i && ms[jj]),
+                                  adjrow, i, j);
         }
         pass[u] = jvalid && lex_less<T>(key[u], j, thr_key, thr_idx);     // false for a NaN key: see the fill-in below
       }
@@ -212,12 +179,8 @@ knn_warp_select_kernel(const SelArgs<T> a) {
     bool nan_rank = false;
     if (j < a.N) {                     // the rank of the scan above, read from global memory
       const T* xj = a.coors + ((size_t)b * a.N + j) * a.C;
-      T d = dist([&](int c) { return xj[c]; });
-      if (a.mask && !(mask_i && a.mask[(size_t)b * a.N + j])) d = T(1e5);
-      if (adjrow) {
-        if (i == j) d = T(-1);
-        else if (adjrow[j]) d = T(0);
-      }
+      const T d = select_rank<T>(dist([&](int c) { return xj[c]; }), a.mask && !(mask_i && a.mask[(size_t)b * a.N + j]),
+                                 adjrow, i, j);
       nan_rank = d != d;
     }
     const unsigned bal = __ballot_sync(0xffffffffu, nan_rank);
@@ -260,21 +223,7 @@ knn_block_sort_kernel(const SelArgs<T> a, int Npad) {
     idxs[j] = jk;
   }
   __syncthreads();
-  for (int size = 2; size <= Npad; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = threadIdx.x; t < Npad / 2; t += blockDim.x) {
-        const int lo = 2 * t - (t & (stride - 1));     // index with the `stride` bit clear
-        const int hi = lo + stride;
-        const bool asc = (lo & size) == 0;
-        const bool hi_less = lex_less<T>(keys[hi], idxs[hi], keys[lo], idxs[lo]);
-        if (hi_less == asc) {
-          T tk = keys[lo]; keys[lo] = keys[hi]; keys[hi] = tk;
-          int ti = idxs[lo]; idxs[lo] = idxs[hi]; idxs[hi] = ti;
-        }
-      }
-      __syncthreads();
-    }
-  }
+  bitonic_sort<T>(keys, idxs, Npad, threadIdx.x, blockDim.x, [] { __syncthreads(); });
   for (int s = threadIdx.x; s < a.k; s += blockDim.x) {
     const size_t o = (size_t)row * a.k + s;
     const bool nan_rank = idxs[s] >= a.N;

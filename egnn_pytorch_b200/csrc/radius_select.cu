@@ -9,7 +9,7 @@
 //
 // Grid, per graph: cell edge cs = sqrt(r2) (1 + 2^-10).  A periodic axis (finite L > 0) has n = max(1, floor(L / cs))
 // cells of width L / n >= cs, positions wrapped into [0, L); an aperiodic axis uses floor(x / cs), clamped to +-2^30.
-// A triclinic cell bins its periodic axes in fractional coordinates instead (frac_cells).
+// A triclinic cell bins its periodic axes in fractional coordinates instead (radius_cells).
 // Binning runs in double.  Cell coordinates hash into Tb = next_pow2(2N) buckets, so the scratch follows from N alone;
 // a collision only adds candidates that the exact rank filter removes.  DESIGN.md section 5 gives the argument that
 // no pair the filter keeps lies outside the 3^C cells around a node.
@@ -65,41 +65,6 @@ static CellWs cell_ws_layout(int B, int N, int C, size_t coord_bytes) {
   return w;
 }
 
-size_t cell_select_ws_bytes(int B, int N, int C, size_t coord_bytes) { return cell_ws_layout(B, N, C, coord_bytes).total; }
-
-bool cell_select_eligible(const EgnnLayerDesc& d) {
-  const int max_k = (d.flags & EGNN_FLAG_CELL_SELECT_WIDE) ? RS_WIDE_MAX_K : 32;
-  if (d.k < 1 || d.k > max_k || d.C < 1 || d.C > 3) return false;
-  if (d.flags & (EGNN_FLAG_ONLY_SPARSE | EGNN_FLAG_ADJ_BATCHED | EGNN_FLAG_EDGES_PER_SLOT)) return false;
-  // the radius in the coordinates' type, as the select compares it; at or above 1e5 padded pairs (rank 1e5) could
-  // take slots in the reference
-  const double r2 = d.dtype == EGNN_DTYPE_F64 ? d.valid_radius : (double)(float)d.valid_radius;
-  return r2 > 0.0 && r2 < 1e5;
-}
-
-size_t knn_grid_ws_bytes(int B, int N, int C, size_t coord_bytes);
-bool knn_grid_eligible(const EgnnLayerDesc& d);
-
-// The radius grid's scratch for a layer it may serve; under EGNN_FLAG_KNN_GRID the kNN grid's, which is larger, for a
-// layer the kNN grid may serve (either can run, depending on the call's mask).
-size_t cell_select_layer_ws_bytes(const EgnnLayerDesc& d) {
-  const size_t cb = d.dtype == EGNN_DTYPE_F64 ? 8 : 4;
-  if (knn_grid_eligible(d)) return knn_grid_ws_bytes(d.B, d.N, d.C, cb);
-  return cell_select_eligible(d) ? cell_select_ws_bytes(d.B, d.N, d.C, cb) : 0;
-}
-
-// Smallest N per graph at which an eligible layer runs the cell grid (DESIGN.md section 6).  EGNN_B200_CELL_SELECT_MIN_N
-// overrides it (0 = always, a huge value = never); read at every call, so one process can run and time both paths.
-constexpr long CELL_SELECT_MIN_N = 4096;
-static long cell_select_min_n() {
-  const char* e = getenv("EGNN_B200_CELL_SELECT_MIN_N");
-  return e ? strtol(e, nullptr, 10) : CELL_SELECT_MIN_N;
-}
-
-bool cell_select_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io) {
-  return io.mask && !io.adj && !io.nbr_idx && cell_select_eligible(d) && d.N >= cell_select_min_n();
-}
-
 // The kNN grid of one graph, set by knn_grid_setup_kernel and read by every later launch (no host round trip).
 // Cell coordinate c of a node: on an aperiodic axis floor((x_c - lo[c]) / cs), in [0, n[c]); on a periodic axis the
 // position (x_c, or the fractional coordinate under a cell) wrapped into [0, L[c]) and cut into n[c] cells.
@@ -114,6 +79,62 @@ struct KGrid {
   int ok;             // 0: no usable grid (fewer than k insertable nodes, a non-finite extent): every row is scanned
 };
 static_assert(sizeof(KGrid) == 176, "KGrid layout");
+
+struct KnnWs { CellWs cell; size_t kg, fb, nfb, total; };
+static KnnWs knn_ws_layout(int B, int N, int C, size_t coord_bytes) {
+  KnnWs w;
+  w.cell = cell_ws_layout(B, N, C, coord_bytes);
+  size_t o = w.cell.total;
+  auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
+  w.kg = take((size_t)B * sizeof(KGrid));
+  w.fb = take((size_t)B * N * sizeof(int));
+  w.nfb = take(sizeof(int));
+  w.total = o;
+  return w;
+}
+
+// The scratch of the radius grid (GRID_RADIUS) or of the kNN grid (GRID_KNN), which contains the radius grid's.
+static size_t grid_ws_bytes(int grid, int B, int N, int C, size_t coord_bytes) {
+  return grid == GRID_KNN ? knn_ws_layout(B, N, C, coord_bytes).total : cell_ws_layout(B, N, C, coord_bytes).total;
+}
+
+// The k, C and flags both grids serve: k <= 32, or <= RS_WIDE_MAX_K under EGNN_FLAG_CELL_SELECT_WIDE; C <= 3; no
+// only_sparse, batched adjacency or per-slot edges.
+static bool grid_eligible(const EgnnLayerDesc& d) {
+  const int max_k = (d.flags & EGNN_FLAG_CELL_SELECT_WIDE) ? RS_WIDE_MAX_K : 32;
+  if (d.k < 1 || d.k > max_k || d.C < 1 || d.C > 3) return false;
+  return !(d.flags & (EGNN_FLAG_ONLY_SPARSE | EGNN_FLAG_ADJ_BATCHED | EGNN_FLAG_EDGES_PER_SLOT));
+}
+
+bool cell_select_eligible(const EgnnLayerDesc& d) {
+  if (!grid_eligible(d)) return false;
+  // the radius in the coordinates' type, as the select compares it; at or above 1e5 padded pairs (rank 1e5) could
+  // take slots in the reference
+  const double r2 = d.dtype == EGNN_DTYPE_F64 ? d.valid_radius : (double)(float)d.valid_radius;
+  return r2 > 0.0 && r2 < 1e5;
+}
+
+static bool knn_grid_eligible(const EgnnLayerDesc& d) { return (d.flags & EGNN_FLAG_KNN_GRID) && grid_eligible(d); }
+
+// The radius grid's scratch for a layer it may serve; under EGNN_FLAG_KNN_GRID the kNN grid's, which is larger, for a
+// layer the kNN grid may serve (either can run, depending on the call's mask).
+size_t cell_select_layer_ws_bytes(const EgnnLayerDesc& d) {
+  const size_t cb = d.dtype == EGNN_DTYPE_F64 ? 8 : 4;
+  if (knn_grid_eligible(d)) return grid_ws_bytes(GRID_KNN, d.B, d.N, d.C, cb);
+  return cell_select_eligible(d) ? grid_ws_bytes(GRID_RADIUS, d.B, d.N, d.C, cb) : 0;
+}
+
+// Smallest N per graph at which an eligible layer runs the cell grid (DESIGN.md section 6).  EGNN_B200_CELL_SELECT_MIN_N
+// overrides it (0 = always, a huge value = never); read at every call, so one process can run and time both paths.
+constexpr long CELL_SELECT_MIN_N = 4096;
+static long cell_select_min_n() {
+  const char* e = getenv("EGNN_B200_CELL_SELECT_MIN_N");
+  return e ? strtol(e, nullptr, 10) : CELL_SELECT_MIN_N;
+}
+
+bool cell_select_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io) {
+  return io.mask && !io.adj && !io.nbr_idx && cell_select_eligible(d) && d.N >= cell_select_min_n();
+}
 
 template <typename T>
 struct RadArgs {
@@ -136,23 +157,6 @@ struct RadArgs {
   int* fb_count;                   // their number
   T vr;                            // ok = rank <= vr
 };
-
-// Axis c of graph b's grid: n[c] > 0 cells of width w[c] on a periodic axis of length L[c]; n[c] = 0 on an aperiodic one.
-template <typename T, int CD, int PBC>
-__device__ __forceinline__ void axis_grids(const RadArgs<T>& a, int b, double (&L)[CD], double (&w)[CD], int (&n)[CD]) {
-#pragma unroll
-  for (int c = 0; c < CD; ++c) {
-    L[c] = 0.0; w[c] = a.cs; n[c] = 0;
-    if constexpr (PBC) {
-      const T l = a.box[(size_t)b * CD + c];
-      if (l > T(0) && l < T(INFINITY)) {
-        const double ld = (double)l;
-        const double q = fmin(fmax(floor(ld / a.cs), 1.0), RS_CLAMP);
-        L[c] = ld; n[c] = (int)q; w[c] = ld / q;
-      }
-    }
-  }
-}
 
 __device__ __forceinline__ int cell_coord(double x, double cs, double L, double w, int n) {
   if (n == 0) return (int)fmin(fmax(floor(x / cs), -RS_CLAMP), RS_CLAMP);
@@ -184,11 +188,6 @@ __device__ __forceinline__ bool load_node(const RadArgs<T>& a, size_t t, T (&x)[
   return ok;
 }
 
-// PBC_CELL: the cell coordinates cc of x in graph b's grid, and the cell count n of every axis (0: aperiodic).  A
-// periodic axis k is binned in the fractional coordinate s_k = sum_d x_d G[d][k], G = A^-1 of the lower-triangular cell
-// A with 1 in place of every aperiodic diagonal, wrapped into [0, 1) and cut into n_k = max(1, floor(w_k / cs)) cells,
-// w_k = 1 / |column k of G| being the cell's perpendicular width along a_k.  An aperiodic axis (its row and column of
-// A are zero but for the diagonal, so s_k = x_k) is binned as without a cell.  Double precision throughout.
 // G = A^-1 of graph b's lower-triangular cell A (m: [CD][CD]) with 1 in place of every aperiodic diagonal (per[r]:
 // axis r is periodic); column k of G by forward substitution down the rows, in double.
 template <typename T, int CD>
@@ -214,38 +213,44 @@ __device__ __forceinline__ void cell_inverse(const T* m, double (&G)[CD][CD], bo
   }
 }
 
-// PBC_CELL: the cell coordinates cc of x in graph b's grid, and the cell count n of every axis (0: aperiodic).  A
-// periodic axis k is binned in the fractional coordinate s_k = sum_d x_d G[d][k] (cell_inverse), wrapped into [0, 1)
-// and cut into n_k = max(1, floor(w_k / cs)) cells, w_k = 1 / |column k of G| being the cell's perpendicular width
-// along a_k.  An aperiodic axis (its row and column of A are zero but for the diagonal, so s_k = x_k) is binned as
-// without a cell.  Double precision throughout.
-template <typename T, int CD>
-__device__ __forceinline__ void frac_cells(const RadArgs<T>& a, int b, const T (&x)[CD], int (&cc)[CD], int (&n)[CD]) {
-  double G[CD][CD];
-  bool per[CD];
-  cell_inverse<T, CD>(a.box + (size_t)b * CD * CD, G, per);
-#pragma unroll
-  for (int k = 0; k < CD; ++k) {
-    double s = 0.0, g2 = 0.0;
-#pragma unroll
-    for (int d = k; d < CD; ++d) { s = fma((double)x[d], G[d][k], s); g2 = fma(G[d][k], G[d][k], g2); }
-    n[k] = per[k] ? (int)fmin(fmax(floor(1.0 / (sqrt(g2) * a.cs)), 1.0), RS_CLAMP) : 0;
-    cc[k] = n[k] > 0 ? cell_coord(s, a.cs, 1.0, 1.0 / n[k], n[k]) : cell_coord(s, a.cs, 0.0, a.cs, 0);
-  }
-}
-
+// The cell coordinates cc of x in graph b's radius grid, and the cell count n of every axis (0: aperiodic).  An
+// aperiodic axis is cut into cells of edge cs = a.cs.  A periodic box axis of length L has n = max(1, floor(L / cs))
+// cells of width L / n >= cs, positions wrapped into [0, L).  Under a cell (PBC_CELL) a periodic axis k is binned in the
+// fractional coordinate s_k = sum_d x_d G[d][k] (cell_inverse), wrapped into [0, 1) and cut into
+// n_k = max(1, floor(w_k / cs)) cells, w_k = 1 / |column k of G| being the cell's perpendicular width along a_k; an
+// aperiodic axis (its row and column of A are zero but for the diagonal, so s_k = x_k) is binned as without a cell.
+// Double precision throughout.
 template <typename T, int CD, int PBC>
-__device__ __forceinline__ int node_bucket(const RadArgs<T>& a, int b, const T (&x)[CD]) {
-  double L[CD], w[CD];
-  int n[CD], cc[CD];
+__device__ __forceinline__ void radius_cells(const RadArgs<T>& a, int b, const T (&x)[CD], int (&cc)[CD], int (&n)[CD]) {
   if constexpr (PBC == PBC_CELL) {
-    frac_cells<T, CD>(a, b, x, cc, n);
-    return cell_bucket<CD>(cc, a.Tb);
-  }
-  axis_grids<T, CD, PBC>(a, b, L, w, n);
+    double G[CD][CD];
+    bool per[CD];
+    cell_inverse<T, CD>(a.box + (size_t)b * CD * CD, G, per);
 #pragma unroll
-  for (int c = 0; c < CD; ++c) cc[c] = cell_coord((double)x[c], a.cs, L[c], w[c], n[c]);
-  return cell_bucket<CD>(cc, a.Tb);
+    for (int k = 0; k < CD; ++k) {
+      double s = 0.0, g2 = 0.0;
+#pragma unroll
+      for (int d = k; d < CD; ++d) { s = fma((double)x[d], G[d][k], s); g2 = fma(G[d][k], G[d][k], g2); }
+      n[k] = per[k] ? (int)fmin(fmax(floor(1.0 / (sqrt(g2) * a.cs)), 1.0), RS_CLAMP) : 0;
+      cc[k] = n[k] > 0 ? cell_coord(s, a.cs, 1.0, 1.0 / n[k], n[k]) : cell_coord(s, a.cs, 0.0, a.cs, 0);
+    }
+  } else {
+    double L[CD], w[CD];
+#pragma unroll
+    for (int c = 0; c < CD; ++c) {
+      L[c] = 0.0; w[c] = a.cs; n[c] = 0;
+      if constexpr (PBC) {
+        const T l = a.box[(size_t)b * CD + c];
+        if (l > T(0) && l < T(INFINITY)) {
+          const double ld = (double)l;
+          const double q = fmin(fmax(floor(ld / a.cs), 1.0), RS_CLAMP);
+          L[c] = ld; n[c] = (int)q; w[c] = ld / q;
+        }
+      }
+    }
+#pragma unroll
+    for (int c = 0; c < CD; ++c) cc[c] = cell_coord((double)x[c], a.cs, L[c], w[c], n[c]);
+  }
 }
 
 // Cell coordinates of x in the kNN grid g, each in [0, g.n[c]).
@@ -276,12 +281,14 @@ __device__ __forceinline__ int knn_index(const KGrid& g, const int (&cc)[CD]) {
 // The bucket node x of graph b goes to: a hashed radius cell, or a dense kNN cell.
 template <typename T, int CD, int PBC, int GRID>
 __device__ __forceinline__ int grid_bucket(const RadArgs<T>& a, int b, const T (&x)[CD]) {
+  int cc[CD];
   if constexpr (GRID == GRID_KNN) {
-    int cc[CD];
     knn_cell<T, CD, PBC>(a.kg[b], x, cc);
     return knn_index<CD>(a.kg[b], cc);
   } else {
-    return node_bucket<T, CD, PBC>(a, b, x);
+    int n[CD];
+    radius_cells<T, CD, PBC>(a, b, x, cc, n);
+    return cell_bucket<CD>(cc, a.Tb);
   }
 }
 
@@ -389,55 +396,20 @@ __device__ __forceinline__ int row_stream(const RadArgs<T>& a, int b, int lane, 
   // hashing alike) is kept by its lowest lane only, so that no node enters the stream twice
   int bkt = -1 - lane;
   if (lane < NB) {
-    double L[CD], w[CD];
     int n[CD], cc[CD];
+    radius_cells<T, CD, PBC>(a, b, xi, cc, n);
     int r = lane;
-    if constexpr (PBC == PBC_CELL) {
-      frac_cells<T, CD>(a, b, xi, cc, n);
 #pragma unroll
-      for (int c = 0; c < CD; ++c) {
-        int v = cc[c] + r % 3 - 1;
-        r /= 3;
-        if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
-        cc[c] = v;
-      }
-    } else {
-      axis_grids<T, CD, PBC>(a, b, L, w, n);
-#pragma unroll
-      for (int c = 0; c < CD; ++c) {
-        int v = cell_coord((double)xi[c], a.cs, L[c], w[c], n[c]) + r % 3 - 1;
-        r /= 3;
-        if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
-        cc[c] = v;
-      }
+    for (int c = 0; c < CD; ++c) {
+      int v = cc[c] + r % 3 - 1;
+      r /= 3;
+      if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
+      cc[c] = v;
     }
     bkt = cell_bucket<CD>(cc, a.Tb);
   }
   const unsigned same = __match_any_sync(0xffffffffu, bkt);
   return bucket_stream(lane, lane < NB && __ffs(same) - 1 == lane, bkt, cnt, end, wexcl, wdelta);
-}
-
-// The rank of the pair (xi, xj), as the all-pairs select computes it (xj(c) reads coordinate c of the other node;
-// bl / binv: the box of the graph under PBC_BOX, pc: its staged cell under PBC_CELL).
-template <typename T, int CD, int PBC, class XJ>
-__device__ __forceinline__ T pair_rank(const T (&xi)[CD], XJ xj, const T (&bl)[CD], const T (&binv)[CD], const T* pc) {
-  T d = T(0);
-  if constexpr (PBC == PBC_CELL) {
-    T r[3];
-#pragma unroll
-    for (int c = 0; c < 3; ++c) r[c] = c < CD ? xi[c < CD ? c : 0] - xj(c < CD ? c : 0) : T(0);
-    cell_wrap<T>(r[0], r[1], r[2], pc);
-#pragma unroll
-    for (int c = 0; c < CD; ++c) d = sq_acc<T>(r[c], d);
-  } else {
-#pragma unroll
-    for (int c = 0; c < CD; ++c) {
-      T r = xi[c] - xj(c);
-      if constexpr (PBC) r = min_image<T>(r, bl[c], binv[c]);
-      d = sq_acc<T>(r, d);
-    }
-  }
-  return d;
 }
 
 // Candidate t of the stream: its node index j and its rank, as the all-pairs select computes it (bl / binv: the box of
@@ -452,7 +424,7 @@ __device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t 
     if (wexcl[s + step] <= t) s += step;
   const size_t pos = g0 + wdelta[s] + t;
   j = a.idx[pos];
-  return pair_rank<T, CD, PBC>(xi, [&](int c) { return a.xs[c * BN + pos]; }, bl, binv, pc);
+  return pair_rank<T, CD, PBC>(xi, [&](int c) { return a.xs[c * BN + pos]; }, CD, bl, binv, pc);
 }
 
 // The prologue of both query kernels: the node at cell-order position p of graph b (false: beyond the nodes the graph
@@ -471,77 +443,6 @@ __device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t 
   } else if constexpr (PBC) {                                                                                           \
     _Pragma("unroll") for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);                        \
   }
-
-// k <= 32: lane l keeps the l-th smallest (rank, j) so far (bkey, bidx); pairs that beat the k-th are queued in the
-// warp's 64 queue slots and merged 32 at a time (warp_merge).
-template <typename T>
-struct LaneList {
-  T* qk;
-  int* qi;
-  int k;
-  T bkey = T(INFINITY), thr_key = T(INFINITY);   // lane l: l-th smallest so far; the k-th smallest so far
-  int bidx = 0x7fffffff, thr_idx = 0x7fffffff;
-  int count = 0;                                 // queued pairs (warp-uniform)
-  __device__ __forceinline__ LaneList(T* qk_, int* qi_, int k_) : qk(qk_), qi(qi_), k(k_) {}
-  __device__ __forceinline__ bool beats(T key, int j) const { return lex_less<T>(key, j, thr_key, thr_idx); }
-  // queues the pairs of the lanes whose `pass` is set; called by the whole warp
-  __device__ __forceinline__ void push(bool pass, T key, int j, int lane) {
-    const unsigned bal = __ballot_sync(0xffffffffu, pass);
-    if (bal == 0) return;
-    if (pass) {
-      const int q = count + __popc(bal & ((1u << lane) - 1));
-      qk[q] = key;
-      qi[q] = j;
-    }
-    count += __popc(bal);
-    __syncwarp();
-    if (count >= 32) {
-      T ckey = qk[lane];
-      int cidx = qi[lane];
-      __syncwarp();
-      if (lane + 32 < count) {         // shift the tail of the queue down
-        T tk = qk[lane + 32]; int ti = qi[lane + 32];
-        qk[lane] = tk; qi[lane] = ti;
-      }
-      count -= 32;
-      __syncwarp();
-      warp_merge<T>(bkey, bidx, ckey, cidx, lane);
-      refresh();
-    }
-  }
-  // merges what is still queued: lane l then holds the l-th smallest of every pair pushed
-  __device__ __forceinline__ void finish(int lane) {
-    if (count > 0) {
-      T ckey = lane < count ? qk[lane] : T(INFINITY);
-      int cidx = lane < count ? qi[lane] : 0x7fffffff;
-      warp_merge<T>(bkey, bidx, ckey, cidx, lane);
-      count = 0;
-    }
-  }
-  __device__ __forceinline__ void refresh() {
-    thr_key = shfl_idx_t<T>(bkey, k - 1);
-    thr_idx = __shfl_sync(0xffffffffu, bidx, k - 1);
-  }
-};
-
-// Sorts n = 2^m (rank, j) pairs in shared memory ascending (lexicographic), one warp: the bitonic network of
-// knn_block_sort_kernel.
-template <typename T>
-__device__ __forceinline__ void warp_smem_sort(T* key, int* idx, int n, int lane) {
-  for (int size = 2; size <= n; size <<= 1) {
-    for (int stride = size >> 1; stride > 0; stride >>= 1) {
-      for (int t = lane; t < n / 2; t += 32) {
-        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-        const bool asc = (lo & size) == 0;
-        if (lex_less<T>(key[hi], idx[hi], key[lo], idx[lo]) == asc) {
-          const T tk = key[lo]; key[lo] = key[hi]; key[hi] = tk;
-          const int ti = idx[lo]; idx[lo] = idx[hi]; idx[hi] = ti;
-        }
-      }
-      __syncwarp();
-    }
-  }
-}
 
 // 32 < k <= RS_WIDE_MAX_K: the top k kept in shared memory instead of lanes.  Per warp, KP = next_pow2(k) (>= 64) pairs
 // `list` (lk, li), sorted ascending (the KP smallest (rank, j) so far, padded with (inf, IMAX)), and KP more `queue`.  A
@@ -568,23 +469,14 @@ struct SmemList {
   __device__ __forceinline__ void flush(int lane) {
     for (int s = count + lane; s < KP; s += 32) { qk[s] = T(INFINITY); qi[s] = 0x7fffffff; }
     __syncwarp();
-    warp_smem_sort<T>(qk, qi, KP, lane);
+    bitonic_sort<T>(qk, qi, KP, lane, 32, [] { __syncwarp(); });
     for (int s = lane; s < KP; s += 32) {
       const T ck = qk[KP - 1 - s];
       const int ci = qi[KP - 1 - s];
       if (lex_less<T>(ck, ci, lk[s], li[s])) { lk[s] = ck; li[s] = ci; }
     }
     __syncwarp();
-    for (int stride = KP >> 1; stride > 0; stride >>= 1) {
-      for (int t = lane; t < KP / 2; t += 32) {
-        const int lo = 2 * t - (t & (stride - 1)), hi = lo + stride;
-        if (lex_less<T>(lk[hi], li[hi], lk[lo], li[lo])) {
-          const T tk = lk[lo]; lk[lo] = lk[hi]; lk[hi] = tk;
-          const int ti = li[lo]; li[lo] = li[hi]; li[hi] = ti;
-        }
-      }
-      __syncwarp();
-    }
+    bitonic_merge<T>(lk, li, KP, lane, 32, [] { __syncwarp(); });
     count = 0;
     thr_key = lk[k - 1];
     thr_idx = li[k - 1];
@@ -716,104 +608,6 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const 
   }
 }
 
-template <typename T, int CD, int PBC>
-static int launch_cell(const RadArgs<T>& a, cudaStream_t st) {
-  const size_t nodes = (size_t)a.B * a.N;
-  const unsigned gn = (unsigned)((nodes + RS_THREADS - 1) / RS_THREADS);
-  EGNN_CUDA_TRY(cudaMemsetAsync(a.cnt, 0, (size_t)a.B * a.Tb * sizeof(int), st));
-  radius_count_kernel<T, CD, PBC><<<gn, RS_THREADS, 0, st>>>(a);
-  EGNN_LAUNCH_CHECK();
-  radius_scan_kernel<<<a.B, RS_SCAN_THREADS, 0, st>>>(a.cnt, a.end, a.Tb);
-  EGNN_LAUNCH_CHECK();
-  radius_scatter_kernel<T, CD, PBC><<<gn, RS_THREADS, 0, st>>>(a);
-  EGNN_LAUNCH_CHECK();
-  if (a.k <= 32) {
-    radius_query_kernel<T, CD, PBC><<<(unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), RS_WARPS * 32, 0, st>>>(a);
-  } else {
-    const int KP = list_kp(a.k), warps = smem_list_warps(KP, sizeof(T));
-    radius_query_wide_kernel<T, CD, PBC><<<(unsigned)((nodes + warps - 1) / warps), warps * 32,
-                                           warps * smem_list_bytes(KP, sizeof(T)), st>>>(a, KP);
-  }
-  EGNN_LAUNCH_CHECK();
-  count_launch(4);
-  return EGNN_OK;
-}
-
-template <typename T>
-static int cell_select(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box, double r2,
-                       int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws, cudaStream_t st, int pbc) {
-  const CellWs L = cell_ws_layout(B, N, C, sizeof(T));
-  char* base = static_cast<char*>(ws);
-  RadArgs<T> a;
-  a.B = B; a.N = N; a.k = k; a.Tb = rs_buckets(N);
-  a.r2 = (T)r2;
-  a.cs = sqrt((double)a.r2) * (1.0 + 0x1p-10);
-  a.coors = static_cast<const T*>(coors); a.mask = mask; a.box = static_cast<const T*>(box);
-  a.cnt = reinterpret_cast<int*>(base + L.cnt);
-  a.end = reinterpret_cast<int*>(base + L.end);
-  a.xs = reinterpret_cast<T*>(base + L.xs);
-  a.idx = reinterpret_cast<int*>(base + L.idx);
-  a.out_idx = out_idx; a.out_ok = out_ok; a.out_count = out_count;
-  if (box && pbc == PBC_CELL) {
-    if (C == 2) return launch_cell<T, 2, PBC_CELL>(a, st);
-    if (C == 3) return launch_cell<T, 3, PBC_CELL>(a, st);
-    return EGNN_ERR_SHAPE;
-  }
-  switch (C * 2 + (box ? 1 : 0)) {
-    case 2: return launch_cell<T, 1, PBC_NONE>(a, st);
-    case 3: return launch_cell<T, 1, PBC_BOX>(a, st);
-    case 4: return launch_cell<T, 2, PBC_NONE>(a, st);
-    case 5: return launch_cell<T, 2, PBC_BOX>(a, st);
-    case 6: return launch_cell<T, 3, PBC_NONE>(a, st);
-    case 7: return launch_cell<T, 3, PBC_BOX>(a, st);
-    default: return EGNN_ERR_UNSUPPORTED;
-  }
-}
-
-static int radius_check(int B, int N, int C, int k, int max_k) {
-  if (B <= 0 || N <= 0 || C <= 0 || k <= 0 || k > N) return EGNN_ERR_SHAPE;
-  if (k > max_k || C > 3) return EGNN_ERR_UNSUPPORTED;
-  if ((long long)B * rs_buckets(N) > 0x7fffffffLL) return EGNN_ERR_SHAPE;    // int bucket and node offsets
-  return EGNN_OK;
-}
-
-// r2 is the radius as the caller passes it; the kernels compare against (T)r2.  k up to RS_WIDE_MAX_K: the callers bound
-// it (egnn_radius_select at 32, cell_select_eligible by the descriptor's flags).
-int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
-                         const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
-                         cudaStream_t st, int pbc) {
-  if (!coors || !out_idx || !ws) return EGNN_ERR_NULL;
-  EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
-  if (dtype == EGNN_DTYPE_F64) {
-    if (!(r2 > 0.0)) return EGNN_ERR_SHAPE;
-    return cell_select<double>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
-  }
-  if (dtype != EGNN_DTYPE_F32) return EGNN_ERR_UNSUPPORTED;
-  if (!((float)r2 > 0.f)) return EGNN_ERR_SHAPE;
-  return cell_select<float>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
-}
-
-// The public entries: egnn_radius_select* with k <= 32, egnn_radius_select_wide* with k <= RS_WIDE_MAX_K.
-static int radius_ws_entry(int max_k, int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
-  if (!out_bytes) return EGNN_ERR_NULL;
-  EGNN_TRY(radius_check(B, N, C, k, max_k));
-  *out_bytes = cell_select_ws_bytes(B, N, C, 8);               // sized for float64 coordinates: covers both types
-  return EGNN_OK;
-}
-
-// lattice: a [B,C] box (pbc = PBC_BOX, may be null) or a [B,C,C] cell (PBC_CELL)
-static int radius_entry(int max_k, int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
-                        const uint8_t* mask, const void* lattice, double r2, int32_t* out_idx, int32_t* out_count,
-                        void* workspace, size_t workspace_bytes, void* stream) {
-  if (!workspace || (pbc == PBC_CELL && !lattice)) return EGNN_ERR_NULL;
-  if (pbc == PBC_CELL && (C < 2 || C > 3)) return EGNN_ERR_SHAPE;    // a cell is 2-D or 3-D (before radius_check's C > 3)
-  EGNN_TRY(radius_check(B, N, C, k, max_k));
-  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
-  if (workspace_bytes < cell_select_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
-  return cell_select_dispatch(dtype, B, N, C, k, coors, mask, lattice, r2, out_idx, nullptr, out_count, workspace,
-                              static_cast<cudaStream_t>(stream), pbc);
-}
-
 // ====================================================================== the kNN grid: k nearest, no cutoff
 //
 // egnn_knn_select's lists (the same rank, (rank, j) order, 1e5 rank of padded pairs, NaN-last rule and ok bytes) in
@@ -829,19 +623,6 @@ constexpr int KG_SETUP_THREADS = 256;
 constexpr double KG_FILL = 8.0;            // nodes aimed at per 3^C block of cells, in units of k (DESIGN.md section 6)
 constexpr int KG_MAX_RING_CELLS = 4096;    // the largest (2R+1)^C cube of cells a row visits before the full scan
 constexpr double KG_MARGIN = 1.0 - 0x1p-10;   // relative rounding margin of the stopping test
-
-struct KnnWs { CellWs cell; size_t kg, fb, nfb, total; };
-static KnnWs knn_ws_layout(int B, int N, int C, size_t coord_bytes) {
-  KnnWs w;
-  w.cell = cell_ws_layout(B, N, C, coord_bytes);
-  size_t o = w.cell.total;
-  auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
-  w.kg = take((size_t)B * sizeof(KGrid));
-  w.fb = take((size_t)B * N * sizeof(int));
-  w.nfb = take(sizeof(int));
-  w.total = o;
-  return w;
-}
 
 struct DMin { __device__ __forceinline__ double operator()(double x, double y) const { return fmin(x, y); } };
 struct DMax { __device__ __forceinline__ double operator()(double x, double y) const { return fmax(x, y); } };
@@ -1120,7 +901,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_scan_kernel(const RadArgs<T
       bool pass = false;
       if (j < a.N) {
         const T* xj = a.coors + (g0 + j) * CD;
-        key = pair_rank<T, CD, PBC>(xi, [&](int c) { return xj[c]; }, bl, binv, pc);
+        key = pair_rank<T, CD, PBC>(xi, [&](int c) { return xj[c]; }, CD, bl, binv, pc);
         if (a.mask && !a.mask[g0 + j]) key = T(1e5);
         jk = j;
         if (key != key) { key = T(INFINITY); jk = j + a.N; }
@@ -1138,79 +919,110 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_scan_kernel(const RadArgs<T
   }
 }
 
-template <typename T, int CD, int PBC>
-static int launch_knn(const RadArgs<T>& a, cudaStream_t st) {
+// ====================================================================== host side of both grids
+
+// One select on the radius grid (GRID_RADIUS) or the kNN grid (GRID_KNN): one memset of the bucket counts, then count /
+// scan / scatter into the grid's buckets and the query, one warp per row: radius_query_kernel; or, on the kNN grid,
+// knn_grid_setup_kernel first, then knn_ring_kernel and knn_scan_kernel for the rows it leaves.
+template <typename T, int CD, int PBC, int GRID>
+static int launch_grid(const RadArgs<T>& a, cudaStream_t st) {
   const size_t nodes = (size_t)a.B * a.N;
   const unsigned gn = (unsigned)((nodes + RS_THREADS - 1) / RS_THREADS);
   EGNN_CUDA_TRY(cudaMemsetAsync(a.cnt, 0, (size_t)a.B * a.Tb * sizeof(int), st));
-  EGNN_CUDA_TRY(cudaMemsetAsync(a.fb_count, 0, sizeof(int), st));
-  knn_grid_setup_kernel<T, CD, PBC><<<a.B, KG_SETUP_THREADS, 0, st>>>(a);
-  EGNN_LAUNCH_CHECK();
-  radius_count_kernel<T, CD, PBC, GRID_KNN><<<gn, RS_THREADS, 0, st>>>(a);
+  if constexpr (GRID == GRID_KNN) {
+    EGNN_CUDA_TRY(cudaMemsetAsync(a.fb_count, 0, sizeof(int), st));
+    knn_grid_setup_kernel<T, CD, PBC><<<a.B, KG_SETUP_THREADS, 0, st>>>(a);
+    EGNN_LAUNCH_CHECK();
+  }
+  radius_count_kernel<T, CD, PBC, GRID><<<gn, RS_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
   radius_scan_kernel<<<a.B, RS_SCAN_THREADS, 0, st>>>(a.cnt, a.end, a.Tb);
   EGNN_LAUNCH_CHECK();
-  radius_scatter_kernel<T, CD, PBC, GRID_KNN><<<gn, RS_THREADS, 0, st>>>(a);
+  radius_scatter_kernel<T, CD, PBC, GRID><<<gn, RS_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
+  // k <= 32: RS_WARPS rows per CTA, lists in lanes; larger k: SmemLists in dynamic shared memory
   const int KP = list_kp(a.k), warps = smem_list_warps(KP, sizeof(T));
   const size_t smem = warps * smem_list_bytes(KP, sizeof(T));
-  if (a.k <= 32) {
-    knn_ring_kernel<T, CD, PBC, false><<<(unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), RS_WARPS * 32, 0, st>>>(a, 0);
+  const unsigned rows = (unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), wide_rows = (unsigned)((nodes + warps - 1) / warps);
+  if constexpr (GRID == GRID_KNN) {
+    if (a.k <= 32) knn_ring_kernel<T, CD, PBC, false><<<rows, RS_WARPS * 32, 0, st>>>(a, 0);
+    else knn_ring_kernel<T, CD, PBC, true><<<wide_rows, warps * 32, smem, st>>>(a, KP);
+    EGNN_LAUNCH_CHECK();
+    int sms = 0;
+    EGNN_TRY(sm_count(&sms));
+    knn_scan_kernel<T, CD, PBC><<<(wide_rows < 4u * sms ? wide_rows : 4u * sms), warps * 32, smem, st>>>(a, KP);
+    EGNN_LAUNCH_CHECK();
+    count_launch(6);
   } else {
-    knn_ring_kernel<T, CD, PBC, true><<<(unsigned)((nodes + warps - 1) / warps), warps * 32, smem, st>>>(a, KP);
+    if (a.k <= 32) radius_query_kernel<T, CD, PBC><<<rows, RS_WARPS * 32, 0, st>>>(a);
+    else radius_query_wide_kernel<T, CD, PBC><<<wide_rows, warps * 32, smem, st>>>(a, KP);
+    EGNN_LAUNCH_CHECK();
+    count_launch(4);
   }
-  EGNN_LAUNCH_CHECK();
-  int sms = 0;
-  EGNN_TRY(sm_count(&sms));
-  const size_t need = (nodes + warps - 1) / warps;
-  knn_scan_kernel<T, CD, PBC><<<(unsigned)(need < (size_t)4 * sms ? need : (size_t)4 * sms), warps * 32, smem, st>>>(
-      a, KP);
-  EGNN_LAUNCH_CHECK();
-  count_launch(6);
   return EGNN_OK;
 }
 
-template <typename T>
-static int knn_grid(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box, double vr,
-                    int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st, int pbc) {
-  const KnnWs L = knn_ws_layout(B, N, C, sizeof(T));
+// r: the squared radius (GRID_RADIUS) or valid_radius (GRID_KNN) as the caller passes it; the kernels compare in T.
+// box: null, a [B,C] box, or a [B,C,C] cell under pbc = PBC_CELL.
+template <typename T, int GRID>
+static int grid_select(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box, double r,
+                       int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws, cudaStream_t st, int pbc) {
+  const KnnWs L = knn_ws_layout(B, N, C, sizeof(T));        // the radius grid's scratch is its cell part
   char* base = static_cast<char*>(ws);
-  RadArgs<T> a;
+  RadArgs<T> a{};
   a.B = B; a.N = N; a.k = k; a.Tb = rs_buckets(N);
-  a.r2 = T(0); a.cs = 0.0;
-  a.vr = (T)vr;
   a.coors = static_cast<const T*>(coors); a.mask = mask; a.box = static_cast<const T*>(box);
   a.cnt = reinterpret_cast<int*>(base + L.cell.cnt);
   a.end = reinterpret_cast<int*>(base + L.cell.end);
   a.xs = reinterpret_cast<T*>(base + L.cell.xs);
   a.idx = reinterpret_cast<int*>(base + L.cell.idx);
-  a.kg = reinterpret_cast<KGrid*>(base + L.kg);
-  a.fb_rows = reinterpret_cast<int*>(base + L.fb);
-  a.fb_count = reinterpret_cast<int*>(base + L.nfb);
-  a.out_idx = out_idx; a.out_ok = out_ok; a.out_count = nullptr;
+  a.out_idx = out_idx; a.out_ok = out_ok; a.out_count = out_count;
+  if constexpr (GRID == GRID_KNN) {
+    a.vr = (T)r;
+    a.kg = reinterpret_cast<KGrid*>(base + L.kg);
+    a.fb_rows = reinterpret_cast<int*>(base + L.fb);
+    a.fb_count = reinterpret_cast<int*>(base + L.nfb);
+  } else {
+    a.r2 = (T)r;
+    a.cs = sqrt((double)a.r2) * (1.0 + 0x1p-10);
+  }
   if (box && pbc == PBC_CELL) {
-    if (C == 2) return launch_knn<T, 2, PBC_CELL>(a, st);
-    if (C == 3) return launch_knn<T, 3, PBC_CELL>(a, st);
+    if (C == 2) return launch_grid<T, 2, PBC_CELL, GRID>(a, st);
+    if (C == 3) return launch_grid<T, 3, PBC_CELL, GRID>(a, st);
     return EGNN_ERR_SHAPE;
   }
   switch (C * 2 + (box ? 1 : 0)) {
-    case 2: return launch_knn<T, 1, PBC_NONE>(a, st);
-    case 3: return launch_knn<T, 1, PBC_BOX>(a, st);
-    case 4: return launch_knn<T, 2, PBC_NONE>(a, st);
-    case 5: return launch_knn<T, 2, PBC_BOX>(a, st);
-    case 6: return launch_knn<T, 3, PBC_NONE>(a, st);
-    case 7: return launch_knn<T, 3, PBC_BOX>(a, st);
+    case 2: return launch_grid<T, 1, PBC_NONE, GRID>(a, st);
+    case 3: return launch_grid<T, 1, PBC_BOX, GRID>(a, st);
+    case 4: return launch_grid<T, 2, PBC_NONE, GRID>(a, st);
+    case 5: return launch_grid<T, 2, PBC_BOX, GRID>(a, st);
+    case 6: return launch_grid<T, 3, PBC_NONE, GRID>(a, st);
+    case 7: return launch_grid<T, 3, PBC_BOX, GRID>(a, st);
     default: return EGNN_ERR_UNSUPPORTED;
   }
 }
 
-size_t knn_grid_ws_bytes(int B, int N, int C, size_t coord_bytes) { return knn_ws_layout(B, N, C, coord_bytes).total; }
+static int radius_check(int B, int N, int C, int k, int max_k) {
+  if (B <= 0 || N <= 0 || C <= 0 || k <= 0 || k > N) return EGNN_ERR_SHAPE;
+  if (k > max_k || C > 3) return EGNN_ERR_UNSUPPORTED;
+  if ((long long)B * rs_buckets(N) > 0x7fffffffLL) return EGNN_ERR_SHAPE;    // int bucket and node offsets
+  return EGNN_OK;
+}
 
-bool knn_grid_eligible(const EgnnLayerDesc& d) {
-  if (!(d.flags & EGNN_FLAG_KNN_GRID)) return false;
-  const int max_k = (d.flags & EGNN_FLAG_CELL_SELECT_WIDE) ? RS_WIDE_MAX_K : 32;
-  if (d.k < 1 || d.k > max_k || d.C < 1 || d.C > 3) return false;
-  return !(d.flags & (EGNN_FLAG_ONLY_SPARSE | EGNN_FLAG_ADJ_BATCHED | EGNN_FLAG_EDGES_PER_SLOT));
+// r2 is the radius as the caller passes it; the kernels compare against (T)r2.  k up to RS_WIDE_MAX_K: the callers bound
+// it (egnn_radius_select at 32, cell_select_eligible by the descriptor's flags).
+int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask,
+                         const void* box, double r2, int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws,
+                         cudaStream_t st, int pbc) {
+  if (!coors || !out_idx || !ws) return EGNN_ERR_NULL;
+  EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
+  if (dtype == EGNN_DTYPE_F64) {
+    if (!(r2 > 0.0)) return EGNN_ERR_SHAPE;
+    return grid_select<double, GRID_RADIUS>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
+  }
+  if (dtype != EGNN_DTYPE_F32) return EGNN_ERR_UNSUPPORTED;
+  if (!((float)r2 > 0.f)) return EGNN_ERR_SHAPE;
+  return grid_select<float, GRID_RADIUS>(B, N, C, k, coors, mask, box, r2, out_idx, out_ok, out_count, ws, st, pbc);
 }
 
 // Smallest N per graph at which a flagged layer selects on the kNN grid (DESIGN.md section 6).
@@ -1230,19 +1042,45 @@ int knn_grid_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coo
   if (!coors || !out_idx || !ws) return EGNN_ERR_NULL;
   EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
   if (dtype == EGNN_DTYPE_F64)
-    return knn_grid<double>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, ws, st, pbc);
+    return grid_select<double, GRID_KNN>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, nullptr, ws, st,
+                                         pbc);
   if (dtype != EGNN_DTYPE_F32) return EGNN_ERR_UNSUPPORTED;
-  return knn_grid<float>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, ws, st, pbc);
+  return grid_select<float, GRID_KNN>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, nullptr, ws, st, pbc);
+}
+
+// The public entries: egnn_radius_select* with k <= 32, egnn_radius_select_wide* and egnn_knn_grid_select* with
+// k <= RS_WIDE_MAX_K.  Workspace sizes are for float64 coordinates, which covers both types.
+static int grid_ws_entry(int grid, int max_k, int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
+  if (!out_bytes) return EGNN_ERR_NULL;
+  EGNN_TRY(radius_check(B, N, C, k, max_k));
+  *out_bytes = grid_ws_bytes(grid, B, N, C, 8);
+  return EGNN_OK;
+}
+
+// The checks of a public select entry before the select's own.  lattice: a [B,C] box (pbc = PBC_BOX, may be null) or
+// a [B,C,C] cell (PBC_CELL).
+static int grid_entry_check(int grid, int max_k, int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k,
+                            const void* lattice, void* workspace, size_t workspace_bytes) {
+  if (!workspace || (pbc == PBC_CELL && !lattice)) return EGNN_ERR_NULL;
+  if (pbc == PBC_CELL && (C < 2 || C > 3)) return EGNN_ERR_SHAPE;    // a cell is 2-D or 3-D (before radius_check's C > 3)
+  EGNN_TRY(radius_check(B, N, C, k, max_k));
+  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
+  if (workspace_bytes < grid_ws_bytes(grid, B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
+  return EGNN_OK;
+}
+
+static int radius_entry(int max_k, int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
+                        const uint8_t* mask, const void* lattice, double r2, int32_t* out_idx, int32_t* out_count,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  EGNN_TRY(grid_entry_check(GRID_RADIUS, max_k, pbc, dtype, B, N, C, k, lattice, workspace, workspace_bytes));
+  return cell_select_dispatch(dtype, B, N, C, k, coors, mask, lattice, r2, out_idx, nullptr, out_count, workspace,
+                              static_cast<cudaStream_t>(stream), pbc);
 }
 
 static int knn_entry(int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
                      const uint8_t* mask, const void* lattice, double valid_radius, int32_t* out_idx, uint8_t* out_ok,
                      void* workspace, size_t workspace_bytes, void* stream) {
-  if (!workspace || (pbc == PBC_CELL && !lattice)) return EGNN_ERR_NULL;
-  if (pbc == PBC_CELL && (C < 2 || C > 3)) return EGNN_ERR_SHAPE;
-  EGNN_TRY(radius_check(B, N, C, k, RS_WIDE_MAX_K));
-  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
-  if (workspace_bytes < knn_grid_ws_bytes(B, N, C, dtype == EGNN_DTYPE_F64 ? 8 : 4)) return EGNN_ERR_WORKSPACE;
+  EGNN_TRY(grid_entry_check(GRID_KNN, RS_WIDE_MAX_K, pbc, dtype, B, N, C, k, lattice, workspace, workspace_bytes));
   return knn_grid_dispatch(dtype, B, N, C, k, coors, mask, lattice, valid_radius, out_idx, out_ok, workspace,
                            static_cast<cudaStream_t>(stream), pbc);
 }
@@ -1250,7 +1088,7 @@ static int knn_entry(int pbc, int32_t dtype, int32_t B, int32_t N, int32_t C, in
 }  // namespace egnn
 
 extern "C" int egnn_radius_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
-  return egnn::radius_ws_entry(32, B, N, C, k, out_bytes);
+  return egnn::grid_ws_entry(egnn::GRID_RADIUS, 32, B, N, C, k, out_bytes);
 }
 
 extern "C" int egnn_radius_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
@@ -1268,7 +1106,7 @@ extern "C" int egnn_radius_select_triclinic(int32_t dtype, int32_t B, int32_t N,
 }
 
 extern "C" int egnn_radius_select_wide_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
-  return egnn::radius_ws_entry(egnn::RS_WIDE_MAX_K, B, N, C, k, out_bytes);
+  return egnn::grid_ws_entry(egnn::GRID_RADIUS, egnn::RS_WIDE_MAX_K, B, N, C, k, out_bytes);
 }
 
 extern "C" int egnn_radius_select_wide(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,
@@ -1287,10 +1125,7 @@ extern "C" int egnn_radius_select_wide_triclinic(int32_t dtype, int32_t B, int32
 }
 
 extern "C" int egnn_knn_grid_select_workspace_bytes(int32_t B, int32_t N, int32_t C, int32_t k, size_t* out_bytes) {
-  if (!out_bytes) return EGNN_ERR_NULL;
-  EGNN_TRY(egnn::radius_check(B, N, C, k, egnn::RS_WIDE_MAX_K));
-  *out_bytes = egnn::knn_grid_ws_bytes(B, N, C, 8);          // sized for float64 coordinates: covers both types
-  return EGNN_OK;
+  return egnn::grid_ws_entry(egnn::GRID_KNN, egnn::RS_WIDE_MAX_K, B, N, C, k, out_bytes);
 }
 
 extern "C" int egnn_knn_grid_select(int32_t dtype, int32_t B, int32_t N, int32_t C, int32_t k, const void* coors,

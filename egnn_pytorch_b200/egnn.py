@@ -29,6 +29,7 @@ import contextlib
 import ctypes as C
 import math
 import os
+import types
 import warnings
 import weakref
 
@@ -841,6 +842,30 @@ def _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff=None):
     return b, n, c
 
 
+@contextlib.contextmanager
+def _grid_call(coors, k, mask, box, cell, entry):
+    """The staging both cell-grid list builders share, on the compute device of `coors` (its device context held while
+    the caller's block runs): coordinates, mask and the box or cell (expanded to one per graph) on that device, the
+    [B, N, k] int32 output, the workspace of `entry` (a library entry point), the entry's function (its `_triclinic`
+    variant under a cell) and the current stream."""
+    b, n, c = coors.shape
+    lib = nat.load()
+    dev = _compute_device(coors)
+    with _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev):
+        if cell is not None:
+            lat = _as(cell, dev, coors.dtype).expand(b, c, c).contiguous()
+        else:
+            lat = None if box is None else _as(box, dev, coors.dtype).expand(b, c).contiguous()
+        nb = C.c_size_t()
+        nat.check(f"{entry}_workspace_bytes", getattr(lib, f"{entry}_workspace_bytes")(b, n, c, k, C.byref(nb)))
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        name = entry + ("_triclinic" if cell is not None else "")
+        yield types.SimpleNamespace(dev=dev, x=_as(coors, dev, coors.dtype), m=_as_u8(mask, dev), lattice=lat,
+                                    out=torch.empty((b, n, k), dtype=torch.int32, device=dev),
+                                    ws=_workspace(dev, nb.value, stream), stream=stream, name=name,
+                                    fn=getattr(lib, name))
+
+
 def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
     """k-nearest-neighbour graph of a point cloud: for every node its `k` nearest nodes (itself included, distance 0),
     as int32 neighbour lists [B, N, k] for `EGNN.forward(..., neighbors=...)`, nearest first, ties to the lower index.
@@ -854,23 +879,10 @@ def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
     [C] or [B, C] periodic box lengths, or `cell` [C, C] or [B, C, C], as `EGNN.forward` takes them (distances of the
     wrapped pair vector).  Nothing synchronises with the host: the call can be captured in a CUDA graph."""
     b, n, c = _check_graph_args("knn_neighbors", 256, coors, k, mask, box, cell)
-    lib = nat.load()
-    dev = _compute_device(coors)
-    ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)
-    with ctx:
-        x = _as(coors, dev, coors.dtype)
-        m = _as_u8(mask, dev)
-        bx = None if box is None else _as(box, dev, coors.dtype).expand(b, c).contiguous()
-        cl = None if cell is None else _as(cell, dev, coors.dtype).expand(b, c, c).contiguous()
-        out = torch.empty((b, n, k), dtype=torch.int32, device=dev)
-        nb = C.c_size_t()
-        nat.check("egnn_knn_grid_select_workspace_bytes", lib.egnn_knn_grid_select_workspace_bytes(b, n, c, k, C.byref(nb)))
-        stream_handle = torch.cuda.current_stream(dev).cuda_stream
-        ws = _workspace(dev, nb.value, stream_handle)
-        lat, entry = (cl, "egnn_knn_grid_select_triclinic") if cl is not None else (bx, "egnn_knn_grid_select")
-        nat.check(entry, getattr(lib, entry)(_KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(lat),
-                                             float("inf"), _ptr(out), None, _ptr(ws), ws.numel(),
-                                             C.c_void_p(stream_handle)))
+    with _grid_call(coors, k, mask, box, cell, "egnn_knn_grid_select") as g:
+        x, m, out = g.x, g.m, g.out
+        nat.check(g.name, g.fn(_KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(g.lattice), float("inf"),
+                                _ptr(out), None, _ptr(g.ws), g.ws.numel(), C.c_void_p(g.stream)))
         usable = torch.isfinite(x).all(dim=-1)                                   # [B, N]: nodes the layer uses
         if m is not None:
             usable = usable & m.bool()
@@ -885,29 +897,12 @@ def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
 def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts):
     b, n, c = _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff)
     r2 = float(cutoff) * float(cutoff)
-    lib = nat.load()
-    dev = _compute_device(coors)
-    ctx = _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev)
-    with ctx:
-        x = _as(coors, dev, coors.dtype)
-        m = _as_u8(mask, dev)
-        bx = None if box is None else _as(box, dev, coors.dtype).expand(b, c).contiguous()
-        cl = None if cell is None else _as(cell, dev, coors.dtype).expand(b, c, c).contiguous()
-        out = torch.empty((b, n, k), dtype=torch.int32, device=dev)
-        counts = torch.empty((b, n), dtype=torch.int32, device=dev) if return_counts else None
-        nb = C.c_size_t()
-        entry = "egnn_radius_select" if max_k == 32 else "egnn_radius_select_wide"
-        nat.check(f"{entry}_workspace_bytes", getattr(lib, f"{entry}_workspace_bytes")(b, n, c, k, C.byref(nb)))
-        stream_handle = torch.cuda.current_stream(dev).cuda_stream
-        ws = _workspace(dev, nb.value, stream_handle)
-        if cl is not None:
-            nat.check(f"{entry}_triclinic", getattr(lib, f"{entry}_triclinic")(
-                _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(cl), r2, _ptr(out), _ptr(counts),
-                _ptr(ws), ws.numel(), C.c_void_p(stream_handle)))
-        else:
-            nat.check(entry, getattr(lib, entry)(
-                _KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(x), _ptr(m), _ptr(bx), r2, _ptr(out), _ptr(counts),
-                _ptr(ws), ws.numel(), C.c_void_p(stream_handle)))
+    entry = "egnn_radius_select" if max_k == 32 else "egnn_radius_select_wide"
+    with _grid_call(coors, k, mask, box, cell, entry) as g:
+        out = g.out
+        counts = torch.empty((b, n), dtype=torch.int32, device=g.dev) if return_counts else None
+        nat.check(g.name, g.fn(_KERNEL_DTYPE[coors.dtype], b, n, c, k, _ptr(g.x), _ptr(g.m), _ptr(g.lattice), r2,
+                                _ptr(out), _ptr(counts), _ptr(g.ws), g.ws.numel(), C.c_void_p(g.stream)))
     if out.device != coors.device:
         out = out.to(coors.device)
         counts = None if counts is None else counts.to(coors.device)
