@@ -157,6 +157,13 @@ SYMBOLS = {
     "egnn_knn_grid_select_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                                  C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
                                                  C.c_size_t, C.c_void_p]),
+    "egnn_knn_select_packed_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, _P(C.c_size_t)]),
+    "egnn_knn_select_packed": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p,
+                                         C.c_void_p, C.c_void_p, C.c_double, C.c_void_p, C.c_void_p, C.c_void_p,
+                                         C.c_size_t, C.c_void_p]),
+    "egnn_knn_select_packed_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p,
+                                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
     "egnn_adj_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_size_t)]),
     "egnn_adj_expand": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -444,75 +444,9 @@ __device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t 
     _Pragma("unroll") for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);                        \
   }
 
-// 32 < k <= RS_WIDE_MAX_K: the top k kept in shared memory instead of lanes.  Per warp, KP = next_pow2(k) (>= 64) pairs
-// `list` (lk, li), sorted ascending (the KP smallest (rank, j) so far, padded with (inf, IMAX)), and KP more `queue`.  A
-// pair that beats the current k-th list entry is queued.  Once the queue could not take another 32, it is padded,
-// sorted and merged into the list: list[s] = min(list[s], queue[KP-1-s]) leaves the KP smallest of both as a bitonic
-// sequence, which log2(KP) merge steps sort.  The list is a function of the set of pairs queued, and every pair the
-// filter drops is beaten by k listed ones, so the k kept pairs are the k smallest of all pairs offered, whatever order
-// they arrive in.
-template <typename T>
-struct SmemList {
-  T* lk;
-  int* li;
-  T* qk;
-  int* qi;
-  int KP, k;
-  T thr_key = T(INFINITY);             // the k-th smallest so far
-  int thr_idx = 0x7fffffff;
-  int count = 0;                       // queued pairs (warp-uniform)
-  __device__ __forceinline__ SmemList(T* lk_, int* li_, int KP_, int k_, int lane)
-      : lk(lk_), li(li_), qk(lk_ + KP_), qi(li_ + KP_), KP(KP_), k(k_) {
-    for (int s = lane; s < KP; s += 32) { lk[s] = T(INFINITY); li[s] = 0x7fffffff; }
-  }
-  __device__ __forceinline__ bool beats(T key, int j) const { return lex_less<T>(key, j, thr_key, thr_idx); }
-  __device__ __forceinline__ void flush(int lane) {
-    for (int s = count + lane; s < KP; s += 32) { qk[s] = T(INFINITY); qi[s] = 0x7fffffff; }
-    __syncwarp();
-    bitonic_sort<T>(qk, qi, KP, lane, 32, [] { __syncwarp(); });
-    for (int s = lane; s < KP; s += 32) {
-      const T ck = qk[KP - 1 - s];
-      const int ci = qi[KP - 1 - s];
-      if (lex_less<T>(ck, ci, lk[s], li[s])) { lk[s] = ck; li[s] = ci; }
-    }
-    __syncwarp();
-    bitonic_merge<T>(lk, li, KP, lane, 32, [] { __syncwarp(); });
-    count = 0;
-    thr_key = lk[k - 1];
-    thr_idx = li[k - 1];
-  }
-  // queues the pairs of the lanes whose `pass` is set; called by the whole warp
-  __device__ __forceinline__ void push(bool pass, T key, int j, int lane) {
-    const unsigned bal = __ballot_sync(0xffffffffu, pass);
-    if (bal == 0) return;
-    if (pass) {
-      const int q = count + __popc(bal & ((1u << lane) - 1));
-      qk[q] = key;
-      qi[q] = j;
-    }
-    count += __popc(bal);
-    if (count > KP - 32) flush(lane);
-  }
-  __device__ __forceinline__ void finish(int lane) {
-    if (count > 0) flush(lane);
-  }
-  __device__ __forceinline__ void refresh() {
-    __syncwarp();
-    thr_key = lk[k - 1];
-    thr_idx = li[k - 1];
-  }
-};
-
-// Dynamic shared memory of a SmemList warp, and the warps per CTA that keep a CTA within RS_WIDE_SMEM (8, or 4 for
-// fp64 at k > 128).
-static inline size_t smem_list_bytes(int KP, size_t tbytes) { return (size_t)2 * KP * (tbytes + sizeof(int)); }
+// The warps per CTA that keep a CTA of SmemLists within RS_WIDE_SMEM (8, or 4 for fp64 at k > 128).
 static inline int smem_list_warps(int KP, size_t tbytes) {
   return smem_list_bytes(KP, tbytes) * RS_WARPS <= RS_WIDE_SMEM ? RS_WARPS : RS_WARPS / 2;
-}
-static inline int list_kp(int k) {
-  int KP = 64;
-  while (KP < k) KP <<= 1;
-  return KP;
 }
 
 // The lists of the warp in dynamic shared memory laid out [warps][2 KP] ranks, then [warps][2 KP] indices.

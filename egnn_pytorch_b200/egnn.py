@@ -382,7 +382,7 @@ class EGNN(nn.Module):
 
     # -------------------------------------------------------------- forward
     def forward(self, feats, coors, edges=None, mask=None, adj_mat=None, *, neighbors=None, neighbor_edges=None, box=None,
-                cell=None, lattice_grad=False, _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
+                cell=None, lattice_grad=False, ptr=None, _edge_labels=None, _label_emb=None, _k_hint=None, _rows=None):
         """Reference signature `forward(feats, coors, edges=None, mask=None, adj_mat=None)` (egnn_pytorch.py:224).
 
         `neighbors` (additive, keyword-only): int tensor [B, N, k] of neighbour indices, -1 = empty slot.  When
@@ -415,7 +415,21 @@ class EGNN(nn.Module):
         it its gradient through autograd, for stress and virial (README).  The wrap is rel = (x_i - x_j) - sum_c n_c a_c
         with integer image counts n, so dL/dcell[c, d] = -sum_pairs n_c dL/drel_d for d <= c (0 above the diagonal),
         dL/dbox[c] = -sum_pairs n_c dL/drel_c, and 0 on aperiodic axes; neighbour selection contributes nothing.  A [C] /
-        [C, C] lattice gets the sum over the batch.  No effect under torch.no_grad()."""
+        [C, C] lattice gets the sum over the batch.  No effect under torch.no_grad().
+
+        `ptr` (additive, keyword-only): a packed batch of variable-size graphs, PyTorch Geometric's layout.  feats
+        [1, T, dim] and coors [1, T, C] hold G graphs end to end, graph g on nodes ptr[g] .. ptr[g+1]-1 of the 1-D integer
+        tensor ptr [G+1] (ptr[0] = 0, non-decreasing, ptr[G] = T; any device).  Every graph gets what it would get
+        alone, to the rounding of the kernel type: with num_nearest_neighbors = k, its k nearest nodes of its own
+        graph (all of its nodes, with mean pooling over them, when it has fewer than k); without, all of its nodes
+        (dense).  The lists are ranked on the device by `egnn_knn_select_packed` in O(sum_g n_g^2) -- the all-pairs
+        cost of each graph alone, not of the batch padded to its largest graph -- and the layer runs on them in
+        edge-list mode, forward and backward.  `mask` [1, T] and one `box` [C] or `cell` [C, C] shared by every graph
+        combine with it; per-graph lattices, `neighbors`, `neighbor_edges`, dense `edges`, adjacency and
+        only_sparse_neighbors do not (ValueError).  ptr's values are read on the host once per tensor version."""
+        if ptr is not None:
+            neighbors, mask = self._packed_lists(feats, coors, ptr, edges, mask, adj_mat, neighbors, neighbor_edges, box,
+                                                 cell, _edge_labels, _rows)
         if neighbor_edges is not None:
             edges = self._check_neighbor_edges(feats, edges, neighbors, neighbor_edges, _label_emb)
         lattice = _check_lattice(box, cell, feats.shape[0], coors.shape[-1], self.__dict__, lattice_grad)
@@ -431,6 +445,40 @@ class EGNN(nn.Module):
                                           _rows, slot_edges=neighbor_edges is not None, box=box, cell=cell)
         return self._forward_impl(feats, coors, edges, mask, adj_mat, neighbors, _edge_labels, _label_emb, _k_hint, _rows,
                                   slot_edges=neighbor_edges is not None, box=box, cell=cell)
+
+    def _packed_lists(self, feats, coors, ptr, edges, mask, adj_mat, neighbors, neighbor_edges, box, cell, labels, rows):
+        """forward(ptr=): the checks (ValueError before anything launches), then -> (neighbour lists [1, T, k], the mask
+        edge-list mode runs with).  kNN: the segmented select's lists; under a caller's mask its ok = 0 slots (rank above
+        valid_radius) are emptied, as the per-graph select's ok bytes drop them there (without a mask the layer keeps
+        every slot, and so do these lists).  Dense: every node of the node's own graph.  Slots past a graph's size are
+        -1.  List mode runs with the caller's mask or with an all-ones one, so that mean pooling divides by the slots
+        the graph fills, as the per-graph call does."""
+        for bad, what in ((neighbors is not None or neighbor_edges is not None, "neighbors= / neighbor_edges= (the lists "
+                           "already define the graphs)"),
+                          (edges is not None, "dense edges [B, N, N, edge_dim]"),
+                          (adj_mat is not None or labels is not None or self.only_sparse_neighbors,
+                           "adj_mat, only_sparse_neighbors or num_adj_degrees"),
+                          (rows is not None, "a row range (_rows)")):
+            if bad:
+                raise ValueError(f"ptr= (a packed batch) cannot be combined with {what}")
+        t, c = coors.shape[1], coors.shape[-1]
+        if feats.shape[:2] != coors.shape[:2]:
+            raise ValueError(f"feats and coors must hold the same [1, T] nodes, got {tuple(feats.shape)} and "
+                             f"{tuple(coors.shape)}")
+        max_n = _check_ptr(ptr, coors.shape[0], t)
+        _check_packed_lattice(box, cell)
+        dev = _compute_device(feats)
+        with _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev):
+            m = _as_u8(mask, dev)
+            if self.num_nearest_neighbors > 0:
+                cdt = torch.float64 if self._kernel_dtype() == torch.float64 else torch.float32   # as the layer's select
+                idx, ok = _packed_select(_as(coors, dev, cdt), ptr, min(self.num_nearest_neighbors, max_n), m,
+                                         _packed_lattice(box, cell, dev, cdt, c), cell is not None, self.valid_radius)
+                lists = idx if m is None else idx.masked_fill(ok == 0, -1)
+            else:
+                lists = _dense_packed_lists(ptr, t, max_n, dev)
+            run_mask = mask if mask is not None else torch.ones((1, t), dtype=torch.bool, device=dev)
+        return lists, run_mask
 
     def _check_neighbor_edges(self, feats, edges, neighbors, neighbor_edges, label_emb):
         """Misuse of `neighbor_edges` raises here, before anything is staged or launched; -> the tensor to run with."""
@@ -746,6 +794,94 @@ def _check_cell(cell, b, c, cache, lattice_grad=False):
     cache["_cell_checked"] = (weakref.ref(cell), cell._version)
 
 
+_PTR_CHECKED: dict = {}
+
+
+def _check_ptr(ptr, b, t):
+    """The checks of `ptr=` (ValueError before anything launches) -> max n_g, the node count of the largest graph.
+    ptr is a 1-D integer tensor of G + 1 >= 2 graph offsets on any device, with ptr[0] == 0, non-decreasing and
+    ptr[-1] == T, for inputs of B == 1 row of T nodes.  The value checks read ptr on the host once per tensor object
+    and version (the caching rule of _check_box, shared by every module and builder), so a repeated call, or a CUDA
+    graph that replays one, does not synchronise; a ptr that was never checked cannot be checked inside a capture."""
+    if (not torch.is_tensor(ptr) or ptr.dim() != 1 or ptr.numel() < 2 or ptr.is_floating_point() or ptr.is_complex()
+            or ptr.dtype == torch.bool):
+        raise ValueError(f"ptr must be a 1-D integer tensor of G + 1 >= 2 graph offsets, got "
+                         f"{type(ptr).__name__ if not torch.is_tensor(ptr) else f'{ptr.dtype} {tuple(ptr.shape)}'}")
+    if b != 1:
+        raise ValueError(f"ptr= takes a packed batch: inputs of shape [1, T, ...] with the graphs end to end, got B={b}")
+    hit = _PTR_CHECKED.get(id(ptr))
+    if hit is not None and hit[0]() is ptr and hit[1] == ptr._version and hit[2] == t:
+        return hit[3]
+    if ptr.is_cuda and torch.cuda.is_current_stream_capturing():
+        raise ValueError("ptr= is checked on the host, which a CUDA graph capture cannot do: run the call once before "
+                         "capturing it (GraphedForward's warm-up does)")
+    p = ptr.detach().to("cpu", torch.int64)
+    if int(p[0]) != 0 or int(p[-1]) != t or bool((p[1:] < p[:-1]).any()):
+        raise ValueError(f"ptr must start at 0, be non-decreasing and end at T = {t} (the node count), got "
+                         f"{p.tolist() if p.numel() <= 16 else f'{p[:8].tolist()} ... {p[-8:].tolist()}'}")
+    max_n = int((p[1:] - p[:-1]).max())
+    if len(_PTR_CHECKED) >= 64:
+        _PTR_CHECKED.clear()
+    _PTR_CHECKED[id(ptr)] = (weakref.ref(ptr), ptr._version, t, max_n)
+    return max_n
+
+
+def _check_packed_lattice(box, cell):
+    """A packed batch takes one box [C] or cell [C, C] shared by every graph (or the [1, C] / [1, C, C] of its one
+    batch row); per-graph lattices would need a graph index in every edge kernel."""
+    if box is not None and torch.is_tensor(box) and box.dim() == 2 and box.shape[0] != 1:
+        raise ValueError(f"ptr= takes one box [C] shared by every graph; per-graph boxes [G, C] are not supported, got "
+                         f"{tuple(box.shape)}")
+    if cell is not None and torch.is_tensor(cell) and cell.dim() == 3 and cell.shape[0] != 1:
+        raise ValueError(f"ptr= takes one cell [C, C] shared by every graph; per-graph cells [G, C, C] are not "
+                         f"supported, got {tuple(cell.shape)}")
+
+
+def _packed_lattice(box, cell, dev, dtype, c):
+    """The shared box [C] or cell [C, C] of a packed batch on `dev` in `dtype`, or None."""
+    if cell is not None:
+        return _as(cell, dev, dtype).reshape(c, c).contiguous()
+    return None if box is None else _as(box, dev, dtype).reshape(c).contiguous()
+
+
+def _packed_select(x, ptr, k, m, lattice, triclinic, valid_radius):
+    """egnn_knn_select_packed on staged inputs on the current device: x [1, T, C] float32 / float64, m uint8 [1, T] or
+    None, lattice [C] or [C, C] (triclinic) in x's type or None -> (idx int32, ok uint8), both [1, T, k]."""
+    lib = nat.load()
+    t, c = x.shape[1], x.shape[2]
+    dev = x.device
+    p32 = ptr.to(device=dev, dtype=torch.int32, non_blocking=True).contiguous()
+    nb = C.c_size_t()
+    nat.check("egnn_knn_select_packed_workspace_bytes",
+              lib.egnn_knn_select_packed_workspace_bytes(p32.numel() - 1, t, c, k, C.byref(nb)))
+    stream = torch.cuda.current_stream(dev).cuda_stream
+    ws = _workspace(dev, nb.value, stream)
+    idx = torch.empty((1, t, k), dtype=torch.int32, device=dev)
+    ok = torch.empty((1, t, k), dtype=torch.uint8, device=dev)
+    name = "egnn_knn_select_packed" + ("_triclinic" if triclinic else "")
+    nat.check(name, getattr(lib, name)(_KERNEL_DTYPE[x.dtype], p32.numel() - 1, t, c, k, _ptr(p32), _ptr(x), _ptr(m),
+                                       _ptr(lattice), float(valid_radius), _ptr(idx), _ptr(ok), _ptr(ws), ws.numel(),
+                                       C.c_void_p(stream)))
+    return idx, ok
+
+
+def _packed_segments(ptr, t, dev):
+    """-> (graph index [T], first node of each graph [G], node counts [G]) of a packed batch, on the device, no sync."""
+    p = ptr.to(device=dev, dtype=torch.int64, non_blocking=True)
+    counts = p[1:] - p[:-1]
+    seg = torch.repeat_interleave(torch.arange(counts.numel(), device=dev), counts, output_size=t)
+    return seg, p[:-1], counts
+
+
+def _dense_packed_lists(ptr, t, max_n, dev):
+    """Dense graphs of a packed batch as neighbour lists [1, T, max n_g]: slot s of a node of graph g is node
+    ptr[g] + s for s < n_g, else -1.  Index arithmetic on the device, no ranking."""
+    seg, start, counts = _packed_segments(ptr, t, dev)
+    s = torch.arange(max_n, device=dev)
+    lists = torch.where(s < counts[seg].unsqueeze(1), start[seg].unsqueeze(1) + s, -1)
+    return lists.to(torch.int32).unsqueeze(0)
+
+
 def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
     """PyG-style `edge_index` [2, E] (messages flow source j = edge_index[0] -> target i = edge_index[1], one graph)
     -> padded neighbour lists [1, N, k] for `EGNN.forward(..., neighbors=...)`; -1 marks empty slots.  Glue code:
@@ -777,7 +913,7 @@ def edge_index_to_neighbors(edge_index, num_nodes, k=None, edge_attr=None):
 _RADIUS_BOX_CHECKED: dict = {}
 
 
-def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return_counts=False):
+def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return_counts=False, ptr=None):
     """Radius graph of a point cloud: for every node the (at most) `k` nearest nodes within distance `cutoff`, as int32
     neighbour lists [B, N, k] for `EGNN.forward(..., neighbors=...)`, nearest first, ties to the lower index, -1 in the
     slots left empty.  A node counts as its own neighbour (distance 0).  Computed on a cell grid (`egnn_radius_select`)
@@ -795,22 +931,30 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return
 
     With `return_counts=True` it returns `(neighbors, counts)`: counts int32 [B, N] is the number of nodes within the
     cutoff before the truncation at k (the node itself included), so `counts > k` shows where k cut the list short.
-    Nothing synchronises with the host: the call can be captured in a CUDA graph."""
-    return _radius_graph("radius_neighbors", 32, coors, cutoff, k, mask, box, cell, return_counts)
+    Nothing synchronises with the host: the call can be captured in a CUDA graph.
+
+    With `ptr` (a packed batch: coors [1, T, C] holding G graphs end to end, `ptr` [G+1] their offsets, as
+    `EGNN.forward(ptr=)` takes them) every node is ranked against the nodes of its own graph only, in O(sum_g n_g^2) by
+    `egnn_knn_select_packed` instead of on the cell grid: the lists equal the per-graph calls' concatenated, indices
+    shifted by ptr[g], with -1 also in the slots past a graph's size (`k` up to 32 whatever the graph sizes).  `box` /
+    `cell` is then one lattice shared by every graph; `return_counts` is not available."""
+    return _radius_graph("radius_neighbors", 32, coors, cutoff, k, mask, box, cell, return_counts, ptr)
 
 
-def radius_neighbors_wide(coors, cutoff, k, *, mask=None, box=None, cell=None, return_counts=False):
+def radius_neighbors_wide(coors, cutoff, k, *, mask=None, box=None, cell=None, return_counts=False, ptr=None):
     """`radius_neighbors` for lists of up to 256 neighbours: `k` in [1, min(256, N)], everything else the same -- the
     lists equal the all-pairs select's kept slots exactly, nearest first, ties to the lower index, -1 in the empty
     slots; `return_counts=True` also returns the in-radius counts before truncation.  For k <= 32 the result is
     `radius_neighbors`'s.  Longer lists (40-100 neighbours within a cutoff are common in condensed-phase atomistic
-    systems) are kept in shared memory instead of one warp's lanes (`egnn_radius_select_wide`)."""
-    return _radius_graph("radius_neighbors_wide", 256, coors, cutoff, k, mask, box, cell, return_counts)
+    systems) are kept in shared memory instead of one warp's lanes (`egnn_radius_select_wide`).  `ptr`: a packed
+    batch, as `radius_neighbors` takes it (O(sum_g n_g^2), `k` up to 256)."""
+    return _radius_graph("radius_neighbors_wide", 256, coors, cutoff, k, mask, box, cell, return_counts, ptr)
 
 
-def _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff=None):
+def _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff=None, ptr=None):
     """The argument checks of the neighbour-list builders (ValueError before anything launches) -> (B, N, C).
-    `cutoff` None: a builder without one (knn_neighbors)."""
+    `cutoff` None: a builder without one (knn_neighbors).  `ptr`: a packed batch (_check_ptr), whose graphs may hold
+    fewer than k nodes."""
     if not torch.is_tensor(coors) or coors.dim() != 3:
         raise ValueError(f"coors must be a [B, N, C] tensor, got {type(coors).__name__}"
                          f"{' of shape ' + str(tuple(coors.shape)) if torch.is_tensor(coors) else ''}")
@@ -821,8 +965,10 @@ def _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff=None):
         raise ValueError(f"coors must hold at least one node in at least one graph, got shape {tuple(coors.shape)}")
     if not 1 <= c <= 3:
         raise ValueError(f"{name} supports C <= 3 coordinates, got C={c}")
-    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= min(max_k, n):
-        raise ValueError(f"k must be an int in [1, min({max_k}, N)] = [1, {min(max_k, n)}], got {k!r}")
+    k_max = max_k if ptr is not None else min(max_k, n)
+    if isinstance(k, bool) or not isinstance(k, int) or not 1 <= k <= k_max:
+        raise ValueError(f"k must be an int in [1, {'' if ptr is not None else 'min('}{max_k}"
+                         f"{'' if ptr is not None else ', N)'}] = [1, {k_max}], got {k!r}")
     if cutoff is not None:
         cutoff = float(cutoff)
         if not (cutoff > 0.0 and math.isfinite(cutoff)):
@@ -833,6 +979,9 @@ def _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff=None):
     if mask is not None and (not torch.is_tensor(mask) or tuple(mask.shape) != (b, n)):
         raise ValueError(f"mask must be a [B, N] = [{b}, {n}] tensor, got "
                          f"{tuple(mask.shape) if torch.is_tensor(mask) else type(mask).__name__}")
+    if ptr is not None:
+        _check_ptr(ptr, b, n)
+        _check_packed_lattice(box, cell)
     if box is not None:
         if cell is not None:
             raise ValueError("pass either box= or cell=, not both")
@@ -866,7 +1015,7 @@ def _grid_call(coors, k, mask, box, cell, entry):
                                     fn=getattr(lib, name))
 
 
-def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
+def knn_neighbors(coors, k, *, mask=None, box=None, cell=None, ptr=None):
     """k-nearest-neighbour graph of a point cloud: for every node its `k` nearest nodes (itself included, distance 0),
     as int32 neighbour lists [B, N, k] for `EGNN.forward(..., neighbors=...)`, nearest first, ties to the lower index.
     The lists are those of the layer's own select (`num_nearest_neighbors=k`, no adjacency), computed on a cell grid
@@ -877,7 +1026,15 @@ def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
     `coors` float32 or float64 [B, N, C] with C <= 3, on any device (CPU tensors are staged to the current CUDA
     device; the result comes back on `coors`'s device).  `k` in [1, min(256, N)].  `mask` [B, N] bool / 0-1.  `box`
     [C] or [B, C] periodic box lengths, or `cell` [C, C] or [B, C, C], as `EGNN.forward` takes them (distances of the
-    wrapped pair vector).  Nothing synchronises with the host: the call can be captured in a CUDA graph."""
+    wrapped pair vector).  Nothing synchronises with the host: the call can be captured in a CUDA graph.
+
+    With `ptr` (a packed batch: coors [1, T, C] holding G graphs end to end, `ptr` [G+1] their offsets, as
+    `EGNN.forward(ptr=)` takes them) every node is ranked against the nodes of its own graph only, in O(sum_g n_g^2) by
+    `egnn_knn_select_packed` instead of on the kNN grid: the lists equal the per-graph calls' concatenated, indices
+    shifted by ptr[g], with -1 also in the slots past a graph's size (`k` up to 256 whatever the graph sizes).  `box` /
+    `cell` is then one lattice shared by every graph."""
+    if ptr is not None:
+        return _packed_graph("knn_neighbors", 256, coors, None, k, mask, box, cell, False, ptr)
     b, n, c = _check_graph_args("knn_neighbors", 256, coors, k, mask, box, cell)
     with _grid_call(coors, k, mask, box, cell, "egnn_knn_grid_select") as g:
         x, m, out = g.x, g.m, g.out
@@ -894,7 +1051,9 @@ def knn_neighbors(coors, k, *, mask=None, box=None, cell=None):
     return out
 
 
-def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts):
+def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts, ptr):
+    if ptr is not None:
+        return _packed_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts, ptr)
     b, n, c = _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff)
     r2 = float(cutoff) * float(cutoff)
     entry = "egnn_radius_select" if max_k == 32 else "egnn_radius_select_wide"
@@ -907,6 +1066,38 @@ def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts)
         out = out.to(coors.device)
         counts = None if counts is None else counts.to(coors.device)
     return (out, counts) if return_counts else out
+
+
+def _packed_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts, ptr):
+    """The builders on a packed batch: the segmented select, then each builder's -1 rules.  kNN (`cutoff` None): -1 in
+    slots that point at a padded node or at a node with a non-finite coordinate, and in every slot of a padded row
+    (knn_neighbors).  Radius: the kept slots are the ok = 1 slots of the select with valid_radius = cutoff^2 and no
+    mask, on coordinates where a padded node's are NaN -- its ranks are then NaN, never kept, and its own row is empty,
+    as the radius grid leaves them; a node with a non-finite coordinate ranks inf or NaN against every node, itself
+    included, and is never kept either."""
+    b, n, c = _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff, ptr)
+    if return_counts:
+        raise ValueError(f"{name}: return_counts is not available with ptr=")
+    dev = _compute_device(coors)
+    with _NULL_CTX if torch.cuda.current_device() == dev.index else torch.cuda.device(dev):
+        x, m = _as(coors, dev, coors.dtype), _as_u8(mask, dev)
+        lat = _packed_lattice(box, cell, dev, coors.dtype, c)
+        if cutoff is None:
+            out, _ = _packed_select(x, ptr, k, m, lat, cell is not None, float("inf"))
+            usable = torch.isfinite(x).all(dim=-1)                               # [1, T]: nodes the layer uses
+            if m is not None:
+                usable = usable & m.bool()
+            row_ok = usable if m is None else m.bool()
+            filled = out >= 0
+            keep = filled & torch.gather(usable, 1, out.clamp_min(0).view(b, n * k).long()).view(b, n, k)
+            keep &= row_ok.unsqueeze(-1)
+        else:
+            if m is not None:
+                x = x.masked_fill(~m.bool().unsqueeze(-1), float("nan"))
+            out, ok = _packed_select(x, ptr, k, None, lat, cell is not None, float(cutoff) * float(cutoff))
+            keep = ok.bool()
+        out = out.masked_fill(~keep, -1)
+    return out if out.device == coors.device else out.to(coors.device)
 
 
 # ----------------------------------------------------------------------------- global attention
@@ -1080,12 +1271,22 @@ class EGNN_Network(nn.Module):
             ]))
 
     def forward(self, feats, coors, adj_mat=None, edges=None, mask=None, return_coor_changes=False, *, box=None,
-                cell=None, lattice_grad=False):
+                cell=None, lattice_grad=False, ptr=None):
         """`box` (additive, keyword-only): periodic box lengths [C] or [B, C], passed to every layer (EGNN.forward).
         `cell` (additive, keyword-only, instead of `box`): a lower-triangular triclinic cell [C, C] or [B, C, C], passed
         to every layer (EGNN.forward).  `lattice_grad` (additive, keyword-only): passed to every layer, so a box / cell
-        that requires grad gets the sum of the layers' lattice gradients, through the chained coordinates too."""
+        that requires grad gets the sum of the layers' lattice gradients, through the chained coordinates too.
+        `ptr` (additive, keyword-only): a packed batch of variable-size graphs, feats [1, T] (tokens) or [1, T, dim] and
+        coors [1, T, C] with graph g on nodes ptr[g] .. ptr[g+1]-1 (EGNN.forward).  Every layer ranks each graph's
+        nodes from its own input coordinates; positions restart at every graph (node i of graph g is at position
+        i - ptr[g], and the largest graph must fit num_positions).  Adjacency, dense edges and global linear
+        attention are not available with it (ValueError)."""
         _check_lattice(box, cell, feats.shape[0], coors.shape[-1], self.__dict__, lattice_grad)
+        if ptr is not None:
+            if adj_mat is not None or exists(self.num_adj_degrees) or exists(edges) or exists(self.global_tokens):
+                raise ValueError("ptr= (a packed batch) cannot be combined with adj_mat / num_adj_degrees, dense edges or "
+                                 "global linear attention")
+            max_n = _check_ptr(ptr, feats.shape[0], feats.shape[1])
         lib = nat.load()
         out_dev = coors.device
         dev = _compute_device(coors)
@@ -1099,11 +1300,11 @@ class EGNN_Network(nn.Module):
             return emb.weight if emb.weight.device == dev else emb.weight.to(dev)
 
         if exists(self.pos_emb):
-            n = feats.shape[1]
+            n = feats.shape[1] if ptr is None else max_n
             assert n <= self.num_positions, \
                 f"given sequence length {n} must be less than the number of positions {self.num_positions} set at init"
         emb_grad = torch.is_grad_enabled() and any(e is not None and e.weight.requires_grad for e in (self.token_emb, self.pos_emb))
-        if exists(self.token_emb) and not emb_grad and self.token_emb.weight.dtype in _KERNEL_DTYPE:
+        if exists(self.token_emb) and not emb_grad and self.token_emb.weight.dtype in _KERNEL_DTYPE and ptr is None:
             # token + positional embedding in ONE launch (egnn_embed_nodes) instead of embedding, arange, embedding, add
             tw = staged(self.token_emb)
             pw = staged(self.pos_emb) if exists(self.pos_emb) else None
@@ -1117,7 +1318,10 @@ class EGNN_Network(nn.Module):
         else:                                        # training through the embedding tables: PyTorch autograd
             if exists(self.token_emb):
                 feats = F.embedding(feats, staged(self.token_emb))                   # reference :401-402
-            if exists(self.pos_emb):
+            if exists(self.pos_emb) and ptr is not None:          # positions restart at every graph of a packed batch
+                seg, start, _ = _packed_segments(ptr, feats.shape[1], dev)
+                feats = feats + staged(self.pos_emb)[torch.arange(feats.shape[1], device=dev) - start[seg]].unsqueeze(0)
+            elif exists(self.pos_emb):
                 feats = feats + staged(self.pos_emb)[:feats.shape[1]].unsqueeze(0)   # :404-408
         if exists(edges) and exists(self.edge_emb):
             edges = F.embedding(edges, staged(self.edge_emb))                        # :410-411
@@ -1174,7 +1378,7 @@ class EGNN_Network(nn.Module):
                 feats, global_tokens = global_attn(feats, global_tokens, mask=mask)
             feats, coors = egnn(feats, coors, edges, mask, adj_mat, _edge_labels=labels, _label_emb=label_emb,
                                 _k_hint=k_hint, neighbors=nbr_lists if exists(mask) else None, box=box, cell=cell,
-                                lattice_grad=lattice_grad)
+                                lattice_grad=lattice_grad, ptr=ptr)
             coor_changes.append(coors)
 
         if out_dev != dev:

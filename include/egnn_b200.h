@@ -361,6 +361,28 @@ int egnn_knn_grid_select_triclinic(int32_t dtype, int32_t B, int32_t N, int32_t 
                                    const uint8_t* mask, const void* cell, double valid_radius, int32_t* out_idx,
                                    uint8_t* out_ok, void* workspace, size_t workspace_bytes, void* stream);
 
+/* k-nearest-neighbour lists of a packed batch: G graphs of n_g = ptr[g+1] - ptr[g] nodes laid end to end on one node
+ * axis of T nodes (PyTorch Geometric's `ptr`).  Every node is ranked against the nodes of its own graph only, in
+ * O(sum_g n_g^2): out_idx and out_ok of node i of graph g equal egnn_knn_select's for that graph alone (B = 1, N = n_g,
+ * the same k, mask, valid_radius and lattice) bit for bit, with indices into the node axis (local index + ptr[g]).
+ * Slots past n_g (n_g < k) hold -1 with ok = 0; an empty graph writes nothing.
+ * ptr int32 [G+1] (device memory, read on the device only, so the call can be captured in a CUDA graph; the graph
+ * bounds are clamped to [0, T], and callers pass ptr[0] = 0, non-decreasing, ptr[G] = T); coors [T,C] (float32, or
+ * float64 when dtype == EGNN_DTYPE_F64), 1 <= C <= 8; mask [T] 0/1 or NULL; box [C] shared by every graph or NULL;
+ * out_idx int32 [T,k]; out_ok uint8 [T,k] or NULL.  1 <= k <= 256 (k > 256: EGNN_ERR_UNSUPPORTED), T <= 2^30.
+ * workspace: egnn_knn_select_packed_workspace_bytes(G, T, C, k) bytes (O(G)), 256-byte aligned.  Enqueued on
+ * `stream`, no host synchronisation. */
+int egnn_knn_select_packed_workspace_bytes(int32_t G, int32_t T, int32_t C, int32_t k, size_t* out_bytes);
+int egnn_knn_select_packed(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, const int32_t* ptr,
+                           const void* coors, const uint8_t* mask, const void* box, double valid_radius, int32_t* out_idx,
+                           uint8_t* out_ok, void* workspace, size_t workspace_bytes, void* stream);
+/* egnn_knn_select_packed under a triclinic cell [C, C] shared by every graph (C in {2, 3}, else EGNN_ERR_SHAPE), as
+ * egnn_knn_grid_select_triclinic takes one graph's cell.  Same workspace. */
+int egnn_knn_select_packed_triclinic(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, const int32_t* ptr,
+                                     const void* coors, const uint8_t* mask, const void* cell, double valid_radius,
+                                     int32_t* out_idx, uint8_t* out_ok, void* workspace, size_t workspace_bytes,
+                                     void* stream);
+
 /* N-th degree adjacency of EGNN_Network (egnn_pytorch.py:414-428) without the dense A@A:
  * adj_in [N,N] or [B,N,N] 0/1; writes the expanded adjacency adj_out [B,N,N] 0/1, the degree
  * labels labels_out [B,N,N] (0 = not connected, d = first reached in round d) and
