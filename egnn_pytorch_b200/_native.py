@@ -164,6 +164,11 @@ SYMBOLS = {
     "egnn_knn_select_packed_triclinic": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_void_p, C.c_double, C.c_void_p,
                                                    C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),
+    **{f"egnn_{g}_select_packed{v}": (C.c_int, [C.c_int32] * 6 + [C.c_void_p] * 4 + [C.c_double] + [C.c_void_p] * 3
+                                      + [C.c_size_t, C.c_void_p])
+       for g in ("radius", "knn_grid") for v in ("", "_triclinic")},
+    **{f"egnn_{g}_select_packed_workspace_bytes": (C.c_int, [C.c_int32] * 4 + [_P(C.c_size_t)])
+       for g in ("radius", "knn_grid")},
     "egnn_adj_workspace_bytes": (C.c_int, [C.c_int32, C.c_int32, _P(C.c_size_t)]),
     "egnn_adj_expand": (C.c_int, [C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p,
                                   C.c_void_p, C.c_void_p, C.c_size_t, C.c_void_p]),

@@ -98,6 +98,14 @@ int cell_select_dispatch(int32_t dtype, int B, int N, int C, int k, const void* 
 bool knn_grid_runs(const EgnnLayerDesc& d, const EgnnLayerIO& io);
 int knn_grid_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box,
                       double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st, int pbc);
+// Either grid on a packed batch (radius_select.cu, for segment_select.cu's grid entries; knn: the kNN grid, else the
+// radius grid): its scratch for T nodes of G graphs (either coordinate type), the smallest graph this call puts on it
+// (INT_MAX: none), and its launches for the graphs of at least min_n nodes while *seg_valid (set on the device).
+size_t packed_grid_ws_bytes(bool knn, int G, int T, int C);
+int packed_grid_min_n(bool knn, int32_t dtype, int k, double r);
+int packed_grid_launch(bool knn, int32_t dtype, int G, int T, int C, int k, int min_n, const int32_t* ptr,
+                       const int* seg_valid, const void* coors, const uint8_t* mask, const void* lattice, int pbc,
+                       double r, int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st);
 
 // ------------------------------------------------------------------ derived sizes
 struct Dims {

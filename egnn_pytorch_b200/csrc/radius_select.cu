@@ -45,18 +45,18 @@ constexpr double RS_CLAMP = 1073741824.0;     // 2^30: aperiodic cell coordinate
 constexpr int GRID_RADIUS = 0, GRID_KNN = 1;  // which grid the count / scatter kernels bin into
 
 // Buckets per graph: next_pow2(2N).
-static inline int rs_buckets(int N) {
+__host__ __device__ inline int rs_buckets(int N) {
   int t = 2;
   while (t < 2 * N) t <<= 1;
   return t;
 }
 
+// The grid's scratch from byte `o` on, for `nodes` nodes in `nb` buckets: B N nodes in B next_pow2(2N) buckets, or
+// the T nodes of a packed batch in 4 T buckets (graph g's from 4 ptr[g] on, next_pow2(2 n_g) <= 4 n_g of them).
 struct CellWs { size_t cnt, end, xs, idx, total; };
-static CellWs cell_ws_layout(int B, int N, int C, size_t coord_bytes) {
+static CellWs cell_ws_layout(size_t nodes, size_t nb, int C, size_t coord_bytes, size_t o = 0) {
   CellWs w;
-  size_t o = 0;
   auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
-  const size_t nb = (size_t)B * rs_buckets(N), nodes = (size_t)B * N;
   w.cnt = take(nb * sizeof(int));
   w.end = take(nb * sizeof(int));
   w.xs = take((size_t)C * nodes * coord_bytes);
@@ -81,13 +81,13 @@ struct KGrid {
 static_assert(sizeof(KGrid) == 176, "KGrid layout");
 
 struct KnnWs { CellWs cell; size_t kg, fb, nfb, total; };
-static KnnWs knn_ws_layout(int B, int N, int C, size_t coord_bytes) {
+static KnnWs knn_ws_layout(int graphs, size_t nodes, size_t nb, int C, size_t coord_bytes, size_t o = 0) {
   KnnWs w;
-  w.cell = cell_ws_layout(B, N, C, coord_bytes);
-  size_t o = w.cell.total;
+  w.cell = cell_ws_layout(nodes, nb, C, coord_bytes, o);
+  o = w.cell.total;
   auto take = [&](size_t bytes) { size_t r = o; o += round_up(bytes, 256); return r; };
-  w.kg = take((size_t)B * sizeof(KGrid));
-  w.fb = take((size_t)B * N * sizeof(int));
+  w.kg = take((size_t)graphs * sizeof(KGrid));
+  w.fb = take(nodes * sizeof(int));
   w.nfb = take(sizeof(int));
   w.total = o;
   return w;
@@ -95,7 +95,9 @@ static KnnWs knn_ws_layout(int B, int N, int C, size_t coord_bytes) {
 
 // The scratch of the radius grid (GRID_RADIUS) or of the kNN grid (GRID_KNN), which contains the radius grid's.
 static size_t grid_ws_bytes(int grid, int B, int N, int C, size_t coord_bytes) {
-  return grid == GRID_KNN ? knn_ws_layout(B, N, C, coord_bytes).total : cell_ws_layout(B, N, C, coord_bytes).total;
+  const size_t nodes = (size_t)B * N, nb = (size_t)B * rs_buckets(N);
+  return grid == GRID_KNN ? knn_ws_layout(B, nodes, nb, C, coord_bytes).total
+                          : cell_ws_layout(nodes, nb, C, coord_bytes).total;
 }
 
 // The k, C and flags both grids serve: k <= 32, or <= RS_WIDE_MAX_K under EGNN_FLAG_CELL_SELECT_WIDE; C <= 3; no
@@ -156,7 +158,62 @@ struct RadArgs {
   int* fb_rows;                    // [B*N] rows (b*N + i) left to knn_scan_kernel
   int* fb_count;                   // their number
   T vr;                            // ok = rank <= vr
+  // the segment form (SEG, a packed batch): B = G graphs, N = T nodes; graph b holds nodes [ptr[b], ptr[b+1]) and
+  // buckets [4 ptr[b], 4 ptr[b] + next_pow2(2 n_b)), idx holds node-axis indices, and one box or cell serves every graph
+  const int32_t* ptr;              // [G+1]
+  const int* seg_valid;            // 1: ptr is non-decreasing within [0, T] (seg_grid_tiles_kernel), else no graph is on the grid
+  int min_n;                       // graphs of fewer nodes are not on the grid (at least k and 1)
 };
+
+// Graph b as the kernels address it: its lattice index lb, bucket count Tb, first node g0 (on the node axis and in
+// xs / idx) and first bucket.
+struct GraphAt { int b, lb, Tb; size_t g0, bkt; };
+
+template <typename T, bool SEG>
+__device__ __forceinline__ GraphAt graph_at(const RadArgs<T>& a, int b) {
+  if constexpr (SEG) {
+    const int lo = a.ptr[b];
+    return {b, 0, rs_buckets(a.ptr[b + 1] - lo), (size_t)lo, 4 * (size_t)lo};
+  } else {
+    return {b, b, a.Tb, (size_t)b * a.N, (size_t)b * a.Tb};
+  }
+}
+
+// The fields of g as the unpacked form reads them straight from its arguments (graph b = g.b), so that its kernels
+// compile as they did before the segment form.
+template <typename T, bool SEG>
+__device__ __forceinline__ int tb_of(const RadArgs<T>& a, const GraphAt& g) { return SEG ? g.Tb : a.Tb; }
+template <bool SEG>
+__device__ __forceinline__ int lb_of(const GraphAt& g) { return SEG ? 0 : g.b; }
+template <typename T, bool SEG>
+__device__ __forceinline__ size_t bkt_of(const RadArgs<T>& a, const GraphAt& g) {
+  return SEG ? g.bkt : (size_t)g.b * a.Tb;
+}
+template <typename T, bool SEG>
+__device__ __forceinline__ size_t g0_of(const RadArgs<T>& a, const GraphAt& g) { return SEG ? g.g0 : (size_t)g.b * a.N; }
+
+// SEG: whether graph b is on the grid (a valid ptr, at least min_n nodes).
+template <typename T>
+__device__ __forceinline__ bool seg_on_grid(const RadArgs<T>& a, int b) {
+  return *a.seg_valid && a.ptr[b + 1] - a.ptr[b] >= a.min_n;
+}
+
+// SEG: the graph b holding node t, if it is on the grid (the last b with ptr[b] <= t; ptr is valid).
+template <typename T>
+__device__ __forceinline__ bool seg_node(const RadArgs<T>& a, int t, int& b) {
+  if (!*a.seg_valid) return false;
+  int lo = 0, hi = a.B - 1;
+  while (lo < hi) {
+    const int mid = (lo + hi + 1) >> 1;
+    if (a.ptr[mid] <= t) lo = mid; else hi = mid - 1;
+  }
+  b = lo;
+  return t >= a.ptr[b] && t < a.ptr[b + 1] && a.ptr[b + 1] - a.ptr[b] >= a.min_n;
+}
+
+// Nodes on the launch's node axis: B N, or T in the segment form.
+template <typename T, bool SEG>
+__device__ __forceinline__ size_t grid_nodes(const RadArgs<T>& a) { return SEG ? (size_t)a.N : (size_t)a.B * a.N; }
 
 __device__ __forceinline__ int cell_coord(double x, double cs, double L, double w, int n) {
   if (n == 0) return (int)fmin(fmax(floor(x / cs), -RS_CLAMP), RS_CLAMP);
@@ -278,29 +335,29 @@ __device__ __forceinline__ int knn_index(const KGrid& g, const int (&cc)[CD]) {
   return t;
 }
 
-// The bucket node x of graph b goes to: a hashed radius cell, or a dense kNN cell.
-template <typename T, int CD, int PBC, int GRID>
-__device__ __forceinline__ int grid_bucket(const RadArgs<T>& a, int b, const T (&x)[CD]) {
+// The bucket node x of graph g goes to, within its region: a hashed radius cell, or a dense kNN cell.
+template <typename T, int CD, int PBC, int GRID, bool SEG>
+__device__ __forceinline__ int grid_bucket(const RadArgs<T>& a, const GraphAt& g, const T (&x)[CD]) {
   int cc[CD];
   if constexpr (GRID == GRID_KNN) {
-    knn_cell<T, CD, PBC>(a.kg[b], x, cc);
-    return knn_index<CD>(a.kg[b], cc);
+    knn_cell<T, CD, PBC>(a.kg[g.b], x, cc);
+    return knn_index<CD>(a.kg[g.b], cc);
   } else {
     int n[CD];
-    radius_cells<T, CD, PBC>(a, b, x, cc, n);
-    return cell_bucket<CD>(cc, a.Tb);
+    radius_cells<T, CD, PBC>(a, lb_of<SEG>(g), x, cc, n);
+    return cell_bucket<CD>(cc, tb_of<T, SEG>(a, g));
   }
 }
 
-// Row t = b*N + i of a node the grid does not hold.  The radius grid leaves it empty.  The kNN grid writes a padded
-// row (every rank 1e5 in egnn_knn_select: slots 0 .. k-1 with ok = (1e5 <= vr)) and leaves a non-finite node's row to
-// the full scan.
+// Row t = b*N + i of a node the grid does not hold (i = t in the segment form).  The radius grid leaves it empty.  The
+// kNN grid writes a padded row (every rank 1e5 in egnn_knn_select: the graph's first k nodes, from node j0, with
+// ok = (1e5 <= vr)) and leaves a non-finite node's row to the full scan.
 template <typename T, int GRID>
-__device__ __forceinline__ void outside_row(const RadArgs<T>& a, size_t t, int i) {
+__device__ __forceinline__ void outside_row(const RadArgs<T>& a, size_t t, int i, int j0) {
   if constexpr (GRID == GRID_KNN) {
     if (a.mask && !a.mask[t]) {
       for (int s = 0; s < a.k; ++s) {
-        a.out_idx[t * a.k + s] = s;
+        a.out_idx[t * a.k + s] = j0 + s;
         if (a.out_ok) a.out_ok[t * a.k + s] = T(1e5) <= a.vr ? 1 : 0;
       }
     } else {
@@ -315,23 +372,38 @@ __device__ __forceinline__ void outside_row(const RadArgs<T>& a, size_t t, int i
   }
 }
 
-template <typename T, int CD, int PBC, int GRID = GRID_RADIUS>
-__global__ void __launch_bounds__(RS_THREADS) radius_count_kernel(const RadArgs<T> a) {
-  const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
-  if (t >= (size_t)a.B * a.N) return;
-  const int b = (int)(t / a.N), i = (int)(t % a.N);
-  T x[CD];
-  if (!load_node<T, CD>(a, t, x)) {                   // not in the grid
-    outside_row<T, GRID>(a, t, i);
-    return;
+// The node (graph b, index i) of thread t: b = t / N, i = t % N; in the segment form (SEG) the graph holding node t,
+// i = t, false when that graph is not on the grid.
+template <typename T, bool SEG>
+__device__ __forceinline__ bool grid_thread_node(const RadArgs<T>& a, size_t t, int& b, int& i) {
+  if constexpr (SEG) {
+    i = (int)t;
+    return seg_node(a, i, b);
+  } else {
+    b = (int)(t / a.N); i = (int)(t % a.N);
+    return true;
   }
-  atomicAdd(a.cnt + (size_t)b * a.Tb + grid_bucket<T, CD, PBC, GRID>(a, b, x), 1);
 }
 
-__global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_kernel(const int* __restrict__ cnt, int* __restrict__ start, int Tb) {
+template <typename T, int CD, int PBC, int GRID = GRID_RADIUS, bool SEG = false>
+__global__ void __launch_bounds__(RS_THREADS) radius_count_kernel(const RadArgs<T> a) {
+  const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
+  if (t >= grid_nodes<T, SEG>(a)) return;
+  int b, i;
+  if (!grid_thread_node<T, SEG>(a, t, b, i)) return;
+  T x[CD];
+  if (!load_node<T, CD>(a, t, x)) {                   // not in the grid
+    outside_row<T, GRID>(a, t, i, SEG ? a.ptr[b] : 0);
+    return;
+  }
+  const GraphAt g = graph_at<T, SEG>(a, b);
+  atomicAdd(a.cnt + bkt_of<T, SEG>(a, g) + grid_bucket<T, CD, PBC, GRID, SEG>(a, g, x), 1);
+}
+
+// The exclusive prefix of the Tb bucket sizes cnt[g ..] into start[g ..], by one CTA.
+__device__ __forceinline__ void scan_buckets(const int* __restrict__ cnt, int* __restrict__ start, size_t g, int Tb) {
   using Scan = cub::BlockScan<int, RS_SCAN_THREADS>;
   __shared__ typename Scan::TempStorage tmp;
-  const size_t g = (size_t)blockIdx.x * Tb;
   int carry = 0;
   for (int base = 0; base < Tb; base += 4 * RS_SCAN_THREADS) {
     int v[4], s = 0;
@@ -355,15 +427,29 @@ __global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_kernel(const int*
   }
 }
 
-template <typename T, int CD, int PBC, int GRID = GRID_RADIUS>
+__global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_kernel(const int* __restrict__ cnt, int* __restrict__ start, int Tb) {
+  scan_buckets(cnt, start, (size_t)blockIdx.x * Tb, Tb);
+}
+
+// The segment form of radius_scan_kernel: graph blockIdx.x's region, if the graph is on the grid.
+template <typename T>
+__global__ void __launch_bounds__(RS_SCAN_THREADS) radius_scan_seg_kernel(const RadArgs<T> a) {
+  if (!seg_on_grid(a, blockIdx.x)) return;
+  const GraphAt g = graph_at<T, true>(a, blockIdx.x);
+  scan_buckets(a.cnt, a.end, g.bkt, g.Tb);
+}
+
+template <typename T, int CD, int PBC, int GRID = GRID_RADIUS, bool SEG = false>
 __global__ void __launch_bounds__(RS_THREADS) radius_scatter_kernel(const RadArgs<T> a) {
   const size_t t = (size_t)blockIdx.x * RS_THREADS + threadIdx.x;
-  if (t >= (size_t)a.B * a.N) return;
-  const int b = (int)(t / a.N), i = (int)(t % a.N);
+  if (t >= grid_nodes<T, SEG>(a)) return;
+  int b, i;
+  if (!grid_thread_node<T, SEG>(a, t, b, i)) return;
   T x[CD];
   if (!load_node<T, CD>(a, t, x)) return;
-  const size_t g0 = (size_t)b * a.N, BN = (size_t)a.B * a.N;
-  const int pos = atomicAdd(a.end + (size_t)b * a.Tb + grid_bucket<T, CD, PBC, GRID>(a, b, x), 1);
+  const GraphAt g = graph_at<T, SEG>(a, b);
+  const size_t g0 = g0_of<T, SEG>(a, g), BN = grid_nodes<T, SEG>(a);
+  const int pos = atomicAdd(a.end + bkt_of<T, SEG>(a, g) + grid_bucket<T, CD, PBC, GRID, SEG>(a, g, x), 1);
 #pragma unroll
   for (int c = 0; c < CD; ++c) a.xs[c * BN + g0 + pos] = x[c];
   a.idx[g0 + pos] = i;
@@ -388,16 +474,16 @@ __device__ __forceinline__ int bucket_stream(int lane, bool keep, int bkt, const
 // The candidate stream of node i of graph b, which its warp reads t = lane, lane + 32, ...: the deduplicated buckets of
 // the 3^C cells around xi, flattened.  Returns its length; wexcl / wdelta (the warp's 32 ints each) receive per kept
 // bucket its first stream position and its cell-order position minus that.
-template <typename T, int CD, int PBC>
-__device__ __forceinline__ int row_stream(const RadArgs<T>& a, int b, int lane, const T (&xi)[CD], const int* cnt,
-                                          const int* end, int* wexcl, int* wdelta) {
+template <typename T, int CD, int PBC, bool SEG>
+__device__ __forceinline__ int row_stream(const RadArgs<T>& a, const GraphAt& g, int lane, const T (&xi)[CD],
+                                          const int* cnt, const int* end, int* wexcl, int* wdelta) {
   constexpr int NB = CD == 1 ? 3 : (CD == 2 ? 9 : 27);           // neighbouring cells
   // lane l < NB: the bucket of neighbouring cell l; a bucket reached twice (a periodic axis of 1 or 2 cells, or two cells
   // hashing alike) is kept by its lowest lane only, so that no node enters the stream twice
   int bkt = -1 - lane;
   if (lane < NB) {
     int n[CD], cc[CD];
-    radius_cells<T, CD, PBC>(a, b, xi, cc, n);
+    radius_cells<T, CD, PBC>(a, lb_of<SEG>(g), xi, cc, n);
     int r = lane;
 #pragma unroll
     for (int c = 0; c < CD; ++c) {
@@ -406,7 +492,7 @@ __device__ __forceinline__ int row_stream(const RadArgs<T>& a, int b, int lane, 
       if (n[c] > 0) v = v < 0 ? v + n[c] : (v >= n[c] ? v - n[c] : v);
       cc[c] = v;
     }
-    bkt = cell_bucket<CD>(cc, a.Tb);
+    bkt = cell_bucket<CD>(cc, tb_of<T, SEG>(a, g));
   }
   const unsigned same = __match_any_sync(0xffffffffu, bkt);
   return bucket_stream(lane, lane < NB && __ffs(same) - 1 == lane, bkt, cnt, end, wexcl, wdelta);
@@ -427,21 +513,40 @@ __device__ __forceinline__ T stream_rank(const RadArgs<T>& a, size_t g0, size_t 
   return pair_rank<T, CD, PBC>(xi, [&](int c) { return a.xs[c * BN + pos]; }, CD, bl, binv, pc);
 }
 
-// The prologue of both query kernels: the node at cell-order position p of graph b (false: beyond the nodes the graph
+// The graph and cell-order position of the query warp gw: graph gw / N, position gw % N; in the segment form (SEG)
+// the graph holding node gw (its region of xs / idx is its node range), false when that graph is not on the grid.
+template <typename T, bool SEG>
+__device__ __forceinline__ bool grid_query_row(const RadArgs<T>& a, size_t gw, GraphAt& g, int& p) {
+  int b;
+  if constexpr (SEG) {
+    if (!seg_node(a, (int)gw, b)) return false;
+    g = graph_at<T, true>(a, b);
+    p = (int)(gw - g.g0);
+  } else {
+    b = (int)(gw / a.N); p = (int)(gw % a.N);
+    g = graph_at<T, false>(a, b);
+  }
+  return true;
+}
+
+// The prologue of the query kernels: the node at cell-order position p of graph g (false: beyond the nodes the graph
 // put into its grid), its coordinates xi and its graph's box (bl, binv) or cell (pc).
 #define RS_QUERY_ROW()                                                                                                  \
-  const int* cnt = a.cnt + (size_t)b * a.Tb;                                                                            \
-  const int* end = a.end + (size_t)b * a.Tb;                                                                            \
-  if (p >= end[a.Tb - 1]) return;                                                                                       \
-  const size_t g0 = (size_t)b * a.N, BN = (size_t)a.B * a.N;                                                            \
+  GraphAt g;                                                                                                            \
+  int p;                                                                                                                \
+  if (!grid_query_row<T, SEG>(a, gw, g, p)) return;                                                                     \
+  const int* cnt = a.cnt + bkt_of<T, SEG>(a, g);                                                                        \
+  const int* end = a.end + bkt_of<T, SEG>(a, g);                                                                        \
+  if (p >= end[tb_of<T, SEG>(a, g) - 1]) return;                                                                        \
+  const size_t g0 = g0_of<T, SEG>(a, g), BN = grid_nodes<T, SEG>(a);                                                    \
   const int i = a.idx[g0 + p];                                                                                          \
   T xi[CD];                                                                                                             \
   _Pragma("unroll") for (int c = 0; c < CD; ++c) xi[c] = a.xs[c * BN + g0 + p];                                         \
   T bl[CD], binv[CD], pc[PBC == PBC_CELL ? CELL_STAGED : 1];                                                            \
   if constexpr (PBC == PBC_CELL) {                                                                                      \
-    _Pragma("unroll") for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, CD, t);                    \
+    _Pragma("unroll") for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, lb_of<SEG>(g), CD, t);        \
   } else if constexpr (PBC) {                                                                                           \
-    _Pragma("unroll") for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);                        \
+    _Pragma("unroll") for (int c = 0; c < CD; ++c) box_axis<T>(a.box, lb_of<SEG>(g), CD, c, bl[c], binv[c]);           \
   }
 
 // The warps per CTA that keep a CTA of SmemLists within RS_WIDE_SMEM (8, or 4 for fp64 at k > 128).
@@ -455,7 +560,7 @@ static inline int smem_list_warps(int KP, size_t tbytes) {
   int* li = reinterpret_cast<int*>(reinterpret_cast<T*>(sm) + (size_t)warps * 2 * KP) + (size_t)warp * 2 * KP;
 
 // k <= 32: the candidate stream, filtered by rank <= r2 and against the current k-th, in a LaneList.
-template <typename T, int CD, int PBC>
+template <typename T, int CD, int PBC, bool SEG = false>
 __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadArgs<T> a) {
   __shared__ T qkey[RS_WARPS][64];
   __shared__ int qidx[RS_WARPS][64];
@@ -463,10 +568,9 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
   __shared__ int sdelta[RS_WARPS][32];
   const int warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const size_t gw = (size_t)blockIdx.x * RS_WARPS + warp;
-  if (gw >= (size_t)a.B * a.N) return;
-  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  if (gw >= grid_nodes<T, SEG>(a)) return;
   RS_QUERY_ROW()
-  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
+  const int total = row_stream<T, CD, PBC, SEG>(a, g, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
 
   LaneList<T> L(qkey[warp], qidx[warp], a.k);
   int nin = 0;                         // this lane's in-radius candidates
@@ -484,7 +588,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
     L.push(pass, key, j, lane);
   }
   L.finish(lane);
-  const size_t row = g0 + i;
+  const size_t row = SEG ? (size_t)i : g0 + i;        // the segment form's idx holds node-axis indices
   if (lane < a.k) {
     const size_t o = row * a.k + lane;
     const bool kept = L.bidx != 0x7fffffff;
@@ -499,17 +603,16 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_kernel(const RadAr
 }
 
 // 32 < k <= RS_WIDE_MAX_K: the candidate stream of radius_query_kernel with the same filter, in a SmemList.
-template <typename T, int CD, int PBC>
+template <typename T, int CD, int PBC, bool SEG = false>
 __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const RadArgs<T> a, int KP) {
   extern __shared__ __align__(16) unsigned char rsw_sm[];
   __shared__ int sexcl[RS_WARPS][32];
   __shared__ int sdelta[RS_WARPS][32];
   const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const size_t gw = (size_t)blockIdx.x * warps + warp;
-  if (gw >= (size_t)a.B * a.N) return;
-  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  if (gw >= grid_nodes<T, SEG>(a)) return;
   RS_QUERY_ROW()
-  const int total = row_stream<T, CD, PBC>(a, b, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
+  const int total = row_stream<T, CD, PBC, SEG>(a, g, lane, xi, cnt, end, sexcl[warp], sdelta[warp]);
 
   RS_SMEM_LIST(rsw_sm)
   SmemList<T> L(lk, li, KP, a.k, lane);
@@ -528,7 +631,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32) radius_query_wide_kernel(const 
     L.push(pass, key, j, lane);
   }
   L.finish(lane);
-  const size_t row = g0 + i;
+  const size_t row = SEG ? (size_t)i : g0 + i;
   for (int s = lane; s < a.k; s += 32) {
     const size_t o = row * a.k + s;
     const bool kept = li[s] != 0x7fffffff;
@@ -566,18 +669,21 @@ struct DMax { __device__ __forceinline__ double operator()(double x, double y) c
 // zero or small extent -- coincident points, a line in 3-D -- gets one cell and leaves the volume), and grows until the
 // dense grid fits the Tb buckets.  Periodic axes have their length L (or the cell's perpendicular width) instead of the
 // extent and n = max(1, floor(L / cs)) cells of width L / n >= cs, as in the radius grid.
-template <typename T, int CD, int PBC>
+template <typename T, int CD, int PBC, bool SEG = false>
 __global__ void __launch_bounds__(KG_SETUP_THREADS) knn_grid_setup_kernel(const RadArgs<T> a) {
   using Red = cub::BlockReduce<double, KG_SETUP_THREADS>;
   __shared__ typename Red::TempStorage tmp;
   __shared__ double res[2 * CD + 2];
   const int b = blockIdx.x;
+  if (SEG && !seg_on_grid(a, b)) return;
+  const int nodes = SEG ? a.ptr[b + 1] - a.ptr[b] : a.N;
+  const int lb = SEG ? 0 : b;                          // the lattice's graph index
   double mn[CD], mx[CD], amax = 0.0, count = 0.0;
 #pragma unroll
   for (int c = 0; c < CD; ++c) { mn[c] = INFINITY; mx[c] = -INFINITY; }
-  for (int i = threadIdx.x; i < a.N; i += KG_SETUP_THREADS) {
+  for (int i = threadIdx.x; i < nodes; i += KG_SETUP_THREADS) {
     T x[CD];
-    if (!load_node<T, CD>(a, (size_t)b * a.N + i, x)) continue;
+    if (!load_node<T, CD>(a, (SEG ? (size_t)a.ptr[b] : (size_t)b * a.N) + i, x)) continue;
     count += 1.0;
 #pragma unroll
     for (int c = 0; c < CD; ++c) {
@@ -610,7 +716,7 @@ __global__ void __launch_bounds__(KG_SETUP_THREADS) knn_grid_setup_kernel(const 
   bool per[CD];
   if constexpr (PBC == PBC_CELL) {
     double G[CD][CD];
-    cell_inverse<T, CD>(a.box + (size_t)b * CD * CD, G, per);
+    cell_inverse<T, CD>(a.box + (size_t)lb * CD * CD, G, per);
 #pragma unroll
     for (int c = 0; c < CD; ++c) {
       double g2 = 0.0;
@@ -623,7 +729,7 @@ __global__ void __launch_bounds__(KG_SETUP_THREADS) knn_grid_setup_kernel(const 
   } else {
 #pragma unroll
     for (int c = 0; c < CD; ++c) {
-      const T l = PBC == PBC_BOX ? a.box[(size_t)b * CD + c] : T(0);
+      const T l = PBC == PBC_BOX ? a.box[(size_t)lb * CD + c] : T(0);
       per[c] = l > T(0) && l < T(INFINITY);
       len[c] = per[c] ? (double)l : res[CD + c] - res[c];
     }
@@ -654,7 +760,7 @@ __global__ void __launch_bounds__(KG_SETUP_THREADS) knn_grid_setup_kernel(const 
         const double q = floor(len[c] / cs);
         cells *= per[c] ? fmax(q, 1.0) : q + 1.0;
       }
-      if (cells <= (double)a.Tb) break;
+      if (cells <= (double)(SEG ? rs_buckets(nodes) : a.Tb)) break;
       cs *= 2.0;
       usable = grow < 2100;
     }
@@ -692,10 +798,10 @@ __global__ void __launch_bounds__(KG_SETUP_THREADS) knn_grid_setup_kernel(const 
 // can rank before or tie with it.  Returns false when the row is left to the full scan: no usable grid, the ring
 // budget exhausted, or a k-th rank that is not finite or (under a mask) reaches the padded pairs' 1e5.
 template <typename T, int CD, int PBC, class List>
-__device__ __forceinline__ bool knn_ring_row(const RadArgs<T>& a, List& L, int b, int lane, const T (&xi)[CD],
+__device__ __forceinline__ bool knn_ring_row(const RadArgs<T>& a, List& L, const GraphAt& ga, int lane, const T (&xi)[CD],
                                              const T (&bl)[CD], const T (&binv)[CD], const T* pc, const int* cnt,
                                              const int* end, size_t g0, size_t BN, int* wexcl, int* wdelta) {
-  const KGrid& g = a.kg[b];
+  const KGrid& g = a.kg[ga.b];
   if (!g.ok) return false;
   int cc[CD], dlo[CD], dhi[CD], n[CD];
   knn_cell<T, CD, PBC>(g, xi, cc);
@@ -766,7 +872,7 @@ __device__ __forceinline__ bool knn_ring_row(const RadArgs<T>& a, List& L, int b
 }
 
 // The ring query: one warp per node in cell order; k <= 32 in a LaneList, larger k in a SmemList (KP > 0).
-template <typename T, int CD, int PBC, bool WIDE>
+template <typename T, int CD, int PBC, bool WIDE, bool SEG = false>
 __global__ void __launch_bounds__(RS_WARPS * 32) knn_ring_kernel(const RadArgs<T> a, int KP) {
   extern __shared__ __align__(16) unsigned char kgr_sm[];
   __shared__ T qkey[WIDE ? 1 : RS_WARPS][64];
@@ -775,14 +881,13 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_ring_kernel(const RadArgs<T
   __shared__ int sdelta[RS_WARPS][32];
   const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
   const size_t gw = (size_t)blockIdx.x * warps + warp;
-  if (gw >= (size_t)a.B * a.N) return;
-  const int b = (int)(gw / a.N), p = (int)(gw % a.N);
+  if (gw >= grid_nodes<T, SEG>(a)) return;
   RS_QUERY_ROW()
-  const size_t row = g0 + i;
+  const size_t row = SEG ? (size_t)i : g0 + i;
   if constexpr (WIDE) {
     RS_SMEM_LIST(kgr_sm)
     SmemList<T> L(lk, li, KP, a.k, lane);
-    if (!knn_ring_row<T, CD, PBC>(a, L, b, lane, xi, bl, binv, pc, cnt, end, g0, BN, sexcl[warp], sdelta[warp])) {
+    if (!knn_ring_row<T, CD, PBC>(a, L, g, lane, xi, bl, binv, pc, cnt, end, g0, BN, sexcl[warp], sdelta[warp])) {
       if (lane == 0) a.fb_rows[atomicAdd(a.fb_count, 1)] = (int)row;
       return;
     }
@@ -792,7 +897,7 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_ring_kernel(const RadArgs<T
     }
   } else {
     LaneList<T> L(qkey[warp], qidx[warp], a.k);
-    if (!knn_ring_row<T, CD, PBC>(a, L, b, lane, xi, bl, binv, pc, cnt, end, g0, BN, sexcl[warp], sdelta[warp])) {
+    if (!knn_ring_row<T, CD, PBC>(a, L, g, lane, xi, bl, binv, pc, cnt, end, g0, BN, sexcl[warp], sdelta[warp])) {
       if (lane == 0) a.fb_rows[atomicAdd(a.fb_count, 1)] = (int)row;
       return;
     }
@@ -805,8 +910,9 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_ring_kernel(const RadArgs<T
 
 // The listed rows, each against all N nodes of its graph with egnn_knn_select's rank: 1e5 to a padded node, and a NaN
 // rank ordered as (+inf, j + N), after every +inf and by index, written as j with ok = 0 (knn_block_sort_kernel's
-// rule).  Grid-stride over the list, whose length only the device knows.
-template <typename T, int CD, int PBC>
+// rule).  Grid-stride over the list, whose length only the device knows.  In the segment form a row is ranked against
+// the n_b nodes of its own graph, j on the node axis and N = T.
+template <typename T, int CD, int PBC, bool SEG = false>
 __global__ void __launch_bounds__(RS_WARPS * 32) knn_scan_kernel(const RadArgs<T> a, int KP) {
   extern __shared__ __align__(16) unsigned char kgs_sm[];
   const int warps = blockDim.x / 32, warp = threadIdx.x / 32, lane = threadIdx.x % 32;
@@ -814,31 +920,37 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_scan_kernel(const RadArgs<T
   const int rows = *a.fb_count;
   for (int r = blockIdx.x * warps + warp; r < rows; r += gridDim.x * warps) {
     const size_t row = (size_t)a.fb_rows[r];
-    const int b = (int)(row / a.N);
-    const size_t g0 = (size_t)b * a.N;
+    int b = (int)(row / a.N), nj = a.N;
+    if constexpr (SEG) {
+      seg_node(a, (int)row, b);                        // listed rows are on the grid
+      nj = a.ptr[b + 1] - a.ptr[b];
+    }
+    const GraphAt ga = graph_at<T, SEG>(a, b);
+    const size_t g0 = g0_of<T, SEG>(a, ga);
+    const int j0 = SEG ? (int)g0 : 0;                  // the node index of candidate 0
     T xi[CD];
 #pragma unroll
     for (int c = 0; c < CD; ++c) xi[c] = a.coors[row * CD + c];
     T bl[CD], binv[CD], pc[PBC == PBC_CELL ? CELL_STAGED : 1];
     if constexpr (PBC == PBC_CELL) {
 #pragma unroll
-      for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, b, CD, t);
+      for (int t = 0; t < CELL_STAGED; ++t) pc[t] = cell_staged<T>(a.box, lb_of<SEG>(ga), CD, t);
     } else if constexpr (PBC) {
 #pragma unroll
-      for (int c = 0; c < CD; ++c) box_axis<T>(a.box, b, CD, c, bl[c], binv[c]);
+      for (int c = 0; c < CD; ++c) box_axis<T>(a.box, lb_of<SEG>(ga), CD, c, bl[c], binv[c]);
     }
     SmemList<T> L(lk, li, KP, a.k, lane);
-    for (int j0 = 0; j0 < a.N; j0 += 32) {
-      const int j = j0 + lane;
+    for (int jb = 0; jb < nj; jb += 32) {
+      const int j = jb + lane;
       T key = T(INFINITY);
       int jk = 0x7fffffff;
       bool pass = false;
-      if (j < a.N) {
+      if (j < nj) {
         const T* xj = a.coors + (g0 + j) * CD;
         key = pair_rank<T, CD, PBC>(xi, [&](int c) { return xj[c]; }, CD, bl, binv, pc);
         if (a.mask && !a.mask[g0 + j]) key = T(1e5);
-        jk = j;
-        if (key != key) { key = T(INFINITY); jk = j + a.N; }
+        jk = j0 + j;
+        if (key != key) { key = T(INFINITY); jk = j0 + j + a.N; }
         pass = L.beats(key, jk);
       }
       L.push(pass, key, jk, lane);
@@ -857,54 +969,80 @@ __global__ void __launch_bounds__(RS_WARPS * 32) knn_scan_kernel(const RadArgs<T
 
 // One select on the radius grid (GRID_RADIUS) or the kNN grid (GRID_KNN): one memset of the bucket counts, then count /
 // scan / scatter into the grid's buckets and the query, one warp per row: radius_query_kernel; or, on the kNN grid,
-// knn_grid_setup_kernel first, then knn_ring_kernel and knn_scan_kernel for the rows it leaves.
-template <typename T, int CD, int PBC, int GRID>
+// knn_grid_setup_kernel first, then knn_ring_kernel and knn_scan_kernel for the rows it leaves.  The segment form (SEG)
+// launches the same sequence over the T nodes and G graphs of a packed batch; graphs off the grid exit at once.
+template <typename T, int CD, int PBC, int GRID, bool SEG = false>
 static int launch_grid(const RadArgs<T>& a, cudaStream_t st) {
-  const size_t nodes = (size_t)a.B * a.N;
+  const size_t nodes = SEG ? (size_t)a.N : (size_t)a.B * a.N;
   const unsigned gn = (unsigned)((nodes + RS_THREADS - 1) / RS_THREADS);
-  EGNN_CUDA_TRY(cudaMemsetAsync(a.cnt, 0, (size_t)a.B * a.Tb * sizeof(int), st));
+  EGNN_CUDA_TRY(cudaMemsetAsync(a.cnt, 0, (SEG ? 4 * nodes : (size_t)a.B * a.Tb) * sizeof(int), st));
   if constexpr (GRID == GRID_KNN) {
     EGNN_CUDA_TRY(cudaMemsetAsync(a.fb_count, 0, sizeof(int), st));
-    knn_grid_setup_kernel<T, CD, PBC><<<a.B, KG_SETUP_THREADS, 0, st>>>(a);
+    knn_grid_setup_kernel<T, CD, PBC, SEG><<<a.B, KG_SETUP_THREADS, 0, st>>>(a);
     EGNN_LAUNCH_CHECK();
   }
-  radius_count_kernel<T, CD, PBC, GRID><<<gn, RS_THREADS, 0, st>>>(a);
+  radius_count_kernel<T, CD, PBC, GRID, SEG><<<gn, RS_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
-  radius_scan_kernel<<<a.B, RS_SCAN_THREADS, 0, st>>>(a.cnt, a.end, a.Tb);
+  if constexpr (SEG) radius_scan_seg_kernel<T><<<a.B, RS_SCAN_THREADS, 0, st>>>(a);
+  else radius_scan_kernel<<<a.B, RS_SCAN_THREADS, 0, st>>>(a.cnt, a.end, a.Tb);
   EGNN_LAUNCH_CHECK();
-  radius_scatter_kernel<T, CD, PBC, GRID><<<gn, RS_THREADS, 0, st>>>(a);
+  radius_scatter_kernel<T, CD, PBC, GRID, SEG><<<gn, RS_THREADS, 0, st>>>(a);
   EGNN_LAUNCH_CHECK();
   // k <= 32: RS_WARPS rows per CTA, lists in lanes; larger k: SmemLists in dynamic shared memory
   const int KP = list_kp(a.k), warps = smem_list_warps(KP, sizeof(T));
   const size_t smem = warps * smem_list_bytes(KP, sizeof(T));
   const unsigned rows = (unsigned)((nodes + RS_WARPS - 1) / RS_WARPS), wide_rows = (unsigned)((nodes + warps - 1) / warps);
   if constexpr (GRID == GRID_KNN) {
-    if (a.k <= 32) knn_ring_kernel<T, CD, PBC, false><<<rows, RS_WARPS * 32, 0, st>>>(a, 0);
-    else knn_ring_kernel<T, CD, PBC, true><<<wide_rows, warps * 32, smem, st>>>(a, KP);
+    if (a.k <= 32) knn_ring_kernel<T, CD, PBC, false, SEG><<<rows, RS_WARPS * 32, 0, st>>>(a, 0);
+    else knn_ring_kernel<T, CD, PBC, true, SEG><<<wide_rows, warps * 32, smem, st>>>(a, KP);
     EGNN_LAUNCH_CHECK();
     int sms = 0;
     EGNN_TRY(sm_count(&sms));
-    knn_scan_kernel<T, CD, PBC><<<(wide_rows < 4u * sms ? wide_rows : 4u * sms), warps * 32, smem, st>>>(a, KP);
+    knn_scan_kernel<T, CD, PBC, SEG><<<(wide_rows < 4u * sms ? wide_rows : 4u * sms), warps * 32, smem, st>>>(a, KP);
     EGNN_LAUNCH_CHECK();
     count_launch(6);
   } else {
-    if (a.k <= 32) radius_query_kernel<T, CD, PBC><<<rows, RS_WARPS * 32, 0, st>>>(a);
-    else radius_query_wide_kernel<T, CD, PBC><<<wide_rows, warps * 32, smem, st>>>(a, KP);
+    if (a.k <= 32) radius_query_kernel<T, CD, PBC, SEG><<<rows, RS_WARPS * 32, 0, st>>>(a);
+    else radius_query_wide_kernel<T, CD, PBC, SEG><<<wide_rows, warps * 32, smem, st>>>(a, KP);
     EGNN_LAUNCH_CHECK();
     count_launch(4);
   }
   return EGNN_OK;
 }
 
+// The C x lattice instantiation of launch_grid.
+template <typename T, int GRID, bool SEG>
+static int grid_dispatch(const RadArgs<T>& a, int C, const void* box, int pbc, cudaStream_t st) {
+  if (box && pbc == PBC_CELL) {
+    if (C == 2) return launch_grid<T, 2, PBC_CELL, GRID, SEG>(a, st);
+    if (C == 3) return launch_grid<T, 3, PBC_CELL, GRID, SEG>(a, st);
+    return EGNN_ERR_SHAPE;
+  }
+  switch (C * 2 + (box ? 1 : 0)) {
+    case 2: return launch_grid<T, 1, PBC_NONE, GRID, SEG>(a, st);
+    case 3: return launch_grid<T, 1, PBC_BOX, GRID, SEG>(a, st);
+    case 4: return launch_grid<T, 2, PBC_NONE, GRID, SEG>(a, st);
+    case 5: return launch_grid<T, 2, PBC_BOX, GRID, SEG>(a, st);
+    case 6: return launch_grid<T, 3, PBC_NONE, GRID, SEG>(a, st);
+    case 7: return launch_grid<T, 3, PBC_BOX, GRID, SEG>(a, st);
+    default: return EGNN_ERR_UNSUPPORTED;
+  }
+}
+
 // r: the squared radius (GRID_RADIUS) or valid_radius (GRID_KNN) as the caller passes it; the kernels compare in T.
 // box: null, a [B,C] box, or a [B,C,C] cell under pbc = PBC_CELL.
+// The segment form (seg non-null: B = G graphs, N = T nodes): seg->ptr, seg->seg_valid and seg->min_n are taken over,
+// and the scratch is laid out for T nodes in 4 T buckets.
 template <typename T, int GRID>
 static int grid_select(int B, int N, int C, int k, const void* coors, const uint8_t* mask, const void* box, double r,
-                       int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws, cudaStream_t st, int pbc) {
-  const KnnWs L = knn_ws_layout(B, N, C, sizeof(T));        // the radius grid's scratch is its cell part
+                       int32_t* out_idx, uint8_t* out_ok, int32_t* out_count, void* ws, cudaStream_t st, int pbc,
+                       const RadArgs<T>* seg = nullptr) {
+  const KnnWs L = seg ? knn_ws_layout(B, (size_t)N, 4 * (size_t)N, C, sizeof(T))
+                      : knn_ws_layout(B, (size_t)B * N, (size_t)B * rs_buckets(N), C, sizeof(T));   // radius: the cell part
   char* base = static_cast<char*>(ws);
   RadArgs<T> a{};
-  a.B = B; a.N = N; a.k = k; a.Tb = rs_buckets(N);
+  a.B = B; a.N = N; a.k = k; a.Tb = seg ? 0 : rs_buckets(N);
+  if (seg) { a.ptr = seg->ptr; a.seg_valid = seg->seg_valid; a.min_n = seg->min_n; }
   a.coors = static_cast<const T*>(coors); a.mask = mask; a.box = static_cast<const T*>(box);
   a.cnt = reinterpret_cast<int*>(base + L.cell.cnt);
   a.end = reinterpret_cast<int*>(base + L.cell.end);
@@ -920,20 +1058,7 @@ static int grid_select(int B, int N, int C, int k, const void* coors, const uint
     a.r2 = (T)r;
     a.cs = sqrt((double)a.r2) * (1.0 + 0x1p-10);
   }
-  if (box && pbc == PBC_CELL) {
-    if (C == 2) return launch_grid<T, 2, PBC_CELL, GRID>(a, st);
-    if (C == 3) return launch_grid<T, 3, PBC_CELL, GRID>(a, st);
-    return EGNN_ERR_SHAPE;
-  }
-  switch (C * 2 + (box ? 1 : 0)) {
-    case 2: return launch_grid<T, 1, PBC_NONE, GRID>(a, st);
-    case 3: return launch_grid<T, 1, PBC_BOX, GRID>(a, st);
-    case 4: return launch_grid<T, 2, PBC_NONE, GRID>(a, st);
-    case 5: return launch_grid<T, 2, PBC_BOX, GRID>(a, st);
-    case 6: return launch_grid<T, 3, PBC_NONE, GRID>(a, st);
-    case 7: return launch_grid<T, 3, PBC_BOX, GRID>(a, st);
-    default: return EGNN_ERR_UNSUPPORTED;
-  }
+  return seg ? grid_dispatch<T, GRID, true>(a, C, box, pbc, st) : grid_dispatch<T, GRID, false>(a, C, box, pbc, st);
 }
 
 static int radius_check(int B, int N, int C, int k, int max_k) {
@@ -980,6 +1105,42 @@ int knn_grid_dispatch(int32_t dtype, int B, int N, int C, int k, const void* coo
                                          pbc);
   if (dtype != EGNN_DTYPE_F32) return EGNN_ERR_UNSUPPORTED;
   return grid_select<float, GRID_KNN>(B, N, C, k, coors, mask, box, valid_radius, out_idx, out_ok, nullptr, ws, st, pbc);
+}
+
+// ---------------------------------------------------------------- packed batches (segment_select.cu's grid entries)
+
+size_t packed_grid_ws_bytes(bool knn, int G, int T, int C) {
+  const KnnWs w = knn_ws_layout(G, (size_t)T, 4 * (size_t)T, C, 8);
+  return knn ? w.total : w.cell.total;
+}
+
+// The smallest graph a packed select puts on the grid: the unpacked threshold, read now, and at least k; INT_MAX when
+// this call puts none there (the radius grid with r outside (0, 1e5) in the coordinates' type, as cell_select_eligible).
+int packed_grid_min_n(bool knn, int32_t dtype, int k, double r) {
+  if (!knn) {
+    const double r2 = dtype == EGNN_DTYPE_F64 ? r : (double)(float)r;
+    if (!(r2 > 0.0 && r2 < 1e5)) return INT_MAX;
+  }
+  const long thr = knn ? knn_grid_min_n() : cell_select_min_n();
+  const long m = thr > k ? thr : k;
+  return m > INT_MAX ? INT_MAX : (int)m;
+}
+
+int packed_grid_launch(bool knn, int32_t dtype, int G, int T, int C, int k, int min_n, const int32_t* ptr,
+                       const int* seg_valid, const void* coors, const uint8_t* mask, const void* lattice, int pbc,
+                       double r, int32_t* out_idx, uint8_t* out_ok, void* ws, cudaStream_t st) {
+  if (dtype == EGNN_DTYPE_F64) {
+    RadArgs<double> s{};
+    s.ptr = ptr; s.seg_valid = seg_valid; s.min_n = min_n;
+    return knn ? grid_select<double, GRID_KNN>(G, T, C, k, coors, mask, lattice, r, out_idx, out_ok, nullptr, ws, st, pbc, &s)
+               : grid_select<double, GRID_RADIUS>(G, T, C, k, coors, mask, lattice, r, out_idx, out_ok, nullptr, ws, st,
+                                                  pbc, &s);
+  }
+  RadArgs<float> s{};
+  s.ptr = ptr; s.seg_valid = seg_valid; s.min_n = min_n;
+  return knn ? grid_select<float, GRID_KNN>(G, T, C, k, coors, mask, lattice, r, out_idx, out_ok, nullptr, ws, st, pbc, &s)
+             : grid_select<float, GRID_RADIUS>(G, T, C, k, coors, mask, lattice, r, out_idx, out_ok, nullptr, ws, st, pbc,
+                                               &s);
 }
 
 // The public entries: egnn_radius_select* with k <= 32, egnn_radius_select_wide* and egnn_knn_grid_select* with

@@ -16,6 +16,13 @@
 //           SEG_JC (coordinates as SoA and mask bytes), rank them and keep the top k in a LaneList (k <= 32) or a
 //           SmemList (k > 32).
 // Segment bounds are clamped to [0, T] on the device, so no ptr can make a kernel read or write out of range.
+//
+// The grid entries (egnn_radius_select_packed, egnn_knn_grid_select_packed) put every graph of at least the unpacked
+// threshold's nodes (and at least k) on the radius or kNN grid of radius_select.cu in its segment form, and the rest on
+// this select: seg_grid_tiles_kernel gives the grid graphs 0 row tiles and checks ptr (non-decreasing within [0, T]:
+// the graphs' node ranges and bucket regions are then disjoint; any other ptr puts every graph on this select), the
+// grid's launches follow, then the select.  A call whose largest graph is below the threshold issues the two launches
+// above and nothing else.
 #include "common.cuh"
 #include "profile.h"
 #include "warp_select.cuh"
@@ -68,6 +75,37 @@ __global__ void __launch_bounds__(SEG_TILE_THREADS) seg_tiles_kernel(const int32
     __syncthreads();                    // tmp is reused by the next chunk
   }
   if (threadIdx.x == 0) tile0[G] = carry;
+}
+
+// seg_tiles_kernel beside a grid: 0 tiles for each graph of at least min_n nodes when ptr is valid, whose validity goes
+// to *valid for the grid's kernels.
+__global__ void __launch_bounds__(SEG_TILE_THREADS) seg_grid_tiles_kernel(const int32_t* __restrict__ ptr, int G, int T,
+                                                                          int min_n, int* __restrict__ tile0,
+                                                                          int* __restrict__ valid) {
+  using Scan = cub::BlockScan<int, SEG_TILE_THREADS>;
+  __shared__ typename Scan::TempStorage tmp;
+  int bad = 0;
+  for (int g = threadIdx.x; g <= G; g += SEG_TILE_THREADS) {
+    const int v = ptr[g];
+    bad |= v < 0 || v > T || (g < G && ptr[g + 1] < v);
+  }
+  const bool ok = !__syncthreads_or(bad);
+  int carry = 0;
+  for (int g0 = 0; g0 < G; g0 += SEG_TILE_THREADS) {
+    const int g = g0 + threadIdx.x;
+    int tiles = 0;
+    if (g < G) {
+      int lo, hi;
+      seg_bounds(ptr, g, T, lo, hi);
+      tiles = ok && hi - lo >= min_n ? 0 : ceil_div(hi - lo, SEG_WARPS);
+    }
+    int excl, total;
+    Scan(tmp).ExclusiveSum(tiles, excl, total);
+    if (g < G) tile0[g] = carry + excl;
+    carry += total;
+    __syncthreads();                    // tmp is reused by the next chunk
+  }
+  if (threadIdx.x == 0) { tile0[G] = carry; *valid = ok ? 1 : 0; }
 }
 
 // Shared memory of the select: staged coordinates [C][SEG_JC], the lists of SEG_WARPS warps, mask bytes [SEG_JC].
@@ -199,10 +237,11 @@ static int seg_check(int G, int T, int C, int k, int pbc) {
   return EGNN_OK;
 }
 
+// tiles_done: tile0 (ws) was written by seg_grid_tiles_kernel, so only the select is launched.
 template <typename T>
 static int seg_select(int G, int Tn, int C, int k, const int32_t* ptr, const void* coors, const uint8_t* mask,
                       const void* lattice, int pbc, double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* ws,
-                      cudaStream_t st) {
+                      cudaStream_t st, bool tiles_done = false) {
   SegArgs<T> a;
   a.G = G; a.T_ = Tn; a.C = C; a.k = k;
   a.ptr = ptr;
@@ -213,9 +252,13 @@ static int seg_select(int G, int Tn, int C, int k, const int32_t* ptr, const voi
   a.out_idx = out_idx; a.out_ok = out_ok;
   a.tile0 = static_cast<const int*>(ws);
   a.KP = k > 32 ? list_kp(k) : 0;
-  seg_tiles_kernel<<<1, SEG_TILE_THREADS, 0, st>>>(ptr, G, Tn, static_cast<int*>(ws));
-  EGNN_LAUNCH_CHECK();
-  count_launch(2);
+  if (tiles_done) {
+    count_launch(1);
+  } else {
+    seg_tiles_kernel<<<1, SEG_TILE_THREADS, 0, st>>>(ptr, G, Tn, static_cast<int*>(ws));
+    EGNN_LAUNCH_CHECK();
+    count_launch(2);
+  }
   if (!lattice) return launch_seg_c<T, PBC_NONE>(a, st);
   if (pbc == PBC_CELL) return launch_seg_c<T, PBC_CELL>(a, st);
   return launch_seg_c<T, PBC_BOX>(a, st);
@@ -233,6 +276,56 @@ static int seg_entry(int pbc, int32_t dtype, int32_t G, int32_t T, int32_t C, in
   if (dtype == EGNN_DTYPE_F64)
     return seg_select<double>(G, T, C, k, ptr, coors, mask, lattice, pbc, valid_radius, out_idx, out_ok, workspace, st);
   return seg_select<float>(G, T, C, k, ptr, coors, mask, lattice, pbc, valid_radius, out_idx, out_ok, workspace, st);
+}
+
+// ---------------------------------------------------------------- the grid entries
+
+// Scratch: tile0 [G+1] and the validity flag, then the grid's (packed_grid_ws_bytes).
+static size_t seg_grid_head_bytes(int G) { return round_up((size_t)(G + 2) * sizeof(int), 256); }
+
+static int seg_grid_check(int G, int T, int C, int k, int pbc) {
+  EGNN_TRY(seg_check(G, T, C, k, pbc));
+  if (4LL * T > 0x7fffffffLL) return EGNN_ERR_SHAPE;   // int bucket offsets 4 ptr[g]
+  return EGNN_OK;
+}
+
+static size_t seg_grid_ws_bytes(bool knn, int G, int T, int C) {
+  return seg_grid_head_bytes(G) + (C <= 3 ? packed_grid_ws_bytes(knn, G, T, C) : 0);
+}
+
+static int seg_grid_entry(bool knn, int pbc, int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                          const int32_t* ptr, const void* coors, const uint8_t* mask, const void* lattice,
+                          double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                          size_t workspace_bytes, void* stream) {
+  if (!ptr || !coors || !out_idx || !workspace || (pbc == PBC_CELL && !lattice) || (!knn && !out_ok))
+    return EGNN_ERR_NULL;
+  EGNN_TRY(seg_grid_check(G, T, C, k, pbc));
+  if (dtype != EGNN_DTYPE_F32 && dtype != EGNN_DTYPE_F64) return EGNN_ERR_UNSUPPORTED;
+  if ((uintptr_t)workspace & 0xFF) return EGNN_ERR_ALIGN;
+  if (workspace_bytes < seg_grid_ws_bytes(knn, G, T, C)) return EGNN_ERR_WORKSPACE;
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const bool f64 = dtype == EGNN_DTYPE_F64;
+  const int min_n = C <= 3 ? packed_grid_min_n(knn, dtype, k, valid_radius) : INT_MAX;
+  if (max_n < min_n)                                 // no graph is large enough: the segmented select alone
+    return f64 ? seg_select<double>(G, T, C, k, ptr, coors, mask, lattice, pbc, valid_radius, out_idx, out_ok, workspace, st)
+               : seg_select<float>(G, T, C, k, ptr, coors, mask, lattice, pbc, valid_radius, out_idx, out_ok, workspace, st);
+  int* tile0 = static_cast<int*>(workspace);
+  seg_grid_tiles_kernel<<<1, SEG_TILE_THREADS, 0, st>>>(ptr, G, T, min_n, tile0, tile0 + G + 1);
+  EGNN_LAUNCH_CHECK();
+  count_launch(1);
+  EGNN_TRY(packed_grid_launch(knn, dtype, G, T, C, k, min_n, ptr, tile0 + G + 1, coors, mask, lattice, pbc, valid_radius,
+                              out_idx, out_ok, static_cast<char*>(workspace) + seg_grid_head_bytes(G), st));
+  return f64 ? seg_select<double>(G, T, C, k, ptr, coors, mask, lattice, pbc, valid_radius, out_idx, out_ok, workspace, st,
+                                  true)
+             : seg_select<float>(G, T, C, k, ptr, coors, mask, lattice, pbc, valid_radius, out_idx, out_ok, workspace, st,
+                                 true);
+}
+
+static int seg_grid_ws_entry(bool knn, int32_t G, int32_t T, int32_t C, int32_t k, size_t* out_bytes) {
+  if (!out_bytes) return EGNN_ERR_NULL;
+  EGNN_TRY(seg_grid_check(G, T, C, k, PBC_NONE));
+  *out_bytes = seg_grid_ws_bytes(knn, G, T, C);
+  return EGNN_OK;
 }
 
 }  // namespace egnn
@@ -259,4 +352,47 @@ extern "C" int egnn_knn_select_packed_triclinic(int32_t dtype, int32_t G, int32_
                                                 void* stream) {
   return egnn::seg_entry(egnn::PBC_CELL, dtype, G, T, C, k, ptr, coors, mask, cell, valid_radius, out_idx, out_ok,
                          workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_radius_select_packed_workspace_bytes(int32_t G, int32_t T, int32_t C, int32_t k, size_t* out_bytes) {
+  return egnn::seg_grid_ws_entry(false, G, T, C, k, out_bytes);
+}
+
+extern "C" int egnn_radius_select_packed(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                                         const int32_t* ptr, const void* coors, const uint8_t* mask, const void* box,
+                                         double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                         size_t workspace_bytes, void* stream) {
+  return egnn::seg_grid_entry(false, egnn::PBC_BOX, dtype, G, T, C, k, max_n, ptr, coors, mask, box, valid_radius,
+                              out_idx, out_ok, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_radius_select_packed_triclinic(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k,
+                                                   int32_t max_n, const int32_t* ptr, const void* coors,
+                                                   const uint8_t* mask, const void* cell, double valid_radius,
+                                                   int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                                   size_t workspace_bytes, void* stream) {
+  return egnn::seg_grid_entry(false, egnn::PBC_CELL, dtype, G, T, C, k, max_n, ptr, coors, mask, cell, valid_radius,
+                              out_idx, out_ok, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_knn_grid_select_packed_workspace_bytes(int32_t G, int32_t T, int32_t C, int32_t k,
+                                                           size_t* out_bytes) {
+  return egnn::seg_grid_ws_entry(true, G, T, C, k, out_bytes);
+}
+
+extern "C" int egnn_knn_grid_select_packed(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                                           const int32_t* ptr, const void* coors, const uint8_t* mask, const void* box,
+                                           double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                           size_t workspace_bytes, void* stream) {
+  return egnn::seg_grid_entry(true, egnn::PBC_BOX, dtype, G, T, C, k, max_n, ptr, coors, mask, box, valid_radius,
+                              out_idx, out_ok, workspace, workspace_bytes, stream);
+}
+
+extern "C" int egnn_knn_grid_select_packed_triclinic(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k,
+                                                     int32_t max_n, const int32_t* ptr, const void* coors,
+                                                     const uint8_t* mask, const void* cell, double valid_radius,
+                                                     int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                                     size_t workspace_bytes, void* stream) {
+  return egnn::seg_grid_entry(true, egnn::PBC_CELL, dtype, G, T, C, k, max_n, ptr, coors, mask, cell, valid_radius,
+                              out_idx, out_ok, workspace, workspace_bytes, stream);
 }

@@ -422,9 +422,11 @@ class EGNN(nn.Module):
         tensor ptr [G+1] (ptr[0] = 0, non-decreasing, ptr[G] = T; any device).  Every graph gets what it would get
         alone, to the rounding of the kernel type: with num_nearest_neighbors = k, its k nearest nodes of its own
         graph (all of its nodes, with mean pooling over them, when it has fewer than k); without, all of its nodes
-        (dense).  The lists are ranked on the device by `egnn_knn_select_packed` in O(sum_g n_g^2) -- the all-pairs
-        cost of each graph alone, not of the batch padded to its largest graph -- and the layer runs on them in
-        edge-list mode, forward and backward.  `mask` [1, T] and one `box` [C] or `cell` [C, C] shared by every graph
+        (dense).  The lists are ranked on the device as each graph's unpacked call would rank them: on the radius grid
+        (a mask and 0 < valid_radius < 1e5) or the kNN grid for graphs of at least EGNN_B200_CELL_SELECT_MIN_N /
+        EGNN_B200_KNN_GRID_MIN_N nodes (C <= 3), in O(n_g); otherwise by the segmented all-pairs select in O(n_g^2) --
+        the cost of each graph alone, not of the batch padded to its largest graph.  The lists are the same either
+        way, and the layer runs on them in edge-list mode, forward and backward.  `mask` [1, T] and one `box` [C] or `cell` [C, C] shared by every graph
         combine with it; per-graph lattices, `neighbors`, `neighbor_edges`, dense `edges`, adjacency and
         only_sparse_neighbors do not (ValueError).  ptr's values are read on the host once per tensor version."""
         if ptr is not None:
@@ -472,8 +474,11 @@ class EGNN(nn.Module):
             m = _as_u8(mask, dev)
             if self.num_nearest_neighbors > 0:
                 cdt = torch.float64 if self._kernel_dtype() == torch.float64 else torch.float32   # as the layer's select
+                # a masked layer with a radius the radius grid serves keeps only in-radius slots: radius mode
+                mode = "radius" if m is not None and _in_cell_radius(self.valid_radius, cdt) else "knn"
                 idx, ok = _packed_select(_as(coors, dev, cdt), ptr, min(self.num_nearest_neighbors, max_n), m,
-                                         _packed_lattice(box, cell, dev, cdt, c), cell is not None, self.valid_radius)
+                                         _packed_lattice(box, cell, dev, cdt, c), cell is not None, self.valid_radius,
+                                         mode, max_n)
                 lists = idx if m is None else idx.masked_fill(ok == 0, -1)
             else:
                 lists = _dense_packed_lists(ptr, t, max_n, dev)
@@ -844,22 +849,47 @@ def _packed_lattice(box, cell, dev, dtype, c):
     return None if box is None else _as(box, dev, dtype).reshape(c).contiguous()
 
 
-def _packed_select(x, ptr, k, m, lattice, triclinic, valid_radius):
-    """egnn_knn_select_packed on staged inputs on the current device: x [1, T, C] float32 / float64, m uint8 [1, T] or
-    None, lattice [C] or [C, C] (triclinic) in x's type or None -> (idx int32, ok uint8), both [1, T, k]."""
+_PACKED_GRID_MAX_T = (1 << 29) - 1       # 4 T bucket offsets stay an int in the grid entries
+
+
+def _packed_entry(mode, t, c, k):
+    """The library entry a packed select in `mode` runs: "knn" (egnn_knn_grid_select_packed: graphs large enough go on
+    the kNN grid) or "radius" (egnn_radius_select_packed: on the radius grid) where the grids serve the call (C <= 3,
+    k <= 256, T within the grid's int offsets), else egnn_knn_select_packed (mode None: the all-pairs select alone)."""
+    if mode is None or c > 3 or k > 256 or t > _PACKED_GRID_MAX_T:
+        return "egnn_knn_select_packed"
+    return "egnn_radius_select_packed" if mode == "radius" else "egnn_knn_grid_select_packed"
+
+
+def _in_cell_radius(r2, dtype):
+    """0 < r2 < 1e5 in `dtype`, as the select compares it: the radius the radius grid serves (above, a padded pair's
+    1e5 rank would count as in range)."""
+    r2 = torch.tensor(float(r2), dtype=dtype).item()
+    return 0.0 < r2 < 1e5
+
+
+def _packed_select(x, ptr, k, m, lattice, triclinic, valid_radius, mode=None, max_n=None):
+    """The packed select on staged inputs on the current device: x [1, T, C] float32 / float64, m uint8 [1, T] or
+    None, lattice [C] or [C, C] (triclinic) in x's type or None -> (idx int32, ok uint8), both [1, T, k].  `mode`
+    (_packed_entry) "knn": idx and ok of egnn_knn_select_packed, with the graphs of at least the kNN grid's threshold
+    on that grid; "radius": its ok, and its idx in every ok = 1 slot, with the graphs of at least the radius grid's
+    threshold on that grid (the callers empty the ok = 0 slots).  max_n: the largest graph's node count."""
     lib = nat.load()
     t, c = x.shape[1], x.shape[2]
     dev = x.device
     p32 = ptr.to(device=dev, dtype=torch.int32, non_blocking=True).contiguous()
+    entry = _packed_entry(mode, t, c, k)
+    grid = entry != "egnn_knn_select_packed"
     nb = C.c_size_t()
-    nat.check("egnn_knn_select_packed_workspace_bytes",
-              lib.egnn_knn_select_packed_workspace_bytes(p32.numel() - 1, t, c, k, C.byref(nb)))
+    nat.check(f"{entry}_workspace_bytes",
+              getattr(lib, f"{entry}_workspace_bytes")(p32.numel() - 1, t, c, k, C.byref(nb)))
     stream = torch.cuda.current_stream(dev).cuda_stream
     ws = _workspace(dev, nb.value, stream)
     idx = torch.empty((1, t, k), dtype=torch.int32, device=dev)
     ok = torch.empty((1, t, k), dtype=torch.uint8, device=dev)
-    name = "egnn_knn_select_packed" + ("_triclinic" if triclinic else "")
-    nat.check(name, getattr(lib, name)(_KERNEL_DTYPE[x.dtype], p32.numel() - 1, t, c, k, _ptr(p32), _ptr(x), _ptr(m),
+    name = entry + ("_triclinic" if triclinic else "")
+    nat.check(name, getattr(lib, name)(_KERNEL_DTYPE[x.dtype], p32.numel() - 1, t, c, k,
+                                       *((int(max_n),) if grid else ()), _ptr(p32), _ptr(x), _ptr(m),
                                        _ptr(lattice), float(valid_radius), _ptr(idx), _ptr(ok), _ptr(ws), ws.numel(),
                                        C.c_void_p(stream)))
     return idx, ok
@@ -934,10 +964,11 @@ def radius_neighbors(coors, cutoff, k, *, mask=None, box=None, cell=None, return
     Nothing synchronises with the host: the call can be captured in a CUDA graph.
 
     With `ptr` (a packed batch: coors [1, T, C] holding G graphs end to end, `ptr` [G+1] their offsets, as
-    `EGNN.forward(ptr=)` takes them) every node is ranked against the nodes of its own graph only, in O(sum_g n_g^2) by
-    `egnn_knn_select_packed` instead of on the cell grid: the lists equal the per-graph calls' concatenated, indices
-    shifted by ptr[g], with -1 also in the slots past a graph's size (`k` up to 32 whatever the graph sizes).  `box` /
-    `cell` is then one lattice shared by every graph; `return_counts` is not available."""
+    `EGNN.forward(ptr=)` takes them) every node is ranked against the nodes of its own graph only
+    (`egnn_radius_select_packed`): on the cell grid for graphs of at least EGNN_B200_CELL_SELECT_MIN_N nodes (4096)
+    and k, by the segmented all-pairs select in O(n_g^2) below: the lists equal the per-graph calls' concatenated,
+    indices shifted by ptr[g], with -1 also in the slots past a graph's size (`k` up to 32 whatever the graph sizes).
+    `box` / `cell` is then one lattice shared by every graph; `return_counts` is not available."""
     return _radius_graph("radius_neighbors", 32, coors, cutoff, k, mask, box, cell, return_counts, ptr)
 
 
@@ -947,7 +978,7 @@ def radius_neighbors_wide(coors, cutoff, k, *, mask=None, box=None, cell=None, r
     slots; `return_counts=True` also returns the in-radius counts before truncation.  For k <= 32 the result is
     `radius_neighbors`'s.  Longer lists (40-100 neighbours within a cutoff are common in condensed-phase atomistic
     systems) are kept in shared memory instead of one warp's lanes (`egnn_radius_select_wide`).  `ptr`: a packed
-    batch, as `radius_neighbors` takes it (O(sum_g n_g^2), `k` up to 256)."""
+    batch, as `radius_neighbors` takes it (the cell grid for large graphs, `k` up to 256)."""
     return _radius_graph("radius_neighbors_wide", 256, coors, cutoff, k, mask, box, cell, return_counts, ptr)
 
 
@@ -1029,10 +1060,11 @@ def knn_neighbors(coors, k, *, mask=None, box=None, cell=None, ptr=None):
     wrapped pair vector).  Nothing synchronises with the host: the call can be captured in a CUDA graph.
 
     With `ptr` (a packed batch: coors [1, T, C] holding G graphs end to end, `ptr` [G+1] their offsets, as
-    `EGNN.forward(ptr=)` takes them) every node is ranked against the nodes of its own graph only, in O(sum_g n_g^2) by
-    `egnn_knn_select_packed` instead of on the kNN grid: the lists equal the per-graph calls' concatenated, indices
-    shifted by ptr[g], with -1 also in the slots past a graph's size (`k` up to 256 whatever the graph sizes).  `box` /
-    `cell` is then one lattice shared by every graph."""
+    `EGNN.forward(ptr=)` takes them) every node is ranked against the nodes of its own graph only
+    (`egnn_knn_grid_select_packed`): on the kNN grid for graphs of at least EGNN_B200_KNN_GRID_MIN_N nodes (8192)
+    and k, by the segmented all-pairs select in O(n_g^2) below: the lists equal the per-graph calls' concatenated,
+    indices shifted by ptr[g], with -1 also in the slots past a graph's size (`k` up to 256 whatever the graph sizes).
+    `box` / `cell` is then one lattice shared by every graph."""
     if ptr is not None:
         return _packed_graph("knn_neighbors", 256, coors, None, k, mask, box, cell, False, ptr)
     b, n, c = _check_graph_args("knn_neighbors", 256, coors, k, mask, box, cell)
@@ -1069,13 +1101,15 @@ def _radius_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts,
 
 
 def _packed_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts, ptr):
-    """The builders on a packed batch: the segmented select, then each builder's -1 rules.  kNN (`cutoff` None): -1 in
-    slots that point at a padded node or at a node with a non-finite coordinate, and in every slot of a padded row
-    (knn_neighbors).  Radius: the kept slots are the ok = 1 slots of the select with valid_radius = cutoff^2 and no
-    mask, on coordinates where a padded node's are NaN -- its ranks are then NaN, never kept, and its own row is empty,
-    as the radius grid leaves them; a node with a non-finite coordinate ranks inf or NaN against every node, itself
-    included, and is never kept either."""
+    """The builders on a packed batch: the packed select (kNN or radius mode, _packed_select), then each builder's -1
+    rules.  kNN (`cutoff` None): -1 in slots that point at a padded node or at a node with a non-finite coordinate, and
+    in every slot of a padded row (knn_neighbors).  Radius: the kept slots are the ok = 1 slots of the select with
+    valid_radius = cutoff^2 and the caller's mask -- a padded node ranks 1e5 > cutoff^2 against every node, so it is
+    never kept and its own row is empty, as the radius grid leaves them; a node with a non-finite coordinate ranks inf
+    or NaN against every node, itself included, and is never kept either.  Where cutoff^2 reaches 1e5 a padded node's
+    coordinates are made NaN instead of passing the mask, to the same effect."""
     b, n, c = _check_graph_args(name, max_k, coors, k, mask, box, cell, cutoff, ptr)
+    max_n = _check_ptr(ptr, b, n)
     if return_counts:
         raise ValueError(f"{name}: return_counts is not available with ptr=")
     dev = _compute_device(coors)
@@ -1083,7 +1117,7 @@ def _packed_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts,
         x, m = _as(coors, dev, coors.dtype), _as_u8(mask, dev)
         lat = _packed_lattice(box, cell, dev, coors.dtype, c)
         if cutoff is None:
-            out, _ = _packed_select(x, ptr, k, m, lat, cell is not None, float("inf"))
+            out, _ = _packed_select(x, ptr, k, m, lat, cell is not None, float("inf"), "knn", max_n)
             usable = torch.isfinite(x).all(dim=-1)                               # [1, T]: nodes the layer uses
             if m is not None:
                 usable = usable & m.bool()
@@ -1092,9 +1126,10 @@ def _packed_graph(name, max_k, coors, cutoff, k, mask, box, cell, return_counts,
             keep = filled & torch.gather(usable, 1, out.clamp_min(0).view(b, n * k).long()).view(b, n, k)
             keep &= row_ok.unsqueeze(-1)
         else:
-            if m is not None:
-                x = x.masked_fill(~m.bool().unsqueeze(-1), float("nan"))
-            out, ok = _packed_select(x, ptr, k, None, lat, cell is not None, float(cutoff) * float(cutoff))
+            r2 = float(cutoff) * float(cutoff)
+            if m is not None and not _in_cell_radius(r2, coors.dtype):
+                x, m = x.masked_fill(~m.bool().unsqueeze(-1), float("nan")), None
+            out, ok = _packed_select(x, ptr, k, m, lat, cell is not None, r2, "radius", max_n)
             keep = ok.bool()
         out = out.masked_fill(~keep, -1)
     return out if out.device == coors.device else out.to(coors.device)

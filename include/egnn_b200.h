@@ -383,6 +383,37 @@ int egnn_knn_select_packed_triclinic(int32_t dtype, int32_t G, int32_t T, int32_
                                      int32_t* out_idx, uint8_t* out_ok, void* workspace, size_t workspace_bytes,
                                      void* stream);
 
+/* egnn_knn_select_packed with the graphs large enough on a cell grid, as each graph's unpacked call would run: the
+ * arguments of egnn_knn_select_packed(_triclinic) plus max_n, the node count of the largest graph (it only decides
+ * whether the grid is launched at all).  Graph g goes on the grid when C <= 3, n_g >= k and n_g reaches the threshold
+ * read at this call; every other graph (and every graph when ptr is not non-decreasing within [0, T]) on the segmented
+ * all-pairs select.  When max_n is below the threshold, the call issues exactly egnn_knn_select_packed's launches.
+ * T <= 2^29 - 1 (4 T bucket offsets stay an int, else EGNN_ERR_SHAPE).  workspace: the entry's _workspace_bytes(G, T,
+ * C, k) bytes (O(G + T), a function of G, T and C).  No host synchronisation.
+ *   egnn_knn_grid_select_packed: the kNN grid from EGNN_B200_KNN_GRID_MIN_N nodes (8192); out_idx and out_ok equal
+ *     egnn_knn_select_packed's bit for bit.
+ *   egnn_radius_select_packed: the radius grid from EGNN_B200_CELL_SELECT_MIN_N nodes (4096), when 0 < valid_radius
+ *     < 1e5 in the coordinates' type (the squared cutoff); out_ok (required) equals egnn_knn_select_packed's and
+ *     out_idx equals its idx in every ok = 1 slot (the kept slots; the rest are unspecified). */
+int egnn_radius_select_packed_workspace_bytes(int32_t G, int32_t T, int32_t C, int32_t k, size_t* out_bytes);
+int egnn_radius_select_packed(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                              const int32_t* ptr, const void* coors, const uint8_t* mask, const void* box,
+                              double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                              size_t workspace_bytes, void* stream);
+int egnn_radius_select_packed_triclinic(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                                        const int32_t* ptr, const void* coors, const uint8_t* mask, const void* cell,
+                                        double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                        size_t workspace_bytes, void* stream);
+int egnn_knn_grid_select_packed_workspace_bytes(int32_t G, int32_t T, int32_t C, int32_t k, size_t* out_bytes);
+int egnn_knn_grid_select_packed(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                                const int32_t* ptr, const void* coors, const uint8_t* mask, const void* box,
+                                double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                size_t workspace_bytes, void* stream);
+int egnn_knn_grid_select_packed_triclinic(int32_t dtype, int32_t G, int32_t T, int32_t C, int32_t k, int32_t max_n,
+                                          const int32_t* ptr, const void* coors, const uint8_t* mask, const void* cell,
+                                          double valid_radius, int32_t* out_idx, uint8_t* out_ok, void* workspace,
+                                          size_t workspace_bytes, void* stream);
+
 /* N-th degree adjacency of EGNN_Network (egnn_pytorch.py:414-428) without the dense A@A:
  * adj_in [N,N] or [B,N,N] 0/1; writes the expanded adjacency adj_out [B,N,N] 0/1, the degree
  * labels labels_out [B,N,N] (0 = not connected, d = first reached in round d) and

@@ -9,7 +9,7 @@ sorted.  The trailing periodic-boundary template argument PBC of the kernels tha
 both logs (it was a bool, false / true, before triclinic cells made it none / box / cell = 0 / 1 / 2), so a kernel
 that existing calls run keeps its name across that change.  pair_bwd3_kernel's trailing lattice-gradient argument
 LAT and tc_knn_kernel's trailing slot-group argument WIDE are dropped from the name when they are false, for the same
-reason.  Prints a unified diff of the two listings: a line present
+reason, and so is the trailing segment-form argument SEG of the cell-grid kernels (SEG_KERNELS).  Prints a unified diff of the two listings: a line present
 in both is an instantiation whose registers, spills, stack and shared memory are unchanged."""
 import difflib
 import re
@@ -19,6 +19,10 @@ import sys
 PBC_KERNELS = ("pair_kernel<", "pair_dense_tiled_kernel<", "pair_bwd1_kernel<", "pair_bwd3_kernel<",
                "knn_warp_select_kernel<", "knn_block_sort_kernel<", "tc_knn_kernel<", "tc_pair_kernel<",
                "radius_count_kernel<", "radius_scatter_kernel<", "radius_query_kernel<")
+
+SEG_KERNELS = {"knn_grid_setup_kernel<": 4, "radius_count_kernel<": 5, "radius_scatter_kernel<": 5,   # template arguments
+               "radius_query_kernel<": 4, "radius_query_wide_kernel<": 4, "knn_ring_kernel<": 5,      # with SEG
+               "knn_scan_kernel<": 4}
 
 
 def entries(path):
@@ -42,6 +46,8 @@ def entries(path):
         if "pair_bwd3_kernel<" in name or "tc_knn_kernel<" in name:     # the trailing LAT / WIDE argument: dropped when false
             name = re.sub(r"(\(int\)\d), \(bool\)([01])>\(",    # before it), written as `true` otherwise
                           lambda m: m.group(1) + (">(" if m.group(2) == "0" else ", (bool)true>("), name, count=1)
+        if any(k in name and name.split(">(", 1)[0].count(",") + 1 == n for k, n in SEG_KERNELS.items()):
+            name = re.sub(r", \(bool\)([01])>\(", lambda m: ">(" if m.group(1) == "0" else ", (bool)true>(", name, count=1)
         if any(k in name for k in PBC_KERNELS):
             name = re.sub(r", \(bool\)([01])>\(", r", (int)\1>(", name, count=1)
         lines.append(f"{name} | {regs} | {frame}\n")
